@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the camera->BEV lift (BASELINE.json metric: lift frames/sec, 6-cam 224x480 -> 200x200).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3_baseline]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3_baseline] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path {head tensor, intrinsics, extrinsics} -> BEV (B', C, X, Y) over one batch of
 synthetic frames (SURVEY.md section 8d).  Prints ONE JSON line (rank 0).
@@ -11,12 +11,16 @@ synthetic frames (SURVEY.md section 8d).  Prints ONE JSON line (rank 0).
   e2e        same metric with HOST (pinned) inputs and a host copy of the BEV inside the timed region
   roofline   the PATH against the measured HBM copy bandwidth (MEASURED_PEAKS.json): algorithmic bytes of the step / step time;
              `kernels` lists every kernel of the step with its OWN algorithmic bytes, the duration of the launches the step really
-             runs (event pairs on their streams, fiery_lift_forward_timed) and the ncu DRAM bytes of the committed capture
+             runs (event pairs on their streams, fiery_lift_forward_timed)
   roofline_bwd  the same for the backward (grad of the head tensor)
   cpu_baseline  the oracle's torch-CPU restatement of the reference op chain on this box's host cores, bounded sample
 
-`--impl reference` times that CPU restatement itself (the reference is pure PyTorch; /root/reference is not on the GPU
-box, oracle/lift_oracle.py restates it op for op and is pinned to it by oracle/gen_golden.py).
+`--impl reference` times that CPU restatement itself (the reference is pure PyTorch; oracle/lift_oracle.py restates it op for op
+and is pinned to it by the golden vectors oracle/gen_golden.py recorded under tests/golden/).
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step as DIR/<name>.npy (float32 / float64, at most
+64 MB in all; a larger output is written as a fixed, seeded sample of its elements).  The inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -39,18 +43,41 @@ from fiery_b200.synthetic import CONFIGS, LiftConfig, make_calibration, make_gra
 
 METRIC = "camera->BEV lift frames/sec (6-cam 224x480 -> 200x200)"
 L2_FLUSH_BYTES = 256 << 20
+DUMP_BUDGET_BYTES = 64 << 20
+# NVIDIA H100 SXM data sheet, for a card allowed up to 700 W: HBM3 bandwidth, dense BF16 tensor-core rate
+H100_HBM_GBS, H100_BF16_TFLOPS = 3350.0, 989.0
 
 
-def load_traffic(workload: str):
-    """ncu DRAM bytes (read + write) per step of every kernel of this workload, from the committed captures
-    (profiles/traffic.json: {workload: {kernel: bytes per step}}); {} when there is no capture."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
+def dump_outputs(out_dir: str, arrays: dict):
+    """Writes every array as out_dir/<name>.npy (float32, or float64 for float64 input).  When the arrays together exceed
+    DUMP_BUDGET_BYTES, each one is cut to the same fraction of its elements: a seeded, sorted sample of flat indices, so the same shape
+    always yields the same positions."""
+    os.makedirs(out_dir, exist_ok=True)
+    host = {}
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+        host[name] = a.astype(np.float64 if a.dtype == np.float64 else np.float32, copy=False)
+    total = sum(a.nbytes for a in host.values())
+    keep = min(1.0, (DUMP_BUDGET_BYTES - 4096) / total) if total else 1.0      # 4 KB of room for the one element every array keeps
+    for name, a in host.items():
+        flat = a.reshape(-1)
+        if keep < 1.0:
+            n = max(1, int(flat.size * keep))
+            flat = flat[np.sort(np.random.default_rng(0).choice(flat.size, size=n, replace=False))]
+            a = flat
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
+
+
+def device_info(index: int):
+    """Name and power limit of the GPU the numbers were measured on (power limit: nvidia-smi, None when it is unavailable)."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
     try:
-        with open(path) as fh:
-            v = json.load(fh).get(workload)
-        return {k: int(b) for k, b in v.items()} if isinstance(v, dict) else {}
-    except (OSError, ValueError):
-        return {}
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return info
 
 
 def load_peaks():
@@ -58,7 +85,7 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return H100_HBM_GBS, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -127,10 +154,11 @@ def _best_thread_count(oracle, head, K, E, candidates):
     return best
 
 
-def time_cpu_reference(cfg: LiftConfig, frames: int, reps: int, warmup: int = 1, backward: bool = False):
+def time_cpu_reference(cfg: LiftConfig, frames: int, reps: int, warmup: int = 1, backward: bool = False, last: dict = None):
     """Times the oracle's torch-CPU restatement of the reference op chain (fiery.py:193-273, encoder.py:99-100,
     geometry.py:283-314) on the host cores, at the thread count that is fastest on this box.
-    Returns (frames_per_s, seconds_per_call, threads)."""
+    Returns (frames_per_s, seconds_per_call, threads); ``last["out"]`` (when given) receives the last rep's result: the BEV, or
+    the gradient of the head tensor with ``backward``."""
     from oracle import lift_oracle as O
     cores = os.cpu_count() or 1
     sub = LiftConfig(**{**cfg.__dict__, "frames": frames})
@@ -150,8 +178,10 @@ def time_cpu_reference(cfg: LiftConfig, frames: int, reps: int, warmup: int = 1,
     ts = []
     for _ in range(reps):
         t0 = time.perf_counter()
-        cpu_lift_once(oracle, head, K, E, gout)
+        out = cpu_lift_once(oracle, head, K, E, gout)
         ts.append(time.perf_counter() - t0)
+    if last is not None:
+        last["out"] = out
     sec = float(np.median(ts))
     return frames / sec, sec, threads
 
@@ -170,8 +200,11 @@ def run_reference(args, cfg: LiftConfig, rank: int):
         return
     frames = cfg.frames                       # the same batch the GPU arm lifts per step
     steps = max(1, args.steps)
+    last = {}
     fps, sec, threads = time_cpu_reference(cfg, frames, reps=steps, warmup=max(1, min(args.warmup, 2)),
-                                           backward=(args.direction == "fwd_bwd"))
+                                           backward=(args.direction == "fwd_bwd"), last=last)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"grad_head" if args.direction == "fwd_bwd" else "bev": last["out"]})
     line = {
         "impl": "reference", "metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": args.gpus, "steps": steps,
         "warmup": args.warmup, "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak",
@@ -231,8 +264,10 @@ def run_train(args, cfg: LiftConfig, rank: int, local_rank: int, world: int):
         torch.cuda.synchronize()
         return float(np.mean([a.elapsed_time(e) for a, e in pairs]))
 
+    last = {}
+
     def step_dev():
-        trainer.step(batch)
+        last["loss"] = trainer.step(batch)
 
     def step_e2e():                                   # the step's inputs come from pinned host memory, its loss goes back to the host
         dev_batch = {k: v.to(dev, non_blocking=True) for k, v in host.items()}
@@ -248,6 +283,9 @@ def run_train(args, cfg: LiftConfig, rank: int, local_rank: int, world: int):
     barrier()
     ms_dev = timed(step_dev)
     barrier()
+    if args.dump_outputs and rank == 0:               # the last timed step's loss and the parameters it produced
+        flat = torch.cat([p.detach().float().reshape(-1) for p in trainer.bucket.params])
+        dump_outputs(args.dump_outputs, {"loss": last["loss"].double().reshape(1), "params": flat})
     for _ in range(2):
         step_e2e()
     barrier()
@@ -286,7 +324,7 @@ def run_train(args, cfg: LiftConfig, rank: int, local_rank: int, world: int):
             "dtype": "f32", "data": "synthetic",
             "config": config_dict(cfg, args, world),          # identical in both arms
             "details": {"batch_per_gpu": b, "time_receptive_field": s,
-                       "precision": precision, "step": "depth_layer (tcgen05 GEMM: half features -> fp32 head; backward: cuDNN) -> fused lift forward (channels-last BEV) -> BEV head "
+                       "precision": precision, "step": "depth_layer (wgmma GEMM: half features -> fp32 head; backward: cuDNN) -> fused lift forward (channels-last BEV) -> BEV head "
                        "+ uncertainty-weighted losses -> fused lift backward (shared geometry plan) -> ONE all-reduce of the flat fp32 "
                        "gradient -> clip 5 -> Adam(3e-4, wd 1e-7); image backbone excluded (feature maps are the input)",
                        "parallelism": f"dp{world}: batch sharded over {world} GPU(s), single NCCL all-reduce of {trainer.bucket.nbytes} gradient bytes per step",
@@ -300,9 +338,9 @@ def run_train(args, cfg: LiftConfig, rank: int, local_rank: int, world: int):
                              "what": "plan + lift forward + lift backward alone (autograd function, channels-last BEV and gradient)"},
             "roofline": {"bound": "hbm", "kernel": "lift_plan_kernel + lift_forward_cols_kernel + lift_backward_kernel",
                          "achieved": alg / (ms_lift * 1e-3) / 1e9, "peak": peak, "peak_source": peak_src, "unit": "GB/s",
-                         "frac": alg / (ms_lift * 1e-3) / 1e9 / peak, "traffic": None, "algorithmic_bytes_per_step": alg,
+                         "frac": alg / (ms_lift * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_step": alg,
                          "how": "algorithmic bytes of lift forward + backward (SURVEY.md 8d) / time of the lift's autograd forward+backward"},
-            "clocks": clocks,
+            "clocks": clocks, "device": device_info(local_rank),
         }
         if not args.no_cpu_baseline:
             fps, sec, threads = time_cpu_reference(cfg, min(frames, args.cpu_frames), reps=max(2, args.cpu_reps // 2), backward=True)
@@ -337,6 +375,8 @@ def main():
                                                       "sizes of the first stages (the last repeats)")
     ap.add_argument("--cpu-frames", type=int, default=3)
     ap.add_argument("--cpu-reps", type=int, default=5)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = CONFIGS[args.workload]
 
@@ -391,7 +431,7 @@ def main():
     def timed_steps(step_fn, n_steps, do_flush=True):
         """Per-step CUDA events on the current stream; L2 flushed (256 MiB write) before each step, outside the events.  All steps
         are enqueued before the host waits, so a step's interval is device time: a descheduled host thread between the start event
-        and the launch would otherwise show up as a multi-millisecond "step" (seen at N = 8, profiles/r02_notes.md)."""
+        and the launch would otherwise show up as a multi-millisecond "step"."""
         pairs = []
         for _ in range(n_steps):
             if do_flush:
@@ -417,7 +457,7 @@ def main():
     graphed_static = lift.capture(head_d, K_d, E_d, static_calibration=True)
 
     # the clock sampler (an nvidia-smi process) starts BEFORE the warm-up: its NVML start-up touches every GPU of the box and showed
-    # up as multi-millisecond outliers in the first timed steps of every rank at N = 8 (profiles/r02_notes.md)
+    # up as multi-millisecond outliers in the first timed steps of every rank
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
@@ -430,6 +470,8 @@ def main():
     barrier()
     t_dev = timed_steps(graphed, S)
     barrier()
+    if args.dump_outputs and rank == 0:               # the BEV of the last timed step (the graph's output buffer)
+        dump_outputs(args.dump_outputs, {"bev": graphed.output})
     t_dev_noflush = timed_steps(graphed, S, do_flush=False)
     t_static = timed_steps(graphed_static, S)
     t_eager = timed_steps(step_eager, S)
@@ -641,7 +683,7 @@ def main():
         except Exception as exc:               # an extra must never take the bench line down
             warp_extra = {"error": f"{type(exc).__name__}: {exc}"[:300]}
 
-    # ---- next row (SURVEY.md section 8f, next-2): Decoder.first_conv 7x7 s2 64->64 on tcgen05, fed by the channel-last lift output ------
+    # ---- next row (SURVEY.md section 8f, next-2): Decoder.first_conv 7x7 s2 64->64 on wgmma, fed by the channel-last lift output ------
     conv_extra = None
     if rank == 0 and not args.no_extras:
         try:
@@ -665,13 +707,13 @@ def main():
                 with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
                     bf16_peak = float(json.load(fh)["bf16_tflops"])
             except (OSError, ValueError, KeyError):
-                bf16_peak = 1590.0
+                bf16_peak = H100_BF16_TFLOPS
             conv_extra = {"frames": frames, "ms_per_call": c_ms, "tflops": flops / (c_ms * 1e-3) / 1e12, "flops": flops,
                           "library_cudnn_tf32_ms": l_ms, "tf32_peak_tflops": bf16_peak / 2,
                           "frac_of_tf32_peak": flops / (c_ms * 1e-3) / 1e12 / (bf16_peak / 2),
-                          "what": "fiery_b200.bev_conv.first_conv_forward (tcgen05 kind::tf32 implicit GEMM, TMA stride-2 im2col) on a "
-                                  "channel-last (B', 200, 200, 64) fp32 BEV; peak = measured cuBLAS bf16 burst / 2 (TF32 runs at half the "
-                                  "bf16 rate); library line: torch conv2d, cuDNN with allow_tf32, same tensors; L2 flushed before every call"}
+                          "what": "fiery_b200.bev_conv.first_conv_forward (wgmma TF32 implicit GEMM, TMA stride-2 im2col) on a "
+                                  "channel-last (B', 200, 200, 64) fp32 BEV; peak = BF16 peak (MEASURED_PEAKS.json, else the H100 SXM data "
+                                  "sheet) / 2 (TF32 runs at half the bf16 rate); library line: torch conv2d, cuDNN with allow_tf32, same tensors; L2 flushed before every call"}
         except Exception as exc:               # an extra must never take the bench line down
             conv_extra = {"error": f"{type(exc).__name__}: {exc}"[:300]}
 
@@ -695,8 +737,8 @@ def main():
             d_bytes = feat16.numel() * 2 + feat16.shape[0] * n_out * fh * fw * 4 + 128 * 128 * 2
             depth_extra = {"frames": frames, "ms_per_call": d_ms, "bytes": d_bytes, "achieved_gbs": d_bytes / (d_ms * 1e-3) / 1e9,
                            "library_cudnn_fp16_ms": dl_ms, "library_cudnn_fp16_plus_widening_ms": dlw_ms,
-                           "what": "fiery_b200.depth_layer.depth_layer_forward (Encoder.depth_layer, encoder.py:36,96: persistent tcgen05 "
-                                   "kind::f16 GEMM, fp16 NCHW features in, fp32 NCHW head tensor out, TMA both ways); bytes = features "
+                           "what": "fiery_b200.depth_layer.depth_layer_forward (Encoder.depth_layer, encoder.py:36,96: persistent wgmma "
+                                   "fp16 GEMM, fp16 NCHW features in, fp32 NCHW head tensor out, TMA both ways); bytes = features "
                                    "read once + head written once + weights; library lines: torch conv2d (cuDNN, fp16 out) alone and "
                                    "followed by the .float() an AMP step needs before the fp32 lift; L2 flushed before every call"}
             del feat16
@@ -735,7 +777,6 @@ def main():
         row_bytes = cfg.out_channels * 4
         own = {"lift_forward_cols_kernel": head_bytes + touched_rows * row_bytes,             # read head once, each touched row written once
                "finalize_tma_kernel": 2 * touched_rows * row_bytes + bev_bytes}               # gather + re-zero touched rows, write the BEV
-        traffic = load_traffic(cfg.name) if args.head_dtype == "f32" else {}
         kernels = []
         for k, name in KIND.items():
             if not per_kind[k]:
@@ -745,8 +786,7 @@ def main():
             kernels.append({"kernel": name, "launches_per_step": n_launch, "ms_per_launch": mean_ms,
                             "algorithmic_bytes_per_launch": own[name] // max(1, n_launch),
                             "achieved": gbs(own[name] / max(1, n_launch), mean_ms), "unit": "GB/s",
-                            "frac": gbs(own[name] / max(1, n_launch), mean_ms) / peak,
-                            "traffic_per_step": traffic.get(name)})
+                            "frac": gbs(own[name] / max(1, n_launch), mean_ms) / peak})
         bwd_alg = cfg.bwd_bytes_per_frame(head_itemsize=4) * frames
         line = {
             "metric": METRIC, "value": total_frames / (ms_dev * 1e-3), "unit": "frames/s", "n_gpus": world, "steps": S,
@@ -777,7 +817,6 @@ def main():
             "roofline": {"bound": "hbm", "kernel": "path: " + " + ".join(k["kernel"] for k in kernels),
                          "achieved": gbs(alg_bytes, ms_dev), "peak": peak, "peak_source": peak_src, "unit": "GB/s",
                          "frac": gbs(alg_bytes, ms_dev) / peak,
-                         "traffic": (sum(v for v in traffic.values()) if traffic else None),
                          "algorithmic_bytes_per_step": alg_bytes, "step_ms": ms_dev,
                          "frac_no_l2_flush": gbs(alg_bytes, ms_dev_noflush) / peak,
                          "frac_static_rig": gbs(alg_bytes, ms_static) / peak,
@@ -790,10 +829,9 @@ def main():
                              "algorithmic_bytes_per_step": bwd_alg, "step_ms": ms_bwd,
                              "channels_last_grad": {"kernel": "lift_backward_kernel", "step_ms": ms_bwd_cl,
                                                     "achieved": gbs(bwd_alg, ms_bwd_cl), "frac": gbs(bwd_alg, ms_bwd_cl) / peak},
-                             "traffic": (sum(load_traffic(cfg.name + "__bwd").values()) or None),
                              "how": "fiery_lift_backward with the forward's plan, eager C-ABI call, L2 flushed before every step; "
                                     "algorithmic bytes = read grad BEV + read head + write grad head (SURVEY.md 8d)"},
-            "clocks": clocks,
+            "clocks": clocks, "device": device_info(local_rank),
         }
         if vs_extra is not None:
             line["voxels_summing_dropin"] = vs_extra

@@ -1,4 +1,4 @@
-"""fiery_b200: Blackwell-native (sm_100a) camera->BEV lift, a drop-in for the Lift-Splat hot path of
+"""fiery_b200: Hopper-native (sm_90a, H100) camera->BEV lift, a drop-in for the Lift-Splat hot path of
 wayveai/fiery (``fiery/models/fiery.py:193-286``, ``fiery/models/encoder.py:96-104``,
 ``fiery/utils/geometry.py:283-314``).  See DESIGN.md.
 

@@ -2,8 +2,8 @@
 
 ``Decoder.first_conv`` (fiery/models/decoder.py:11,59) is ``nn.Conv2d(64, 64, kernel_size=7, stride=2, padding=3, bias=False)``,
 followed by ``bn1`` and ``relu`` (decoder.py:60-61).  ``FirstConv`` carries the same parameter (``weight`` (64, 64, 7, 7), so a
-reference ``state_dict`` entry ``first_conv.weight`` loads unchanged) and runs the layer as a tcgen05 implicit GEMM
-(fiery_b200/csrc/bev_conv.cu: TF32 operands, fp32 accumulation in tensor memory).  It takes the lift's channel-last BEV directly
+reference ``state_dict`` entry ``first_conv.weight`` loads unchanged) and runs the layer as a wgmma implicit GEMM
+(fiery_b200/csrc/bev_conv.cu: TF32 operands, fp32 accumulation).  It takes the lift's channel-last BEV directly
 (``LiftSplat(output_layout="channels_last")``), so the lift's NCHW layout pass is not on this path.
 
 Inference op: no backward (training keeps ``nn.Conv2d``; the reference trains this layer under cuDNN).  No CPU path.

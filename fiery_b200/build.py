@@ -1,4 +1,4 @@
-"""Build libfiery_b200.so in-tree with nvcc for sm_100a (no torch, no cmake).
+"""Build libfiery_b200.so in-tree with nvcc for sm_90a (H100; no torch, no cmake).
 
     python -m fiery_b200.build [--force] [--verbose]
 
@@ -20,7 +20,7 @@ LIB_PATH = os.path.join(PKG_DIR, "libfiery_b200.so")
 STAMP_PATH = os.path.join(PKG_DIR, "csrc", ".build_stamp")
 SOURCES = ["c_api.cu", "lift_plan.cu", "lift_fwd.cu", "lift_fwd_cols.cu", "lift_bwd.cu", "bev_conv.cu", "depth_layer.cu", "voxels_summing.cu", "warp.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math=false",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
@@ -58,7 +58,7 @@ def is_current() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, out: str = None, obj_suffix: str = "") -> str:
-    """Compiles every .cu under csrc/ for sm_100a into fiery_b200/libfiery_b200.so; returns its path.
+    """Compiles every .cu under csrc/ for sm_90a into fiery_b200/libfiery_b200.so; returns its path.
     ``out`` / ``obj_suffix``: build a second library next to it (experiment builds with FIERY_NVCC_EXTRA) without touching the
     in-tree one."""
     if out is not None:
@@ -93,7 +93,7 @@ def _build_to(lib_path: str, obj_suffix: str, verbose: bool) -> str:
             print(f"nvcc failed on {src}", file=sys.stderr)
     if failed:
         raise RuntimeError("nvcc compilation failed")
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", lib_path, *objs, "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib_path, *objs, "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     subprocess.run(link, check=True)
     return lib_path
 

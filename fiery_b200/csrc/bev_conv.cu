@@ -1,4 +1,4 @@
-// First BEV convolution on the 5th-generation tensor cores (SURVEY.md section 8f, next-2): Decoder.first_conv, 7x7 stride 2 padding 3,
+// First BEV convolution on the tensor cores (SURVEY.md section 8f, next-2): Decoder.first_conv, 7x7 stride 2 padding 3,
 // 64 -> 64 channels, no bias (fiery/models/decoder.py:11,59), with the folded bn1 + relu of decoder.py:60-61 as an optional epilogue.
 //
 // It is the first dense contraction after the lift and it consumes the lift's CHANNEL-LAST result directly: (B', X, Y, C) fp32 is
@@ -8,17 +8,18 @@
 //   M = 128 output pixels (a 16 wide x 8 tall patch), N = 64 output channels, K = 49 taps x 64 channels = 3136
 //
 // One CTA per output patch, warp-specialised:
-//   warp 0    TMA producer: per tap, two 4-D tiled loads (box 32 ch x 16 px x 8 rows, ELEMENT STRIDE 2 along X and Y: the copy
-//             engine does the stride-2 im2col; out-of-range coordinates are zero-filled = the padding) and two loads of the tap's
-//             (64 out x 32 in) weight slices, all with the 128-byte swizzle the MMA expects; 4-stage ring, mbarrier full/empty
-//   warp 1    MMA issuer: one thread issues tcgen05.mma kind::tf32 (M128 N64 K8), 8 per tap, fp32 accumulator in TMEM (64
-//             columns); tcgen05.commit releases the stage / signals the epilogue
-//   warps 2-5 epilogue: tcgen05.ld the 128 x 64 accumulator (one output pixel per thread), per-channel scale/shift (+ relu),
-//             16-byte stores into the channel-last output
+//   warp 8     TMA producer: per tap, two 4-D tiled loads (box 32 ch x 16 px x 8 rows, ELEMENT STRIDE 2 along X and Y: the copy
+//              engine does the stride-2 im2col; out-of-range coordinates are zero-filled = the padding) and two loads of the tap's
+//              (64 out x 32 in) weight slices, all with the 128-byte swizzle the MMA expects; 4-stage ring, mbarrier full/empty
+//   warps 0-7  two consumer warpgroups, warpgroup g owns output pixels 64g .. 64g + 63 (patch rows 4g .. 4g + 3): wgmma m64n64k8
+//              TF32, 8 per tap, fp32 accumulator in registers; one tap's MMAs stay in flight while the next tap's are issued, a
+//              stage is released once its MMAs have completed.  Epilogue: per-channel scale/shift (+ relu), 8-byte stores into the
+//              channel-last output
 // Operands are TF32 (10-bit mantissa: weights rounded when they are packed, activations read from fp32 by truncation), accumulation
 // fp32 -- the precision cuDNN uses for this layer under torch's default allow_tf32; the parity bar (tests/test_bev_conv_gpu.py) is
-// stated against an fp64 convolution: normwise < 1e-3 (measured 6-8e-4; cuDNN's TF32 path, which rounds both operands: 3e-4).
+// stated against an fp64 convolution: normwise < 1e-3.
 #include "lift_plan.cuh"
+#include "wgmma.cuh"
 
 namespace fiery {
 
@@ -29,8 +30,9 @@ constexpr int CV_STAGES = 4;
 constexpr int CV_A_ATOM = 128 * 128;          // 128 rows x 128 bytes (32 fp32 channels), swizzle-128B atom rows
 constexpr int CV_B_ATOM = 64 * 128;           // 64 output channels x 32 input channels
 constexpr int CV_STAGE_BYTES = 2 * CV_A_ATOM + 2 * CV_B_ATOM;      // 48 KB
-constexpr int CV_THREADS = 192;
-constexpr int CV_TMEM_COLS = 64;
+constexpr int CV_CONSUMERS = 2;               // warpgroups
+constexpr int CV_PRODUCER_WARP = 4 * CV_CONSUMERS;
+constexpr int CV_THREADS = 128 * CV_CONSUMERS + 32;
 
 struct ConvMaps {
     CUtensorMap x;       // (C, W, H, B) fp32, box (32, 32, 16, 1), element strides (1, 2, 2, 1), swizzle 128B
@@ -44,33 +46,6 @@ __device__ __forceinline__ void tma_load_3d_sw(void* dst, const CUtensorMap* map
         : "memory");
 }
 
-// shared-memory matrix descriptor of a K-major operand tile with 128-byte rows and the 128-byte swizzle (canonical layout
-// ((8,n),2):((8,SBO),1) in 16-byte units): rows 128 B apart inside a group of 8, groups 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_byte_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_byte_addr >> 4) & 0x3fff);        // start address
-    d |= static_cast<uint64_t>(1) << 16;                               // leading byte offset (unused for swizzled K-major): 1
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;                       // stride byte offset: 8 rows x 128 B
-    d |= static_cast<uint64_t>(1) << 46;                               // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;                               // SWIZZLE_128B
-    return d;
-}
-
-// instruction descriptor: D fp32, A and B TF32, both K-major, N = 64, M = 128
-constexpr uint32_t CV_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(CV_IDESC), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-
 __global__ void __launch_bounds__(CV_THREADS, 1)
 bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restrict__ scale, const float* __restrict__ shift,
                      int relu, float* __restrict__ y, int Ho, int Wo, int tiles_x, int tiles_y) {
@@ -79,8 +54,6 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + CV_STAGES * CV_STAGE_BYTES);
     uint64_t* empty = full + CV_STAGES;
-    uint64_t* accum_ready = empty + CV_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_ready + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
@@ -88,26 +61,18 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
     const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
     const int oy0 = ty * CV_TH, ox0 = tx * CV_TW;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == CV_PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w);
         for (int s = 0; s < CV_STAGES; ++s) {
             mbar_init(full + s, 1);
-            mbar_init(empty + s, 1);
+            mbar_init(empty + s, 4 * CV_CONSUMERS);   // one arrival per consumer warp
         }
-        mbar_init(accum_ready, 1);
         fence_mbar_init();
     }
-    if (warp == 1) {                                  // one warp allocates the accumulator columns in tensor memory
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(tmem_slot)), "r"(CV_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == CV_PRODUCER_WARP) {
         if (lane == 0) {                              // ===== TMA producer =====
             for (int it = 0; it < CV_TAPS; ++it) {
                 const int st = it % CV_STAGES;
@@ -123,64 +88,56 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
                 tma_load_3d_sw(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, it);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {                              // ===== MMA issuer =====
-            for (int it = 0; it < CV_TAPS; ++it) {
-                const int st = it % CV_STAGES;
-                mbar_wait(full + st, (it / CV_STAGES) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_addr = smem_addr(smem + st * CV_STAGE_BYTES);
-                const uint32_t b_addr = a_addr + 2 * CV_A_ATOM;
+        return;
+    }
+
+    // ===== consumers: warpgroup g takes accumulator rows 64g .. 64g + 63 =====
+    const int g = warp >> 2, wq = warp & 3;
+    float acc[CV_C / 2];
 #pragma unroll
-                for (int atom = 0; atom < 2; ++atom) {
-                    const uint64_t da = umma_desc_k_sw128(a_addr + atom * CV_A_ATOM);
-                    const uint64_t db = umma_desc_k_sw128(b_addr + atom * CV_B_ATOM);
+    for (int i = 0; i < CV_C / 2; ++i) acc[i] = 0.f;
+    wgmma_fence();
+    for (int it = 0; it < CV_TAPS; ++it) {
+        const int st = it % CV_STAGES;
+        mbar_wait(full + st, (it / CV_STAGES) & 1);
+        const uint32_t a_addr = smem_addr(smem + st * CV_STAGE_BYTES) + g * 64 * 128;
+        const uint32_t b_addr = smem_addr(smem + st * CV_STAGE_BYTES) + 2 * CV_A_ATOM;
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)       // 8 TF32 values (32 bytes) per MMA along K: the start address advances by 2 units
-                        umma_tf32(tmem_base, da + 2 * k, db + 2 * k, (it | atom | k) ? 1u : 0u);
-                }
-                umma_commit(empty + st);              // the stage may be refilled once these MMAs have read it
-            }
-            umma_commit(accum_ready);                 // all 392 MMAs done: the accumulator is complete
+        for (int atom = 0; atom < 2; ++atom) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k)               // 8 TF32 values (32 bytes) per MMA along K
+                wgmma_m64n64k8_tf32_ss(acc, gmma_desc_sw128(a_addr + atom * CV_A_ATOM + 32 * k, 16, 1024),
+                                       gmma_desc_sw128(b_addr + atom * CV_B_ATOM + 32 * k, 16, 1024));
         }
-    } else {                                          // ===== epilogue: warps 2..5, tensor-memory lanes 32 * (warp % 4) .. =====
-        mbar_wait(accum_ready, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int q = warp & 3;
-        const int m = q * 32 + lane;                  // accumulator row = output pixel of the patch
+        wgmma_commit();
+        if (it > 0) {                                 // the previous tap's MMAs are complete: its stage may be refilled
+            wgmma_wait<1>();
+            __syncwarp();
+            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + (it - 1) % CV_STAGES)) : "memory");
+        }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        const int m = 64 * g + 16 * wq + (lane >> 2) + 8 * half;   // accumulator row = output pixel of the patch
         const int oy = oy0 + m / CV_TW, ox = ox0 + m % CV_TW;
-        uint32_t v[CV_C];
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll
-        for (int c = 0; c < CV_C; c += 16) {
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(v[c + 0]), "=r"(v[c + 1]), "=r"(v[c + 2]), "=r"(v[c + 3]), "=r"(v[c + 4]), "=r"(v[c + 5]), "=r"(v[c + 6]), "=r"(v[c + 7]),
-                  "=r"(v[c + 8]), "=r"(v[c + 9]), "=r"(v[c + 10]), "=r"(v[c + 11]), "=r"(v[c + 12]), "=r"(v[c + 13]), "=r"(v[c + 14]), "=r"(v[c + 15])
-                : "r"(taddr + c)
-                : "memory");
-        }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
         if (oy < Ho && ox < Wo) {
-            float4* dst = reinterpret_cast<float4*>(y + ((static_cast<size_t>(b) * Ho + oy) * Wo + ox) * CV_C);
+            float* dst = y + ((static_cast<size_t>(b) * Ho + oy) * Wo + ox) * CV_C;
 #pragma unroll
-            for (int c = 0; c < CV_C; c += 4) {
-                float o[4];
+            for (int j = 0; j < CV_C / 8; ++j) {
+                const int c = 8 * j + cq;
+                float o[2];
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    float t = __uint_as_float(v[c + e]);
+                for (int e = 0; e < 2; ++e) {
+                    float t = acc[4 * j + 2 * half + e];
                     if (scale) t = fmaf(t, __ldg(scale + c + e), __ldg(shift + c + e));
                     o[e] = relu ? fmaxf(t, 0.f) : t;
                 }
-                dst[c / 4] = make_float4(o[0], o[1], o[2], o[3]);
+                *reinterpret_cast<float2*>(dst + c) = make_float2(o[0], o[1]);
             }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(CV_TMEM_COLS) : "memory");
     }
 }
 
@@ -250,7 +207,7 @@ int launch_bev_conv(int n_frames, int H, int W, const float* x_nhwc, const float
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (conv weights) failed with CUresult %d", (int)r);
     }
-    const int smem = CV_STAGES * CV_STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers, tensor-memory slot */;
+    const int smem = CV_STAGES * CV_STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
     static OncePerDevice once;
     int rc = once.run([smem]() -> int {
         FIERY_CUDA_CHECK(cudaFuncSetAttribute(bev_conv7x7s2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

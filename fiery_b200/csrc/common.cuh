@@ -1,4 +1,4 @@
-// Shared device helpers: mbarrier / TMA / vector-reduction PTX wrappers for sm_100a, error plumbing.
+// Shared device helpers: mbarrier / TMA / vector-reduction PTX wrappers for sm_90a, error plumbing.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -1,91 +1,77 @@
 // Encoder.depth_layer on the tensor cores (SURVEY.md section 8f, next-3): the 1x1 convolution 128 -> D + C that produces the head
-// tensor the lift consumes (fiery/models/encoder.py:36,96), as a tcgen05 GEMM that reads the feature map in the dtype the backbone
+// tensor the lift consumes (fiery/models/encoder.py:36,96), as a wgmma GEMM that reads the feature map in the dtype the backbone
 // emits it (fp16 / bf16 under AMP, fp32 otherwise) and writes the fp32 NCHW head tensor directly -- so an AMP step has no separate
 // widening pass between the 1x1 convolution and the lift (the reference's softmax / outer product run in fp32 under autocast,
 // encoder.py:99-100, and so do the tile kernels).
 //
 //   head[img][o][p] = bias[o] + sum_i W[o][i] * feat[img][i][p]          o < D + C <= 128,  i < 128,  p < h*w
 //
-// Per CTA one tile of 128 pixels of one image:  D (M = 128 output channels x N = 128 pixels, fp32 in TMEM)
-//     = A (W, 128 x 128, K-major, 128-byte swizzle: the padded weight matrix, loaded once per CTA)
-//     x B (feat tile, K = 128 channels x N = 128 pixels, taken as it lies in the NCHW feature map: N contiguous = "MN-major" operand,
-//          TMA boxes of (128 bytes of pixels) x (128 channels), 128-byte swizzle)
-// Because the accumulator's rows are output CHANNELS and its columns consecutive PIXELS, the epilogue thread that owns row o writes
-// 512 contiguous bytes of plane o of the NCHW head tensor -- no transposition anywhere.
-// Warp roles: warp 0 TMA producer, warp 1 TMEM allocation + MMA issue (8 x kind::f16 K16 or 16 x kind::tf32 K8), warps 2-9 epilogue
-// (two warps per TMEM lane quarter; tcgen05.ld 2 x 32 columns, + bias, swizzled staging boxes, TMA stores).
+// Per CTA one tile of 128 pixels of one image at a time (persistent: CTA b takes tiles b, b + grid, ...).  The padded weight matrix
+// (128 x 128, K-major, 128-byte swizzle) is loaded once per CTA; feature tiles (K = 128 channels x 128 pixels, taken as they lie in
+// the NCHW feature map: pixels contiguous) run through a STAGES-deep TMA ring.  Warp roles: warps 0-7 are two consumer warpgroups,
+// warp 8 the TMA producer.
+//   fp16 / bf16: D (128 output channels x 128 pixels) = W x feat, both operands from shared memory, the feature tile as the
+//                MN-major ("transposed") B operand; warpgroup g owns output channels 64g .. 64g + 63.  An accumulator row is an output
+//                channel, so a thread's float2 stores go to consecutive pixels of one plane of the head tensor.
+//   fp32 (TF32): wgmma has no MN-major TF32 operand, so the product is taken transposed, D (128 pixels x 128 output channels) =
+//                feat^T x W^T: the weight matrix is the K-major B operand as it lies, the feature tile is the A operand, read from
+//                shared memory into registers.  Warpgroup g owns pixel rows 64g .. 64g + 63, in the order dl_pixel() gives them
+//                (conflict-free fragment loads from the swizzled tile).
 #include "lift_plan.cuh"
+#include "wgmma.cuh"
 
 namespace fiery {
 
 constexpr int DL_K = 128;                 // input channels (upsampling_out_channels, encoder.py:33)
 constexpr int DL_M = 128;                 // padded output channels
 constexpr int DL_N = 128;                 // pixels per tile
-constexpr int DL_EPI_WARPS = 8;              // two per TMEM lane quarter, each takes half of the tile's pixel columns
-constexpr int DL_THREADS = 64 + 32 * DL_EPI_WARPS;
-constexpr int DL_TMEM_COLS = 256;             // two accumulators
+constexpr int DL_CONSUMERS = 2;           // warpgroups
+constexpr int DL_PRODUCER_WARP = 4 * DL_CONSUMERS;
+constexpr int DL_THREADS = 128 * DL_CONSUMERS + 32;
 
 struct DepthLayerMaps {
     CUtensorMap w;        // (K, M) padded weights, box (128 bytes of K, 128 rows), swizzle 128B
     CUtensorMap feat;     // (pixels, K, images), box (128 bytes of pixels, 128 channels, 1), swizzle 128B
-    CUtensorMap out;      // (pixels, n_out, images) fp32, box (32 pixels, 32 channels, 1), swizzle 128B
-    int pixels;
 };
 
 __device__ __forceinline__ void tma_load_2d_sw(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1) : "memory");
 }
-
-// matrix descriptors, 128-byte swizzle, version 1 (Blackwell).  K-major: rows of 128 bytes along K, 8-row groups 1024 B apart (SBO).
-// MN-major: rows of 128 bytes along N (one k each), 8 consecutive k = one 1024-byte atom (SBO = stride between k-groups),
-// LBO = stride between blocks of 128 bytes along N.
-// 32-bit operands in MN-major form exist only in the "128-byte swizzle, 32-byte atoms" layout (type 1): 32-byte chunks of a 128-byte row
-// XOR-ed with the row number mod 4, so the k-group the SBO steps over is 4 rows (512 B); TMA writes it with SWIZZLE_128B_ATOM_32B.
-__device__ __forceinline__ uint64_t dl_desc(uint32_t smem_byte_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_byte_addr >> 4) & 0x3fff);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fff) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(layout_type) << 61;
-    return d;
-}
-
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
 
 template <int ES>
 struct DlShape {
     static constexpr int EPR = 128 / ES;                      // elements per 128-byte row
-    static constexpr int ATOMS = DL_K / EPR;                  // K-major A: atoms of (128 rows x 128 B) along K
-    static constexpr int NBLK = DL_N / EPR;                   // MN-major B: blocks of 128 B along N
-    static constexpr int UMMA_K = 32 / ES;
-    static constexpr int A_ATOM = DL_M * 128, B_BLK = DL_K * 128;
-    static constexpr int A_BYTES = ATOMS * A_ATOM, B_BYTES = NBLK * B_BLK;
-    static constexpr int STAGES = ES == 2 ? 3 : 2;            // feature tiles in flight (32 KB / 64 KB each)
-    static constexpr int OUT_BUF = 32 * 128;                  // one epilogue warp's staging box: 32 channels x 32 pixels fp32
-    static constexpr int OUT_BUFS = ES == 2 ? 2 : 1;          // staging boxes per warp (the fp32 variant's feature ring leaves room for one)
-    static constexpr int OUT_BYTES = DL_EPI_WARPS * OUT_BUFS * OUT_BUF;
-    static constexpr int SMEM = A_BYTES + STAGES * B_BYTES + OUT_BYTES + 1024 + 256;
+    static constexpr int ATOMS = DL_K / EPR;                  // weights: atoms of (128 rows x 128 B) along K
+    static constexpr int NBLK = DL_N / EPR;                   // feature tile: blocks of (128 channels x 128 B) along the pixels
+    static constexpr int MMA_K = 32 / ES;                     // K of one MMA: 16 (fp16 / bf16), 8 (TF32)
+    static constexpr int W_ATOM = DL_M * 128, B_BLK = DL_K * 128;
+    static constexpr int W_BYTES = ATOMS * W_ATOM, B_BYTES = NBLK * B_BLK;
+    static constexpr int STAGES = ES == 2 ? 4 : 2;            // feature tiles in flight (32 KB / 64 KB each)
+    static constexpr int SMEM = W_BYTES + STAGES * B_BYTES + 1024 + 256;
 };
 
-// ES: element size of the operands (2: fp16 / bf16, kind::f16, K = 16 per MMA; 4: fp32 read as TF32, kind::tf32, K = 8 per MMA).
-// Persistent: CTA b takes tiles b, b + grid, ...; the weights are loaded once; feature tiles run through a STAGES-deep ring, the
-// accumulator is double-buffered in TMEM (2 x 128 columns), so the loads of tile t + 2, the MMAs of tile t + 1 and the epilogue of tile t
-// overlap.  The epilogue goes TMEM -> registers (+ bias) -> swizzled shared-memory boxes -> TMA stores (full 128-byte lines per plane).
-template <int ES>
+// fp32 path: accumulator row r (0..127) -> pixel of the tile.  The 8 rows one fragment load covers (r = 8t .. 8t + 7) are 4 pixels
+// from the first half of a 128-byte row of the swizzled tile and 4 from the second half, so with the 4 channels of the load they hit
+// 32 different banks.
+__device__ __forceinline__ int dl_pixel(int r) {
+    const int t = r >> 3, q = r & 7;
+    return (t >> 2) * 32 + (q >> 2) * 16 + (t & 3) * 4 + (q & 3);
+}
+
+// byte offset of (channel, pixel) in a feature tile of fp32 blocks (32 pixels x 128 channels, 128-byte swizzle)
+__device__ __forceinline__ uint32_t dl_feat_offset(int ch, int px) {
+    return (px >> 5) * DlShape<4>::B_BLK + ch * 128 + ((((px & 31) >> 2) ^ (ch & 7)) << 4) + (px & 3) * 4;
+}
+
+// ES: element size of the operands (2: fp16 / bf16; 4: fp32 read as TF32).  BF16 selects the 16-bit type.
+template <int ES, bool BF16>
 __global__ void __launch_bounds__(DL_THREADS, 1)
-depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __restrict__ bias, int n_out, int tiles_per_image,
-                   int n_tiles, uint32_t idesc, int skip_arg) {
+depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __restrict__ bias, float* __restrict__ head, int n_out,
+                   int pixels, int tiles_per_image, int n_tiles, int skip_arg) {
     using S = DlShape<ES>;
 #ifdef FIERY_COLS_AB
     const int skip = skip_arg;                         // experiment builds: leave out stores (1) / MMAs (2) / feature loads (4)
@@ -94,47 +80,31 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
 #endif
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    unsigned char* s_a = smem;
-    unsigned char* s_b = s_a + S::A_BYTES;
-    unsigned char* s_out = s_b + S::STAGES * S::B_BYTES;
-    uint64_t* a_full = reinterpret_cast<uint64_t*>(s_out + S::OUT_BYTES);
-    uint64_t* b_full = a_full + 1;
+    unsigned char* s_w = smem;
+    unsigned char* s_b = s_w + S::W_BYTES;
+    uint64_t* w_full = reinterpret_cast<uint64_t*>(s_b + S::STAGES * S::B_BYTES);
+    uint64_t* b_full = w_full + 1;
     uint64_t* b_empty = b_full + S::STAGES;
-    uint64_t* acc_full = b_empty + S::STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == DL_PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&maps.w);
         tma_prefetch_desc(&maps.feat);
-        tma_prefetch_desc(&maps.out);
-        mbar_init(a_full, 1);
+        mbar_init(w_full, 1);
         for (int i = 0; i < S::STAGES; ++i) {
             mbar_init(b_full + i, 1);
-            mbar_init(b_empty + i, 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(acc_full + i, 1);
-            mbar_init(acc_empty + i, DL_EPI_WARPS);     // one arrival per epilogue warp
+            mbar_init(b_empty + i, 4 * DL_CONSUMERS);  // one arrival per consumer warp
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(tmem_slot)), "r"(DL_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == DL_PRODUCER_WARP) {
         if (lane == 0) {                               // ===== TMA producer: weights once, then this CTA's feature tiles =====
-            mbar_arrive_expect_tx(a_full, S::A_BYTES);
+            mbar_arrive_expect_tx(w_full, S::W_BYTES);
 #pragma unroll
-            for (int a = 0; a < S::ATOMS; ++a) tma_load_2d_sw(s_a + a * S::A_ATOM, &maps.w, a_full, a * S::EPR, 0);
+            for (int a = 0; a < S::ATOMS; ++a) tma_load_2d_sw(s_w + a * S::W_ATOM, &maps.w, w_full, a * S::EPR, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
                 const int st = it % S::STAGES, use = it / S::STAGES;
@@ -147,101 +117,90 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
                 for (int b = 0; b < S::NBLK; ++b) tma_load_3d(dst + b * S::B_BLK, &maps.feat, b_full + st, p0 + b * S::EPR, 0, img);   // pixels past the image: zeros
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {                               // ===== MMA issuer =====
-            mbar_wait(a_full, 0);
-            const uint32_t a_addr = smem_addr(s_a);
-            int it = 0;
-            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-                const int st = it % S::STAGES, use = it / S::STAGES;
-                const int acc = it & 1, acc_use = it >> 1;
-                mbar_wait(b_full + st, use & 1);
-                if (acc_use > 0) mbar_wait(acc_empty + acc, (acc_use - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t b_addr = smem_addr(s_b + st * S::B_BYTES);
-                const uint32_t d_addr = tmem_base + acc * DL_N;
-#pragma unroll
-                for (int k = 0; k < ((skip & 2) ? 0 : DL_K / S::UMMA_K); ++k) {
-                    const int k0 = k * S::UMMA_K;
-                    // A: atom k0 / EPR, 32 bytes per K step inside the atom.  B: k0 rows of 128 bytes down the block; blocks along N 16 KB apart.
-                    const uint64_t da = dl_desc(a_addr + (k0 / S::EPR) * S::A_ATOM + (k0 % S::EPR) * ES, 16, 1024);
-                    const uint64_t db = ES == 2 ? dl_desc(b_addr + k0 * 128, S::B_BLK, 1024) : dl_desc(b_addr + k0 * 128, S::B_BLK, 512, 1);
-                    if (ES == 2)
-                        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                                     ::"r"(d_addr), "l"(da), "l"(db), "r"(idesc), "r"(k ? 1u : 0u) : "memory");
-                    else
-                        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                                     ::"r"(d_addr), "l"(da), "l"(db), "r"(idesc), "r"(k ? 1u : 0u) : "memory");
-                }
-                umma_commit(b_empty + st);             // the feature stage is free once these MMAs have read it
-                umma_commit(acc_full + acc);
-            }
-        }
-    } else {                                           // ===== epilogue: accumulator row = output channel, columns = pixels =====
-        const int q = warp & 3;                        // TMEM lane quarter this warp may read
-        const int half = (warp - 2) >> 2;              // which 64 pixel columns of the tile
-        const int o = q * 32 + lane;
-        const float bo = (o < n_out && bias) ? __ldg(bias + o) : 0.f;
-        unsigned char* my_out = s_out + (warp - 2) * S::OUT_BUFS * S::OUT_BUF;
-        const bool rows_live = q * 32 < n_out;         // channels past n_out: the store's box lies outside the tensor
-        const int pixels = maps.pixels;
-        int it = 0, nbox = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-            const int acc = it & 1, acc_use = it >> 1;
-            const int img = t / tiles_per_image, p0 = (t % tiles_per_image) * DL_N + half * 64;
-            mbar_wait(acc_full + acc, acc_use & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * DL_N + half * 64;
-            uint32_t v[2][32];
-#pragma unroll
-            for (int c = 0; c < 2; ++c)
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[c][0]), "=r"(v[c][1]), "=r"(v[c][2]), "=r"(v[c][3]), "=r"(v[c][4]), "=r"(v[c][5]), "=r"(v[c][6]), "=r"(v[c][7]),
-                      "=r"(v[c][8]), "=r"(v[c][9]), "=r"(v[c][10]), "=r"(v[c][11]), "=r"(v[c][12]), "=r"(v[c][13]), "=r"(v[c][14]),
-                      "=r"(v[c][15]), "=r"(v[c][16]), "=r"(v[c][17]), "=r"(v[c][18]), "=r"(v[c][19]), "=r"(v[c][20]), "=r"(v[c][21]),
-                      "=r"(v[c][22]), "=r"(v[c][23]), "=r"(v[c][24]), "=r"(v[c][25]), "=r"(v[c][26]), "=r"(v[c][27]), "=r"(v[c][28]),
-                      "=r"(v[c][29]), "=r"(v[c][30]), "=r"(v[c][31])
-                    : "r"(taddr + c * 32)
-                    : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");      // the accumulator is in registers: hand it back
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty + acc);
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                if (rows_live && p0 + c * 32 < pixels && !(skip & 1)) {
-                    unsigned char* buf = my_out + (nbox % S::OUT_BUFS) * S::OUT_BUF;
-                    if (nbox >= S::OUT_BUFS) {         // the store that last read this buffer must have drained it
-                        if (lane == 0) {
-                            if (S::OUT_BUFS == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                            else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                        }
-                        __syncwarp();
-                    }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)        // row = lane (128 B), 16-byte chunk j at j ^ (row % 8): the 128-byte swizzle of the store's map
-                        *reinterpret_cast<float4*>(buf + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                            make_float4(__uint_as_float(v[c][4 * j]) + bo, __uint_as_float(v[c][4 * j + 1]) + bo,
-                                        __uint_as_float(v[c][4 * j + 2]) + bo, __uint_as_float(v[c][4 * j + 3]) + bo);
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0) {
-                        tma_store_3d(&maps.out, buf, p0 + c * 32, q * 32, img);     // clipped at the image's last pixel and at channel n_out
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
-                    ++nbox;
-                }
-            }
-        }
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the stores' reads
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
+
+    // ===== consumers: warpgroup g, warp wq of it =====
+    const int g = warp >> 2, wq = warp & 3;
+    const int r0 = 64 * g + 16 * wq + (lane >> 2);     // accumulator rows r0 and r0 + 8 of this thread
+    const int cq = 2 * (lane & 3);                     // accumulator columns 8j + cq, 8j + cq + 1
+    const uint32_t w_addr = smem_addr(s_w);
+    mbar_wait(w_full, 0);
+    int it = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
+        const int st = it % S::STAGES, use = it / S::STAGES;
+        const int img = t / tiles_per_image, p0 = (t % tiles_per_image) * DL_N;
+        const unsigned char* tile = s_b + st * S::B_BYTES;
+        mbar_wait(b_full + st, use & 1);
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        if constexpr (ES == 2) {
+            wgmma_fence();
+            const uint32_t b_addr = smem_addr(tile);
+#pragma unroll
+            for (int k = 0; k < ((skip & 2) ? 0 : DL_K / S::MMA_K); ++k) {
+                const int k0 = k * S::MMA_K;
+                // A: atom k0 / EPR, rows 64g.., 32 bytes per K step inside the atom.  B: k0 rows of 128 bytes down the block (8-row
+                // groups 1024 B apart), blocks of 64 pixels B_BLK apart.
+                const uint64_t da = gmma_desc_sw128(w_addr + (k0 / S::EPR) * S::W_ATOM + g * 64 * 128 + (k0 % S::EPR) * ES, 16, 1024);
+                const uint64_t db = gmma_desc_sw128(b_addr + k0 * 128, S::B_BLK, 1024);
+                if (BF16) wgmma_m64n128k16_bf16_ss_tb(acc, da, db);
+                else wgmma_m64n128k16_f16_ss_tb(acc, da, db);
+            }
+        } else {
+            const int pa = dl_pixel(r0), pb = dl_pixel(r0 + 8);
+            uint32_t a[DL_K / 8][4];
+#pragma unroll
+            for (int k = 0; k < DL_K / 8; ++k) {
+                const int ch = 8 * k + (lane & 3);
+                a[k][0] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch, pa));
+                a[k][1] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch, pb));
+                a[k][2] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch + 4, pa));
+                a[k][3] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch + 4, pb));
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < ((skip & 2) ? 0 : DL_K / 8); ++k) {
+                const int k0 = 8 * k;
+                wgmma_m64n128k8_tf32_rs(acc, a[k], gmma_desc_sw128(w_addr + (k0 / 32) * S::W_ATOM + (k0 % 32) * 4, 16, 1024));
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
         __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(DL_TMEM_COLS) : "memory");
+        if (lane == 0) mbar_arrive(b_empty + st);      // this warp's part of the tile has been read
+        if (skip & 1) continue;
+        if constexpr (ES == 2) {                       // rows = output channels r0, r0 + 8; columns = pixels
+            float* out = head + (static_cast<size_t>(img) * n_out + r0) * pixels + p0;
+            const float b0 = (bias && r0 < n_out) ? __ldg(bias + r0) : 0.f;
+            const float b1 = (bias && r0 + 8 < n_out) ? __ldg(bias + r0 + 8) : 0.f;
+#pragma unroll
+            for (int j = 0; j < DL_N / 8; ++j) {
+                const int p = 8 * j + cq;
+                if (p0 + p < pixels) {                 // pixels is a multiple of 4: p + 1 is inside too
+                    if (r0 < n_out) *reinterpret_cast<float2*>(out + p) = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b0);
+                    if (r0 + 8 < n_out)
+                        *reinterpret_cast<float2*>(out + 8 * static_cast<size_t>(pixels) + p) = make_float2(acc[4 * j + 2] + b1, acc[4 * j + 3] + b1);
+                }
+            }
+        } else {                                       // rows = pixels dl_pixel(r0), dl_pixel(r0 + 8); columns = output channels
+            const int pa = p0 + dl_pixel(r0), pb = p0 + dl_pixel(r0 + 8);
+            float* out = head + static_cast<size_t>(img) * n_out * pixels;
+#pragma unroll
+            for (int j = 0; j < DL_M / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int o = 8 * j + cq + e;
+                    if (o < n_out) {
+                        const float bo = bias ? __ldg(bias + o) : 0.f;
+                        if (pa < pixels) out[static_cast<size_t>(o) * pixels + pa] = acc[4 * j + e] + bo;
+                        if (pb < pixels) out[static_cast<size_t>(o) * pixels + pb] = acc[4 * j + 2 + e] + bo;
+                    }
+                }
+            }
+        }
     }
 }
 
@@ -293,27 +252,15 @@ int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, in
         cuuint32_t box[3] = {epr, DL_K, 1};
         cuuint32_t estr[3] = {1, 1, 1};
         CUresult r = fn(&maps.feat, dt, 3, const_cast<void*>(feat), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        es == 4 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (feature map) failed with CUresult %d", (int)r);
     }
-    {
-        cuuint64_t dims[3] = {static_cast<cuuint64_t>(pixels), static_cast<cuuint64_t>(n_out), static_cast<cuuint64_t>(n_images)};
-        cuuint64_t strides[2] = {static_cast<cuuint64_t>(pixels) * 4, static_cast<cuuint64_t>(pixels) * n_out * 4};
-        cuuint32_t box[3] = {32, 32, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = fn(&maps.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, head, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (head tensor) failed with CUresult %d", (int)r);
-    }
-    maps.pixels = pixels;
-    // instruction descriptor: D fp32; A/B format F16 = 0, BF16 = 1, TF32 = 2; A K-major, B MN-major; N = 128, M = 128
-    const uint32_t fmt = dtype == 0 ? 2u : (dtype == 1 ? 0u : 1u);
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 16) | ((DL_N >> 3) << 17) | ((DL_M >> 4) << 24);
     static OncePerDevice once;
     static int n_sm[64];
     int rc = once.run([]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<2>::SMEM));
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<4>::SMEM));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<2>::SMEM));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<2>::SMEM));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<4>::SMEM));
         int dev = 0;
         FIERY_CUDA_CHECK(cudaGetDevice(&dev));
         FIERY_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev));
@@ -324,15 +271,19 @@ int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, in
     FIERY_CUDA_CHECK(cudaGetDevice(&dev));
     const int tiles_per_image = (pixels + DL_N - 1) / DL_N;
     const int n_tiles = n_images * tiles_per_image;
-    const int sms = n_sm[dev & 63] > 0 ? n_sm[dev & 63] : 148;
+    const int sms = n_sm[dev & 63];
     const int waves = (n_tiles + sms - 1) / sms;                       // one persistent CTA per SM, the tiles spread evenly over them
     const unsigned grid = static_cast<unsigned>((n_tiles + waves - 1) / waves);
     int skip = 0;
 #ifdef FIERY_COLS_AB
     if (const char* e = getenv("FIERY_DL_SKIP")) skip = atoi(e);      // experiment builds only: 1 no stores, 2 no MMAs, 4 no feature loads
 #endif
-    if (es == 2) depth_layer_kernel<2><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, n_out, tiles_per_image, n_tiles, idesc, skip);
-    else depth_layer_kernel<4><<<grid, DL_THREADS, DlShape<4>::SMEM, stream>>>(maps, bias, n_out, tiles_per_image, n_tiles, idesc, skip);
+    if (dtype == 0)
+        depth_layer_kernel<4, false><<<grid, DL_THREADS, DlShape<4>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
+    else if (dtype == 1)
+        depth_layer_kernel<2, false><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
+    else
+        depth_layer_kernel<2, true><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

@@ -1,4 +1,4 @@
-// Backward of the camera->BEV lift for sm_100a: gradient of the BEV features w.r.t. the head tensor (depth logits + context), i.e.
+// Backward of the camera->BEV lift for sm_90a: gradient of the BEV features w.r.t. the head tensor (depth logits + context), i.e.
 // autograd through fiery/models/encoder.py:99-100 (softmax, outer product) and fiery/utils/geometry.py:305-314
 // (VoxelsSumming.backward = "send the voxel's gradient to every point summed into it") without ever materialising the (N, C) point
 // gradient the reference builds.
@@ -70,7 +70,7 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void*
                  : "memory");
 }
 
-// packed fp32x2 helpers (SASS FFMA2 / FMUL2)
+// helpers on pairs of fp32 values held in one 64-bit register pair (two FFMA / FMUL each)
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
     unsigned long long r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -80,16 +80,22 @@ __device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& 
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ void fma2_acc(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %0;\n\t"
+        "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
+        "mov.b64 %0, {c0, c1};\n\t}" : "+l"(acc) : "l"(a), "l"(b));
 }
 __device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
     unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\t"
+        "mul.rn.f32 a0, a0, b0;\n\tmul.rn.f32 a1, a1, b1;\n\t"
+        "mov.b64 %0, {a0, a1};\n\t}" : "=l"(r) : "l"(a), "l"(b));
     return r;
 }
 
 // One step of a slot's gather pipeline, for the lanes where `pred` != 0, as one block of straight-line predicated code (a
-// conditional C++ assignment inside the unrolled row loop makes ptxas shuffle the whole register set, profiles/r01_notes.md):
+// conditional C++ assignment inside the unrolled row loop makes ptxas shuffle the whole register set):
 //   G   <- Gn                        the run that was "next" becomes current
 //   Gn  <- gradient row of `pnn`     (zeros for a masked run, pnn < 0): 2 x 16-byte loads of this lane's 8 channels
 //   pnn <- streams[sp], sp += 1      the pillar of the run after that

@@ -1,4 +1,4 @@
-// Forward camera->BEV lift for sm_100a, host side and the passes around the tile kernel (lift_fwd_cols.cu): the NCHW layout
+// Forward camera->BEV lift for sm_90a, host side and the passes around the tile kernel (lift_fwd_cols.cu): the NCHW layout
 // pass, the integer index dump and the calibration composition used by the parity checks, and the launchers.
 //
 // Replaces, per call: Fiery.get_geometry (fiery/models/fiery.py:193-208), the tail of Encoder.forward
@@ -284,9 +284,8 @@ __global__ void compose_calibration_kernel(int n, const float* __restrict__ K, c
 // ---------------------------------------------------------------------------------------------------------------------
 // host launchers (called from c_api.cu)
 // ---------------------------------------------------------------------------------------------------------------------
-// Frames per launch.  Measured on B200 (profiles/r01_notes.md): chunks small enough to keep the accumulator L2-resident (3 frames,
-// 31 MB) are slower end to end (152.9 us vs 122.7 us for 9 frames) -- the extra launches and the single-wave grids cost more than the
-// saved HBM traffic -- so the chunk only bounds the scratch footprint (1 GiB: accumulator + marks of a chunk).
+// Frames per launch.  Chunks small enough to keep the accumulator L2-resident pay for extra launches and single-wave grids, so the
+// chunk only bounds the scratch footprint (1 GiB: accumulator + marks of a chunk).
 static std::atomic<int> g_max_chunk_frames{0};       // fiery_lift_set_max_chunk_frames (test hook: forces the multi-pass path)
 void lift_set_max_chunk_frames(int n) { g_max_chunk_frames.store(n > 0 ? n : 0); }
 
@@ -338,14 +337,15 @@ static int chain_resources(ChainResources** out) {
 
 // NCHW output: the frames of a chunk are cut into groups, each a (plan kernel ->) tile kernel -> layout pass chain on its own stream.
 // The layout pass of one group (DRAM-bound) runs under the tile kernels of the others (issue-bound); only the last pass is
-// exposed.  Measured on B200 (profiles/r01_notes.md), 8 frames: 1 chain 84.7 us, 2 chains 78.3 us, 4 chains 73.3 us; 8 chains of
-// one frame (90 tiles) each fall back to 79.6 us, so a group keeps at least one tile per SM (148).
+// exposed.  A group whose tile kernel cannot fill the GPU once loses more than the overlap gains, so a group keeps at least one
+// tile per SM of an H100 SXM (132).  The count is host logic (fiery_lift_forward_launches answers without a device), hence a
+// constant rather than the device's SM count.
 #ifdef FIERY_COLS_AB
 static int g_max_chains = MAX_CHAINS;      // FIERY_CHAINS (A/B builds)
-static int g_chain_min_tiles = 148;        // FIERY_CHAIN_MIN_TILES (A/B builds)
+static int g_chain_min_tiles = 132;        // FIERY_CHAIN_MIN_TILES (A/B builds)
 #else
 constexpr int g_max_chains = MAX_CHAINS;
-constexpr int g_chain_min_tiles = 148;
+constexpr int g_chain_min_tiles = 132;
 #endif
 int lift_forward_groups(const LiftParams& P, int frames_in_chunk) {
     if (P.bev_layout == FIERY_BEV_NHWC) return 1;          // no layout pass to hide

@@ -19,7 +19,7 @@
 //     channel split is a 5-D tensor map, so the permutation is done by the copy engine).  One 16-byte shared load is then
 //     "4 adjacent columns of one (row, depth)" or "... of one (row, channel)";
 //   * a thread owns 2 depths x 4 columns x CPL channels, held as packed pairs of ADJACENT COLUMNS, so the outer product is
-//     4*CPL FFMA2 per row whose operands are exactly the register pairs the loads return;
+//     8*CPL FFMA per row whose operands are exactly the register pairs the loads return;
 //   * the tile's pillar runs are read from the plan and expanded into run-end events while the TMA is in flight;
 //   * the softmax runs in place on prob (lane = (depth mod 8, column): conflict free, reductions by shuffle);
 //   * run ends are detected warp-uniformly (one 32-bit load + one warp reduction per row, fetched a row ahead).
@@ -73,9 +73,12 @@ __device__ __forceinline__ void cp_async_8(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_addr(dst)), "l"(src) : "memory");
 }
 
-// packed fp32x2 FMA (SASS FFMA2) on two adjacent columns: acc.lo += a.lo * b.lo, acc.hi += a.hi * b.hi
+// FMA on a pair of adjacent columns held in one 64-bit register pair: acc.lo += a.lo * b.lo, acc.hi += a.hi * b.hi (two FFMA)
 __device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %0;\n\t"
+        "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
+        "mov.b64 %0, {c0, c1};\n\t}" : "+l"(acc) : "l"(a), "l"(b));
 }
 
 template <int HALF>
@@ -130,8 +133,7 @@ constexpr int GEO_OFF_CAM = 0, GEO_OFF_U = 48, GEO_OFF_V = 64, GEO_OFF_D = 192;
 
 // Calls WITHOUT a plan (a forward-only call whose calibration is new: nothing to share the geometry with): the geometry of the tile
 // is evaluated here, while the head tile is in flight -- the tile kernel waits for the copy engine at that point anyway, so this
-// costs no time (measured on B200: tile kernel 49-51 us for 8 frames with or without it), whereas a separate plan kernel in front of
-// every frame group does (step 81.6 vs 71.4 us).  Same device functions as the plan kernel (geometry.cuh), same result:
+// costs little, whereas a separate plan kernel in front of every frame group adds a launch and a dependency to every chain.  Same device functions as the plan kernel (geometry.cuh), same result:
 // the pillar (rank, fiery.py:236-256; -1 = masked) of every point, evaluated with the reference arithmetic, reduced on the fly to
 // what the pooling loop consumes:
 //   ev[unit][row]      bit j (slot j = dd*4 + col: depth DD*unit + dd, column col) set <=> pair j changes pillar between
@@ -333,7 +335,7 @@ __device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL]
 // One (depth, column) slot of the run-end handling.  `mw` is warp-uniform, so the test is a plain branch; the lanes that own
 // the ending run reduce their channels into the accumulator and restart.  The "+ 0.0f" copies are real instructions on
 // purpose: they gather the values into the consecutive registers the vector reduction needs HERE, instead of letting the
-// register allocator keep the accumulators in that order and un-shuffle them around every FFMA2.
+// register allocator keep the accumulators in that order and un-shuffle them around every FMA pair.
 template <int CPL, int DD, int SD, int COL>
 __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
                                            const int* plp, char* out) {
@@ -524,14 +526,12 @@ static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStre
     return FIERY_OK;
 }
 
-// Unit shape (CPL channels per lane, DD depths per unit), measured on B200.  The pooling loop is bound by shared-memory wavefronts
-// (a broadcast LDS.128 costs 2, a 512-byte one 4) and by the run-end control flow, so the shape trades context re-reads (48 / DD per
-// row), registers (4 * CPL * DD accumulators) and resident warps.  CPL 4 and DD 4 shapes lose (profiles/r01_notes.md,
-// profiles/r02_notes.md).
-//   * geometry in the tile (no plan): DD = 3 (512 threads, 57 registers) is 7-8 % faster when the grid fills whole waves of 2 tiles
-//     per SM (9 frames: 55.3 vs 60.2 us); DD = 2 (768 threads, row loop not unrolled) is faster while tiles run alone on an SM, i.e.
-//     when the last wave is at most half full (8 frames: 51.1 vs 53.4 us);
-//   * geometry from a plan: DD = 3 always (8 frames: 49.2 vs 53.3 us, 9 frames: 51.1 vs 55.4 us).
+// Unit shape (CPL channels per lane, DD depths per unit).  The pooling loop is bound by shared-memory wavefronts (a broadcast LDS.128
+// costs 2, a 512-byte one 4) and by the run-end control flow, so the shape trades context re-reads (48 / DD per row), registers
+// (4 * CPL * DD accumulators) and resident warps; CPL 4 and DD 4 shapes lose.
+//   * geometry in the tile (no plan): DD = 3 (512 threads) when the grid fills whole waves of 2 tiles per SM; DD = 2 (768 threads, row
+//     loop not unrolled) while tiles run alone on an SM, i.e. when the last wave is at most half full;
+//   * geometry from a plan: DD = 3 always.
 int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream) {
     FIERY_REQUIRE(P.hh <= 32, "feat_h=%d not supported by this build (<= 32)", P.hh);
     FIERY_REQUIRE(P.C == 64 && P.D <= COLS_DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);

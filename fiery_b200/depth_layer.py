@@ -3,7 +3,7 @@
 The reference builds ``self.depth_layer = nn.Conv2d(upsampling_out_channels=128, C + D, kernel_size=1, padding=0)``
 (fiery/models/encoder.py:36) and applies it to the backbone features (encoder.py:96); its output is the head tensor the lift
 consumes.  ``DepthLayer`` carries the same parameters (``weight`` (C + D, 128, 1, 1), ``bias`` (C + D,): a reference ``state_dict``
-loads unchanged) and runs the layer as a tcgen05 GEMM (fiery_b200/csrc/depth_layer.cu) that reads the features in the dtype the
+loads unchanged) and runs the layer as a wgmma GEMM (fiery_b200/csrc/depth_layer.cu) that reads the features in the dtype the
 backbone emits (fp16 / bf16 under AMP, fp32 otherwise) and writes the **fp32** head tensor directly -- the dtype the lift computes in
 (the reference's softmax and outer product run in fp32 under autocast, encoder.py:99-100), so an AMP step needs no widening pass
 between the two.  The backward (gradients of features, weight and bias) is one library call, ``aten::convolution_backward``.

@@ -87,7 +87,7 @@ def _require_cuda(t: torch.Tensor, name: str) -> None:
 
 
 class VoxelsSumming(torch.autograd.Function):
-    """Drop-in for ``fiery.utils.geometry.VoxelsSumming`` (geometry.py:283-314) on sm_100a.
+    """Drop-in for ``fiery.utils.geometry.VoxelsSumming`` (geometry.py:283-314) on sm_90a.
 
     ``forward(ctx, x, geometry, ranks) -> (x_sum, geometry_kept)``: ``x`` (Nm, C) features and ``geometry`` (Nm, 3)
     int64 voxel coordinates, both ordered by ``ranks`` (Nm,) int64 ascending.  Returns the per-voxel sums (U, C) and

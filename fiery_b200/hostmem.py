@@ -1,6 +1,6 @@
 """Host-side placement for the host-buffer entry point (``LiftSplat.lift_from_host``): one process per GPU, each bound to the
 CPU cores of its GPU's NUMA node BEFORE it allocates pinned memory, so the 36 MB up / 82 MB down per 8-frame step cross PCIe
-into local DRAM instead of the inter-socket link (an HGX B200 box has GPUs 0-3 on socket 0 and 4-7 on socket 1).
+into local DRAM instead of the inter-socket link (an 8-GPU HGX box has GPUs 0-3 on socket 0 and 4-7 on socket 1).
 
 Linux only (sysfs); everything degrades to a no-op with a reason string when the information is not available.
 """

@@ -30,8 +30,8 @@ _TORCH_TO_DTYPE = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16}
 
 # Half-precision head tensors (AMP, baseline.yml PRECISION 16): False (default) = the tensor is widened to fp32 on the device
 # first and takes the TMA path; True = the forward tile kernel reads the fp16 tensor itself (cp.async pieces widened in shared
-# memory).  Both compute the same fp32 arithmetic on exactly converted values.  Measured on B200, 8 frames: the 8-byte pieces
-# make the tile kernel slower (77.0 vs 51.0 us) than the widening pass costs (~10 us), so widening stays the default.
+# memory).  Both compute the same fp32 arithmetic on exactly converted values.  The 8-byte cp.async pieces slow the tile kernel
+# down by more than the widening pass costs, so widening stays the default.
 # Overridable with FIERY_B200_NATIVE_FP16=0/1.
 NATIVE_FP16_FORWARD = os.environ.get("FIERY_B200_NATIVE_FP16", "0") == "1"
 
@@ -451,7 +451,7 @@ class LiftSplat(nn.Module):
 
 class _LiftWarpedFn(torch.autograd.Function):
     """Fused forward (lift + warp epilogue); backward = the warp's adjoint (gather kernel), then the lift's backward.  Folding the
-    adjoint into the gradient's re-layout pass was built and measured slower (profiles/r02_notes.md), so the two stay separate."""
+    adjoint into the gradient's re-layout pass was built and measured slower, so the two stay separate."""
 
     @staticmethod
     def forward(ctx, head, intrinsics, extrinsics, plan, theta, copy_mask, module):

@@ -1,5 +1,5 @@
 /*
- * fiery_b200 -- C ABI of the Blackwell-native (sm_100a) camera->BEV lift.
+ * fiery_b200 -- C ABI of the Hopper-native (sm_90a, H100) camera->BEV lift.
  *
  * The reference (wayveai/fiery) has no FFI: its "operator API" for this path is three Python call sites
  * (SURVEY.md section 8b).  Each entry point below replaces one of them and is what a binding for the path would
@@ -228,7 +228,7 @@ FIERY_API int fiery_warp_theta(int32_t n_sequences, int32_t T, int32_t cumulativ
                                float spatial_extent_y, float* theta, uint8_t* copy_mask, void* stream);
 
 /*
- * First BEV convolution on the tensor cores (tcgen05, TF32 operands, fp32 accumulation in tensor memory) -- Decoder.first_conv
+ * First BEV convolution on the tensor cores (wgmma, TF32 operands, fp32 accumulation) -- Decoder.first_conv
  * (fiery/models/decoder.py:11,59): Conv2d(64, 64, kernel_size=7, stride=2, padding=3, bias=False), optionally followed by a per-channel
  * affine (bn1 folded for inference, decoder.py:60) and relu (decoder.py:61).  [SURVEY.md section 8f, next-2]
  * It consumes the lift's channel-last result directly: x_nhwc (B', H, W, 64) fp32 = FIERY_BEV_NHWC output of fiery_lift_forward;
@@ -241,7 +241,7 @@ FIERY_API int fiery_bev_first_conv_forward(int32_t n_frames, int32_t height, int
 
 /*
  * Encoder.depth_layer on the tensor cores -- the 1x1 convolution 128 -> D + C that produces the head tensor
- * (fiery/models/encoder.py:36,96): head_out (n_images, n_out, pixels) fp32 = weight @ feat + bias, computed by tcgen05 (fp16 / bf16
+ * (fiery/models/encoder.py:36,96): head_out (n_images, n_out, pixels) fp32 = weight @ feat + bias, computed by wgmma (fp16 / bf16
  * operands under AMP, TF32 for fp32 features; fp32 accumulation).  feat: (n_images, 128, pixels) with pixels = h*w, dtype 0 fp32 /
  * 1 fp16 / 2 bf16; weight_padded: (128, 128) row-major in the SAME dtype, rows >= n_out zero; bias: n_out floats or NULL.  Writing the
  * fp32 head directly removes the widening pass an AMP step otherwise needs in front of the lift.  [SURVEY.md section 8f, next-3]

@@ -2,7 +2,7 @@
 
 Run from the repo root:   python oracle/gen_golden.py
 
-The reference (wayveai/fiery, mounted read-only at /root/reference) is pure Python; its hot-path functions are
+The reference (a wayveai/fiery checkout, located by FIERY_REFERENCE) is pure Python; its hot-path functions are
 imported here with two stub modules for unused third-party imports (SURVEY.md appendix A) and called unbound on
 a namespace carrying the attributes ``Fiery.__init__`` would have built.  This executes the reference's own
 bytecode for fiery.py:109-128,193-208,221-273 and geometry.py:39-58,283-314; the encoder tail
@@ -12,8 +12,8 @@ bytecode for fiery.py:109-128,193-208,221-273 and geometry.py:39-58,283-314; the
 Two things happen:
   1. every oracle function is compared with the reference function it restates (bit-exact for integers and for
      float outputs that come from identical torch calls) -- a mismatch aborts;
-  2. small golden fixtures are written so the same pin holds on a box without /root/reference.
-/root/reference is never read by tests, smoke() or bench.py.
+  2. small golden fixtures are written so the same pin holds on a machine without the reference.
+The reference is never read by tests, smoke() or bench.py.
 """
 from __future__ import annotations
 
@@ -28,7 +28,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REFERENCE = "/root/reference"
+REFERENCE = os.environ.get("FIERY_REFERENCE", "")       # path of a wayveai/fiery checkout
 
 from fiery_b200.synthetic import CONFIGS, LiftConfig, make_calibration, make_head, make_grad_bev  # noqa: E402
 from oracle import lift_oracle as O  # noqa: E402
@@ -40,6 +40,8 @@ def import_reference():
             m = types.ModuleType(name)
             setattr(m, attr, object)
             sys.modules[name] = m
+    if not os.path.isdir(os.path.join(REFERENCE, "fiery")):
+        raise SystemExit("set FIERY_REFERENCE to a wayveai/fiery checkout")
     sys.path.insert(0, REFERENCE)
     from fiery.models.fiery import Fiery
     from fiery.utils.geometry import VoxelsSumming, calculate_birds_eye_view_parameters
@@ -226,11 +228,14 @@ def main():
         gpick = np.random.default_rng(6).integers(0, grad_ref.size, size=4096)
         lift[f"{tag}__grad_pick"] = gpick
         lift[f"{tag}__grad_ref_at_pick"] = grad_ref.reshape(-1)[gpick]
-        if cname == "cfg1_tiny":                     # small enough to keep whole
+        if cname == "cfg1_tiny":                     # indices and gradient whole; the BEV at 2048 of its non-zero elements
             lift[f"{tag}__idx"] = idx_r.numpy().astype(np.int32)
             lift[f"{tag}__keep"] = keep_o.numpy()
-            lift[f"{tag}__bev_ref"] = bev_ref.detach().numpy()
-            lift[f"{tag}__bev_exact"] = exact.numpy()
+            nz = np.flatnonzero(bev_ref.detach().numpy().reshape(-1))
+            dense = np.sort(np.random.default_rng(7).choice(nz, size=min(2048, nz.size), replace=False)).astype(np.int32)
+            lift[f"{tag}__bev_dense_pick"] = dense
+            lift[f"{tag}__bev_ref_at_dense_pick"] = bev_ref.detach().numpy().reshape(-1)[dense]
+            lift[f"{tag}__bev_exact_at_dense_pick"] = exact.numpy().reshape(-1)[dense]
             lift[f"{tag}__grad_ref"] = grad_ref
     np.savez_compressed(os.path.join(out_dir, "lift.npz"), **lift)
     for f in sorted(os.listdir(out_dir)):

@@ -1,5 +1,5 @@
 """Pin oracle/warp_oracle.py against the REAL reference (fiery/utils/geometry.py:82-253) and write tests/golden/warp.npz.
-Dev container only (needs /root/reference).  Run from the repo root: python oracle/gen_golden_warp.py"""
+Needs a wayveai/fiery checkout in FIERY_REFERENCE.  Run from the repo root: python oracle/gen_golden_warp.py"""
 import os
 import sys
 import types
@@ -14,7 +14,9 @@ for name, attr in (("pyquaternion", "Quaternion"), ("efficientnet_pytorch", "Eff
         m = types.ModuleType(name)
         setattr(m, attr, object)
         sys.modules[name] = m
-sys.path.insert(0, "/root/reference")
+if not os.path.isdir(os.path.join(os.environ.get("FIERY_REFERENCE", ""), "fiery")):
+    raise SystemExit("set FIERY_REFERENCE to a wayveai/fiery checkout")
+sys.path.insert(0, os.environ["FIERY_REFERENCE"])
 from fiery.utils import geometry as R  # noqa: E402
 from oracle import warp_oracle as W  # noqa: E402
 from fiery_b200.synthetic import make_egomotion  # noqa: E402

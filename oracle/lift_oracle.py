@@ -2,7 +2,7 @@
 
 This file is a CPU restatement (torch-CPU / numpy) of the reference's Lift-Splat hot path.  It exists so that
 ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline leg can check / time the algorithm on a
-box where ``/root/reference`` does not exist.  Nothing under ``fiery_b200/`` may import it: the product path
+machine without the reference.  Nothing under ``fiery_b200/`` may import it: the product path
 is the CUDA library and fails loudly without it.
 
 Where the arithmetic lives: the reference (wayveai/fiery @ fd03f16) is pure Python calling PyTorch
@@ -11,7 +11,7 @@ these torch calls: ``softmax`` (encoder.py:99), ``inverse``/``matmul`` (fiery.py
 truncation (fiery.py:237), ``argsort`` (fiery.py:257), ``cumsum`` (geometry.py:289), ``index_put``
 (fiery.py:265).  The oracle calls the same torch-CPU primitives in the same order, so it *is* the reference's
 algorithm on this torch build; ``oracle/gen_golden.py`` checks it against the real reference bytecode imported
-from ``/root/reference`` (dev container only) and commits golden vectors under ``tests/golden/``.
+from a reference checkout (``FIERY_REFERENCE``) and commits golden vectors under ``tests/golden/``.
 
 Pinned: the reference ships no tests or fixtures (SURVEY.md section 4), so parity is pinned by (i) golden
 vectors generated from the reference's own functions by ``oracle/gen_golden.py`` and (ii) the live

@@ -4,7 +4,7 @@ The small golden cases (tests/test_lift_gpu.py) run one or two frames; these bat
 on forked streams, the other unit shape of the tile kernel), so they are compared here directly, in ONE call each, with
   * the oracle's restatement of the reference op chain (fiery/models/fiery.py:193-273, encoder.py:99-100, geometry.py:283-314),
   * the fp64 exact pooling, and
-  * the reference's own recorded bytes (tests/golden/lift.npz, written by oracle/gen_golden.py from /root/reference): SHA-256 of
+  * the reference's own recorded bytes (tests/golden/lift.npz, written by oracle/gen_golden.py from the reference): SHA-256 of
     every point's voxel index and validity, sampled BEV values and gradients, norms.
 """
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 first BEV convolution (fiery_b200/csrc/bev_conv.cu; Decoder.first_conv + bn1 + relu, fiery/models/decoder.py:11,
+"""GPU: the wgmma first BEV convolution (fiery_b200/csrc/bev_conv.cu; Decoder.first_conv + bn1 + relu, fiery/models/decoder.py:11,
 59-61) against torch convolutions of the same layer.
 
 Parity bar: the kernel multiplies TF32 operands (10-bit mantissa; weights rounded at packing time, activations truncated by the

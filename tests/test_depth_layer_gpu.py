@@ -1,4 +1,4 @@
-"""GPU: Encoder.depth_layer (fiery/models/encoder.py:36,96) as a tcgen05 GEMM writing the fp32 head tensor
+"""GPU: Encoder.depth_layer (fiery/models/encoder.py:36,96) as a wgmma GEMM writing the fp32 head tensor
 (fiery_b200/csrc/depth_layer.cu).  Parity bar: fp16 / bf16 / TF32 operands with fp32 accumulation -- what cuDNN does for this layer
 under autocast / allow_tf32 -- against an fp64 convolution of the SAME rounded operands: 1e-5 normwise (only the fp32 accumulation
 order differs), and against the unrounded fp64 convolution: 2e-3 (fp16), 1e-2 (bf16), 1e-3 (TF32)."""

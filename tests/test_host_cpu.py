@@ -53,7 +53,7 @@ def test_argument_validation_without_gpu():
 
 def test_forward_launch_plan_without_gpu():
     """fiery_lift_forward_launches is host logic: one tile kernel for channel-last output; for NCHW one (tile kernel, layout
-    pass) chain per frame group, a group holding at least one tile per SM (148) and at most four groups per call."""
+    pass) chain per frame group, a group holding at least one tile per SM of an H100 (132) and at most four groups per call."""
     lib = _lib.load()
     d = _lib.LiftDesc()
     d.n_cameras, d.depth_bins, d.channels, d.feat_h, d.feat_w = 6, 48, 64, 28, 60        # 90 tiles per frame

@@ -100,7 +100,7 @@ def test_unsupported_configuration_runs_the_reference_method(fake_fiery):
 
 
 def test_depth_layer_swap_keeps_parameters_and_state_dict_keys():
-    """use_tensor_core_depth_layer: Encoder.depth_layer (encoder.py:36) becomes the tcgen05 layer with the SAME Parameters."""
+    """use_tensor_core_depth_layer: Encoder.depth_layer (encoder.py:36) becomes the tensor-core (wgmma) layer with the SAME Parameters."""
     import types
     import torch.nn as nn
     import fiery_b200.install as fb

@@ -1,6 +1,6 @@
 """CPU: the oracle (oracle/lift_oracle.py) reproduces the golden vectors that oracle/gen_golden.py recorded from the
 REAL reference functions (fiery/models/fiery.py:109-128,193-208,221-273; fiery/utils/geometry.py:39-58,283-314).
-This is what pins the oracle on a box where /root/reference does not exist."""
+This is what pins the oracle on a machine without the reference."""
 import numpy as np
 import pytest
 import torch
@@ -80,8 +80,15 @@ def test_lift_matches_reference(golden_lift, case):
     oracle = O.LiftOracle.from_config(cfg)
     comb = torch.from_numpy(golden_lift[f"{tag}__combined"])
     head.requires_grad_(True)
-    bev = oracle.lift(head, K, E, combined=comb)
-    bev.backward(gout)
+    # torch's CPU argsort / cumsum split the work by thread count, which moves the cumsum rounding of the reference's pooling
+    # (1.5e-6 normwise at 3 threads); one thread reproduces the recorded run on any host
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)
+    try:
+        bev = oracle.lift(head, K, E, combined=comb)
+        bev.backward(gout)
+    finally:
+        torch.set_num_threads(threads)
     pick = golden_lift[f"{tag}__bev_pick"]
     ref = golden_lift[f"{tag}__bev_ref_at_pick"]
     got = bev.detach().flatten()[pick].numpy()
@@ -95,8 +102,9 @@ def test_lift_matches_reference(golden_lift, case):
     assert np.abs(ggot - gref).max() <= 2e-5 * float(np.abs(gref).max())
     occupied = bev.detach().abs().sum(1) > 0
     assert np.array_equal(occupied.flatten(1).sum(1).numpy(), golden_lift[f"{tag}__occupied_count"])
-    if "cfg1" in case[0]:
-        assert O.normwise_error(bev, torch.from_numpy(golden_lift[f"{tag}__bev_ref"])) < 1e-6
+    if "cfg1" in case[0]:                            # the reference's values at a seeded sample of its non-zero BEV elements
+        dense = golden_lift[f"{tag}__bev_dense_pick"]
+        assert O.normwise_error(bev.detach().flatten()[dense], torch.from_numpy(golden_lift[f"{tag}__bev_ref_at_dense_pick"])) < 1e-6
         assert O.normwise_error(head.grad, torch.from_numpy(golden_lift[f"{tag}__grad_ref"])) < 1e-6
 
 
@@ -108,9 +116,11 @@ def test_exact_pooling_is_the_adjudicator(golden_lift):
     tag = golden_tag(case)
     oracle = O.LiftOracle.from_config(cfg)
     exact = oracle.lift_exact(head, K, E, combined=torch.from_numpy(golden_lift[f"{tag}__combined"]))
-    assert O.normwise_error(exact, torch.from_numpy(golden_lift[f"{tag}__bev_exact"])) < 1e-12
-    ref = torch.from_numpy(golden_lift[f"{tag}__bev_ref"])
-    assert O.normwise_error(ref, exact) < 1e-4
+    dense = golden_lift[f"{tag}__bev_dense_pick"]
+    assert O.normwise_error(exact.flatten()[dense], torch.from_numpy(golden_lift[f"{tag}__bev_exact_at_dense_pick"])) < 1e-12
+    assert np.allclose(exact.flatten(1).norm(dim=1).numpy(), golden_lift[f"{tag}__exact_norm"], rtol=1e-12)
+    ref = torch.from_numpy(golden_lift[f"{tag}__bev_ref_at_dense_pick"])
+    assert O.normwise_error(ref, exact.flatten()[dense]) < 1e-4
 
 
 @pytest.mark.parametrize("case", FAST_CASES, ids=case_id)

@@ -195,7 +195,7 @@ def test_multi_pass_path_matches_oracle(layout):
         from fiery_b200 import lift as lift_mod
         lift_mod._scratch.clear()
         assert int(lib.fiery_lift_scratch_bytes(desc)) < full or layout == "channels_last"
-        groups_per_pass = 2 if layout == "contiguous" else 1         # 4 frames = 360 tiles: two chains of >= 148 tiles
+        groups_per_pass = 2 if layout == "contiguous" else 1         # 4 frames = 360 tiles: two chains of >= 132 tiles
         per_group = 2 if layout == "contiguous" else 1
         assert int(lib.fiery_lift_forward_launches(desc)) == (2 * groups_per_pass + 1) * per_group
         with torch.no_grad():

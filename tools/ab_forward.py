@@ -75,7 +75,7 @@ best = min((v for v in res["tile"] if "us_mean" in res["tile"][v] and res["tile"
 res["best_tile"] = best
 out_nchw = torch.empty((F, cfg.out_channels, X, Y), dtype=torch.float32, device=dev)
 ref_nchw = ref.permute(0, 3, 1, 2)
-combos = os.environ.get("AB_COMBOS", "1:148 2:148 4:148").split()
+combos = os.environ.get("AB_COMBOS", "1:132 2:132 4:132").split()
 from fiery_b200.synthetic import make_grad_bev
 gout = torch.from_numpy(make_grad_bev(cfg, seed=100)).to(dev)
 for combo in combos:

@@ -1,4 +1,4 @@
-"""Time Encoder.depth_layer (1x1 conv 128 -> 112) on the tcgen05 kernel against cuDNN (+ the widening pass an AMP step needs)."""
+"""Time Encoder.depth_layer (1x1 conv 128 -> 112) on the wgmma kernel against cuDNN (+ the widening pass an AMP step needs)."""
 import sys
 import torch
 import torch.nn.functional as F
@@ -36,4 +36,4 @@ for dtype in ((torch.float16,) if only == 'fp16' else (torch.float16, torch.bflo
     t_conv = timeit(lambda: F.conv2d(feat, wd, bd)) if only is None else 0.0
     t_conv_widen = timeit(lambda: F.conv2d(feat, wd, bd).float()) if only is None else 0.0
     byts = feat.numel() * feat.element_size() + N * n_out * h * w * 4
-    print(f"{dtype}: tcgen05 {t_ours:.1f} us ({byts / t_ours * 1e-3:.0f} GB/s algorithmic) | cuDNN {t_conv:.1f} us | cuDNN + .float() {t_conv_widen:.1f} us")
+    print(f"{dtype}: wgmma {t_ours:.1f} us ({byts / t_ours * 1e-3:.0f} GB/s algorithmic) | cuDNN {t_conv:.1f} us | cuDNN + .float() {t_conv_widen:.1f} us")

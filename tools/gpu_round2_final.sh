@@ -1,5 +1,5 @@
 #!/bin/bash
-# round-2 final evidence on ONE B200: GPU tests, smoke, bench lines (all workloads, both directions, reference arm), launch list of the
+# round-2 final evidence on ONE GPU: GPU tests, smoke, bench lines (all workloads, both directions, reference arm), launch list of the
 # bench command, full captures of the kernels of the step.  Everything lands in gpurun_out/ with the tag given as $1.
 T=${1:-r02final}
 mkdir -p gpurun_out

@@ -1,5 +1,5 @@
 // Microbenchmark: why is the accumulator -> NCHW finalize pass slow?  Variants isolate reads / zero-writes / store shape.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o finalize_variants finalize_variants.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o finalize_variants finalize_variants.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

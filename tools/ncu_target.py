@@ -6,8 +6,8 @@
     python tools/ncu_target.py <workload> warp_bwd      # backward of cumulative_warp_features (3, 3, 64, X, Y): the gather adjoint, 3 calls
     python tools/ncu_target.py <workload> step_warped   # lift with the warp folded into the layout pass (finalize_warp_kernel), 3 calls
     python tools/ncu_target.py <workload> bwd     # NCHW backward (re-layout + backward tile kernel), 3 calls
-    python tools/ncu_target.py <workload> depth   # the tcgen05 depth_layer (fp16 features -> fp32 head tensor) at the workload's size, 4 calls
-    python tools/ncu_target.py <workload> conv    # the tcgen05 first BEV convolution on a channel-last BEV of the workload's size, 4 calls
+    python tools/ncu_target.py <workload> depth   # the wgmma depth_layer (fp16 features -> fp32 head tensor) at the workload's size, 4 calls
+    python tools/ncu_target.py <workload> conv    # the wgmma first BEV convolution on a channel-last BEV of the workload's size, 4 calls
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
