@@ -73,10 +73,33 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// L2 eviction-priority policies (createpolicy: a 64-bit descriptor covering the whole access) for the .L2::cache_hint forms:
+// evict_first for data used once (it streams past what should stay), evict_last for data that is used again soon,
+// evict_normal to hand lines back to the default priority.
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_last() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_normal() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
 // 1-D bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP); 16-byte aligned, size a multiple of 16
 __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)), "l"(policy) : "memory");
 }
 
 // 3-D tiled TMA load global -> shared, completion signalled on an mbarrier (SASS: UTMALDG)
@@ -92,6 +115,14 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
     asm volatile(
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
         ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3,
+                                            uint64_t policy) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
+        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
+          "l"(policy)
         : "memory");
 }
 

@@ -67,20 +67,27 @@ finalize_nchw_kernel(float* __restrict__ accum, unsigned char* __restrict__ flag
 constexpr int FT_P = 64;
 constexpr int FT_THREADS = 256;
 
-__device__ __forceinline__ void bulk_store_1d(void* dst, const void* src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_addr(src)), "r"(bytes) : "memory");
+__device__ __forceinline__ void bulk_store_1d(void* dst, const void* src, uint32_t bytes, uint64_t policy) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+                 ::"l"(dst), "r"(smem_addr(src)), "r"(bytes), "l"(policy) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, uint64_t policy) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
+                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(src)), "r"(c0), "r"(c1), "r"(c2), "l"(policy) : "memory");
+}
+
+// L2 priority of the restored zeros: evict_last while another frame group of the lane reduces into the same rows next, evict_normal
+// after the lane's last group so that a call leaves no raised-priority lines behind
+__device__ __forceinline__ uint64_t l2_restore_policy(int last_in_lane) {
+    return last_in_lane ? l2_evict_normal() : l2_evict_last();
 }
 
 __global__ void __launch_bounds__(FT_THREADS)
 finalize_tma_kernel(const __grid_constant__ CUtensorMap bev_map, float* __restrict__ accum, unsigned char* __restrict__ touched,
-                    long long pillars, int tiles_per_frame, int frame_out0, int clear_marks) {
+                    long long pillars, int tiles_per_frame, int frame_out0, int clear_marks, int last_in_lane) {
     constexpr int C = 64;
     __shared__ __align__(128) float s_in[FT_P * C];      // [pillar][channel]: bulk-copy destination
     __shared__ __align__(128) float s_out[C * FT_P];     // [channel][pillar]: TMA store source
@@ -110,7 +117,7 @@ finalize_tma_kernel(const __grid_constant__ CUtensorMap bev_map, float* __restri
         if (f) {
             row = accum + (static_cast<size_t>(frame) * pillars + p) * C;
             mbar_arrive_expect_tx(&bar, C * 4);
-            bulk_load_1d(s_in + tid * C, row, C * 4, &bar);
+            bulk_load_1d(s_in + tid * C, row, C * 4, &bar, l2_evict_last());
         } else {
             mbar_arrive(&bar);
         }
@@ -140,9 +147,9 @@ finalize_tma_kernel(const __grid_constant__ CUtensorMap bev_map, float* __restri
     }
     fence_proxy_async();                                // generic-proxy writes (s_out, s_zero) -> visible to the copy engine
     __syncthreads();
-    if (tid == 0) tma_store_3d(&bev_map, s_out, static_cast<int>(p0), 0, frame_out0 + frame);
+    if (tid == 0) tma_store_3d(&bev_map, s_out, static_cast<int>(p0), 0, frame_out0 + frame, l2_evict_first());   // written once
     if (row) {                                          // restore the all-zero scratch
-        bulk_store_1d(row, s_zero, C * 4);
+        bulk_store_1d(row, s_zero, C * 4, l2_restore_policy(last_in_lane));
         if (clear_marks) *mark = 0;             // marks of a caller-owned plan stay: the plan is reused
     }
     if (tid == 0 || row) tma_store_commit_and_wait();   // the shared sources must outlive the copies
@@ -212,13 +219,16 @@ finalize_warp_kernel(const float* __restrict__ accum, const unsigned char* __res
     }
     __syncthreads();
     float* dst = bev + static_cast<size_t>(gframe) * C * pillars + p0;
+    const uint64_t once = l2_evict_first();             // the output is written once
 #pragma unroll
     for (int cc = 0; cc < C / (FW_THREADS / 32); ++cc) {
         const int c = warp * (C / (FW_THREADS / 32)) + cc;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const int px = half * 32 + lane;
-            if (p0 + px < pillars) __stcs(dst + static_cast<size_t>(c) * pillars + px, s_out[c][px]);
+            if (p0 + px < pillars)
+                asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;"
+                             ::"l"(dst + static_cast<size_t>(c) * pillars + px), "f"(s_out[c][px]), "l"(once) : "memory");
         }
     }
 }
@@ -226,16 +236,19 @@ finalize_warp_kernel(const float* __restrict__ accum, const unsigned char* __res
 // Restores the all-zero scratch after finalize_warp_kernel: a warp looks at 32 marks and zeroes the 256-byte accumulator row of
 // every marked pillar with one 8-byte store per lane; marks that live in the scratch are cleared too (a caller's plan keeps its own).
 __global__ void __launch_bounds__(256)
-clear_touched_kernel(float* __restrict__ accum, unsigned char* __restrict__ touched, long long n_pillars, int clear_marks) {
+clear_touched_kernel(float* __restrict__ accum, unsigned char* __restrict__ touched, long long n_pillars, int clear_marks,
+                     int last_in_lane) {
     const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
     const unsigned char f = p < n_pillars ? touched[p] : 0;
     unsigned m = __ballot_sync(0xffffffffu, f != 0);
     const long long base = p - lane;
+    const uint64_t policy = l2_restore_policy(last_in_lane);
     while (m) {
         const int i = __ffs(m) - 1;
         m &= m - 1;
-        reinterpret_cast<float2*>(accum + static_cast<size_t>(base + i) * 64)[lane] = make_float2(0.f, 0.f);
+        asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %1}, %2;"
+                     ::"l"(accum + static_cast<size_t>(base + i) * 64 + 2 * lane), "f"(0.f), "l"(policy) : "memory");
     }
     if (f && clear_marks) touched[p] = 0;
 }
@@ -298,23 +311,17 @@ int lift_chunk_frames(const LiftParams& P) {
     return static_cast<int>(c < 1 ? 1 : c);
 }
 
-// scratch of one pass (NCHW output): [accumulator (chunk, X*Y, C) fp32][marks (chunk, X*Y) bytes, padded to 128]; all zero between calls
-size_t lift_scratch_bytes(const LiftParams& P) {
-    if (P.bev_layout != FIERY_BEV_NCHW || P.n_frames <= 0) return 0;
-    const size_t chunk = static_cast<size_t>(lift_chunk_frames(P));
-    return chunk * P.pillars * P.C * 4 + ((chunk * P.pillars + 127) & ~static_cast<size_t>(127));
-}
-
 int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream);
 int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels, int n_frames, int box_pillars);
 
 // Side streams and fork/join events of the forward chains: created once per host thread and device (thread_local, so concurrent
 // callers never share or race on them), reused by every call -- nothing is created or destroyed on the launch path.
-constexpr int MAX_CHAINS = 4;
+constexpr int MAX_CHAINS = 4;     // frame groups of a pass
+constexpr int MAX_LANES = 2;      // streams (and scratch slices) they run on, see lane_layout
 struct ChainResources {
-    cudaStream_t side[MAX_CHAINS - 1] = {};
+    cudaStream_t side[MAX_LANES - 1] = {};
     cudaEvent_t fork = nullptr;
-    cudaEvent_t done[MAX_CHAINS - 1] = {};
+    cudaEvent_t done[MAX_LANES - 1] = {};
     bool ready = false;
 };
 static int chain_resources(ChainResources** out) {
@@ -324,7 +331,7 @@ static int chain_resources(ChainResources** out) {
     FIERY_REQUIRE(dev >= 0 && dev < 16, "device %d out of range for the chain resources", dev);
     ChainResources& r = pool[dev];
     if (!r.ready) {
-        for (int i = 0; i < MAX_CHAINS - 1; ++i) {
+        for (int i = 0; i < MAX_LANES - 1; ++i) {
             FIERY_CUDA_CHECK(cudaStreamCreateWithFlags(&r.side[i], cudaStreamNonBlocking));
             FIERY_CUDA_CHECK(cudaEventCreateWithFlags(&r.done[i], cudaEventDisableTiming));
         }
@@ -335,8 +342,8 @@ static int chain_resources(ChainResources** out) {
     return FIERY_OK;
 }
 
-// NCHW output: the frames of a chunk are cut into groups, each a (plan kernel ->) tile kernel -> layout pass chain on its own stream.
-// The layout pass of one group (DRAM-bound) runs under the tile kernels of the others (issue-bound); only the last pass is
+// NCHW output: the frames of a chunk are cut into groups, each a tile kernel -> layout pass chain, spread over the lanes below.
+// The layout pass of one group (DRAM-bound) runs beside the tile kernel of the other lane (issue-bound); only the last pass is
 // exposed.  A group whose tile kernel cannot fill the GPU once loses more than the overlap gains, so a group keeps at least one
 // tile per SM of an H100 SXM (132).  The count is host logic (fiery_lift_forward_launches answers without a device), hence a
 // constant rather than the device's SM count.
@@ -353,6 +360,52 @@ int lift_forward_groups(const LiftParams& P, int frames_in_chunk) {
     const long long tiles_per_frame = static_cast<long long>(P.n_cameras) * P.n_wtiles;
     while (groups > 1 && (frames_in_chunk / groups) * tiles_per_frame < g_chain_min_tiles) --groups;
     return groups < 1 ? 1 : groups;
+}
+
+// Scratch lanes.  The frame groups of a pass share the scratch in (at most MAX_LANES) slices: group g runs on lane g % lanes, i.e. on
+// that lane's stream and in that lane's slice, so a lane runs tile(g) -> layout(g) -> tile(g + lanes) -> ...  Stream order alone
+// guarantees that the layout pass of one group has restored the zeros before the next group of the lane reduces into the slice.
+// Frames of one rig touch nearly the same pillars, so the next group's reductions land on lines the layout pass has just re-zeroed
+// in L2 (kept there with evict_last hints) instead of fetching zeros from DRAM, and the scratch of a pass is the largest group of
+// each lane, not the whole chunk.  Fewer lanes move fewer bytes but overlap less of the layout passes with tile kernels: on an H100
+// two lanes beat three and four on every bench workload (DESIGN.md section 2.3).  Host logic, like the group count.
+struct LaneLayout {
+    int groups, lanes;
+    int frames;                               // scratch frames of the pass
+    int slice0[MAX_LANES];                    // first scratch frame of each lane's slice
+};
+static int group_start(int nf, int groups, int g) { return static_cast<int>(static_cast<long long>(nf) * g / groups); }
+static LaneLayout lane_layout(const LiftParams& P, int frames_in_chunk) {
+    LaneLayout L;
+    L.groups = lift_forward_groups(P, frames_in_chunk);
+    L.lanes = L.groups < MAX_LANES ? L.groups : MAX_LANES;
+    L.frames = 0;
+    for (int l = 0; l < L.lanes; ++l) {
+        int largest = 0;
+        for (int g = l; g < L.groups; g += L.lanes) {
+            const int n = group_start(frames_in_chunk, L.groups, g + 1) - group_start(frames_in_chunk, L.groups, g);
+            largest = n > largest ? n : largest;
+        }
+        L.slice0[l] = L.frames;
+        L.frames += largest;
+    }
+    return L;
+}
+
+// frames of scratch a call needs: the lanes' frames of its largest pass
+static int scratch_frames(const LiftParams& P) {
+    const int chunk = lift_chunk_frames(P);
+    const int full = lane_layout(P, chunk).frames;
+    if (P.n_frames % chunk == 0) return full;
+    const int tail = lane_layout(P, P.n_frames % chunk).frames;     // the last pass is shorter and may be cut into fewer groups
+    return tail > full ? tail : full;
+}
+
+// scratch (NCHW output): [accumulator (F, X*Y, C) fp32][marks (F, X*Y) bytes, padded to 128], F = scratch_frames; all zero between calls
+size_t lift_scratch_bytes(const LiftParams& P) {
+    if (P.bev_layout != FIERY_BEV_NCHW || P.n_frames <= 0) return 0;
+    const size_t f = static_cast<size_t>(scratch_frames(P));
+    return f * P.pillars * P.C * 4 + ((f * P.pillars + 127) & ~static_cast<size_t>(127));
 }
 
 // kernel launches of one forward call (include/fiery_b200.h: fiery_lift_forward_launches)
@@ -405,8 +458,9 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
     // lift into a channel-last accumulator (NHWC: the caller's zero-filled output itself), then the layout pass for NCHW; several
     // passes only to bound the scratch footprint
     const int chunk = lift_chunk_frames(P);
-    float* accum = static_cast<float*>(scratch);    // [accumulator floats of one pass][one mark byte per pillar]
-    unsigned char* scratch_marks = nchw ? reinterpret_cast<unsigned char*>(accum + static_cast<size_t>(chunk) * P.pillars * P.C) : nullptr;
+    float* accum = static_cast<float*>(scratch);    // [accumulator floats of the lanes][one mark byte per pillar]
+    unsigned char* scratch_marks =
+        nchw ? reinterpret_cast<unsigned char*>(accum + static_cast<size_t>(scratch_frames(P)) * P.pillars * P.C) : nullptr;
     const bool tma_pass = P.pillars % 4 == 0;      // the output map needs a 16-byte row pitch
     CUtensorMap bev_map;
     if (nchw && tma_pass && !warp_theta) {
@@ -416,21 +470,23 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
     ChainResources* res = nullptr;
     for (int f0 = 0; f0 < P.n_frames; f0 += chunk) {
         const int nf = (P.n_frames - f0 < chunk) ? P.n_frames - f0 : chunk;
-        const int groups = lift_forward_groups(P, nf);
-        cudaStream_t chain[MAX_CHAINS] = {stream};
-        if (groups > 1) {                           // fork: the side streams start behind everything queued on the caller's
+        const LaneLayout lanes = lane_layout(P, nf);
+        cudaStream_t chain[MAX_LANES] = {stream};
+        if (lanes.lanes > 1) {                      // fork: the side streams start behind everything queued on the caller's
             if (!res) {
                 rc = chain_resources(&res);
                 if (rc != FIERY_OK) return rc;
             }
-            for (int g = 1; g < groups; ++g) chain[g] = res->side[g - 1];
+            for (int l = 1; l < lanes.lanes; ++l) chain[l] = res->side[l - 1];
             FIERY_CUDA_CHECK(cudaEventRecord(res->fork, stream));
         }
-        for (int g = 0; g < groups; ++g) {
-            const int s0 = static_cast<int>(static_cast<long long>(nf) * g / groups);
-            const int s1 = static_cast<int>(static_cast<long long>(nf) * (g + 1) / groups);
-            cudaStream_t st = chain[g];
-            if (g > 0) FIERY_CUDA_CHECK(cudaStreamWaitEvent(st, res->fork, 0));
+        for (int g = 0; g < lanes.groups; ++g) {
+            const int s0 = group_start(nf, lanes.groups, g), s1 = group_start(nf, lanes.groups, g + 1);
+            const int lane = g % lanes.lanes;
+            const bool last_in_lane = g + lanes.lanes >= lanes.groups;
+            const size_t slice = static_cast<size_t>(lanes.slice0[lane]);
+            cudaStream_t st = chain[lane];
+            if (lane > 0 && g < lanes.lanes) FIERY_CUDA_CHECK(cudaStreamWaitEvent(st, res->fork, 0));
             Q.frame0 = f0 + s0;
             Q.n_frames = s1 - s0;
             unsigned char* marks = nullptr;         // "pillar receives a point" bytes the layout pass reads
@@ -441,10 +497,10 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
                 marks = const_cast<unsigned char*>(v.touched);
             } else {                                // the tile kernel evaluates the geometry itself and marks into the scratch
                 Q.plan_tiles = nullptr;
-                marks = nchw ? scratch_marks + static_cast<size_t>(s0) * P.pillars : nullptr;
+                marks = nchw ? scratch_marks + slice * P.pillars : nullptr;
                 Q.touched = marks;
             }
-            Q.accum = nchw ? accum + static_cast<size_t>(s0) * P.pillars * P.C
+            Q.accum = nchw ? accum + slice * P.pillars * P.C
                            : bev_out + static_cast<size_t>(Q.frame0) * P.pillars * P.C;
             timer_begin(st, 1);
             rc = launch_forward_cols(Q, head, st);
@@ -457,11 +513,12 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
                     finalize_warp_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FW_THREADS, 0, st>>>(
                         Q.accum, marks, bev_out, P.pillars, P.grid.X, P.grid.Y, tpf, Q.frame0, warp_theta, warp_copy);
                     const long long n = P.pillars * Q.n_frames;
-                    clear_touched_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(Q.accum, marks, n, plan ? 0 : 1);
+                    clear_touched_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(Q.accum, marks, n, plan ? 0 : 1,
+                                                                                                 last_in_lane ? 1 : 0);
                 } else if (tma_pass) {
                     const int tpf = static_cast<int>((P.pillars + FT_P - 1) / FT_P);
-                    finalize_tma_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FT_THREADS, 0, st>>>(bev_map, Q.accum, marks, P.pillars,
-                                                                                                     tpf, Q.frame0, plan ? 0 : 1);
+                    finalize_tma_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FT_THREADS, 0, st>>>(
+                        bev_map, Q.accum, marks, P.pillars, tpf, Q.frame0, plan ? 0 : 1, last_in_lane ? 1 : 0);
                 } else {
                     const int bpf = static_cast<int>((P.pillars + FIN_THREADS - 1) / FIN_THREADS);
                     finalize_nchw_kernel<<<static_cast<unsigned>(bpf) * Q.n_frames, FIN_THREADS, 0, st>>>(
@@ -470,9 +527,9 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
                 timer_end(st);
                 FIERY_CUDA_CHECK(cudaGetLastError());
             }
-            if (g > 0) {                            // join the chain back into the caller's stream
-                FIERY_CUDA_CHECK(cudaEventRecord(res->done[g - 1], st));
-                FIERY_CUDA_CHECK(cudaStreamWaitEvent(stream, res->done[g - 1], 0));
+            if (lane > 0 && last_in_lane) {         // join the lane back into the caller's stream
+                FIERY_CUDA_CHECK(cudaEventRecord(res->done[lane - 1], st));
+                FIERY_CUDA_CHECK(cudaStreamWaitEvent(stream, res->done[lane - 1], 0));
             }
         }
     }

@@ -67,8 +67,17 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, u
         ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4,
+                                            uint64_t policy) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;"
+        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4),
+          "l"(policy)
+        : "memory");
+}
 
 // 8-byte asynchronous copy global -> shared (SASS LDGSTS.64): one (channel, row) piece = 4 half-precision columns
+// (no L2 policy here: ptxas 12.9 gives the .L2::cache_hint form of this instruction a descriptor operand it never writes)
 __device__ __forceinline__ void cp_async_8(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_addr(dst)), "l"(src) : "memory");
 }
@@ -321,50 +330,57 @@ __device__ __forceinline__ void softmax_cols(const LiftParams& P, const ColsLayo
     }
 }
 
-// predicated vector reduction of CPL adjacent channels
-template <int CPL>
-__device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL], unsigned bit) {
-    if (CPL == 4)
+// predicated vector reduction of CPL adjacent channels; HINT: with an L2 `policy` (the scratch accumulator stays in L2 for the layout pass)
+template <int CPL, bool HINT>
+__device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL], unsigned bit, uint64_t policy) {
+    if (!HINT && CPL == 4)
         asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %5, 0;\n\t@p red.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n\t}"
                      :: "l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[CPL > 2 ? 2 : 0]), "f"(v[CPL > 3 ? 3 : 0]), "r"(bit) : "memory");
-    else
+    else if (!HINT)
         asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\t@p red.global.add.v2.f32 [%0], {%1, %2};\n\t}"
                      :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit) : "memory");
+    else if (CPL == 4)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %5, 0;\n\t@p red.global.add.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %6;\n\t}"
+                     :: "l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[CPL > 2 ? 2 : 0]), "f"(v[CPL > 3 ? 3 : 0]), "r"(bit), "l"(policy) : "memory");
+    else
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\t@p red.global.add.L2::cache_hint.v2.f32 [%0], {%1, %2}, %4;\n\t}"
+                     :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit), "l"(policy) : "memory");
 }
 
 // One (depth, column) slot of the run-end handling.  `mw` is warp-uniform, so the test is a plain branch; the lanes that own
 // the ending run reduce their channels into the accumulator and restart.  The "+ 0.0f" copies are real instructions on
 // purpose: they gather the values into the consecutive registers the vector reduction needs HERE, instead of letting the
 // register allocator keep the accumulators in that order and un-shuffle them around every FMA pair.
-template <int CPL, int DD, int SD, int COL>
+template <int CPL, int DD, int SD, int COL, bool HINT>
 __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
-                                           const int* plp, char* out) {
+                                           const int* plp, char* out, uint64_t policy) {
     constexpr int j = SD * 4 + COL;
     if (mw & (1u << j)) {
         const unsigned pl = static_cast<unsigned>(plp[j]);
         float v[CPL];
 #pragma unroll
         for (int k = 0; k < CPL; ++k) v[k] = __fadd_rn(half_of<COL & 1>(acc[k][SD][COL >> 1]), 0.0f);
-        red_channels_if<CPL>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j));
+        red_channels_if<CPL, HINT>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j), policy);
         const unsigned keep = ((own >> j) & 1u) - 1u;          // 0 where my run ends, ~0 otherwise
 #pragma unroll
         for (int k = 0; k < CPL; ++k) clear_half<COL & 1>(acc[k][SD][COL >> 1], keep);
     }
 }
 
-template <int CPL, int DD, int SD>
+template <int CPL, int DD, int SD, bool HINT>
 __device__ __forceinline__ void flush_depth(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
-                                            const int* plp, char* out) {
+                                            const int* plp, char* out, uint64_t policy) {
     if (mw & (0xfu << (4 * SD))) {
-        flush_slot<CPL, DD, SD, 0>(acc, mw, own, flush, plp, out); flush_slot<CPL, DD, SD, 1>(acc, mw, own, flush, plp, out);
-        flush_slot<CPL, DD, SD, 2>(acc, mw, own, flush, plp, out); flush_slot<CPL, DD, SD, 3>(acc, mw, own, flush, plp, out);
+        flush_slot<CPL, DD, SD, 0, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<CPL, DD, SD, 1, HINT>(acc, mw, own, flush, plp, out, policy);
+        flush_slot<CPL, DD, SD, 2, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<CPL, DD, SD, 3, HINT>(acc, mw, own, flush, plp, out, policy);
     }
-    if constexpr (SD + 1 < DD) flush_depth<CPL, DD, SD + 1>(acc, mw, own, flush, plp, out);
+    if constexpr (SD + 1 < DD) flush_depth<CPL, DD, SD + 1, HINT>(acc, mw, own, flush, plp, out, policy);
 }
 
 // CPL channels per lane, DD depths per unit: a unit is 64 / CPL lanes, a tile 48 / DD units.
 //   CPL 2, DD 2: 768 threads (a unit is a warp)      CPL 2, DD 4: 384 threads      CPL 4, DD 4: 192 threads (a unit is a half-warp)
-template <int CPL, int DD, int MINB, int UNR = 2, bool HALF = false, bool PLANNED = false>
+// HINTS: NCHW output, L2 policies on the head loads and the reductions into the scratch (lift_fwd.cu: lanes)
+template <int CPL, int DD, int MINB, int UNR = 2, bool HALF = false, bool PLANNED = false, bool HINTS = false>
 __global__ void __launch_bounds__((COLS_DPAD / DD) * (64 / CPL), MINB)
 lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const LiftParams P) {
     constexpr int LPU = 64 / CPL;                     // lanes per unit
@@ -401,8 +417,14 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
         tma_prefetch_desc(&head_maps.ctx);
         const uint32_t prob_bytes = P.use_depth ? static_cast<uint32_t>(hh * COLS_DPAD * WT * 4) : 0u;
         mbar_arrive_expect_tx(bar, prob_bytes + static_cast<uint32_t>(hh * L.C * WT * 4));
-        if (P.use_depth) tma_load_4d(smem + L.off_prob, &head_maps.depth, bar, w0, 0, 0, img);
-        tma_load_5d(smem + L.off_ctx, &head_maps.ctx, bar, w0, 0, 0, 0, img);
+        if (HINTS) {
+            const uint64_t once = l2_evict_first();                                  // the head is read once
+            if (P.use_depth) tma_load_4d(smem + L.off_prob, &head_maps.depth, bar, w0, 0, 0, img, once);
+            tma_load_5d(smem + L.off_ctx, &head_maps.ctx, bar, w0, 0, 0, 0, img, once);
+        } else {
+            if (P.use_depth) tma_load_4d(smem + L.off_prob, &head_maps.depth, bar, w0, 0, 0, img);
+            tma_load_5d(smem + L.off_ctx, &head_maps.ctx, bar, w0, 0, 0, 0, img);
+        }
     }
     {
         unsigned* s_ev = reinterpret_cast<unsigned*>(smem + L.off_ev);
@@ -448,6 +470,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
     const int* plp = reinterpret_cast<const int*>(smem + L.off_pillar) + unit * SLOTS - COLS_NPAIR;          // row h-1
     char* out = reinterpret_cast<char*>(P.accum + static_cast<size_t>(frame) * P.pillars * P.C + cl * CPL);
     const unsigned* evp = reinterpret_cast<const unsigned*>(smem + L.off_ev) + unit * COLS_EVS + 1;         // row h+1
+    const uint64_t keep = HINTS ? l2_evict_last() : 0;   // the scratch accumulator: the layout pass reads these lines next
 
     unsigned long long acc[CPL][DD][2];               // [channel k][depth dd][column pair]
 #pragma unroll
@@ -463,7 +486,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
 #pragma unroll UNR
     for (int h = 0; h < hh; ++h, pp += COLS_DPAD * WT, cp += 64 * WT, plp += COLS_NPAIR, ++evp) {
         const unsigned ev_next = *evp;                                // the word after the last row stays 0
-        if (mw) flush_depth<CPL, DD, 0>(acc, mw, own, flush, plp, out);
+        if (mw) flush_depth<CPL, DD, 0, HINTS>(acc, mw, own, flush, plp, out, keep);
         ulonglong2 dv[DD];
 #pragma unroll
         for (int dd = 0; dd < DD; ++dd) dv[dd] = *reinterpret_cast<const ulonglong2*>(pp + dd * WT);   // columns (0,1) (2,3)
@@ -491,21 +514,21 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
             const unsigned long long a = acc[k][j >> 2][(j & 3) >> 1];
             v[k] = (j & 1) ? half_of<1>(a) : half_of<0>(a);
         }
-        red_channels_if<CPL>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u);
+        red_channels_if<CPL, HINTS>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u, keep);
     }
 }
 
 int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane);
 
-template <int CPL, int DD, int MINB, int UNR, bool HALF, bool PLANNED>
+template <int CPL, int DD, int MINB, int UNR, bool HALF, bool PLANNED, bool HINTS>
 static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStream_t stream) {
     constexpr int NU = COLS_DPAD / DD, NT = NU * (64 / CPL);
     const ColsLayout L(P.hh, P.C, NU);
     static OncePerDevice once;                        // zero-initialised (static storage)
     int rc = once.run([]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         // ask for the full shared-memory carve-out (two or three tiles of ~75 KB per SM for the reference shape)
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                               cudaSharedmemCarveoutMaxShared));
         return FIERY_OK;
     });
@@ -521,9 +544,17 @@ static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStre
         if (rc != FIERY_OK) return rc;
     }
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
-    lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED><<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
+    lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS><<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
+}
+
+// L2 hints for NCHW output only: with channel-last output the tile kernel reduces into the caller's output, and hinted there it
+// measured slower on an H100 than with the plain instructions
+template <int DD, int UNR, bool HALF, bool PLANNED>
+static int launch_layout_t(const LiftParams& P, const void* head, cudaStream_t stream) {
+    return P.bev_layout == FIERY_BEV_NCHW ? launch_forward_cols_t<2, DD, 2, UNR, HALF, PLANNED, true>(P, head, stream)
+                                          : launch_forward_cols_t<2, DD, 2, UNR, HALF, PLANNED, false>(P, head, stream);
 }
 
 // Unit shape (CPL channels per lane, DD depths per unit).  The pooling loop is bound by shared-memory wavefronts (a broadcast LDS.128
@@ -547,11 +578,11 @@ int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stre
 #endif
     const bool half = P.head_f16 != nullptr;
     if (planned) {
-        if (dd3) return half ? launch_forward_cols_t<2, 3, 2, 2, true, true>(P, head, stream) : launch_forward_cols_t<2, 3, 2, 2, false, true>(P, head, stream);
-        return half ? launch_forward_cols_t<2, 2, 2, 1, true, true>(P, head, stream) : launch_forward_cols_t<2, 2, 2, 1, false, true>(P, head, stream);
+        if (dd3) return half ? launch_layout_t<3, 2, true, true>(P, head, stream) : launch_layout_t<3, 2, false, true>(P, head, stream);
+        return half ? launch_layout_t<2, 1, true, true>(P, head, stream) : launch_layout_t<2, 1, false, true>(P, head, stream);
     }
-    if (dd3) return half ? launch_forward_cols_t<2, 3, 2, 2, true, false>(P, head, stream) : launch_forward_cols_t<2, 3, 2, 2, false, false>(P, head, stream);
-    return half ? launch_forward_cols_t<2, 2, 2, 1, true, false>(P, head, stream) : launch_forward_cols_t<2, 2, 2, 1, false, false>(P, head, stream);
+    if (dd3) return half ? launch_layout_t<3, 2, true, false>(P, head, stream) : launch_layout_t<3, 2, false, false>(P, head, stream);
+    return half ? launch_layout_t<2, 1, true, false>(P, head, stream) : launch_layout_t<2, 1, false, false>(P, head, stream);
 }
 
 }  // namespace fiery
