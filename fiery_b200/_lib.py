@@ -9,8 +9,7 @@ import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
 
-# FIERY_B200_LIB: another build of the same library (experiment builds of tools/gpu_ab.sh); default: the in-tree one
-LIB_PATH = os.environ.get("FIERY_B200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libfiery_b200.so")
+LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libfiery_b200.so")
 ABI_VERSION = 2
 
 DTYPE_F32, DTYPE_F16 = 0, 1

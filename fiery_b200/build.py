@@ -26,11 +26,6 @@ NVCC_FLAGS = [
 ]
 
 
-def _extra_flags():
-    """FIERY_NVCC_EXTRA: extra nvcc flags for experiment builds (e.g. -DFIERY_COLS_AB for tools/gpu_ab.sh); part of the stamp."""
-    return os.environ.get("FIERY_NVCC_EXTRA", "").split()
-
-
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
@@ -46,7 +41,7 @@ def _source_hash() -> str:
         with open(f, "rb") as fh:
             h.update(f.encode())
             h.update(fh.read())
-    h.update(" ".join(NVCC_FLAGS + _extra_flags()).encode())
+    h.update(" ".join(NVCC_FLAGS).encode())
     return h.hexdigest()
 
 
@@ -57,27 +52,16 @@ def is_current() -> bool:
         return fh.read().strip() == _source_hash()
 
 
-def build(force: bool = False, verbose: bool = False, out: str = None, obj_suffix: str = "") -> str:
-    """Compiles every .cu under csrc/ for sm_90a into fiery_b200/libfiery_b200.so; returns its path.
-    ``out`` / ``obj_suffix``: build a second library next to it (experiment builds with FIERY_NVCC_EXTRA) without touching the
-    in-tree one."""
-    if out is not None:
-        return _build_to(out, obj_suffix or ".ab", verbose)
+def build(force: bool = False, verbose: bool = False) -> str:
+    """Compiles every .cu under csrc/ for sm_90a into fiery_b200/libfiery_b200.so; returns its path."""
     if not force and is_current():
         return LIB_PATH
-    _build_to(LIB_PATH, "", verbose)
-    with open(STAMP_PATH, "w") as fh:
-        fh.write(_source_hash())
-    return LIB_PATH
-
-
-def _build_to(lib_path: str, obj_suffix: str, verbose: bool) -> str:
     nvcc = _nvcc()
     objs = []
     procs = []
     for src in SOURCES:
-        obj = os.path.join(CSRC, src.replace(".cu", obj_suffix + ".o"))
-        cmd = [nvcc, *[f for f in NVCC_FLAGS if f != "--use_fast_math=false"], *_extra_flags(), "-c", os.path.join(CSRC, src), "-o", obj]
+        obj = os.path.join(CSRC, src.replace(".cu", ".o"))
+        cmd = [nvcc, *[f for f in NVCC_FLAGS if f != "--use_fast_math=false"], "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
             print(" ".join(cmd), flush=True)
@@ -93,15 +77,16 @@ def _build_to(lib_path: str, obj_suffix: str, verbose: bool) -> str:
             print(f"nvcc failed on {src}", file=sys.stderr)
     if failed:
         raise RuntimeError("nvcc compilation failed")
-    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib_path, *objs, "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH, *objs, "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     subprocess.run(link, check=True)
-    return lib_path
+    with open(STAMP_PATH, "w") as fh:
+        fh.write(_source_hash())
+    return LIB_PATH
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--force", action="store_true")
     ap.add_argument("--verbose", action="store_true")
-    ap.add_argument("--out", default=None, help="write an experiment build here instead of the in-tree library")
     a = ap.parse_args()
-    print(build(force=a.force, verbose=a.verbose, out=a.out))
+    print(build(force=a.force, verbose=a.verbose))

@@ -41,49 +41,7 @@ static encode_tiled_fn get_encode_fn() {
     return fn;
 }
 
-// One 4-D view (column, row, channel-within-image, image) of `channels` channels starting at channel `ch0` of every image.
-static int encode_view(CUtensorMap* map, const void* head, long long n_images, int head_channels, int ch0, int channels,
-                       int hh, int ww) {
-    encode_tiled_fn fn = get_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const size_t es = 4;
-    const char* base = static_cast<const char*>(head) + static_cast<size_t>(ch0) * hh * ww * es;
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "head tensor (or its context slice) is not 16-byte aligned");
-    FIERY_REQUIRE(hh <= 256, "feat_h=%d exceeds the TMA box limit of 256", hh);
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(ww), static_cast<cuuint64_t>(hh), static_cast<cuuint64_t>(channels),
-                          static_cast<cuuint64_t>(n_images)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(ww) * es, static_cast<cuuint64_t>(ww) * hh * es,
-                             static_cast<cuuint64_t>(ww) * hh * head_channels * es};
-    cuuint32_t box[4] = {WT, static_cast<cuuint32_t>(hh), CH_BOX, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<char*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-    return FIERY_OK;
-}
-
-int encode_head_maps(HeadMaps* maps, const void* head, int dtype, const LiftParams& P) {
-    FIERY_REQUIRE(dtype == FIERY_DTYPE_F32, "TMA map: only fp32 head tensors are supported");
-    const long long n_images = static_cast<long long>(P.frame0 + P.n_frames) * P.n_cameras;
-    int rc = FIERY_OK;
-    if (P.use_depth) {
-        rc = encode_view(&maps->depth, head, n_images, P.head_channels, 0, P.D, P.hh, P.ww);
-        if (rc != FIERY_OK) return rc;
-    } else {
-        memset(&maps->depth, 0, sizeof(CUtensorMap));
-    }
-    return encode_view(&maps->ctx, head, n_images, P.head_channels, P.use_depth ? P.D : 0, P.C, P.hh, P.ww);
-}
-
-// Tensor maps of the column-packed forward kernel (lift_fwd_cols.cu): the tile arrives as prob[row][depth][col4] and
-// ctx[row][k][cl][col4] with channel = CPL*cl + k -- the dimension order of the maps is the shared-memory order, the strides do
-// the permutation.
-struct HeadMapsCols {
-    CUtensorMap depth;
-    CUtensorMap ctx;
-};
-
+// Tensor maps of the lift's tile kernels (lift_tile.cuh: HeadMapsCols)
 int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane) {
     encode_tiled_fn fn = get_encode_fn();
     if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");

@@ -71,13 +71,8 @@ __device__ __forceinline__ uint32_t dl_feat_offset(int ch, int px) {
 template <int ES, bool BF16>
 __global__ void __launch_bounds__(DL_THREADS, 1)
 depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __restrict__ bias, float* __restrict__ head, int n_out,
-                   int pixels, int tiles_per_image, int n_tiles, int skip_arg) {
+                   int pixels, int tiles_per_image, int n_tiles) {
     using S = DlShape<ES>;
-#ifdef FIERY_COLS_AB
-    const int skip = skip_arg;                         // experiment builds: leave out stores (1) / MMAs (2) / feature loads (4)
-#else
-    constexpr int skip = 0;
-#endif
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     unsigned char* s_w = smem;
@@ -111,7 +106,6 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
                 if (use > 0) mbar_wait(b_empty + st, (use - 1) & 1);
                 const int img = t / tiles_per_image, p0 = (t % tiles_per_image) * DL_N;
                 unsigned char* dst = s_b + st * S::B_BYTES;
-                if (skip & 4) { mbar_arrive(b_full + st); continue; }
                 mbar_arrive_expect_tx(b_full + st, S::B_BYTES);
 #pragma unroll
                 for (int b = 0; b < S::NBLK; ++b) tma_load_3d(dst + b * S::B_BLK, &maps.feat, b_full + st, p0 + b * S::EPR, 0, img);   // pixels past the image: zeros
@@ -139,7 +133,7 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
             wgmma_fence();
             const uint32_t b_addr = smem_addr(tile);
 #pragma unroll
-            for (int k = 0; k < ((skip & 2) ? 0 : DL_K / S::MMA_K); ++k) {
+            for (int k = 0; k < DL_K / S::MMA_K; ++k) {
                 const int k0 = k * S::MMA_K;
                 // A: atom k0 / EPR, rows 64g.., 32 bytes per K step inside the atom.  B: k0 rows of 128 bytes down the block (8-row
                 // groups 1024 B apart), blocks of 64 pixels B_BLK apart.
@@ -161,7 +155,7 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
             }
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < ((skip & 2) ? 0 : DL_K / 8); ++k) {
+            for (int k = 0; k < DL_K / 8; ++k) {
                 const int k0 = 8 * k;
                 wgmma_m64n128k8_tf32_rs(acc, a[k], gmma_desc_sw128(w_addr + (k0 / 32) * S::W_ATOM + (k0 % 32) * 4, 16, 1024));
             }
@@ -171,7 +165,6 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
         wgmma_fence_operands(acc);
         __syncwarp();
         if (lane == 0) mbar_arrive(b_empty + st);      // this warp's part of the tile has been read
-        if (skip & 1) continue;
         if constexpr (ES == 2) {                       // rows = output channels r0, r0 + 8; columns = pixels
             float* out = head + (static_cast<size_t>(img) * n_out + r0) * pixels + p0;
             const float b0 = (bias && r0 < n_out) ? __ldg(bias + r0) : 0.f;
@@ -274,16 +267,12 @@ int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, in
     const int sms = n_sm[dev & 63];
     const int waves = (n_tiles + sms - 1) / sms;                       // one persistent CTA per SM, the tiles spread evenly over them
     const unsigned grid = static_cast<unsigned>((n_tiles + waves - 1) / waves);
-    int skip = 0;
-#ifdef FIERY_COLS_AB
-    if (const char* e = getenv("FIERY_DL_SKIP")) skip = atoi(e);      // experiment builds only: 1 no stores, 2 no MMAs, 4 no feature loads
-#endif
     if (dtype == 0)
-        depth_layer_kernel<4, false><<<grid, DL_THREADS, DlShape<4>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
+        depth_layer_kernel<4, false><<<grid, DL_THREADS, DlShape<4>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles);
     else if (dtype == 1)
-        depth_layer_kernel<2, false><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
+        depth_layer_kernel<2, false><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles);
     else
-        depth_layer_kernel<2, true><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles, skip);
+        depth_layer_kernel<2, true><<<grid, DL_THREADS, DlShape<2>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

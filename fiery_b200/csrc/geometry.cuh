@@ -1,4 +1,4 @@
-// Frustum -> ego -> voxel arithmetic shared by every kernel (lift fwd/bwd, index dump).
+// Frustum -> ego -> voxel arithmetic shared by every kernel (geometry plan, forward tile kernel, index dump).
 //
 // The reference computes, per frustum point (u, v, d) of camera i (fiery/models/fiery.py:199-205, 236-247):
 //     q   = (u*d, v*d, d)
@@ -187,5 +187,28 @@ __device__ __forceinline__ int select_pillar(float sx, float sy, float az, float
         : "f"(sx), "f"(sy), "f"(az), "f"(Xf), "f"(Yf), "f"(z_lo), "f"(z_hi), "r"(rank));
     return r;
 }
+
+// Point -> pillar evaluation of the plan and the forward tile kernel: pillar_of after ego_point, with the grid constants hoisted
+// out of the point loop into plain floats.  POW2: both horizontal resolutions are powers of two, so the scale is an exact multiply.
+template <bool POW2>
+struct PillarMap {
+    float offx, offy, offz, kx, ky, Xf, Yf, z_lo, z_hi;
+    int Y;
+
+    __device__ __forceinline__ explicit PillarMap(const GridParams& g)
+        : offx(g.off[0]), offy(g.off[1]), offz(g.off[2]), kx(POW2 ? g.inv_res[0] : g.res[0]), ky(POW2 ? g.inv_res[1] : g.res[1]),
+          Xf(static_cast<float>(g.X)), Yf(static_cast<float>(g.Y)), z_lo(g.z_lo), z_hi(g.z_hi), Y(g.Y) {}
+
+    // pillar (rank) of the point at frustum row coordinate v and depth d of the column `ct`, or -1 if it is masked out
+    __device__ __forceinline__ int operator()(const CameraTransform& T, const ColumnTerms& ct, float v, float d) const {
+        float p[3];
+        ego_point(T, ct, v, d, p);                                        // fiery.py:199-205
+        const float ax = __fsub_rn(p[0], offx), ay = __fsub_rn(p[1], offy), az = __fsub_rn(p[2], offz);
+        const float sx = POW2 ? __fmul_rn(ax, kx) : __fdiv_rn(ax, kx);    // fiery.py:236 (the scale is exact when res is 2^k)
+        const float sy = POW2 ? __fmul_rn(ay, ky) : __fdiv_rn(ay, ky);
+        const int rank = static_cast<int>(sx) * Y + static_cast<int>(sy); // truncation, fiery.py:237,252-256
+        return select_pillar(sx, sy, az, Xf, Yf, z_lo, z_hi, rank);       // mask, fiery.py:240-247
+    }
+};
 
 }  // namespace fiery

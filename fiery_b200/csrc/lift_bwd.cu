@@ -20,25 +20,15 @@
 //     channel lanes with a transposing shuffle butterfly (4 SHFL per row and depth group);
 //   * G gathers are software-pipelined two runs deep: registers hold the current run's gradient row, the next run's row
 //     (already in flight) and the pillar of the run after that, so neither the pillar lookup nor the 256-byte gather is waited for.
-#include <atomic>
-#include <mutex>
-
 #include "lift_plan.cuh"
 
 namespace fiery {
 
-constexpr int BW_DPAD = 48;                  // depth slots (D <= 48)
 constexpr int BW_CH = 8;                     // channels per lane: 8 lanes cover C = 64
 constexpr int BW_ND = PLAN_ND;               // depths per depth group
-constexpr int BW_NG = BW_DPAD / BW_ND;       // depth groups
+constexpr int BW_NG = DPAD / BW_ND;          // depth groups
 constexpr int BW_NT = 32 * PLAN_RG;          // threads: one warp per row group
 constexpr int BW_MAXR = PLAN_MAX_ROWS / PLAN_RG;   // rows per thread
-
-struct HeadMapsCols {
-    CUtensorMap depth;    // 4-D (w, d, h, image), box (4, 48, h, 1)
-    CUtensorMap ctx;      // 5-D (w, cl, k, h, image), box (4, 8, 8, h, 1): channel = 8*cl + k
-};
-int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane);
 
 struct BwdLayout {
     int hh;
@@ -49,26 +39,14 @@ struct BwdLayout {
         off_mask = o;   o += PLAN_PAIRS * 4;
         off_soff = o;   o += PLAN_STREAMS * 2;
         o = (o + 127) & ~127;
-        off_prob = o;   o += hh * BW_DPAD * WT * 4;     // prob[row][depth][col4]
+        off_prob = o;   o += hh * DPAD * WT * 4;        // prob[row][depth][col4]
         o = (o + 127) & ~127;
-        off_gprob = o;  o += hh * BW_DPAD * WT * 4;     // g_prob, then g_logit, same layout
+        off_gprob = o;  o += hh * DPAD * WT * 4;        // g_prob, then g_logit, same layout
         o = (o + 127) & ~127;
         off_ctx = o;    o += hh * 64 * WT * 4;          // ctx[row][k][cl][col4], overwritten by g_ctx at the end
         total = o;
     }
 };
-
-__device__ __forceinline__ void tma_load_5d_b(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3, int c4) {
-    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-                 : "memory");
-}
 
 // helpers on pairs of fp32 values held in one 64-bit register pair (two FFMA / FMUL each)
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
@@ -78,12 +56,6 @@ __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
 }
 __device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ void fma2_acc(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
-        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %0;\n\t"
-        "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
-        "mov.b64 %0, {c0, c1};\n\t}" : "+l"(acc) : "l"(a), "l"(b));
 }
 __device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
     unsigned long long r;
@@ -120,46 +92,8 @@ __device__ __forceinline__ void advance_slot(unsigned long long (&G)[4], unsigne
         : "memory");
 }
 
-// softmax over depth (encoder.py:99) in place on prob[row][d][col]; lane = (d mod 8, col): conflict free, reductions by shuffle
-__device__ __forceinline__ void softmax_rows(const LiftParams& P, float* s_prob, int hh) {
-    constexpr float L2E = 1.4426950408889634f;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int c8 = lane >> 2, col = lane & 3;
-    for (int row = warp; row < hh; row += BW_NT / 32) {
-        float* base = s_prob + (row * BW_DPAD + c8) * WT + col;
-        float x[BW_DPAD / 8];
-        if (P.use_depth) {
-            float m = -INFINITY;
-#pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) {
-                x[k] = (c8 + 8 * k < P.D) ? base[k * 8 * WT] : -INFINITY;
-                m = fmaxf(m, x[k]);
-            }
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-            const float m2 = m * L2E;
-            float sum = 0.f;
-#pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) {
-                x[k] = exp2f(fmaf(x[k], L2E, -m2));         // exp(x - max); padding (-inf) gives 0
-                sum += x[k];
-            }
-            sum += __shfl_xor_sync(0xffffffffu, sum, 4);
-            sum += __shfl_xor_sync(0xffffffffu, sum, 8);
-            sum += __shfl_xor_sync(0xffffffffu, sum, 16);
-            const float inv = __fdiv_rn(1.0f, sum);
-#pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) base[k * 8 * WT] = x[k] * inv;
-        } else {
-#pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) base[k * 8 * WT] = (c8 + 8 * k < P.D) ? 1.0f : 0.f;   // encoder.py:102
-        }
-    }
-}
-
 // MAXR: rows per thread the row loop is unrolled for (ceil(h / 4) <= MAXR); the g_ctx accumulators take 8 registers per row
-template <int MAXR, bool LDS_EARLY>
+template <int MAXR>
 __global__ void __launch_bounds__(BW_NT, 3)
 lift_backward_kernel(const __grid_constant__ HeadMapsCols head_maps, const __grid_constant__ HeadMapsCols grad_maps, const LiftParams P) {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -183,16 +117,16 @@ lift_backward_kernel(const __grid_constant__ HeadMapsCols head_maps, const __gri
         tma_prefetch_desc(&head_maps.ctx);
         mbar_init(bar, 1);
         fence_mbar_init();
-        const uint32_t prob_bytes = P.use_depth ? static_cast<uint32_t>(hh * BW_DPAD * WT * 4) : 0u;
+        const uint32_t prob_bytes = P.use_depth ? static_cast<uint32_t>(hh * DPAD * WT * 4) : 0u;
         mbar_arrive_expect_tx(bar, prob_bytes + static_cast<uint32_t>(hh * 64 * WT * 4));
         if (P.use_depth) tma_load_4d(s_prob, &head_maps.depth, bar, w0, 0, 0, img);
-        tma_load_5d_b(s_ctx, &head_maps.ctx, bar, w0, 0, 0, 0, img);
+        tma_load_5d(s_ctx, &head_maps.ctx, bar, w0, 0, 0, 0, img);
     }
     for (int i = tid; i < PLAN_PAIRS; i += BW_NT) s_mask[i] = __ldg(reinterpret_cast<const unsigned*>(rec + PLAN_OFF_MASK) + i);
     if (tid < PLAN_STREAMS) s_soff[tid] = __ldg(reinterpret_cast<const unsigned short*>(rec + PLAN_OFF_SOFF) + tid);
     __syncthreads();                                   // plan header staged, the mbarrier is set up
     mbar_wait(bar, 0);                                 // head tile has landed
-    softmax_rows(P, s_prob, hh);
+    softmax_depth<BW_NT>(P, s_prob, hh);
     __syncthreads();
 
     // ---- main loop: warp = row group, lane = (column, 8-channel lane) ------------------------------------------------------------
@@ -258,52 +192,43 @@ lift_backward_kernel(const __grid_constant__ HeadMapsCols head_maps, const __gri
             for (int i = 0; i < MAXR; ++i) {
                 if (i < R) {
                     const int h = r_lo + i;
-                    // operands of this row first: the shared loads are in flight while the run changes are handled
-                    const float* pr = s_prob + (h * BW_DPAD + g * BW_ND) * WT + col;
+                    const float* pr = s_prob + (h * DPAD + g * BW_ND) * WT + col;
                     const float* cx = s_ctx + h * 64 * WT + cl * WT + col;
-                    // LDS_EARLY: operands of the row are requested before the run changes are handled (more registers live)
-                    float pv[BW_ND];
-                    unsigned long long cp[4];
-                    if (LDS_EARLY) {
-#pragma unroll
-                        for (int j = 0; j < BW_ND; ++j) pv[j] = pr[j * WT];
-#pragma unroll
-                        for (int m = 0; m < 4; ++m) cp[m] = pack2(cx[(2 * m) * 8 * WT], cx[(2 * m + 1) * 8 * WT]);
-                    }
                     if (i > 0 && ((anyrow >> h) & 1u)) {            // warp-uniform: some slot of some column changes pillar here
 #pragma unroll
                         for (int j = 0; j < BW_ND; ++j)
                             if ((anyj[j] >> h) & 1u) advance_slot(G[j], Gn[j], pnn[j], sp[j], gbev, streams, (cm[j] >> h) & 1u);
                     }
-                    if (!LDS_EARLY) {
+                    // the operands of the row after the run changes (loading them before keeps more registers live)
+                    float pv[BW_ND];
+                    unsigned long long cp[4];
 #pragma unroll
-                        for (int j = 0; j < BW_ND; ++j) pv[j] = pr[j * WT];
+                    for (int j = 0; j < BW_ND; ++j) pv[j] = pr[j * WT];
 #pragma unroll
-                        for (int m = 0; m < 4; ++m) cp[m] = pack2(cx[(2 * m) * 8 * WT], cx[(2 * m + 1) * 8 * WT]);
-                    }
+                    for (int m = 0; m < 4; ++m) cp[m] = pack2(cx[(2 * m) * 8 * WT], cx[(2 * m + 1) * 8 * WT]);
                     float sj[BW_ND];
 #pragma unroll
                     for (int j = 0; j < BW_ND; ++j) {
                         const unsigned long long pp = pack2(pv[j], pv[j]);
 #pragma unroll
-                        for (int m = 0; m < 4; ++m) fma2_acc(gc[i][m], pp, G[j][m]);          // g_ctx += prob * G
+                        for (int m = 0; m < 4; ++m) ffma2(gc[i][m], pp, G[j][m]);          // g_ctx += prob * G
                         unsigned long long t = mul2(cp[0], G[j][0]);                          // ctx . G over my 8 channels
-                        fma2_acc(t, cp[1], G[j][1]);
-                        fma2_acc(t, cp[2], G[j][2]);
-                        fma2_acc(t, cp[3], G[j][3]);
+                        ffma2(t, cp[1], G[j][1]);
+                        ffma2(t, cp[2], G[j][2]);
+                        ffma2(t, cp[3], G[j][3]);
                         float lo, hi;
                         unpack2(t, lo, hi);
                         sj[j] = lo + hi;
                     }
                     if (P.use_depth) {
-                        if (i > 0) reduce_and_store(ps, ((h - 1) * BW_DPAD + g * BW_ND) * WT + col);   // the previous row's g_prob
+                        if (i > 0) reduce_and_store(ps, ((h - 1) * DPAD + g * BW_ND) * WT + col);   // the previous row's g_prob
 #pragma unroll
                         for (int j = 0; j < BW_ND; ++j) ps[j] = sj[j];
                     }
                 }
             }
             // the last row of the group: its shuffles overlap with the set-up of the next depth group
-            if (P.use_depth) reduce_and_store(ps, ((r_lo + R - 1) * BW_DPAD + g * BW_ND) * WT + col);
+            if (P.use_depth) reduce_and_store(ps, ((r_lo + R - 1) * DPAD + g * BW_ND) * WT + col);
         }
     }
     // ---- g_ctx registers -> the ctx region, same layout (every thread overwrites exactly the entries only it read) -------------------
@@ -326,11 +251,11 @@ lift_backward_kernel(const __grid_constant__ HeadMapsCols head_maps, const __gri
     if (P.use_depth) {
         const int c8 = lane >> 2, scol = lane & 3;
         for (int row = warp; row < hh; row += BW_NT / 32) {
-            const int o = (row * BW_DPAD + c8) * WT + scol;
-            float pv[BW_DPAD / 8], gv[BW_DPAD / 8];
+            const int o = (row * DPAD + c8) * WT + scol;
+            float pv[DPAD / 8], gv[DPAD / 8];
             float dot = 0.f;
 #pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) {
+            for (int k = 0; k < DPAD / 8; ++k) {
                 pv[k] = s_prob[o + k * 8 * WT];
                 gv[k] = s_gprob[o + k * 8 * WT];
                 dot = fmaf(pv[k], gv[k], dot);
@@ -339,7 +264,7 @@ lift_backward_kernel(const __grid_constant__ HeadMapsCols head_maps, const __gri
             dot += __shfl_xor_sync(0xffffffffu, dot, 8);
             dot += __shfl_xor_sync(0xffffffffu, dot, 16);
 #pragma unroll
-            for (int k = 0; k < BW_DPAD / 8; ++k) s_gprob[o + k * 8 * WT] = pv[k] * (gv[k] - dot);
+            for (int k = 0; k < DPAD / 8; ++k) s_gprob[o + k * 8 * WT] = pv[k] * (gv[k] - dot);
         }
     }
     fence_proxy_async();       // generic-proxy writes -> visible to the TMA (async proxy)
@@ -392,7 +317,7 @@ size_t lift_backward_relayout_bytes(const LiftParams& P) {
 int launch_lift_backward(const LiftParams& P, const void* head, int head_dtype, float* workspace, const void* plan, cudaStream_t stream) {
     FIERY_REQUIRE(head_dtype == FIERY_DTYPE_F32, "head dtype %d not supported by this build (fp32 only)", head_dtype);
     FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
-    FIERY_REQUIRE(P.D >= 1 && P.D <= BW_DPAD, "depth_bins=%d not supported by this build (1..48)", P.D);
+    FIERY_REQUIRE(P.D >= 1 && P.D <= DPAD, "depth_bins=%d not supported by this build (1..48)", P.D);
     FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
     FIERY_REQUIRE(P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
     HeadMapsCols hm, gm;
@@ -420,33 +345,20 @@ int launch_lift_backward(const LiftParams& P, const void* head, int head_dtype, 
     }
     const BwdLayout L(P.hh);
     FIERY_REQUIRE(L.total <= 227 * 1024, "tile needs %d bytes of shared memory", L.total);
-    const bool small = (P.hh + PLAN_RG - 1) / PLAN_RG <= 7;     // the reference's h = 28: 7 rows per thread
-    bool early = false;
-#ifdef FIERY_COLS_AB
-    if (const char* e = getenv("FIERY_BWD_EARLY")) early = atoi(e) != 0;      // A/B builds only
-#endif
     typedef void (*kernel_t)(const HeadMapsCols, const HeadMapsCols, const LiftParams);
-    const kernel_t variants[4] = {lift_backward_kernel<7, false>, lift_backward_kernel<7, true>,
-                                  lift_backward_kernel<BW_MAXR, false>, lift_backward_kernel<BW_MAXR, true>};
-    {
-        static std::mutex mu;
-        static std::atomic<int> configured_on[64];    // function attributes are per device; zero-initialised
-        int dev_id = 0;
-        FIERY_CUDA_CHECK(cudaGetDevice(&dev_id));
-        std::atomic<int>& configured = configured_on[dev_id & 63];
-        if (!configured.load(std::memory_order_acquire)) {
-            std::lock_guard<std::mutex> lock(mu);
-            if (!configured.load(std::memory_order_relaxed)) {
-                for (kernel_t k : variants) {
-                    FIERY_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-                    FIERY_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-                }
-                configured.store(1, std::memory_order_release);
-            }
+    static const kernel_t kernels[2] = {lift_backward_kernel<7>, lift_backward_kernel<BW_MAXR>};
+    static OncePerDevice once;
+    rc = once.run([]() -> int {
+        for (kernel_t k : kernels) {
+            FIERY_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            FIERY_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         }
-    }
+        return FIERY_OK;
+    });
+    if (rc != FIERY_OK) return rc;
+    const bool small = (P.hh + PLAN_RG - 1) / PLAN_RG <= 7;     // the reference's h = 28: 7 rows per thread
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
-    variants[(small ? 0 : 2) + (early ? 1 : 0)]<<<static_cast<unsigned>(n_tiles), BW_NT, L.total, stream>>>(hm, gm, Q);
+    kernels[small ? 0 : 1]<<<static_cast<unsigned>(n_tiles), BW_NT, L.total, stream>>>(hm, gm, Q);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

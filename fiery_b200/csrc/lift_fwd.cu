@@ -347,18 +347,12 @@ static int chain_resources(ChainResources** out) {
 // exposed.  A group whose tile kernel cannot fill the GPU once loses more than the overlap gains, so a group keeps at least one
 // tile per SM of an H100 SXM (132).  The count is host logic (fiery_lift_forward_launches answers without a device), hence a
 // constant rather than the device's SM count.
-#ifdef FIERY_COLS_AB
-static int g_max_chains = MAX_CHAINS;      // FIERY_CHAINS (A/B builds)
-static int g_chain_min_tiles = 132;        // FIERY_CHAIN_MIN_TILES (A/B builds)
-#else
-constexpr int g_max_chains = MAX_CHAINS;
-constexpr int g_chain_min_tiles = 132;
-#endif
+constexpr int CHAIN_MIN_TILES = 132;
 int lift_forward_groups(const LiftParams& P, int frames_in_chunk) {
     if (P.bev_layout == FIERY_BEV_NHWC) return 1;          // no layout pass to hide
-    int groups = frames_in_chunk < g_max_chains ? frames_in_chunk : g_max_chains;
+    int groups = frames_in_chunk < MAX_CHAINS ? frames_in_chunk : MAX_CHAINS;
     const long long tiles_per_frame = static_cast<long long>(P.n_cameras) * P.n_wtiles;
-    while (groups > 1 && (frames_in_chunk / groups) * tiles_per_frame < g_chain_min_tiles) --groups;
+    while (groups > 1 && (frames_in_chunk / groups) * tiles_per_frame < CHAIN_MIN_TILES) --groups;
     return groups < 1 ? 1 : groups;
 }
 
@@ -451,10 +445,6 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
     int rc = FIERY_OK;
     LiftParams Q = P;
     Q.head_f16 = head_dtype == FIERY_DTYPE_F16 ? head : nullptr;
-#ifdef FIERY_COLS_AB
-    if (const char* e = getenv("FIERY_CHAINS")) g_max_chains = atoi(e) < MAX_CHAINS ? atoi(e) : MAX_CHAINS;
-    if (const char* e = getenv("FIERY_CHAIN_MIN_TILES")) g_chain_min_tiles = atoi(e);
-#endif
     // lift into a channel-last accumulator (NHWC: the caller's zero-filled output itself), then the layout pass for NCHW; several
     // passes only to bound the scratch footprint
     const int chunk = lift_chunk_frames(P);

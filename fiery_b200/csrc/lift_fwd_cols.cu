@@ -18,30 +18,26 @@
 //   * the two TMA loads deliver the tile as  prob[row][depth][col4]  and  ctx[row][k][cl][col4]  (channel CPL*cl + k; the
 //     channel split is a 5-D tensor map, so the permutation is done by the copy engine).  One 16-byte shared load is then
 //     "4 adjacent columns of one (row, depth)" or "... of one (row, channel)";
-//   * a thread owns 2 depths x 4 columns x CPL channels, held as packed pairs of ADJACENT COLUMNS, so the outer product is
-//     8*CPL FFMA per row whose operands are exactly the register pairs the loads return;
+//   * a thread owns DD depths x 4 columns x 2 channels, held as packed pairs of ADJACENT COLUMNS, so the outer product is
+//     8*DD FFMA per row whose operands are exactly the register pairs the loads return;
 //   * the tile's pillar runs are read from the plan and expanded into run-end events while the TMA is in flight;
 //   * the softmax runs in place on prob (lane = (depth mod 8, column): conflict free, reductions by shuffle);
-//   * run ends are detected warp-uniformly (one 32-bit load + one warp reduction per row, fetched a row ahead).
+//   * run ends are detected warp-uniformly (one 32-bit load per row, fetched a row ahead).
 #include <string.h>
 
 #include "lift_plan.cuh"
 
 namespace fiery {
 
-constexpr int COLS_DPAD = 48;                 // depth slots (D <= 48)
-constexpr int COLS_NPAIR = COLS_DPAD * WT;    // (depth, column) pairs of a tile: each is one image column of points
+constexpr int COLS_NPAIR = DPAD * WT;         // (depth, column) pairs of a tile: each is one image column of points
 constexpr int COLS_EVS = 33;                  // event words per unit: rows 0..31 + one that stays 0
 constexpr int COLS_PLAN_STAGE = 4096;         // bytes of the tile's plan record staged in shared memory by one bulk copy ...
 constexpr int COLS_RUNS_STAGED = (COLS_PLAN_STAGE - PLAN_OFF_RUNS) / 4;   // ... = header + this many runs; later runs are read from global
-// A "unit" is DD adjacent depths x the 4 columns of the tile (4*DD pairs = "slots"); the 64 / CPL lanes of a unit own CPL
-// channels each.  DD trades shared-memory traffic for registers: per image row a unit reads the whole 1 KB context row of the
-// tile, so the tile's context traffic is (48 / DD) KB per row.
-
-struct HeadMapsCols {
-    CUtensorMap depth;    // 4-D (w, d, h, image), box (4, 48, h, 1)
-    CUtensorMap ctx;      // 5-D (w, cl, k, h, image), box (4, 64/CPL, CPL, h, 1): channel = CPL*cl + k
-};
+// A "unit" is DD adjacent depths x the 4 columns of the tile (4*DD pairs = "slots"); the 32 lanes of a unit, one warp, own
+// CPL = 2 channels each.  DD trades shared-memory traffic for registers: per image row a unit reads the whole 1 KB context row of
+// the tile, so the tile's context traffic is (48 / DD) KB per row.
+constexpr int CPL = 2;                        // channels per lane
+constexpr int LPU = 64 / CPL;                 // lanes per unit
 
 struct ColsLayout {
     int hh, C;
@@ -52,7 +48,7 @@ struct ColsLayout {
         off_plan = o;   o += COLS_PLAN_STAGE;           // head of the tile's plan record: masks, offsets, the first runs
         off_ev = o;     o += n_units * COLS_EVS * 4;   // run-end events: [unit][row], see expand_plan
         o = (o + 127) & ~127;
-        off_prob = o;   o += hh * COLS_DPAD * WT * 4;
+        off_prob = o;   o += hh * DPAD * WT * 4;
         o = (o + 127) & ~127;
         off_ctx = o;    o += hh * C * WT * 4;
         o = (o + 127) & ~127;
@@ -61,33 +57,10 @@ struct ColsLayout {
     }
 };
 
-__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4,
-                                            uint64_t policy) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;"
-        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4),
-          "l"(policy)
-        : "memory");
-}
-
 // 8-byte asynchronous copy global -> shared (SASS LDGSTS.64): one (channel, row) piece = 4 half-precision columns
 // (no L2 policy here: ptxas 12.9 gives the .L2::cache_hint form of this instruction a descriptor operand it never writes)
 __device__ __forceinline__ void cp_async_8(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_addr(dst)), "l"(src) : "memory");
-}
-
-// FMA on a pair of adjacent columns held in one 64-bit register pair: acc.lo += a.lo * b.lo, acc.hi += a.hi * b.hi (two FFMA)
-__device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
-        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %0;\n\t"
-        "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
-        "mov.b64 %0, {c0, c1};\n\t}" : "+l"(acc) : "l"(a), "l"(b));
 }
 
 template <int HALF>
@@ -142,7 +115,8 @@ constexpr int GEO_OFF_CAM = 0, GEO_OFF_U = 48, GEO_OFF_V = 64, GEO_OFF_D = 192;
 
 // Calls WITHOUT a plan (a forward-only call whose calibration is new: nothing to share the geometry with): the geometry of the tile
 // is evaluated here, while the head tile is in flight -- the tile kernel waits for the copy engine at that point anyway, so this
-// costs little, whereas a separate plan kernel in front of every frame group adds a launch and a dependency to every chain.  Same device functions as the plan kernel (geometry.cuh), same result:
+// costs little, whereas a separate plan kernel in front of every frame group adds a launch and a dependency to every chain.  Same
+// evaluator as the plan kernel (geometry.cuh: PillarMap), same result:
 // the pillar (rank, fiery.py:236-256; -1 = masked) of every point, evaluated with the reference arithmetic, reduced on the fly to
 // what the pooling loop consumes:
 //   ev[unit][row]      bit j (slot j = dd*4 + col: depth DD*unit + dd, column col) set <=> pair j changes pillar between
@@ -167,11 +141,7 @@ __device__ __forceinline__ void stage_geometry_cols(const LiftParams& P, const C
     for (int i = 0; i < 9; ++i) T.m[i] = s_cam[i];
 #pragma unroll
     for (int i = 0; i < 3; ++i) T.t[i] = s_cam[9 + i];
-    const float offx = P.grid.off[0], offy = P.grid.off[1], offz = P.grid.off[2];
-    const float kx = POW2 ? P.grid.inv_res[0] : P.grid.res[0], ky = POW2 ? P.grid.inv_res[1] : P.grid.res[1];
-    const float Xf = static_cast<float>(P.grid.X), Yf = static_cast<float>(P.grid.Y);
-    const float z_lo = P.grid.z_lo, z_hi = P.grid.z_hi;
-    const int Y = P.grid.Y;
+    const PillarMap<POW2> pillar(P.grid);
     const int hh = L.hh;
     const int pair = threadIdx.x / NRS, rs = threadIdx.x % NRS;
     const bool idle = pair >= COLS_NPAIR;                    // NT is not always a multiple of the pair count
@@ -197,13 +167,7 @@ __device__ __forceinline__ void stage_geometry_cols(const LiftParams& P, const C
         int h = h_lo;
 #pragma unroll 2
         for (; h < h_hi; ++h) {
-            float p[3];
-            ego_point(T, ct, s_v[h], depth, p);                               // fiery.py:199-205
-            const float ax = __fsub_rn(p[0], offx), ay = __fsub_rn(p[1], offy), az = __fsub_rn(p[2], offz);
-            const float sx = POW2 ? __fmul_rn(ax, kx) : __fdiv_rn(ax, kx);    // fiery.py:236 (x scale exact when res is 2^k)
-            const float sy = POW2 ? __fmul_rn(ay, ky) : __fdiv_rn(ay, ky);
-            const int rank = static_cast<int>(sx) * Y + static_cast<int>(sy); // truncation, fiery.py:237,252-256
-            const int cur = select_pillar(sx, sy, az, Xf, Yf, z_lo, z_hi, rank);   // mask, fiery.py:240-247
+            const int cur = pillar(T, ct, s_v[h], depth);
             if (h == h_lo) first = cur;
             else if (cur != prev) run_ends(h, prev, cur);
             prev = cur;
@@ -228,13 +192,12 @@ __device__ __forceinline__ void stage_geometry_cols(const LiftParams& P, const C
 // piece order.  After the geometry phase the pieces are widened in place: every thread reads its pieces, one barrier, every
 // thread writes them as fp32 (exact: fp16 -> fp32 conversion, then the same fp32 arithmetic as for an fp32 head, which is what
 // autocast does to the reference's softmax and outer product, encoder.py:99-100).
-template <int CPL, int NT>
+template <int NT>
 __device__ __forceinline__ void issue_half_tile(const LiftParams& P, const ColsLayout& L, unsigned char* smem, int img, int w0) {
-    constexpr int LPU = 64 / CPL;
     const int hh = L.hh;
-    const int n_pp = P.use_depth ? hh * COLS_DPAD : 0;
+    const int n_pp = P.use_depth ? hh * DPAD : 0;
     const int n_cp = hh * 64;
-    unsigned char* prob_stage = smem + L.off_prob + hh * COLS_DPAD * WT * 2;     // upper half of prob[row][depth][col4]
+    unsigned char* prob_stage = smem + L.off_prob + hh * DPAD * WT * 2;     // upper half of prob[row][depth][col4]
     unsigned char* ctx_stage = smem + L.off_ctx + hh * 64 * WT * 2;              // upper half of ctx[row][k][cl][col4]
     const __half* head = static_cast<const __half*>(P.head_f16);
     const size_t plane = static_cast<size_t>(hh) * P.ww;
@@ -242,7 +205,7 @@ __device__ __forceinline__ void issue_half_tile(const LiftParams& P, const ColsL
     const int ctx_ch0 = P.use_depth ? P.D : 0;
     for (int p = threadIdx.x; p < n_pp + n_cp; p += NT) {
         if (p < n_pp) {
-            const int row = p / COLS_DPAD, d = p - row * COLS_DPAD;
+            const int row = p / DPAD, d = p - row * DPAD;
             if (d < P.D) cp_async_8(prob_stage + p * 8, img_base + d * plane + static_cast<size_t>(row) * P.ww);
         } else {
             const int q = p - n_pp;
@@ -256,13 +219,13 @@ __device__ __forceinline__ void issue_half_tile(const LiftParams& P, const ColsL
 
 template <int NT>
 __device__ __forceinline__ void widen_half_tile(const LiftParams& P, const ColsLayout& L, unsigned char* smem) {
-    constexpr int MAXP = (32 * (COLS_DPAD + 64) + NT - 1) / NT;                  // pieces per thread at h = 32
+    constexpr int MAXP = (32 * (DPAD + 64) + NT - 1) / NT;                  // pieces per thread at h = 32
     const int hh = L.hh;
-    const int n_pp = P.use_depth ? hh * COLS_DPAD : 0;
+    const int n_pp = P.use_depth ? hh * DPAD : 0;
     const int total = n_pp + hh * 64;
     unsigned char* prob_base = smem + L.off_prob;
     unsigned char* ctx_base = smem + L.off_ctx;
-    const int prob_half = hh * COLS_DPAD * WT * 2, ctx_half = hh * 64 * WT * 2;
+    const int prob_half = hh * DPAD * WT * 2, ctx_half = hh * 64 * WT * 2;
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncthreads();                                  // every thread's pieces have landed
     uint2 v[MAXP];
@@ -271,7 +234,7 @@ __device__ __forceinline__ void widen_half_tile(const LiftParams& P, const ColsL
         const int p = threadIdx.x + i * NT;
         v[i] = make_uint2(0u, 0u);                     // depth slots >= D stay zero (the tensor maps zero-fill them too)
         if (p < n_pp) {
-            if (p % COLS_DPAD < P.D) v[i] = *reinterpret_cast<const uint2*>(prob_base + prob_half + p * 8);
+            if (p % DPAD < P.D) v[i] = *reinterpret_cast<const uint2*>(prob_base + prob_half + p * 8);
         } else if (p < total) {
             v[i] = *reinterpret_cast<const uint2*>(ctx_base + ctx_half + (p - n_pp) * 8);
         }
@@ -290,58 +253,12 @@ __device__ __forceinline__ void widen_half_tile(const LiftParams& P, const ColsL
     __syncthreads();                                  // the fp32 tile is complete
 }
 
-// softmax over depth (encoder.py:99) in place on prob[row][d][col]; lane = (d mod 8, col)
-template <int NT>
-__device__ __forceinline__ void softmax_cols(const LiftParams& P, const ColsLayout& L, unsigned char* smem) {
-    constexpr float L2E = 1.4426950408889634f;
-    float* s_prob = reinterpret_cast<float*>(smem + L.off_prob);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int c8 = lane >> 2, col = lane & 3;
-    for (int row = warp; row < L.hh; row += NT / 32) {
-        float* base = s_prob + (row * COLS_DPAD + c8) * WT + col;
-        float x[COLS_DPAD / 8];
-        if (P.use_depth) {
-            float m = -INFINITY;
-#pragma unroll
-            for (int k = 0; k < COLS_DPAD / 8; ++k) {
-                x[k] = (c8 + 8 * k < P.D) ? base[k * 8 * WT] : -INFINITY;
-                m = fmaxf(m, x[k]);
-            }
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-            const float m2 = m * L2E;
-            float sum = 0.f;
-#pragma unroll
-            for (int k = 0; k < COLS_DPAD / 8; ++k) {
-                x[k] = exp2f(fmaf(x[k], L2E, -m2));         // exp(x - max); padding (-inf) gives 0
-                sum += x[k];
-            }
-            sum += __shfl_xor_sync(0xffffffffu, sum, 4);
-            sum += __shfl_xor_sync(0xffffffffu, sum, 8);
-            sum += __shfl_xor_sync(0xffffffffu, sum, 16);
-            const float inv = __fdiv_rn(1.0f, sum);
-#pragma unroll
-            for (int k = 0; k < COLS_DPAD / 8; ++k) base[k * 8 * WT] = x[k] * inv;
-        } else {
-#pragma unroll
-            for (int k = 0; k < COLS_DPAD / 8; ++k) base[k * 8 * WT] = (c8 + 8 * k < P.D) ? 1.0f : 0.f;   // encoder.py:102
-        }
-    }
-}
-
 // predicated vector reduction of CPL adjacent channels; HINT: with an L2 `policy` (the scratch accumulator stays in L2 for the layout pass)
-template <int CPL, bool HINT>
+template <bool HINT>
 __device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL], unsigned bit, uint64_t policy) {
-    if (!HINT && CPL == 4)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %5, 0;\n\t@p red.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n\t}"
-                     :: "l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[CPL > 2 ? 2 : 0]), "f"(v[CPL > 3 ? 3 : 0]), "r"(bit) : "memory");
-    else if (!HINT)
+    if (!HINT)
         asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\t@p red.global.add.v2.f32 [%0], {%1, %2};\n\t}"
                      :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit) : "memory");
-    else if (CPL == 4)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %5, 0;\n\t@p red.global.add.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %6;\n\t}"
-                     :: "l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[CPL > 2 ? 2 : 0]), "f"(v[CPL > 3 ? 3 : 0]), "r"(bit), "l"(policy) : "memory");
     else
         asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\t@p red.global.add.L2::cache_hint.v2.f32 [%0], {%1, %2}, %4;\n\t}"
                      :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit), "l"(policy) : "memory");
@@ -351,7 +268,7 @@ __device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL]
 // the ending run reduce their channels into the accumulator and restart.  The "+ 0.0f" copies are real instructions on
 // purpose: they gather the values into the consecutive registers the vector reduction needs HERE, instead of letting the
 // register allocator keep the accumulators in that order and un-shuffle them around every FMA pair.
-template <int CPL, int DD, int SD, int COL, bool HINT>
+template <int DD, int SD, int COL, bool HINT>
 __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
                                            const int* plp, char* out, uint64_t policy) {
     constexpr int j = SD * 4 + COL;
@@ -360,34 +277,34 @@ __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2]
         float v[CPL];
 #pragma unroll
         for (int k = 0; k < CPL; ++k) v[k] = __fadd_rn(half_of<COL & 1>(acc[k][SD][COL >> 1]), 0.0f);
-        red_channels_if<CPL, HINT>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j), policy);
+        red_channels_if<HINT>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j), policy);
         const unsigned keep = ((own >> j) & 1u) - 1u;          // 0 where my run ends, ~0 otherwise
 #pragma unroll
         for (int k = 0; k < CPL; ++k) clear_half<COL & 1>(acc[k][SD][COL >> 1], keep);
     }
 }
 
-template <int CPL, int DD, int SD, bool HINT>
+template <int DD, int SD, bool HINT>
 __device__ __forceinline__ void flush_depth(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
                                             const int* plp, char* out, uint64_t policy) {
     if (mw & (0xfu << (4 * SD))) {
-        flush_slot<CPL, DD, SD, 0, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<CPL, DD, SD, 1, HINT>(acc, mw, own, flush, plp, out, policy);
-        flush_slot<CPL, DD, SD, 2, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<CPL, DD, SD, 3, HINT>(acc, mw, own, flush, plp, out, policy);
+        flush_slot<DD, SD, 0, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 1, HINT>(acc, mw, own, flush, plp, out, policy);
+        flush_slot<DD, SD, 2, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 3, HINT>(acc, mw, own, flush, plp, out, policy);
     }
-    if constexpr (SD + 1 < DD) flush_depth<CPL, DD, SD + 1, HINT>(acc, mw, own, flush, plp, out, policy);
+    if constexpr (SD + 1 < DD) flush_depth<DD, SD + 1, HINT>(acc, mw, own, flush, plp, out, policy);
 }
 
-// CPL channels per lane, DD depths per unit: a unit is 64 / CPL lanes, a tile 48 / DD units.
-//   CPL 2, DD 2: 768 threads (a unit is a warp)      CPL 2, DD 4: 384 threads      CPL 4, DD 4: 192 threads (a unit is a half-warp)
+// DD depths per unit, a tile is 48 / DD units of one warp: DD 2 is 768 threads, DD 3 512.  The row loop is unrolled twice for DD 3
+// and not at all for DD 2.  Two tiles per SM.
 // HINTS: NCHW output, L2 policies on the head loads and the reductions into the scratch (lift_fwd.cu: lanes)
-template <int CPL, int DD, int MINB, int UNR = 2, bool HALF = false, bool PLANNED = false, bool HINTS = false>
-__global__ void __launch_bounds__((COLS_DPAD / DD) * (64 / CPL), MINB)
+template <int DD, bool HALF, bool PLANNED, bool HINTS>
+__global__ void __launch_bounds__((DPAD / DD) * LPU, 2)
 lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const LiftParams P) {
-    constexpr int LPU = 64 / CPL;                     // lanes per unit
-    constexpr int NU = COLS_DPAD / DD;                // units per tile
+    constexpr int NU = DPAD / DD;                     // units per tile
     constexpr int NT = NU * LPU;
     constexpr int SLOTS = 4 * DD;
-    static_assert(COLS_DPAD % DD == 0 && SLOTS <= 16 && (LPU == 16 || LPU == 32), "unsupported unit shape");
+    constexpr int UNR = DD == 3 ? 2 : 1;              // row-loop unroll
+    static_assert(DPAD % DD == 0 && SLOTS <= 16, "unsupported unit shape");
     extern __shared__ __align__(128) unsigned char smem[];
     const ColsLayout L(P.hh, P.C, NU);
     const int wtile = blockIdx.x % P.n_wtiles;
@@ -411,11 +328,11 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
         }
     }
     if (HALF) {
-        issue_half_tile<CPL, NT>(P, L, smem, img, w0);
+        issue_half_tile<NT>(P, L, smem, img, w0);
     } else if (tid == 0) {
         tma_prefetch_desc(&head_maps.depth);
         tma_prefetch_desc(&head_maps.ctx);
-        const uint32_t prob_bytes = P.use_depth ? static_cast<uint32_t>(hh * COLS_DPAD * WT * 4) : 0u;
+        const uint32_t prob_bytes = P.use_depth ? static_cast<uint32_t>(hh * DPAD * WT * 4) : 0u;
         mbar_arrive_expect_tx(bar, prob_bytes + static_cast<uint32_t>(hh * L.C * WT * 4));
         if (HINTS) {
             const uint64_t once = l2_evict_first();                                  // the head is read once
@@ -436,7 +353,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
         float* s_d = reinterpret_cast<float*>(smem + L.off_plan + GEO_OFF_D);
         if (tid < WT) s_u[tid] = (w0 + tid < P.ww) ? P.fu[w0 + tid] : 0.f;
         if (tid >= 32 && tid < 64) s_v[tid - 32] = P.fv[min(tid - 32, hh - 1)];
-        if (tid >= 64 && tid < 64 + COLS_DPAD) s_d[tid - 64] = (tid - 64 < P.D) ? P.fd[tid - 64] : 0.f;
+        if (tid >= 64 && tid < 64 + DPAD) s_d[tid - 64] = (tid - 64 < P.D) ? P.fd[tid - 64] : 0.f;
         if (tid == NT - 1) {
             CameraTransform T;
             load_camera(P.calib_mode, P.calib_a, P.calib_b, img, T);
@@ -459,7 +376,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
     }
     if (HALF) widen_half_tile<NT>(P, L, smem);         // fp16 pieces -> the fp32 tile, in place
     else mbar_wait(bar, 0);                           // head tile has landed
-    softmax_cols<NT>(P, L, smem);
+    softmax_depth<NT>(P, reinterpret_cast<float*>(smem + L.off_prob), hh);
     __syncthreads();
 
     // ---- pooling: thread = (unit of DD depths, 4 columns, channels CPL*cl .. CPL*cl + CPL-1) ---------------------------
@@ -479,14 +396,13 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
         for (int dd = 0; dd < DD; ++dd) acc[k][dd][0] = acc[k][dd][1] = 0ull;
 
     // own: my slots whose run ends at this row, flush: ... and must be flushed.  mw: slots that end a run anywhere in the
-    // warp -- a warp reduction when two units share a warp, so every run-end branch is warp-uniform (half-warps that own
-    // different depths would otherwise diverge on every event).  All are fetched one row ahead: the chain load -> reduce ->
-    // branch is long.
+    // warp; a unit is one warp, so that is `own` and every run-end branch is warp-uniform.  Both are fetched one row ahead: the
+    // chain load -> branch is long.
     unsigned own = 0, flush = 0, mw = 0;              // row 0 starts every run
 #pragma unroll UNR
-    for (int h = 0; h < hh; ++h, pp += COLS_DPAD * WT, cp += 64 * WT, plp += COLS_NPAIR, ++evp) {
+    for (int h = 0; h < hh; ++h, pp += DPAD * WT, cp += 64 * WT, plp += COLS_NPAIR, ++evp) {
         const unsigned ev_next = *evp;                                // the word after the last row stays 0
-        if (mw) flush_depth<CPL, DD, 0, HINTS>(acc, mw, own, flush, plp, out, keep);
+        if (mw) flush_depth<DD, 0, HINTS>(acc, mw, own, flush, plp, out, keep);
         ulonglong2 dv[DD];
 #pragma unroll
         for (int dd = 0; dd < DD; ++dd) dv[dd] = *reinterpret_cast<const ulonglong2*>(pp + dd * WT);   // columns (0,1) (2,3)
@@ -502,7 +418,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
         }
         own = ev_next & ((1u << SLOTS) - 1u);
         flush = ev_next >> SLOTS;
-        mw = LPU == 32 ? own : __reduce_or_sync(0xffffffffu, own);
+        mw = own;
     }
     // the runs that reach the last row (plp now points at it)
 #pragma unroll
@@ -514,21 +430,19 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
             const unsigned long long a = acc[k][j >> 2][(j & 3) >> 1];
             v[k] = (j & 1) ? half_of<1>(a) : half_of<0>(a);
         }
-        red_channels_if<CPL, HINTS>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u, keep);
+        red_channels_if<HINTS>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u, keep);
     }
 }
 
-int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane);
-
-template <int CPL, int DD, int MINB, int UNR, bool HALF, bool PLANNED, bool HINTS>
+template <int DD, bool HALF, bool PLANNED, bool HINTS>
 static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStream_t stream) {
-    constexpr int NU = COLS_DPAD / DD, NT = NU * (64 / CPL);
+    constexpr int NU = DPAD / DD, NT = NU * LPU;
     const ColsLayout L(P.hh, P.C, NU);
     static OncePerDevice once;                        // zero-initialised (static storage)
     int rc = once.run([]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         // ask for the full shared-memory carve-out (two or three tiles of ~75 KB per SM for the reference shape)
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                               cudaSharedmemCarveoutMaxShared));
         return FIERY_OK;
     });
@@ -544,45 +458,39 @@ static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStre
         if (rc != FIERY_OK) return rc;
     }
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
-    lift_forward_cols_kernel<CPL, DD, MINB, UNR, HALF, PLANNED, HINTS><<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
+    lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS><<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
 
 // L2 hints for NCHW output only: with channel-last output the tile kernel reduces into the caller's output, and hinted there it
 // measured slower on an H100 than with the plain instructions
-template <int DD, int UNR, bool HALF, bool PLANNED>
+template <int DD, bool HALF, bool PLANNED>
 static int launch_layout_t(const LiftParams& P, const void* head, cudaStream_t stream) {
-    return P.bev_layout == FIERY_BEV_NCHW ? launch_forward_cols_t<2, DD, 2, UNR, HALF, PLANNED, true>(P, head, stream)
-                                          : launch_forward_cols_t<2, DD, 2, UNR, HALF, PLANNED, false>(P, head, stream);
+    return P.bev_layout == FIERY_BEV_NCHW ? launch_forward_cols_t<DD, HALF, PLANNED, true>(P, head, stream)
+                                          : launch_forward_cols_t<DD, HALF, PLANNED, false>(P, head, stream);
 }
 
-// Unit shape (CPL channels per lane, DD depths per unit).  The pooling loop is bound by shared-memory wavefronts (a broadcast LDS.128
-// costs 2, a 512-byte one 4) and by the run-end control flow, so the shape trades context re-reads (48 / DD per row), registers
-// (4 * CPL * DD accumulators) and resident warps; CPL 4 and DD 4 shapes lose.
+// Unit shape (DD depths per unit of one warp, 2 channels per lane).  The pooling loop is bound by shared-memory wavefronts (a
+// broadcast LDS.128 costs 2, a 512-byte one 4) and by the run-end control flow, so the shape trades context re-reads (48 / DD per
+// row), registers (8 * DD accumulators) and resident warps:
 //   * geometry in the tile (no plan): DD = 3 (512 threads) when the grid fills whole waves of 2 tiles per SM; DD = 2 (768 threads, row
 //     loop not unrolled) while tiles run alone on an SM, i.e. when the last wave is at most half full;
 //   * geometry from a plan: DD = 3 always.
 int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream) {
     FIERY_REQUIRE(P.hh <= 32, "feat_h=%d not supported by this build (<= 32)", P.hh);
-    FIERY_REQUIRE(P.C == 64 && P.D <= COLS_DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);
-    const bool planned = P.plan_tiles != nullptr;
+    FIERY_REQUIRE(P.C == 64 && P.D <= DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);
+    const bool half = P.head_f16 != nullptr;
+    if (P.plan_tiles != nullptr)
+        return half ? launch_layout_t<3, true, true>(P, head, stream) : launch_layout_t<3, false, true>(P, head, stream);
     int n_sm = 0, dev = 0;
     FIERY_CUDA_CHECK(cudaGetDevice(&dev));
     FIERY_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
     const long long rem = n_tiles % (2ll * n_sm);
-    bool dd3 = planned || !(rem > 0 && rem <= n_sm);
-#ifdef FIERY_COLS_AB
-    if (const char* e = getenv("FIERY_COLS_VARIANT")) dd3 = atoi(e) < 0 ? dd3 : atoi(e) == 2;      // A/B builds only: 0 = DD 2, 2 = DD 3
-#endif
-    const bool half = P.head_f16 != nullptr;
-    if (planned) {
-        if (dd3) return half ? launch_layout_t<3, 2, true, true>(P, head, stream) : launch_layout_t<3, 2, false, true>(P, head, stream);
-        return half ? launch_layout_t<2, 1, true, true>(P, head, stream) : launch_layout_t<2, 1, false, true>(P, head, stream);
-    }
-    if (dd3) return half ? launch_layout_t<3, 2, true, false>(P, head, stream) : launch_layout_t<3, 2, false, false>(P, head, stream);
-    return half ? launch_layout_t<2, 1, true, false>(P, head, stream) : launch_layout_t<2, 1, false, false>(P, head, stream);
+    if (!(rem > 0 && rem <= n_sm))
+        return half ? launch_layout_t<3, true, false>(P, head, stream) : launch_layout_t<3, false, false>(P, head, stream);
+    return half ? launch_layout_t<2, true, false>(P, head, stream) : launch_layout_t<2, false, false>(P, head, stream);
 }
 
 }  // namespace fiery

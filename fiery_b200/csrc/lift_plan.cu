@@ -13,7 +13,7 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
     __shared__ float s_cam[12];
     __shared__ float s_u[WT];
     __shared__ float s_v[PLAN_MAX_ROWS];
-    __shared__ float s_d[48];
+    __shared__ float s_d[DPAD];
     __shared__ unsigned s_mask[PLAN_PAIRS];
     __shared__ int s_warp_sum[PLAN_PAIRS / 32];
     __shared__ unsigned short s_seg[PLAN_RG * PLAN_PAIRS];   // segment lengths, then offsets, in (rg, col, j, g) order
@@ -30,7 +30,7 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
 
     if (tid < WT) s_u[tid] = (w0 + tid < P.ww) ? P.fu[w0 + tid] : 0.f;
     if (tid >= 32 && tid < 64) s_v[tid - 32] = P.fv[min(tid - 32, hh - 1)];
-    if (tid >= 64 && tid < 64 + 48) s_d[tid - 64] = (tid - 64 < P.D) ? P.fd[tid - 64] : 0.f;
+    if (tid >= 64 && tid < 64 + DPAD) s_d[tid - 64] = (tid - 64 < P.D) ? P.fd[tid - 64] : 0.f;
     if (tid == PLAN_PAIRS - 1) {                        // one lane composes R @ K^-1 (fiery.py:203)
         CameraTransform T;
         load_camera(P.calib_mode, P.calib_a, P.calib_b, img, T);
@@ -54,11 +54,7 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
         for (int i = 0; i < 9; ++i) T.m[i] = s_cam[i];
 #pragma unroll
         for (int i = 0; i < 3; ++i) T.t[i] = s_cam[9 + i];
-        const float offx = P.grid.off[0], offy = P.grid.off[1], offz = P.grid.off[2];
-        const float kx = POW2 ? P.grid.inv_res[0] : P.grid.res[0], ky = POW2 ? P.grid.inv_res[1] : P.grid.res[1];
-        const float Xf = static_cast<float>(P.grid.X), Yf = static_cast<float>(P.grid.Y);
-        const float z_lo = P.grid.z_lo, z_hi = P.grid.z_hi;
-        const int Y = P.grid.Y;
+        const PillarMap<POW2> pillar(P.grid);
         unsigned char* tmap = touched ? touched + static_cast<size_t>(frame) * P.pillars : nullptr;
         const float depth = s_d[d];
         const ColumnTerms ct = column_terms(T, s_u[col], depth);
@@ -66,13 +62,7 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
         n = 0;
 #pragma unroll 4
         for (int h = 0; h < hh; ++h) {
-            float p[3];
-            ego_point(T, ct, s_v[h], depth, p);                               // fiery.py:199-205
-            const float ax = __fsub_rn(p[0], offx), ay = __fsub_rn(p[1], offy), az = __fsub_rn(p[2], offz);
-            const float sx = POW2 ? __fmul_rn(ax, kx) : __fdiv_rn(ax, kx);    // fiery.py:236 (the scale is exact when res is 2^k)
-            const float sy = POW2 ? __fmul_rn(ay, ky) : __fdiv_rn(ay, ky);
-            const int rank = static_cast<int>(sx) * Y + static_cast<int>(sy); // truncation, fiery.py:237,252-256
-            const int cur = select_pillar(sx, sy, az, Xf, Yf, z_lo, z_hi, rank);   // mask, fiery.py:240-247
+            const int cur = pillar(T, ct, s_v[h], depth);
             if (h == 0 || cur != prev) {
                 if (h) mask |= 1u << h;
                 s_tmp[n * PLAN_PAIRS + pair] = cur;
@@ -115,7 +105,7 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
     // A segment = the runs of one pair inside one row group: the run that contains the group's first row + the runs that start
     // inside the group.  Stream (rg, col, j) = segments of depth groups g = 0..11 in order + two pad entries; the streams follow each
     // other in streams[].  Offsets: exclusive scan over the 768 segment lengths in (rg, col, j, g) order, + 2 per preceding stream.
-    constexpr int NG = 48 / PLAN_ND;
+    constexpr int NG = DPAD / PLAN_ND;
     const int g_of = d / PLAN_ND, j_of = d % PLAN_ND;
     unsigned in_group[PLAN_RG], upto[PLAN_RG];
 #pragma unroll

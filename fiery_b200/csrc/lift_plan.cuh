@@ -28,7 +28,7 @@
 
 namespace fiery {
 
-constexpr int PLAN_PAIRS = 48 * WT;          // (depth, column) pairs of a tile
+constexpr int PLAN_PAIRS = DPAD * WT;         // (depth, column) pairs of a tile
 constexpr int PLAN_RG = 4;                   // row groups of the backward kernel
 constexpr int PLAN_ND = 4;                   // depths per backward depth group (slots j)
 constexpr int PLAN_STREAMS = PLAN_RG * WT * PLAN_ND;

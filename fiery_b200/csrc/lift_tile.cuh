@@ -1,22 +1,17 @@
-// Tile staging of the backward lift kernel (the forward kernel, lift_fwd_cols.cu, has its own transposition-free layout).
+// What the lift's tile kernels share: the forward (lift_fwd_cols.cu), the backward (lift_bwd.cu) and the geometry plan
+// (lift_plan.cu).
 //
-// Work unit ("tile"): one camera image of one frame, WT = 4 adjacent feature-map columns, all h rows, all D depth
-// bins, all C channels.  A tile is fetched from the NCHW head tensor (fiery/models/encoder.py:96 output) with 3-D TMA
-// boxes of (4 columns, h rows, 8 channels) straight into shared memory, where it lands as raw[ch][row][col].
-// The pooling loops want the transposed layouts
-//     prob[pix][d]   (pix = col*h + row, row stride dpad)            depth distribution, encoder.py:99
-//     ctx [pix][c]   (row stride C)                                 context features,  encoder.py:100
-//     pillar[pix][d] (row stride dpad)                              rank of the point, fiery.py:236-256, -1 = masked
-// so the tile is transposed in place through registers (all reads, one barrier, all writes) with a diagonal
-// lane->element mapping that keeps both sides (almost) bank-conflict free.
+// Work unit ("tile"): one camera image of one frame, WT = 4 adjacent feature-map columns, all h rows, all D depth bins, all C
+// channels.  The forward and the backward fetch the tile from the NCHW head tensor (fiery/models/encoder.py:96 output) with two
+// TMA loads that deliver it as prob[row][depth][col4] and ctx[row][k][cl][col4]: the tensor maps do the permutation, nothing is
+// transposed in shared memory.
 #pragma once
 #include "geometry.cuh"
 
 namespace fiery {
 
 constexpr int WT = 4;        // feature-map columns per tile (16 B: the minimum TMA inner box)
-constexpr int CH_BOX = 8;    // channels per TMA box
-constexpr int CG = 16;       // channel groups of 4 -> C = 64
+constexpr int DPAD = 48;     // depth slots of a tile (D <= 48)
 
 struct LiftParams {
     int n_frames, n_cameras;
@@ -42,270 +37,61 @@ struct LiftParams {
     GridParams grid;
 };
 
-template <int DBLKS>
-struct TileLayout {
-    static constexpr int DPAD = 8 * DBLKS;
-    static constexpr int PS = DPAD;              // prob row stride (floats)
-    static constexpr int NT = 64 * DBLKS;        // threads: WT columns x DBLKS depth blocks x 16 channel groups
-    static constexpr int NWARPS = NT / 32;
-
-    int hh, C, PX;                               // PX = hh * WT pixels per tile
-    // byte offsets into dynamic shared memory
-    int off_bar, off_cam, off_brk, off_u, off_v, off_d, off_red, off_prob, off_ctx, off_pillar, off_chg, total;
-
-    __host__ __device__ TileLayout(int hh_, int C_) : hh(hh_), C(C_), PX(hh_ * WT) {
-        int o = 0;
-        off_bar = o;    o += 16;
-        off_cam = o;    o += 12 * 4;
-        off_brk = o;    o += WT * DBLKS * 4;     // per (column, depth block): bit h set <=> a pillar changes at row h
-        off_u = o;      o += WT * 4;
-        off_d = o;      o += DPAD * 4;
-        off_v = o;      o += ((hh + 3) & ~3) * 4;
-        // softmax partial max / sum per (depth group of 16, pixel); dead after transform_tile, so the change bits, which
-        // are written after the barrier that follows stage_pillars, share the bytes
-        const int red_bytes = 2 * (DPAD / 16) * PX * 4;
-        const int chg_bytes = (PX * DBLKS + 15) & ~15;
-        off_red = o;    off_chg = o;
-        o += (red_bytes > chg_bytes ? red_bytes : chg_bytes);
-        o = (o + 127) & ~127;
-        const int prob_raw = DPAD * PX * 4, prob_t = PX * PS * 4;
-        off_prob = o;   o += (prob_raw > prob_t ? prob_raw : prob_t);
-        o = (o + 127) & ~127;
-        off_ctx = o;    o += C * PX * 4;
-        o = (o + 127) & ~127;
-        off_pillar = o; o += PX * DPAD * 4;
-        total = o;
-    }
-};
-
-// ---- phase 0: constants of the tile -------------------------------------------------------------------------------
-template <int DBLKS>
-__device__ __forceinline__ void stage_constants(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem,
-                                                int cam_flat, int w0) {
-    float* s_u = reinterpret_cast<float*>(smem + L.off_u);
-    float* s_v = reinterpret_cast<float*>(smem + L.off_v);
-    float* s_d = reinterpret_cast<float*>(smem + L.off_d);
-    const int tid = threadIdx.x;
-    if (tid < WT) s_u[tid] = (w0 + tid < P.ww) ? P.fu[w0 + tid] : 0.f;
-    for (int i = tid; i < L.hh; i += blockDim.x) s_v[i] = P.fv[i];
-    for (int i = tid; i < TileLayout<DBLKS>::DPAD; i += blockDim.x) s_d[i] = (i < P.D) ? P.fd[i] : 0.f;
-    unsigned* s_brk = reinterpret_cast<unsigned*>(smem + L.off_brk);
-    if (tid < WT * DBLKS) s_brk[tid] = 0u;
-}
-
-// One lane composes R @ K^-1 (fiery.py:203) while the TMA is in flight and the other warps run the softmax.
-template <int DBLKS>
-__device__ __forceinline__ void stage_camera(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem, int cam_flat) {
-    CameraTransform T;
-    load_camera(P.calib_mode, P.calib_a, P.calib_b, cam_flat, T);
-    float* s_cam = reinterpret_cast<float*>(smem + L.off_cam);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) s_cam[i] = T.m[i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) s_cam[9 + i] = T.t[i];
-}
-
-// ---- pillar (rank, fiery.py:236-256) of every point of the tile: WT x D x h evaluations of the reference arithmetic -------
-template <int DBLKS, bool POW2>
-__device__ __forceinline__ void stage_pillars_impl(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem, int w0) {
-    constexpr int DPAD = TileLayout<DBLKS>::DPAD;
-    constexpr int NHS = 2;                                  // row halves, so that WT*DPAD*NHS == NT work items
-    const float* s_cam = reinterpret_cast<const float*>(smem + L.off_cam);
-    const float* s_u = reinterpret_cast<const float*>(smem + L.off_u);
-    const float* s_v = reinterpret_cast<const float*>(smem + L.off_v);
-    const float* s_d = reinterpret_cast<const float*>(smem + L.off_d);
-    int* s_pillar = reinterpret_cast<int*>(smem + L.off_pillar);
-    CameraTransform T;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) T.m[i] = s_cam[i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) T.t[i] = s_cam[9 + i];
-    // grid constants as plain floats (hoisted out of the point loop)
-    const float offx = P.grid.off[0], offy = P.grid.off[1], offz = P.grid.off[2];
-    const float kx = POW2 ? P.grid.inv_res[0] : P.grid.res[0], ky = POW2 ? P.grid.inv_res[1] : P.grid.res[1];
-    const float Xf = static_cast<float>(P.grid.X), Yf = static_cast<float>(P.grid.Y);
-    const float z_lo = P.grid.z_lo, z_hi = P.grid.z_hi;
-    const int Y = P.grid.Y;
-    for (int item = threadIdx.x; item < WT * DPAD * NHS; item += blockDim.x) {
-        const int d = item % DPAD;
-        const int wt = (item / DPAD) % WT;
-        const int hs = item / (DPAD * WT);
-        const int h_lo = (L.hh * hs) / NHS, h_hi = (L.hh * (hs + 1)) / NHS;
-        int* out = s_pillar + (wt * L.hh + h_lo) * DPAD + d;
-        if (d >= P.D || w0 + wt >= P.ww) {
-            for (int h = h_lo; h < h_hi; ++h, out += DPAD) *out = -1;
-            continue;
-        }
-        const float depth = s_d[d];
-        const ColumnTerms ct = column_terms(T, s_u[wt], depth);
-#pragma unroll 2
-        for (int h = h_lo; h < h_hi; ++h, out += DPAD) {
-            float p[3];
-            ego_point(T, ct, s_v[h], depth, p);                               // fiery.py:199-205
-            const float ax = __fsub_rn(p[0], offx), ay = __fsub_rn(p[1], offy), az = __fsub_rn(p[2], offz);
-            const float sx = POW2 ? __fmul_rn(ax, kx) : __fdiv_rn(ax, kx);    // fiery.py:236 (x scale exact when res is 2^k)
-            const float sy = POW2 ? __fmul_rn(ay, ky) : __fdiv_rn(ay, ky);
-            const int rank = static_cast<int>(sx) * Y + static_cast<int>(sy); // truncation, fiery.py:237,252-256
-            *out = select_pillar(sx, sy, az, Xf, Yf, z_lo, z_hi, rank);       // mask, fiery.py:240-247
-        }
-    }
-}
-
-template <int DBLKS>
-__device__ __forceinline__ void stage_pillars(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem, int w0) {
-    if (P.grid.pow2[0] && P.grid.pow2[1]) stage_pillars_impl<DBLKS, true>(P, L, smem, w0);
-    else stage_pillars_impl<DBLKS, false>(P, L, smem, w0);
-}
-
-// chg[pix][dblk]: bit j set <=> pillar[pix][8*dblk+j] differs from the previous row's (same column).  Row 0 -> 0.
-template <int DBLKS>
-__device__ __forceinline__ void stage_change_bits(const TileLayout<DBLKS>& L, unsigned char* smem) {
-    constexpr int DPAD = TileLayout<DBLKS>::DPAD;
-    const int* s_pillar = reinterpret_cast<const int*>(smem + L.off_pillar);
-    unsigned char* s_chg = smem + L.off_chg;
-    unsigned* s_brk = reinterpret_cast<unsigned*>(smem + L.off_brk);
-    for (int item = threadIdx.x; item < L.PX * DBLKS; item += blockDim.x) {
-        const int dblk = item % DBLKS;
-        const int pix = item / DBLKS;               // col*hh + row
-        const int row = pix % L.hh;
-        unsigned m = 0;
-        if (row > 0) {
-            const int4* cur = reinterpret_cast<const int4*>(s_pillar + pix * DPAD + dblk * 8);
-            const int4* prv = reinterpret_cast<const int4*>(s_pillar + (pix - 1) * DPAD + dblk * 8);
-            const int4 c0 = cur[0], c1 = cur[1], p0 = prv[0], p1 = prv[1];
-            m = (c0.x != p0.x) | ((c0.y != p0.y) << 1) | ((c0.z != p0.z) << 2) | ((c0.w != p0.w) << 3) |
-                ((c1.x != p1.x) << 4) | ((c1.y != p1.y) << 5) | ((c1.z != p1.z) << 6) | ((c1.w != p1.w) << 7);
-        }
-        s_chg[item] = static_cast<unsigned char>(m);
-        if (m) atomicOr(s_brk + (pix / L.hh) * DBLKS + dblk, 1u << row);
-    }
-}
-
-// ---- TMA issue: DBLKS + C/8 boxes of (4 cols, hh rows, 8 channels, 1 image) ------------------------------------------------
-// Two 4-D views of the head tensor: `depth` covers channels [0, D) of every image, `ctx` channels [D, D+C).  Boxes that
-// stick out of a view (D not a multiple of 8, last column tile) are zero-filled on load and clipped on store.
-struct HeadMaps {
+// Tensor maps of a head tensor (or of its gradient) in the tile layouts: depth is 4-D (w, d, h, image) with box (4, 48, h, 1);
+// ctx is 5-D (w, cl, k, h, image) with box (4, C / channels_per_lane, channels_per_lane, h, 1), channel = channels_per_lane*cl + k.
+// The dimension order of the maps is the shared-memory order; the strides do the permutation.  Defined in c_api.cu.
+struct HeadMapsCols {
     CUtensorMap depth;
     CUtensorMap ctx;
 };
+int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane);
 
-template <int DBLKS>
-__device__ __forceinline__ void issue_tile_loads(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem,
-                                                 const HeadMaps* maps, int img, int w0) {
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + L.off_bar);
-    const int box_bytes = CH_BOX * L.PX * 4;
-    const int n_dbox = P.use_depth ? DBLKS : 0;
-    const int n_cbox = L.C / CH_BOX;
-    mbar_arrive_expect_tx(bar, static_cast<uint32_t>((n_dbox + n_cbox) * box_bytes));
-    for (int i = 0; i < n_dbox; ++i)
-        tma_load_4d(smem + L.off_prob + i * box_bytes, &maps->depth, bar, w0, 0, i * CH_BOX, img);
-    for (int i = 0; i < n_cbox; ++i)
-        tma_load_4d(smem + L.off_ctx + i * box_bytes, &maps->ctx, bar, w0, 0, i * CH_BOX, img);
+// FMA on a pair of adjacent values held in one 64-bit register pair: acc.lo += a.lo * b.lo, acc.hi += a.hi * b.hi (two FFMA)
+__device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
+    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %0;\n\t"
+        "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
+        "mov.b64 %0, {c0, c1};\n\t}" : "+l"(acc) : "l"(a), "l"(b));
 }
 
-// ---- phase 2: softmax over depth + in-place transposes ---------------------------------------------------------------
-// Every warp takes one depth unit (16 depths x 32 raw pixels) and one or two context units (16 channels x 32 raw pixels).
-// Lane l owns raw pixel p0+l and walks its 16 values on the diagonal (l+k) mod 16: bank = (16*((l+k)&1) + l + const) mod 32
-// is a bijection in l for the reference pixel pitch (and conflict-free for any pitch that is a multiple of 32), so the raw
-// reads are conflict free; the transposed stores are at worst 2-way conflicted.  The softmax (encoder.py:99) over the
-// DPAD/16 depth units of a pixel is combined through two small shared arrays (max, then sum).  All raw values sit in
-// registers across the first barrier, so both transposes are in place.
-template <int DBLKS>
-__device__ __forceinline__ void transform_tile(const LiftParams& P, const TileLayout<DBLKS>& L, unsigned char* smem) {
-    constexpr int DPAD = TileLayout<DBLKS>::DPAD;
-    constexpr int PS = TileLayout<DBLKS>::PS;
-    constexpr int NWARPS = TileLayout<DBLKS>::NWARPS;
-    constexpr int NG = DPAD / 16;                           // depth units per pixel block
+// softmax over depth (encoder.py:99) in place on prob[row][d][col] of a block of NT threads; lane = (d mod 8, col): conflict free,
+// reductions by shuffle
+template <int NT>
+__device__ __forceinline__ void softmax_depth(const LiftParams& P, float* s_prob, int hh) {
     constexpr float L2E = 1.4426950408889634f;
-    float* s_prob = reinterpret_cast<float*>(smem + L.off_prob);
-    float* s_ctx = reinterpret_cast<float*>(smem + L.off_ctx);
-    float* s_max = reinterpret_cast<float*>(smem + L.off_red);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int PX = L.PX, hh = L.hh;
-    float* s_sum = s_max + NG * PX;
-    const int n_pblk = (PX + 31) >> 5;
-    const int n_punits = n_pblk * NG;
-    const int n_cunits = (L.C >> 4) * n_pblk;
-
-    // ---- read phase ----
-    const bool p_unit = warp < n_punits;
-    const int pg = p_unit ? warp / n_pblk : 0, ppb = p_unit ? warp % n_pblk : 0;
-    const int ppix = ppb * 32 + lane;
-    const bool p_act = p_unit && ppix < PX;
-    float pv[16];
-    float mx = -INFINITY;
-    if (p_act && P.use_depth) {
-        const float* src = s_prob + (pg * 16) * PX + ppix;
-#pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const int dd = (lane + k) & 15;
-            pv[k] = (pg * 16 + dd < P.D) ? src[dd * PX] : -INFINITY;
-            mx = fmaxf(mx, pv[k]);
-        }
-        s_max[pg * PX + ppix] = mx;
-    }
-    float cv[2][16];
-    int cpix[2], cc0[2];
-    bool c_act[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        const int u = warp + r * NWARPS;
-        c_act[r] = u < n_cunits;
-        cc0[r] = c_act[r] ? (u / n_pblk) * 16 : 0;
-        cpix[r] = (c_act[r] ? (u % n_pblk) : 0) * 32 + lane;
-        c_act[r] = c_act[r] && cpix[r] < PX;
-        if (c_act[r]) {
-            const float* src = s_ctx + cc0[r] * PX + cpix[r];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) cv[r][k] = src[((lane + k) & 15) * PX];
-        }
-    }
-    __syncthreads();      // every raw value is in registers; partial maxima published
-
-    // ---- context: transposed stores (overlap with the depth units' second pass) ----
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        if (c_act[r]) {
-            const int pixT = (cpix[r] % WT) * hh + cpix[r] / WT;
-            float* dst = s_ctx + pixT * L.C + cc0[r];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) dst[(lane + k) & 15] = cv[r][k];
-        }
-    }
-    // ---- depth: exp and partial sums ----
-    if (p_act) {
+    const int c8 = lane >> 2, col = lane & 3;
+    for (int row = warp; row < hh; row += NT / 32) {
+        float* base = s_prob + (row * DPAD + c8) * WT + col;
+        float x[DPAD / 8];
         if (P.use_depth) {
-            float m = s_max[ppix];
+            float m = -INFINITY;
 #pragma unroll
-            for (int g = 1; g < NG; ++g) m = fmaxf(m, s_max[g * PX + ppix]);
+            for (int k = 0; k < DPAD / 8; ++k) {
+                x[k] = (c8 + 8 * k < P.D) ? base[k * 8 * WT] : -INFINITY;
+                m = fmaxf(m, x[k]);
+            }
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
             const float m2 = m * L2E;
             float sum = 0.f;
 #pragma unroll
-            for (int k = 0; k < 16; ++k) {
-                pv[k] = exp2f(fmaf(pv[k], L2E, -m2));       // exp(x - max); padding (-inf) gives 0
-                sum += pv[k];
+            for (int k = 0; k < DPAD / 8; ++k) {
+                x[k] = exp2f(fmaf(x[k], L2E, -m2));         // exp(x - max); padding (-inf) gives 0
+                sum += x[k];
             }
-            s_sum[pg * PX + ppix] = sum;
+            sum += __shfl_xor_sync(0xffffffffu, sum, 4);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 8);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 16);
+            const float inv = __fdiv_rn(1.0f, sum);
+#pragma unroll
+            for (int k = 0; k < DPAD / 8; ++k) base[k * 8 * WT] = x[k] * inv;
         } else {
 #pragma unroll
-            for (int k = 0; k < 16; ++k) pv[k] = (pg * 16 + ((lane + k) & 15) < P.D) ? 1.0f : 0.f;   // encoder.py:102
+            for (int k = 0; k < DPAD / 8; ++k) base[k * 8 * WT] = (c8 + 8 * k < P.D) ? 1.0f : 0.f;   // encoder.py:102
         }
     }
-    __syncthreads();      // partial sums published
-    if (p_act) {
-        float inv = 1.0f;
-        if (P.use_depth) {
-            float tot = s_sum[ppix];
-#pragma unroll
-            for (int g = 1; g < NG; ++g) tot += s_sum[g * PX + ppix];
-            inv = __fdiv_rn(1.0f, tot);
-        }
-        const int pixT = (ppix % WT) * hh + ppix / WT;
-        float* dst = s_prob + pixT * PS + pg * 16;
-#pragma unroll
-        for (int k = 0; k < 16; ++k) dst[(lane + k) & 15] = pv[k] * inv;
-    }
-    // no barrier here: the next reader of prob/ctx (the pooling loop) is behind the barriers of the rank staging
 }
 
 }  // namespace fiery
