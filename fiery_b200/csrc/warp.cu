@@ -64,19 +64,21 @@ __global__ void __launch_bounds__(WARP_THREADS, 2)
 warp_backward_gather_kernel(int C, int H, int W, const float* __restrict__ gout, long long gout_stride, const float* __restrict__ theta,
                             const unsigned char* __restrict__ copy_mask, float* __restrict__ gx, long long gx_stride, int nearest) {
     const int plane = PLANE ? PLANE : H * W;
+    // channel stride in 64 bits: 31 * plane passes 2^31 once H * W > 69.3 M, well inside the accepted H * W < 2^27
+    const long long cstride = plane;
     const int pix = blockIdx.x * WARP_THREADS + threadIdx.x;
     if (pix >= plane) return;
     const int map = blockIdx.z, c0 = blockIdx.y * WB_CH;
     const int nc = C - c0;
-    const float* g = gout + map * gout_stride + static_cast<long long>(c0) * plane;
-    float* dst = gx + map * gx_stride + static_cast<long long>(c0) * plane + pix;
+    const float* g = gout + map * gout_stride + c0 * cstride;
+    float* dst = gx + map * gx_stride + c0 * cstride + pix;
     if (copy_mask && copy_mask[map]) {                       // the present frame passed through: so does its gradient
         float v[WB_CH];                                      // all loads first: a store between them would order them
 #pragma unroll
-        for (int c = 0; c < WB_CH; ++c) v[c] = c < nc ? __ldcs(g + c * plane + pix) : 0.f;
+        for (int c = 0; c < WB_CH; ++c) v[c] = c < nc ? __ldcs(g + c * cstride + pix) : 0.f;
 #pragma unroll
         for (int c = 0; c < WB_CH; ++c)
-            if (c < nc) __stcs(dst + c * plane, v[c]);
+            if (c < nc) __stcs(dst + c * cstride, v[c]);
         return;
     }
     const float* th = theta + map * 6;
@@ -94,7 +96,7 @@ warp_backward_gather_kernel(int C, int H, int W, const float* __restrict__ gout,
 #pragma unroll
             for (int c = 0; c < 8; ++c)
 #pragma unroll
-                for (int k = 0; k < WB_M; ++k) v[c][k] = (k < n_match && cb + c < nc) ? __ldg(g + m_off[k] + (cb + c) * plane) : 0.f;
+                for (int k = 0; k < WB_M; ++k) v[c][k] = (k < n_match && cb + c < nc) ? __ldg(g + m_off[k] + (cb + c) * cstride) : 0.f;
 #pragma unroll
             for (int c = 0; c < 8; ++c)
 #pragma unroll
@@ -103,7 +105,7 @@ warp_backward_gather_kernel(int C, int H, int W, const float* __restrict__ gout,
     }
 #pragma unroll
     for (int c = 0; c < WB_CH; ++c)
-        if (c < nc) __stcs(dst + c * plane, acc[c]);
+        if (c < nc) __stcs(dst + c * cstride, acc[c]);
 }
 
 // ---- pose algebra: flow (b, T, 6) -> theta (b*T, 2, 3) -------------------------------------------------------------------

@@ -25,7 +25,7 @@ __device__ __forceinline__ void sample_coords(const float* __restrict__ th, int 
     sample_coords_norm(th, norm_centre(i, W), norm_centre(j, H), W, H, ix, iy);
 }
 
-// The adjoint as a gather (warp_backward_gather_kernel, warp_adjoint_nhwc_kernel): the output pixels that sample a given source
+// The adjoint as a gather (warp_backward_gather_kernel): the output pixels that sample a given source
 // pixel lie in a small window around the inverse image of that pixel.  InverseMap: inverse of the linear part of (i, j) -> (ix, iy)
 // in pixel units, and whether that window is small enough to enumerate -- every map warp_features builds is a rotation
 // (determinant 1); for anything else (strong scaling, singular or non-finite maps) the scan covers the whole image: slow, but any
