@@ -109,11 +109,18 @@ struct GridParams {
     int pow2[2];
     float z_lo, z_hi;   // closed interval of (z - off_z) that maps to 0 <= iz < Z
     int X, Y;
+    float x_lim, y_lim; // smallest float >= X (>= Y): for every float s, trunc(s) < X  <=>  s < x_lim
 };
 
 __host__ inline bool is_pow2_float(float r) {
     int e;
     return r > 0.f && frexpf(r, &e) == 0.5f;
+}
+
+// float(n) rounds to nearest, so above 2^24 it can fall below n (2^24 + 1 -> 2^24), and s < float(n) would drop s = n - 1
+__host__ inline float float_at_or_above(int n) {
+    const float f = static_cast<float>(n);
+    return static_cast<double>(f) < n ? nextafterf(f, INFINITY) : f;
 }
 
 __host__ inline GridParams make_grid_params(const fiery_lift_desc_t& d) {
@@ -122,6 +129,7 @@ __host__ inline GridParams make_grid_params(const fiery_lift_desc_t& d) {
     for (int a = 0; a < 2; ++a) { g.pow2[a] = is_pow2_float(g.res[a]) ? 1 : 0; g.inv_res[a] = 1.0f / g.res[a]; }
     g.z_lo = d.z_valid_lo; g.z_hi = d.z_valid_hi;
     g.X = d.bev_x; g.Y = d.bev_y;
+    g.x_lim = float_at_or_above(d.bev_x); g.y_lim = float_at_or_above(d.bev_y);
     return g;
 }
 
@@ -160,12 +168,12 @@ __device__ __forceinline__ float scaled_xy(const GridParams& g, int axis, float 
 }
 
 // Pillar (= rank, fiery.py:252-256 with Z == 1) of an ego-frame point, or -1 if it is masked out
-// (fiery.py:240-247).  trunc(s) >= 0  <=>  s > -1 ;  trunc(s) < X  <=>  s < X ; NaN fails both.
+// (fiery.py:240-247).  trunc(s) >= 0  <=>  s > -1 ;  trunc(s) < X  <=>  s < x_lim ; NaN fails both.
 __device__ __forceinline__ int pillar_of(const GridParams& g, const float p[3]) {
     const float sx = scaled_xy(g, 0, p[0]);
     const float sy = scaled_xy(g, 1, p[1]);
     const float az = __fsub_rn(p[2], g.off[2]);
-    const bool ok = (sx > -1.0f) && (sx < static_cast<float>(g.X)) && (sy > -1.0f) && (sy < static_cast<float>(g.Y)) &&
+    const bool ok = (sx > -1.0f) && (sx < g.x_lim) && (sy > -1.0f) && (sy < g.y_lim) &&
                     (az >= g.z_lo) && (az <= g.z_hi);
     const int ix = static_cast<int>(sx);   // cvt.rzi: truncation toward zero, like .long()
     const int iy = static_cast<int>(sy);
@@ -197,7 +205,7 @@ struct PillarMap {
 
     __device__ __forceinline__ explicit PillarMap(const GridParams& g)
         : offx(g.off[0]), offy(g.off[1]), offz(g.off[2]), kx(POW2 ? g.inv_res[0] : g.res[0]), ky(POW2 ? g.inv_res[1] : g.res[1]),
-          Xf(static_cast<float>(g.X)), Yf(static_cast<float>(g.Y)), z_lo(g.z_lo), z_hi(g.z_hi), Y(g.Y) {}
+          Xf(g.x_lim), Yf(g.y_lim), z_lo(g.z_lo), z_hi(g.z_hi), Y(g.Y) {}
 
     // pillar (rank) of the point at frustum row coordinate v and depth d of the column `ct`, or -1 if it is masked out
     __device__ __forceinline__ int operator()(const CameraTransform& T, const ColumnTerms& ct, float v, float d) const {

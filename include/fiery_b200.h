@@ -173,6 +173,8 @@ FIERY_API int fiery_lift_backward(const fiery_lift_desc_t* desc, const void* hea
  * (camera, depth, row, column) (fiery.py:233).  idx_out: (B',N,3) int64 = trunc((p - offset)/res) (fiery.py:236-237);
  * valid_out: (B',N) uint8 (fiery.py:240-247); pillar_out: (B',N) int32 = rank (fiery.py:252-256) or -1 -- taken
  * from the same device function the lift kernels use.  Any output pointer may be NULL.
+ * Where a scaled coordinate s = (p - offset)/res is NaN, +-inf or |s| >= 2^63, idx_out of that axis is unspecified (torch's .long()
+ * itself gives different values on CPU and CUDA there); valid_out is 0 and pillar_out is -1 for such a point.
  */
 FIERY_API int fiery_lift_point_indices(const fiery_lift_desc_t* desc, const float* calib_a, const float* calib_b,
                              const float* frustum_u, const float* frustum_v, const float* frustum_d,

@@ -20,7 +20,7 @@ from oracle import lift_oracle as O
 from oracle import warp_oracle as W
 from tests.test_lift_backward_gpu import _oracle_grad
 from tests.test_lift_launch_plan_cpu import forward_groups, group_bounds, passes, scratch_bytes
-from tests.test_plan_gpu import PAIRS, _decode
+from tests._plan_layout import PAIRS, _decode
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
