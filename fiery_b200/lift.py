@@ -9,6 +9,10 @@ Reference call sites replaced (SURVEY.md section 8b):
 
 ``LiftSplat`` carries what ``Fiery.__init__`` builds for this path (fiery.py:18-29): the frustum and the three BEV
 grid tensors, under the same names, so a reference ``state_dict`` loads into it unchanged.
+
+The plain lift (``LiftSplat.forward``) and the lift with the warp in its layout pass (``LiftSplat.forward_warped``) run through one
+dispatcher operator, ``torch.ops.fiery_b200.lift_splat`` (fiery_b200/ops.py: autograd formula, fake implementation, autocast rule,
+and the choice of a geometry plan for the backward).  This module holds the C-ABI launches behind it.
 """
 from __future__ import annotations
 
@@ -24,7 +28,17 @@ from . import _lib
 from .geometry import (_require_cuda, _stream_ptr, bev_offset_fp32, calculate_birds_eye_view_parameters, create_frustum,
                        split_frustum, z_valid_interval)
 
-_PLAN_OFF_COUNTS = 192 * 4 + 192 * 2 + 64 * 2      # mask[192] u32, off[192] u16, soff[64] u16, then (n_runs, n_stream) u32
+# The geometry plan's byte layout (fiery_b200/csrc/lift_plan.cuh): one record per (frame, camera, 4-column tile), then the touched
+# maps (one byte per frame and pillar).  A record holds mask[192] u32, off[192] u16, soff[64] u16, the counts (n_runs, n_stream) u32
+# in 16 bytes, runs[192 * 32] i32 and streams[192 * 32 + 2 * 64] i32, padded to 128 bytes.
+_PLAN_OFF_COUNTS = 192 * 4 + 192 * 2 + 64 * 2
+_PLAN_TILE_BYTES = (_PLAN_OFF_COUNTS + 16 + 192 * 32 * 4 + (192 * 32 + 2 * 64) * 4 + 127) // 128 * 128
+
+
+def _plan_touched_offset(n_frames: int, n_cameras: int, feat_w: int) -> int:
+    """Byte offset of the touched maps in a plan of ``n_frames`` frames: the end of the tile records."""
+    return n_frames * n_cameras * ((feat_w + 3) // 4) * _PLAN_TILE_BYTES
+
 
 _TORCH_TO_DTYPE = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16}
 
@@ -193,17 +207,29 @@ class LiftSplat(nn.Module):
             return _lib.CALIB_COMPOSED, combined.float().contiguous(), translation.float().contiguous()
         return _lib.CALIB_RAW, intrinsics.float().contiguous(), extrinsics.float().contiguous()
 
+    def _abi_args(self, dev: torch.device, intrinsics: torch.Tensor, extrinsics: torch.Tensor, head_dtype: torch.dtype, layout: int):
+        """(descriptor, geometry) of a C-ABI call on these calibrations (B', n, ...) on ``dev``: ``geometry`` is the five tensors
+        behind the calls' geometry pointers (calibration a and b, frustum u, v and d).  Hold it until the call is queued: the
+        calibration pair may be a temporary."""
+        c = self._constants(dev)
+        mode, a, b = self._calibration(intrinsics.to(dev), extrinsics.to(dev))
+        B, n = intrinsics.shape[:2]
+        return self._desc(c, B, n, head_dtype, mode, layout), (a, b, c["u"], c["v"], c["d"])
+
     # -- public entry points --------------------------------------------------------------------------------------
     def forward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
-                plan: Optional[torch.Tensor] = None) -> torch.Tensor:
+                plan: Optional[torch.Tensor] = None, warp: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
         """head (B'*n, D+C, h, w) [= Encoder.depth_layer output, encoder.py:96], intrinsics (B', n, 3, 3),
         extrinsics (B', n, 4, 4) -> BEV features (B', C, X, Y) float32 (fiery.py:225-227 allocates float32).
         ``plan``: the geometry of this calibration from ``self.plan(intrinsics, extrinsics)`` -- pass it while the camera rig
-        is static and the per-call geometry pass disappears; ``None`` computes it inside the call."""
+        is static and the per-call geometry pass disappears; ``None`` computes it inside the call.
+        ``warp``: (theta (B', 2, 3) float32, copy_mask (B',) uint8) samples every frame under its map in the layout pass (see
+        ``forward_warped``); the BEV is then NCHW whatever ``output_layout`` says."""
         from . import ops
         _require_cuda(head, "head")                     # loud and specific: the operators are registered for CUDA only
         make_plan = plan is None and torch.is_grad_enabled() and head.requires_grad      # a training step shares one plan
-        bev, _plan = torch.ops.fiery_b200.lift_splat(head, intrinsics, extrinsics, plan, ops.register_module(self, head.device), make_plan)
+        bev, _plan = torch.ops.fiery_b200.lift_splat(head, intrinsics, extrinsics, plan, ops.register_module(self, head.device), make_plan,
+                                                     *(warp if warp is not None else (None, None)))
         return bev
 
     def forward_warped(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor, flow: torch.Tensor,
@@ -222,11 +248,8 @@ class LiftSplat(nn.Module):
             return self.forward(head, intrinsics, extrinsics, plan).unflatten(0, (b, s)).contiguous()
         if flow.shape[1] < 2:
             raise IndexError("flow needs at least two timesteps")
-        theta, copy_mask = _device_theta(flow.to(head.device), spatial_extent, cumulative=True)
-        if plan is None and torch.is_grad_enabled() and head.requires_grad:
-            plan = self.plan(intrinsics, extrinsics)
-        bev = _LiftWarpedFn.apply(head, intrinsics, extrinsics, plan, theta, copy_mask, self)
-        return bev.unflatten(0, (b, s))
+        warp = _device_theta(flow.to(head.device), spatial_extent, cumulative=True)
+        return self.forward(head, intrinsics, extrinsics, plan, warp).unflatten(0, (b, s))
 
     def plan(self, intrinsics: torch.Tensor, extrinsics: torch.Tensor) -> torch.Tensor:
         """The geometry plan of a batch of calibrations (fiery_lift_plan): where every frustum point lands -- get_geometry
@@ -235,14 +258,10 @@ class LiftSplat(nn.Module):
         _require_cuda(intrinsics, "intrinsics")
         lib = _lib.load()
         dev = intrinsics.device
-        c = self._constants(dev)
-        B, n = intrinsics.shape[:2]
-        mode, a, b = self._calibration(intrinsics, extrinsics.to(dev))
-        desc = self._desc(c, B, n, torch.float32, mode, _lib.BEV_NCHW)
+        desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, _lib.BEV_NCHW)
         buf = torch.empty(max(1, int(lib.fiery_lift_plan_bytes(desc))), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.fiery_lift_plan(desc, a.data_ptr(), b.data_ptr(), c["u"].data_ptr(), c["v"].data_ptr(), c["d"].data_ptr(),
-                                           buf.data_ptr(), _stream_ptr(dev)), "fiery_lift_plan")
+            _lib.check(lib.fiery_lift_plan(desc, *(t.data_ptr() for t in geo), buf.data_ptr(), _stream_ptr(dev)), "fiery_lift_plan")
         return buf
 
     def point_indices(self, intrinsics: torch.Tensor, extrinsics: torch.Tensor):
@@ -251,17 +270,13 @@ class LiftSplat(nn.Module):
         _require_cuda(intrinsics, "intrinsics")
         lib = _lib.load()
         dev = intrinsics.device
-        c = self._constants(dev)
-        B, n = intrinsics.shape[:2]
-        mode, a, b = self._calibration(intrinsics, extrinsics)
-        desc = self._desc(c, B, n, torch.float32, mode, _lib.BEV_NCHW)
-        N = n * c["D"] * c["h"] * c["w"]
+        desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, _lib.BEV_NCHW)
+        B, N = desc.n_frames, desc.n_cameras * desc.depth_bins * desc.feat_h * desc.feat_w
         idx = torch.empty((B, N, 3), dtype=torch.int64, device=dev)
         valid = torch.empty((B, N), dtype=torch.uint8, device=dev)
         pillar = torch.empty((B, N), dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.fiery_lift_point_indices(desc, a.data_ptr(), b.data_ptr(), c["u"].data_ptr(), c["v"].data_ptr(),
-                                                    c["d"].data_ptr(), idx.data_ptr(), valid.data_ptr(),
+            _lib.check(lib.fiery_lift_point_indices(desc, *(t.data_ptr() for t in geo), idx.data_ptr(), valid.data_ptr(),
                                                     pillar.data_ptr(), _stream_ptr(dev)), "fiery_lift_point_indices")
         return idx, valid.bool(), pillar
 
@@ -285,14 +300,13 @@ class LiftSplat(nn.Module):
         """Counts read back from a plan buffer (layout: fiery_b200/csrc/lift_plan.cuh): pillar runs, backward stream entries and
         pillars that receive a point.  Diagnostic (bench.py uses it for the per-kernel algorithmic bytes); synchronises."""
         c = self._constants(plan.device)
-        n_tiles = n_frames * n_cameras * ((c["w"] + 3) // 4)
         X, Y, _ = c["dim"]
-        touched_bytes = (n_frames * X * Y + 127) // 128 * 128
-        tile_bytes = (plan.numel() - touched_bytes) // max(1, n_tiles)
-        counts = plan[:n_tiles * tile_bytes].view(n_tiles, tile_bytes)[:, _PLAN_OFF_COUNTS:_PLAN_OFF_COUNTS + 8].contiguous().view(torch.int32)
-        touched = plan[n_tiles * tile_bytes:n_tiles * tile_bytes + n_frames * X * Y]
+        t0 = _plan_touched_offset(n_frames, n_cameras, c["w"])
+        records = plan[:t0].view(t0 // _PLAN_TILE_BYTES, _PLAN_TILE_BYTES)
+        counts = records[:, _PLAN_OFF_COUNTS:_PLAN_OFF_COUNTS + 8].contiguous().view(torch.int32)
+        touched = plan[t0:t0 + n_frames * X * Y]
         return {"runs": int(counts[:, 0].sum()), "stream_entries": int(counts[:, 1].sum()), "touched_pillars": int(touched.ne(0).sum()),
-                "tile_record_bytes": int(tile_bytes)}
+                "tile_record_bytes": _PLAN_TILE_BYTES}
 
     # -- CUDA graph and host-buffer entry points ------------------------------------------------------------------------
     def capture(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
@@ -366,7 +380,7 @@ class LiftSplat(nn.Module):
             cache[key] = tuple(torch.cuda.Stream(device=dev) for _ in range(3))
         return cache[key]
 
-    # -- raw launches (used by the autograd function and by bench.py) ------------------------------------------------
+    # -- raw launches (used by the operators in ops.py and by bench.py) ----------------------------------------------
     def _launch_forward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
                         scratch: Optional[torch.Tensor] = None, plan: Optional[torch.Tensor] = None,
                         warp: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
@@ -386,36 +400,30 @@ class LiftSplat(nn.Module):
         if head.dtype != torch.float32 and not (head.dtype == torch.float16 and NATIVE_FP16_FORWARD):
             head = head.float()                      # half-precision heads: widen first (see NATIVE_FP16_FORWARD)
         head = head.contiguous()
-        mode, a, b = self._calibration(intrinsics.to(dev), extrinsics.to(dev))
+        nhwc = self.output_layout == "channels_last" and warp is None
+        desc, geo = self._abi_args(dev, intrinsics, extrinsics, head.dtype, _lib.BEV_NHWC if nhwc else _lib.BEV_NCHW)
         X, Y, _ = c["dim"]
         pooled = 0
         with torch.cuda.device(dev):
-            if self.output_layout == "channels_last" and warp is None:
-                desc = self._desc(c, B, n, head.dtype, mode, _lib.BEV_NHWC)
+            if nhwc:
                 store = torch.zeros((B, X, Y, C), dtype=torch.float32, device=dev)
                 out = store.permute(0, 3, 1, 2)
             else:
-                desc = self._desc(c, B, n, head.dtype, mode, _lib.BEV_NCHW)
-                store = torch.empty((B, C, X, Y), dtype=torch.float32, device=dev)
-                out = store
+                store = out = torch.empty((B, C, X, Y), dtype=torch.float32, device=dev)
             if plan is not None and plan.numel() < int(lib.fiery_lift_plan_bytes(desc)):
                 raise ValueError("plan was made for another batch shape: rebuild it with LiftSplat.plan(intrinsics, extrinsics)")
-            if scratch is None and B and (self.output_layout != "channels_last" or warp is not None):
+            if scratch is None and B and not nhwc:
                 pooled = int(lib.fiery_lift_scratch_bytes(desc))
                 scratch = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
-            scratch_ptr = scratch.data_ptr() if (B and scratch is not None) else 0
+            args = (desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(),
+                    scratch.data_ptr() if (B and scratch is not None) else 0, plan.data_ptr() if plan is not None else 0)
             if warp is None:
-                status = lib.fiery_lift_forward(desc, head.data_ptr(), a.data_ptr(), b.data_ptr(), c["u"].data_ptr(),
-                                                c["v"].data_ptr(), c["d"].data_ptr(), store.data_ptr(), scratch_ptr,
-                                                plan.data_ptr() if plan is not None else 0, _stream_ptr(dev))
+                status = lib.fiery_lift_forward(*args, _stream_ptr(dev))
             else:
                 theta, copy_mask = warp
                 if theta.numel() != B * 6 or copy_mask.numel() != B or theta.dtype != torch.float32 or copy_mask.dtype != torch.uint8:
                     raise ValueError("warp must be (theta (B', 2, 3) float32, copy_mask (B',) uint8) for the B' frames of this call")
-                status = lib.fiery_lift_forward_warped(desc, head.data_ptr(), a.data_ptr(), b.data_ptr(), c["u"].data_ptr(),
-                                                       c["v"].data_ptr(), c["d"].data_ptr(), store.data_ptr(), scratch_ptr,
-                                                       plan.data_ptr() if plan is not None else 0, theta.data_ptr(),
-                                                       copy_mask.data_ptr(), _stream_ptr(dev))
+                status = lib.fiery_lift_forward_warped(*args, theta.data_ptr(), copy_mask.data_ptr(), _stream_ptr(dev))
             if status != 0 and pooled:
                 _scratch.discard(dev, pooled)          # a launch sequence that stopped half way may have left it dirty
             _lib.check(status, "fiery_lift_forward_warped" if warp is not None else "fiery_lift_forward")
@@ -423,59 +431,27 @@ class LiftSplat(nn.Module):
 
     def _launch_backward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
                          grad_bev: torch.Tensor, plan: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Gradient of the BEV w.r.t. ``head``, in ``head``'s dtype; the backward kernel reads the head widened to fp32."""
         lib = _lib.load()
         dev = head.device
-        c = self._constants(dev)
-        B, n = intrinsics.shape[:2]
-        head = head.contiguous()
-        mode, a, b = self._calibration(intrinsics.to(dev), extrinsics.to(dev))
+        h32 = head.float().contiguous()
         g = grad_bev.float()
         if g.permute(0, 2, 3, 1).is_contiguous() and not g.is_contiguous():
             layout = _lib.BEV_NHWC
         else:
             layout = _lib.BEV_NCHW
             g = g.contiguous()
-        desc = self._desc(c, B, n, head.dtype, mode, layout)
-        grad_head = torch.empty_like(head)
+        desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, layout)
+        grad_head = torch.empty_like(h32)
         with torch.cuda.device(dev):
             ws = None
             if plan is None or layout == _lib.BEV_NCHW:        # re-layout of an NCHW gradient and/or room for the plan records
                 ws = torch.empty(max(1, int(lib.fiery_lift_workspace_bytes(desc)) // 4), dtype=torch.float32, device=dev)
-            _lib.check(lib.fiery_lift_backward(desc, head.data_ptr(), a.data_ptr(), b.data_ptr(), c["u"].data_ptr(),
-                                               c["v"].data_ptr(), c["d"].data_ptr(), g.data_ptr(), grad_head.data_ptr(),
+            _lib.check(lib.fiery_lift_backward(desc, h32.data_ptr(), *(t.data_ptr() for t in geo), g.data_ptr(), grad_head.data_ptr(),
                                                ws.data_ptr() if ws is not None else 0,
                                                plan.data_ptr() if plan is not None else 0, _stream_ptr(dev)),
                        "fiery_lift_backward")
-        return grad_head
-
-
-class _LiftWarpedFn(torch.autograd.Function):
-    """Fused forward (lift + warp epilogue); backward = the warp's adjoint (gather kernel), then the lift's backward.  Folding the
-    adjoint into the gradient's re-layout pass was built and measured slower, so the two stay separate."""
-
-    @staticmethod
-    def forward(ctx, head, intrinsics, extrinsics, plan, theta, copy_mask, module):
-        ctx.module = module
-        ctx.save_for_backward(head, intrinsics, extrinsics, theta, copy_mask, plan if plan is not None else torch.empty(0, device=head.device))
-        ctx.has_plan = plan is not None
-        return module._launch_forward(head.detach(), intrinsics, extrinsics, plan=plan, warp=(theta, copy_mask))
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        head, intrinsics, extrinsics, theta, copy_mask, plan = ctx.saved_tensors
-        lib = _lib.load()
-        g = grad_out.float().contiguous()
-        n, C, H, W = g.shape
-        g_bev = torch.empty_like(g)                         # overwritten by the gather adjoint
-        with torch.cuda.device(g.device):
-            _lib.check(lib.fiery_warp_features_backward(n, C, H, W, g.data_ptr(), C * H * W, theta.data_ptr(), copy_mask.data_ptr(),
-                                                        g_bev.data_ptr(), C * H * W, 0, _stream_ptr(g.device)),
-                       "fiery_warp_features_backward")
-        h32 = head.detach()
-        if h32.dtype != torch.float32:
-            h32 = h32.float()
-        g_head = ctx.module._launch_backward(h32, intrinsics, extrinsics, g_bev, plan if ctx.has_plan else None)
-        return g_head.to(head.dtype), None, None, None, None, None, None
+        return grad_head.to(head.dtype)
 
 
 class GraphedLift:
@@ -494,11 +470,9 @@ class GraphedLift:
                 module._launch_forward(head, intrinsics, extrinsics, plan=self.plan)
         torch.cuda.current_stream(dev).wait_stream(side)
         # the graph owns its accumulation scratch (zeroed once here; every replay leaves it zeroed again)
-        c = module._constants(dev)
-        B, n = intrinsics.shape[:2]
         self.scratch = None
-        if module.output_layout != "channels_last" and B:
-            desc = module._desc(c, B, n, head.dtype, _lib.CALIB_RAW, _lib.BEV_NCHW)
+        if module.output_layout != "channels_last" and intrinsics.shape[0]:
+            desc, _ = module._abi_args(dev, intrinsics, extrinsics, head.dtype, _lib.BEV_NCHW)
             self.scratch = torch.zeros(int(_lib.load().fiery_lift_scratch_bytes(desc)) // 4, dtype=torch.float32, device=dev)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()

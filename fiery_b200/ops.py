@@ -6,6 +6,10 @@ dispatcher knows: it has a fake (meta) implementation for tracing / ``torch.comp
 the reference's softmax and outer product run in fp32 (fiery/models/encoder.py:99-100 under autocast), so the operator's inputs are
 cast to fp32.
 
+One operator serves both lifts: the plain lift (``LiftSplat.forward``) and, given the warp's ``theta`` and ``copy_mask``, the lift with
+``cumulative_warp_features`` in its layout pass (``LiftSplat.forward_warped``).  The operator also decides whether to make the
+geometry plan that the forward and the backward share.
+
 The operators take plain tensors plus an integer ``handle`` naming the ``LiftSplat`` module that holds the frustum / BEV-grid
 constants (a registry of weak references; the constants are tiny host-derived tensors, not operator inputs).
 """
@@ -15,6 +19,8 @@ import weakref
 from typing import Optional, Tuple
 
 import torch
+
+from .warp import _warp_adjoint
 
 _REGISTRY = {}          # handle -> (weakref to the LiftSplat module, (C, X, Y, channels_last) as python values for the fake impl)
 
@@ -39,57 +45,62 @@ def _module(handle: int):
 
 @torch.library.custom_op("fiery_b200::lift_splat", mutates_args=(), device_types="cuda")
 def lift_splat(head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor, plan: Optional[torch.Tensor], handle: int,
-               make_plan: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+               make_plan: bool, theta: Optional[torch.Tensor] = None,
+               copy_mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """(head (B'n, D+C, h, w), intrinsics (B', n, 3, 3), extrinsics (B', n, 4, 4)) -> (BEV (B', C, X, Y) fp32, plan).
     ``plan``: a geometry plan of this calibration, or None.  ``make_plan``: compute one (returned, for the backward) when none was
-    passed; otherwise the second output is an empty tensor and the tile kernels evaluate the geometry themselves."""
-    from . import lift as L
+    passed; otherwise the second output is an empty tensor and the tile kernels evaluate the geometry themselves.
+    ``theta`` (B', 2, 3) fp32 and ``copy_mask`` (B',) uint8: the warped lift -- every frame is sampled under its map in the layout
+    pass (fiery_lift_forward_warped) and the BEV is NCHW whatever the module's output layout."""
     m = _module(handle)
-    native = head.dtype == torch.float32 or (head.dtype == torch.float16 and L.NATIVE_FP16_FORWARD)
-    head_in = head if native else head.float()
     made = None
     if plan is None and make_plan and intrinsics.shape[0]:
         made = m.plan(intrinsics.to(head.device), extrinsics)
-    out = m._launch_forward(head_in, intrinsics, extrinsics, plan=plan if plan is not None else made)
+    out = m._launch_forward(head, intrinsics, extrinsics, plan=plan if plan is not None else made,
+                            warp=(theta, copy_mask) if theta is not None else None)
     # the second output is the plan MADE here (an operator output may not alias an input: a plan that was passed in is not returned)
     return out, (made if made is not None else torch.empty(0, dtype=torch.uint8, device=head.device))
 
 
 @lift_splat.register_fake
-def _(head, intrinsics, extrinsics, plan, handle, make_plan):
+def _(head, intrinsics, extrinsics, plan, handle, make_plan, theta=None, copy_mask=None):
     C, X, Y, channels_last = _REGISTRY[handle][1]                   # python values only: nothing here touches a real tensor
     B = intrinsics.shape[0]
-    bev = head.new_empty((B, X, Y, C), dtype=torch.float32).permute(0, 3, 1, 2) if channels_last \
+    bev = head.new_empty((B, X, Y, C), dtype=torch.float32).permute(0, 3, 1, 2) if channels_last and theta is None \
         else head.new_empty((B, C, X, Y), dtype=torch.float32)
     return bev, head.new_empty((0,), dtype=torch.uint8)
 
 
 @torch.library.custom_op("fiery_b200::lift_splat_backward", mutates_args=(), device_types="cuda")
 def lift_splat_backward(head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor, grad_bev: torch.Tensor,
-                        plan: Optional[torch.Tensor], handle: int) -> torch.Tensor:
-    """Gradient of the BEV w.r.t. the head tensor (same shape and dtype as ``head``); the calibration gets none (geometry.py:300)."""
-    m = _module(handle)
-    h32 = head if head.dtype == torch.float32 else head.float()          # the backward kernel reads an fp32 head tensor
-    g = m._launch_backward(h32, intrinsics, extrinsics, grad_bev, plan=plan if (plan is not None and plan.numel()) else None)
-    return g if g.dtype == head.dtype else g.to(head.dtype)
+                        plan: Optional[torch.Tensor], handle: int, theta: Optional[torch.Tensor] = None,
+                        copy_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Gradient of the BEV w.r.t. the head tensor (same shape and dtype as ``head``); the calibration gets none (geometry.py:300).
+    With ``theta`` / ``copy_mask`` (the warped lift) ``grad_bev`` first goes through the warp's adjoint.  Both steps run inside this
+    operator, so the backward graph holds dispatcher operators only.  Folding the adjoint into the gradient's re-layout pass was
+    built and measured slower, so the two launches stay separate."""
+    if theta is not None:
+        grad_bev = _warp_adjoint(grad_bev, theta, copy_mask, 0)      # the warped lift samples bilinearly
+    return _module(handle)._launch_backward(head, intrinsics, extrinsics, grad_bev,
+                                            plan=plan if (plan is not None and plan.numel()) else None)
 
 
 @lift_splat_backward.register_fake
-def _(head, intrinsics, extrinsics, grad_bev, plan, handle):
+def _(head, intrinsics, extrinsics, grad_bev, plan, handle, theta=None, copy_mask=None):
     return torch.empty_like(head)
 
 
 def _setup_context(ctx, inputs, output):
-    head, intrinsics, extrinsics, plan, handle, _make_plan = inputs
+    head, intrinsics, extrinsics, plan, handle, _make_plan, theta, copy_mask = inputs
     _bev, plan_out = output
     ctx.handle = handle
-    ctx.save_for_backward(head, intrinsics, extrinsics, plan if plan is not None else plan_out)
+    ctx.save_for_backward(head, intrinsics, extrinsics, plan if plan is not None else plan_out, theta, copy_mask)
 
 
 def _backward(ctx, grad_bev, _grad_plan):
-    head, intrinsics, extrinsics, plan = ctx.saved_tensors
-    grad_head = torch.ops.fiery_b200.lift_splat_backward(head, intrinsics, extrinsics, grad_bev, plan, ctx.handle)
-    return grad_head, None, None, None, None, None
+    head, intrinsics, extrinsics, plan, theta, copy_mask = ctx.saved_tensors
+    grad_head = torch.ops.fiery_b200.lift_splat_backward(head, intrinsics, extrinsics, grad_bev, plan, ctx.handle, theta, copy_mask)
+    return grad_head, None, None, None, None, None, None, None
 
 
 lift_splat.register_autograd(_backward, setup_context=_setup_context)

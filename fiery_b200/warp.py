@@ -50,23 +50,29 @@ class _WarpMaps(torch.autograd.Function):
             _lib.check(lib.fiery_warp_features_forward(n, C, H, W, xs.data_ptr(), xs.stride(0) if n else 0, th.data_ptr(),
                                                        copy_mask.data_ptr() if copy_mask is not None else 0, out.data_ptr(),
                                                        C * H * W, nearest, _stream_ptr(x.device)), "fiery_warp_features_forward")
-        ctx.save_for_backward(th, copy_mask if copy_mask is not None else torch.empty(0, dtype=torch.uint8, device=x.device))
-        ctx.has_mask = copy_mask is not None
-        ctx.nearest, ctx.shape, ctx.dtype = nearest, tuple(x.shape), x.dtype
+        ctx.save_for_backward(th, copy_mask)
+        ctx.nearest, ctx.dtype = nearest, x.dtype
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         th, mask = ctx.saved_tensors
-        lib = _lib.load()
-        n, C, H, W = ctx.shape
-        g = _dense_maps(grad_out)
-        grad_x = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)       # overwritten by the gather adjoint
-        with torch.cuda.device(g.device):
-            _lib.check(lib.fiery_warp_features_backward(n, C, H, W, g.data_ptr(), g.stride(0) if n else 0, th.data_ptr(),
-                                                        mask.data_ptr() if ctx.has_mask else 0, grad_x.data_ptr(), C * H * W,
-                                                        ctx.nearest, _stream_ptr(g.device)), "fiery_warp_features_backward")
-        return grad_x.to(ctx.dtype), None, None, None
+        return _warp_adjoint(grad_out, th, mask, ctx.nearest).to(ctx.dtype), None, None, None
+
+
+def _warp_adjoint(grad_out: torch.Tensor, theta: torch.Tensor, copy_mask, nearest: int) -> torch.Tensor:
+    """Gradient (n, C, H, W) float32 of the maps sampled under theta (n, 2, 3) float32 w.r.t. their sources, for the upstream
+    gradient ``grad_out`` (n, C, H, W); maps flagged in ``copy_mask`` (n,) uint8 or None pass it through (the gather adjoint,
+    fiery_warp_features_backward).  Used by ``_WarpMaps`` and by the warped lift's backward (fiery_b200/ops.py)."""
+    lib = _lib.load()
+    n, C, H, W = grad_out.shape
+    g = _dense_maps(grad_out)
+    grad_x = torch.empty((n, C, H, W), dtype=torch.float32, device=g.device)       # overwritten by the gather adjoint
+    with torch.cuda.device(g.device):
+        _lib.check(lib.fiery_warp_features_backward(n, C, H, W, g.data_ptr(), g.stride(0) if n else 0, theta.data_ptr(),
+                                                    copy_mask.data_ptr() if copy_mask is not None else 0, grad_x.data_ptr(),
+                                                    C * H * W, nearest, _stream_ptr(g.device)), "fiery_warp_features_backward")
+    return grad_x
 
 
 def _device_theta(flow: torch.Tensor, spatial_extent, cumulative: bool):

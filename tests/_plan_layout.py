@@ -1,14 +1,15 @@
-"""Mirror of the geometry plan's buffer layout (fiery_b200/csrc/lift_plan.cuh) and a decoder of plan bytes back to one pillar per
-frustum point, shared by the tests that read plans."""
+"""A decoder of the geometry plan's bytes (layout: fiery_b200/csrc/lift_plan.cuh) back to one pillar per frustum point, shared by
+the tests that read plans.  The record size, the counts offset and the touched maps' offset are the host layer's own
+(fiery_b200/lift.py); decoding plans against the oracle pins them and the field offsets below."""
 import numpy as np
+
+from fiery_b200.lift import _PLAN_OFF_COUNTS as OFF_COUNTS, _PLAN_TILE_BYTES as TILE_BYTES, _plan_touched_offset
 
 PAIRS, RG, ND, STREAMS, MAX_ROWS = 192, 4, 4, 64, 32
 CAP = PAIRS * MAX_ROWS
 OFF_MASK, OFF_OFF, OFF_SOFF = 0, PAIRS * 4, PAIRS * 4 + PAIRS * 2
-OFF_COUNTS = OFF_SOFF + STREAMS * 2
 OFF_RUNS = OFF_COUNTS + 16
 OFF_STREAMS = OFF_RUNS + CAP * 4
-TILE_BYTES = (OFF_STREAMS + (CAP + 2 * STREAMS) * 4 + 127) // 128 * 128
 
 
 def _decode(plan: np.ndarray, cfg):
@@ -45,7 +46,8 @@ def _decode(plan: np.ndarray, cfg):
                     dense[f, cam, d, :, wt * 4 + c] = per_pair[d * 4 + c]
         tiles.append(dict(mask=mask.copy(), off=off.copy(), soff=soff.copy(), n_runs=int(n_runs), n_stream=int(n_stream),
                           runs=runs, streams=streams, per_pair=per_pair))
-    touched = plan[n_tiles * TILE_BYTES:n_tiles * TILE_BYTES + B * X * Y].reshape(B, X * Y)
+    t0 = _plan_touched_offset(B, n, w)
+    touched = plan[t0:t0 + B * X * Y].reshape(B, X * Y)
     return dense, tiles, touched
 
 

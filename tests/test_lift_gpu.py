@@ -413,34 +413,50 @@ def test_all_points_masked_and_degenerate_calibration():
 def test_lift_is_a_dispatcher_operator():
     """torch.ops.fiery_b200.lift_splat (torch.library.custom_op over the C ABI): autograd formula registered on the operator, fake
     implementation for tracing (torch.compile, fullgraph), autocast rule = fp32 like the reference's softmax / outer product under
-    AMP (fiery/models/encoder.py:99-100)."""
+    AMP (fiery/models/encoder.py:99-100).  The same for the warped lift (LiftSplat.forward_warped): the operator with the warp's
+    theta / copy_mask."""
     from fiery_b200 import ops
+    from fiery_b200.synthetic import make_egomotion
+    from fiery_b200.warp import _device_theta
+    from oracle import warp_oracle as W
     cfg = LiftConfig(**{**CONFIGS["cfg1_tiny"].__dict__, "frames": 2})
     dev = _dev()
     K, E = make_calibration(cfg, seed=3)
     Kd, Ed = torch.from_numpy(K).to(dev), torch.from_numpy(E).to(dev)
     head = torch.from_numpy(make_head(cfg, seed=3)).to(dev)
+    flow = torch.from_numpy(make_egomotion(1, 2, seed=3))                # one sequence of the two frames
+    ext = (float(cfg.x_bound[1]), float(cfg.y_bound[1]))
+    warp = _device_theta(flow.to(dev), ext, cumulative=True)
     lift = LiftSplat.from_config(cfg).to(dev)
     handle = ops.register_module(lift, dev)
-    h = head.clone().requires_grad_(True)
-    bev, plan = torch.ops.fiery_b200.lift_splat(h, Kd, Ed, None, handle, True)
-    assert plan.numel() > 0 and bev.grad_fn is not None and not plan.requires_grad
-    bev.sum().backward()
-    h2 = head.clone().requires_grad_(True)
-    lift(h2, Kd, Ed).sum().backward()                               # the module goes through the same operator
-    assert torch.equal(h.grad, h2.grad)
-    exact = O.LiftOracle.from_config(cfg).lift_exact(head.cpu(), torch.from_numpy(K), torch.from_numpy(E))
-    assert O.normwise_error(bev.detach().cpu(), exact) < TOL
-    # autocast: an fp16 head inside an autocast region is lifted in fp32; the gradient comes back in fp16
-    h16 = head.half().requires_grad_(True)
-    with torch.autocast("cuda", dtype=torch.float16):
-        out = lift(h16, Kd, Ed)
-    assert out.dtype == torch.float32
-    out.sum().backward()
-    assert h16.grad.dtype == torch.float16
-    assert O.normwise_error(out.detach().cpu(), O.LiftOracle.from_config(cfg).lift_exact(h16.detach().float().cpu(), torch.from_numpy(K),
-                                                                                         torch.from_numpy(E))) < TOL
-    # traceable: dynamo captures the call as ONE operator node (fake implementation gives shapes / dtypes)
-    fn = torch.compile(lambda x: torch.ops.fiery_b200.lift_splat(x, Kd, Ed, None, handle, False)[0] * 2.0, backend="eager", fullgraph=True)
-    with torch.no_grad():
-        assert O.normwise_error((fn(head) / 2.0).cpu(), bev.detach().cpu()) < 1e-6
+    oracle = O.LiftOracle.from_config(cfg)
+
+    def warped_exact(h):
+        exact = oracle.lift_exact(h, torch.from_numpy(K), torch.from_numpy(E)).float().unflatten(0, (1, 2))
+        return W.cumulative_warp_features(exact.clone(), flow, mode="bilinear", spatial_extent=ext).flatten(0, 1)
+
+    for name, extra, module_call, exact_of in (
+            ("plain", (), lambda x: lift(x, Kd, Ed),
+             lambda h: oracle.lift_exact(h, torch.from_numpy(K), torch.from_numpy(E))),
+            ("warped", warp, lambda x: lift.forward_warped(x, Kd, Ed, flow.to(dev), ext).flatten(0, 1), warped_exact)):
+        h = head.clone().requires_grad_(True)
+        bev, plan = torch.ops.fiery_b200.lift_splat(h, Kd, Ed, None, handle, True, *extra)
+        assert plan.numel() > 0 and bev.grad_fn is not None and not plan.requires_grad, name
+        bev.sum().backward()
+        h2 = head.clone().requires_grad_(True)
+        module_call(h2).sum().backward()                            # the module goes through the same operator
+        assert torch.equal(h.grad, h2.grad), name
+        assert O.normwise_error(bev.detach().cpu(), exact_of(head.cpu())) < TOL, name
+        # autocast: an fp16 head inside an autocast region is lifted in fp32; the gradient comes back in fp16
+        h16 = head.half().requires_grad_(True)
+        with torch.autocast("cuda", dtype=torch.float16):
+            out = module_call(h16)
+        assert out.dtype == torch.float32, name
+        out.sum().backward()
+        assert h16.grad.dtype == torch.float16, name
+        assert O.normwise_error(out.detach().cpu(), exact_of(h16.detach().float().cpu())) < TOL, name
+        # traceable: dynamo captures the call as ONE operator node (fake implementation gives shapes / dtypes)
+        fn = torch.compile(lambda x: torch.ops.fiery_b200.lift_splat(x, Kd, Ed, None, handle, False, *extra)[0] * 2.0, backend="eager",
+                           fullgraph=True)
+        with torch.no_grad():
+            assert O.normwise_error((fn(head) / 2.0).cpu(), bev.detach().cpu()) < 1e-6, name
