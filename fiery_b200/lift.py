@@ -216,6 +216,17 @@ class LiftSplat(nn.Module):
         B, n = intrinsics.shape[:2]
         return self._desc(c, B, n, head_dtype, mode, layout), (a, b, c["u"], c["v"], c["d"])
 
+    @staticmethod
+    def _check_plan(plan: Optional[torch.Tensor], desc: _lib.LiftDesc, dev: torch.device) -> None:
+        """A caller-owned plan must be the buffer ``plan()`` makes for this call's (B', n): exactly fiery_lift_plan_bytes(desc)
+        bytes of uint8 on ``dev`` (one byte for B' = 0).  The kernels find the touched maps at an offset computed from this call's
+        frame count, so a plan of another batch would be read at the wrong place, not merely out of range."""
+        if plan is None:
+            return
+        want = max(1, int(_lib.load().fiery_lift_plan_bytes(desc)))
+        if plan.dtype != torch.uint8 or plan.device != dev or plan.numel() != want:
+            raise ValueError("plan was made for another batch shape: rebuild it with LiftSplat.plan(intrinsics, extrinsics)")
+
     # -- public entry points --------------------------------------------------------------------------------------
     def forward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
                 plan: Optional[torch.Tensor] = None, warp: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
@@ -254,7 +265,9 @@ class LiftSplat(nn.Module):
     def plan(self, intrinsics: torch.Tensor, extrinsics: torch.Tensor) -> torch.Tensor:
         """The geometry plan of a batch of calibrations (fiery_lift_plan): where every frustum point lands -- get_geometry
         (fiery.py:193-208) + voxel index / mask / rank (fiery.py:236-256) -- as pillar runs, in a device byte tensor.  Valid for
-        forward and backward calls with the same (B', n) and these calibrations."""
+        forward and backward calls with the same (B', n) and these calibrations.  A call rejects a plan whose size is not that
+        of its own (B', n) (``ValueError``); a plan of the same size made by another module, BEV grid or frustum, or for other
+        calibrations, cannot be detected and gives a wrong BEV."""
         _require_cuda(intrinsics, "intrinsics")
         lib = _lib.load()
         dev = intrinsics.device
@@ -402,6 +415,7 @@ class LiftSplat(nn.Module):
         head = head.contiguous()
         nhwc = self.output_layout == "channels_last" and warp is None
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, head.dtype, _lib.BEV_NHWC if nhwc else _lib.BEV_NCHW)
+        self._check_plan(plan, desc, dev)
         X, Y, _ = c["dim"]
         pooled = 0
         with torch.cuda.device(dev):
@@ -410,8 +424,6 @@ class LiftSplat(nn.Module):
                 out = store.permute(0, 3, 1, 2)
             else:
                 store = out = torch.empty((B, C, X, Y), dtype=torch.float32, device=dev)
-            if plan is not None and plan.numel() < int(lib.fiery_lift_plan_bytes(desc)):
-                raise ValueError("plan was made for another batch shape: rebuild it with LiftSplat.plan(intrinsics, extrinsics)")
             if scratch is None and B and not nhwc:
                 pooled = int(lib.fiery_lift_scratch_bytes(desc))
                 scratch = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
@@ -442,6 +454,7 @@ class LiftSplat(nn.Module):
             layout = _lib.BEV_NCHW
             g = g.contiguous()
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, layout)
+        self._check_plan(plan, desc, dev)
         grad_head = torch.empty_like(h32)
         with torch.cuda.device(dev):
             ws = None
