@@ -49,6 +49,9 @@ SIGNATURES = {
     "fiery_lift_forward_timed": (c_int32, [POINTER(LiftDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_int32, POINTER(c_float), POINTER(c_int32),
                                            POINTER(c_int32)]),
+    "fiery_lift_deterministic_workspace_bytes": (c_size_t, [POINTER(LiftDesc)]),
+    "fiery_lift_forward_deterministic": (c_int32, [POINTER(LiftDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_lift_set_max_chunk_frames": (None, [c_int32]),
     "fiery_lift_workspace_bytes": (c_size_t, [POINTER(LiftDesc)]),
     "fiery_lift_backward": (c_int32, [POINTER(LiftDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -60,6 +63,9 @@ SIGNATURES = {
     "fiery_voxels_summing_forward": (c_int32, [c_int64, c_int32, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                                                c_void_p, c_void_p, c_void_p]),
     "fiery_voxels_summing_backward": (c_int32, [c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_voxels_summing_deterministic_workspace_bytes": (c_size_t, [c_int64, c_int32]),
+    "fiery_voxels_summing_forward_deterministic": (c_int32, [c_int64, c_int32, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
+                                                             c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_depth_layer_forward": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_bev_conv_pack_weights": (c_int32, [c_void_p, c_void_p, c_void_p]),
     "fiery_bev_first_conv_forward": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),

@@ -96,6 +96,9 @@ int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels
 int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* scratch, const void* plan,
                         const float* warp_theta, const unsigned char* warp_copy,
                         cudaStream_t);
+int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* workspace, const void* plan,
+                            const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream);
+size_t lift_det_workspace_bytes(const LiftParams& P);
 int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
 int lift_chunk_frames(const LiftParams& P);
 size_t lift_scratch_bytes(const LiftParams& P);
@@ -119,6 +122,9 @@ int vs_plan(int64_t n_rows, const int64_t* ranks, int32_t* seg, int64_t* host_n,
 int vs_forward(int64_t n_rows, int channels, int64_t feat_stride, const float* feats, const int64_t* coords,
                const int32_t* seg, int64_t n_seg, float* sums, int64_t* coords_out, cudaStream_t);
 int vs_backward(int64_t n_rows, int channels, const float* grad_sums, const int32_t* seg, float* grad_feats, cudaStream_t);
+size_t vs_det_workspace_bytes(int64_t n_rows, int channels);
+int vs_forward_det(int64_t n_rows, int channels, int64_t feat_stride, const float* feats, const int64_t* coords, const int32_t* seg,
+                   float* sums, int64_t* coords_out, float* edge, cudaStream_t);
 
 static int make_params(const fiery_lift_desc_t* d, const float* calib_a, const float* calib_b, const float* fu,
                        const float* fv, const float* fd, LiftParams& P) {
@@ -234,6 +240,26 @@ FIERY_API int fiery_lift_forward_warped(const fiery_lift_desc_t* desc, const voi
     return launch_lift_forward(P, head, desc->head_dtype, bev_out, scratch, plan, theta, copy_mask, static_cast<cudaStream_t>(stream));
 }
 
+FIERY_API size_t fiery_lift_deterministic_workspace_bytes(const fiery_lift_desc_t* d) {
+    LiftParams P;
+    if (!shape_params(d, P) || P.n_frames == 0) return 0;
+    return lift_det_workspace_bytes(P);
+}
+
+FIERY_API int fiery_lift_forward_deterministic(const fiery_lift_desc_t* desc, const void* head, const float* calib_a,
+                                               const float* calib_b, const float* frustum_u, const float* frustum_v,
+                                               const float* frustum_d, float* bev_out, void* workspace, const void* plan,
+                                               const float* theta, const uint8_t* copy_mask, void* stream) {
+    LiftParams P;
+    int rc = make_params(desc, calib_a, calib_b, frustum_u, frustum_v, frustum_d, P);
+    if (rc != FIERY_OK) return rc;
+    if (P.n_frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(head && bev_out, "head / bev_out is NULL");
+    FIERY_REQUIRE((theta == nullptr) == (copy_mask == nullptr), "theta and copy_mask go together (the warped lift) or are both NULL");
+    FIERY_REQUIRE(!theta || desc->bev_layout == FIERY_BEV_NCHW, "the warped lift writes the NCHW layout only");
+    return launch_lift_forward_det(P, head, desc->head_dtype, bev_out, workspace, plan, theta, copy_mask, static_cast<cudaStream_t>(stream));
+}
+
 FIERY_API int fiery_lift_forward_timed(const fiery_lift_desc_t* desc, const void* head, const float* calib_a, const float* calib_b,
                                        const float* frustum_u, const float* frustum_v, const float* frustum_d, float* bev_out,
                                        void* scratch, const void* plan, void* stream, int32_t max_launches, float* host_ms,
@@ -306,6 +332,24 @@ FIERY_API int fiery_voxels_summing_forward(int64_t n_rows, int32_t channels, int
     FIERY_REQUIRE(feats && coords && segment_of_row && sums_out && coords_out, "NULL pointer");
     return vs_forward(n_rows, channels, feat_stride, feats, coords, segment_of_row, n_segments, sums_out, coords_out,
                       static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_voxels_summing_deterministic_workspace_bytes(int64_t n_rows, int32_t channels) {
+    if (n_rows <= 0 || channels < 1) return 0;
+    return vs_det_workspace_bytes(n_rows, channels);
+}
+
+FIERY_API int fiery_voxels_summing_forward_deterministic(int64_t n_rows, int32_t channels, int64_t feat_stride, const float* feats,
+                                                         const int64_t* coords, const int32_t* segment_of_row, int64_t n_segments,
+                                                         float* sums_out, int64_t* coords_out, void* workspace, void* stream) {
+    FIERY_REQUIRE(n_rows >= 0 && channels >= 1 && feat_stride >= channels, "bad shape n_rows=%lld C=%d stride=%lld",
+                  (long long)n_rows, channels, (long long)feat_stride);
+    if (n_rows == 0) return FIERY_OK;
+    FIERY_REQUIRE(feats && coords && segment_of_row && sums_out && coords_out, "NULL pointer");
+    FIERY_REQUIRE(workspace != nullptr, "NULL workspace (fiery_voxels_summing_deterministic_workspace_bytes)");
+    (void)n_segments;
+    return vs_forward_det(n_rows, channels, feat_stride, feats, coords, segment_of_row, sums_out, coords_out,
+                          static_cast<float*>(workspace), static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API int fiery_voxels_summing_backward(int64_t n_rows, int32_t channels, const float* grad_sums, const int32_t* segment_of_row,

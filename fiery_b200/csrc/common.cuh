@@ -163,4 +163,29 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
+// inclusive prefix sum of v over the block (every thread must call it); warp_sums: >= 32 ints of shared memory
+__device__ __forceinline__ int block_inclusive_scan(int v, int* warp_sums) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += t;
+    }
+    if (lane == 31) warp_sums[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+        int w = (lane < (blockDim.x >> 5)) ? warp_sums[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += t;
+        }
+        warp_sums[lane] = w;
+    }
+    __syncthreads();
+    const int base = warp > 0 ? warp_sums[warp - 1] : 0;
+    __syncthreads();
+    return v + base;
+}
+
 }  // namespace fiery

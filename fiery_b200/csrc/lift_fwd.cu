@@ -526,6 +526,116 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
     return FIERY_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Deterministic forward (fiery_lift_forward_deterministic; kernels and summation order: lift_det.cu).  Per pass of frames, in the
+// workspace: [plan of the pass (internal plan only)][partial sums: a row of 64 floats per possible run][channel-last accumulator
+// (NCHW output only)][list starts][list cursors][lists].  Everything is sized for the worst case -- one run per frustum point -- so
+// no count ever comes back to the host, and a pass holds as many frames as fit the cap the default path's scratch has (1 GiB).
+// ---------------------------------------------------------------------------------------------------------------------
+struct DetLayout {
+    int frames;                                          // frames per pass
+    size_t plan, partials, accum, start, cursor, lists, total;   // byte offsets into the workspace, and its size
+};
+static size_t det_align(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
+static DetLayout det_layout(const LiftParams& P) {
+    const size_t tpf = static_cast<size_t>(P.n_cameras) * P.n_wtiles;
+    const size_t rows = tpf * det_runs_per_tile(P.hh);
+    const bool nchw = P.bev_layout == FIERY_BEV_NCHW;
+    const size_t per_frame = tpf * PLAN_TILE_BYTES + P.pillars + rows * 64 * 4 + (nchw ? P.pillars * 64 * 4 : 0) + P.pillars * 8 + rows * 4;
+    long long c = static_cast<long long>((1ull << 30) / per_frame);
+    const int forced = g_max_chunk_frames.load();
+    if (forced > 0 && forced < c) c = forced;
+    if (c > P.n_frames) c = P.n_frames;
+    DetLayout L;
+    L.frames = static_cast<int>(c < 1 ? 1 : c);
+    const size_t f = L.frames;
+    L.plan = 0;
+    L.partials = det_align(plan_bytes(L.frames, P.n_cameras, P.n_wtiles, P.pillars));
+    L.accum = L.partials + det_align(f * rows * 64 * 4);
+    L.start = L.accum + (nchw ? det_align(f * P.pillars * 64 * 4) : 0);
+    L.cursor = L.start + det_align(f * P.pillars * 4);
+    L.lists = L.cursor + det_align(f * P.pillars * 4);
+    L.total = L.lists + det_align(f * rows * 4);
+    return L;
+}
+
+size_t lift_det_workspace_bytes(const LiftParams& P) { return P.n_frames > 0 ? det_layout(P).total : 0; }
+
+int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t stream);
+int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
+int launch_det_reduce(const LiftParams& P, int nf, const unsigned char* tiles, const float* partials, int* start, int* cursor,
+                      int* lists, float* out, int zero_empty, cudaStream_t stream);
+
+int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* workspace, const void* plan,
+                            const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream) {
+    FIERY_REQUIRE(head_dtype == FIERY_DTYPE_F32 || head_dtype == FIERY_DTYPE_F16, "head dtype %d not supported (fp32 / fp16)", head_dtype);
+    FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
+    FIERY_REQUIRE(P.D >= 1 && P.D <= 48, "depth_bins=%d not supported by this build (1..48)", P.D);
+    FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
+    FIERY_REQUIRE(P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
+    const bool nchw = P.bev_layout == FIERY_BEV_NCHW;
+    FIERY_REQUIRE(!warp_theta || nchw, "the warped lift writes the NCHW layout only");
+    FIERY_REQUIRE(workspace != nullptr, "the deterministic forward needs the workspace of fiery_lift_deterministic_workspace_bytes()");
+    const DetLayout W = det_layout(P);
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    float* partials = reinterpret_cast<float*>(ws + W.partials);
+    float* accum = reinterpret_cast<float*>(ws + W.accum);
+    int* start = reinterpret_cast<int*>(ws + W.start);
+    int* cursor = reinterpret_cast<int*>(ws + W.cursor);
+    int* lists = reinterpret_cast<int*>(ws + W.lists);
+    const bool tma_pass = P.pillars % 4 == 0;
+    CUtensorMap bev_map;
+    if (nchw && tma_pass && !warp_theta) {
+        const int rc = encode_bev_map(&bev_map, bev_out, P.pillars, P.C, P.n_frames, FT_P);
+        if (rc != FIERY_OK) return rc;
+    }
+    LiftParams Q = P;
+    Q.head_f16 = head_dtype == FIERY_DTYPE_F16 ? head : nullptr;
+    Q.touched = nullptr;
+    for (int f0 = 0; f0 < P.n_frames; f0 += W.frames) {
+        Q.frame0 = f0;
+        Q.n_frames = (P.n_frames - f0 < W.frames) ? P.n_frames - f0 : W.frames;
+        const unsigned char* marks;
+        if (plan) {
+            const PlanView v = plan_view(plan, P.n_frames, P.n_cameras, P.n_wtiles, P.pillars, f0);
+            Q.plan_tiles = v.tiles;
+            marks = v.touched;
+        } else {                                     // a forward-only plan of this pass's frames (no backward streams)
+            const PlanView v = plan_view(ws + W.plan, Q.n_frames, P.n_cameras, P.n_wtiles, P.pillars, 0);
+            FIERY_CUDA_CHECK(cudaMemsetAsync(const_cast<unsigned char*>(v.touched), 0, static_cast<size_t>(Q.n_frames) * P.pillars, stream));
+            const int rc = launch_lift_plan(Q, const_cast<unsigned char*>(v.tiles), const_cast<unsigned char*>(v.touched), 0, stream);
+            if (rc != FIERY_OK) return rc;
+            Q.plan_tiles = v.tiles;
+            marks = v.touched;
+        }
+        Q.accum = partials;
+        int rc = launch_forward_cols_det(Q, head, stream);
+        if (rc != FIERY_OK) return rc;
+        float* out = nchw ? accum : bev_out + static_cast<size_t>(f0) * P.pillars * P.C;
+        rc = launch_det_reduce(Q, Q.n_frames, Q.plan_tiles, partials, start, cursor, lists, out, nchw ? 0 : 1, stream);
+        if (rc != FIERY_OK) return rc;
+        if (!nchw) continue;
+        // the layout passes of the default path, unchanged; they read exactly the marked rows, which the reduction has written.  The
+        // workspace needs no restoring, so marks are never cleared and the accumulator's rows need not be re-zeroed after the warp.
+        unsigned char* m = const_cast<unsigned char*>(marks);
+        if (warp_theta) {
+            const int tpf = static_cast<int>((P.pillars + FW_P - 1) / FW_P);
+            finalize_warp_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FW_THREADS, 0, stream>>>(
+                accum, m, bev_out, P.pillars, P.grid.X, P.grid.Y, tpf, f0, warp_theta, warp_copy);
+        } else if (tma_pass) {
+            const int tpf = static_cast<int>((P.pillars + FT_P - 1) / FT_P);
+            finalize_tma_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FT_THREADS, 0, stream>>>(
+                bev_map, accum, m, P.pillars, tpf, f0, 0, 1);
+        } else {
+            const int bpf = static_cast<int>((P.pillars + FIN_THREADS - 1) / FIN_THREADS);
+            finalize_nchw_kernel<<<static_cast<unsigned>(bpf) * Q.n_frames, FIN_THREADS, 0, stream>>>(
+                accum, m, bev_out + static_cast<size_t>(f0) * P.C * P.pillars, P.pillars, bpf, 0);
+        }
+        FIERY_CUDA_CHECK(cudaGetLastError());
+    }
+    return FIERY_OK;
+}
+
 int launch_point_indices(const LiftParams& P, int64_t* idx_out, uint8_t* valid_out, int32_t* pillar_out, cudaStream_t stream) {
     const long long total = static_cast<long long>(P.n_frames) * P.n_cameras * P.D * P.hh * P.ww;
     if (total == 0) return FIERY_OK;

@@ -83,7 +83,9 @@ __device__ __forceinline__ void clear_half(unsigned long long& v, unsigned keep)
 //   pillar[row][pair]  written only where it is read: the last row of every run
 // thread = (depth, column) pair; a pair has ~2.8 runs on average, so this is a few dozen instructions per thread (the 37
 // instructions per POINT of the reference arithmetic are spent once per batch in the plan kernel, not per tile pass).
-template <int NT, int DD>
+// DET (the deterministic forward): pillar[row][pair] holds the run's index k in the record's runs[] instead of its pillar -- the row
+// of the tile's partial sums the run is stored to -- and -1 for a masked run that reaches the last row.
+template <int NT, int DD, bool DET = false>
 __device__ __forceinline__ void expand_plan(const ColsLayout& L, unsigned char* smem, const unsigned char* __restrict__ rec) {
     static_assert(NT >= COLS_NPAIR, "one thread per (depth, column) pair at least");
     const int pair = threadIdx.x;
@@ -104,10 +106,15 @@ __device__ __forceinline__ void expand_plan(const ColsLayout& L, unsigned char* 
         m &= m - 1;
         const int nxt = run(++k);
         atomicOr(ev + h, (1u << j) | (cur >= 0 ? (1u << (4 * DD + j)) : 0u));
-        if (cur >= 0) tab[(h - 1) * COLS_NPAIR] = cur;
+        if constexpr (DET) {
+            if (cur >= 0) tab[(h - 1) * COLS_NPAIR] = k - 1;
+        } else {
+            if (cur >= 0) tab[(h - 1) * COLS_NPAIR] = cur;
+        }
         cur = nxt;
     }
-    tab[(L.hh - 1) * COLS_NPAIR] = cur;                   // the run that reaches the last row
+    if constexpr (DET) tab[(L.hh - 1) * COLS_NPAIR] = cur >= 0 ? k : -1;
+    else tab[(L.hh - 1) * COLS_NPAIR] = cur;              // the run that reaches the last row
 }
 
 // constants of the in-tile geometry live where a planned tile stages its plan record
@@ -264,11 +271,18 @@ __device__ __forceinline__ void red_channels_if(char* dst, const float (&v)[CPL]
                      :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit), "l"(policy) : "memory");
 }
 
+// the deterministic forward's flush: a predicated plain store of CPL adjacent channels into the run's row of partial sums
+__device__ __forceinline__ void st_channels_if(char* dst, const float (&v)[CPL], unsigned bit) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\t@p st.global.v2.f32 [%0], {%1, %2};\n\t}"
+                 :: "l"(dst), "f"(v[0]), "f"(v[1]), "r"(bit) : "memory");
+}
+
 // One (depth, column) slot of the run-end handling.  `mw` is warp-uniform, so the test is a plain branch; the lanes that own
 // the ending run reduce their channels into the accumulator and restart.  The "+ 0.0f" copies are real instructions on
 // purpose: they gather the values into the consecutive registers the vector reduction needs HERE, instead of letting the
 // register allocator keep the accumulators in that order and un-shuffle them around every FMA pair.
-template <int DD, int SD, int COL, bool HINT>
+// DET: plp holds run indices and `out` is the tile's rows of partial sums; the run's sum is stored, not reduced.
+template <int DD, int SD, int COL, bool HINT, bool DET>
 __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
                                            const int* plp, char* out, uint64_t policy) {
     constexpr int j = SD * 4 + COL;
@@ -277,29 +291,33 @@ __device__ __forceinline__ void flush_slot(unsigned long long (&acc)[CPL][DD][2]
         float v[CPL];
 #pragma unroll
         for (int k = 0; k < CPL; ++k) v[k] = __fadd_rn(half_of<COL & 1>(acc[k][SD][COL >> 1]), 0.0f);
-        red_channels_if<HINT>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j), policy);
+        if constexpr (DET) st_channels_if(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j));
+        else red_channels_if<HINT>(out + static_cast<size_t>(pl) * (64 * 4), v, flush & (1u << j), policy);
         const unsigned keep = ((own >> j) & 1u) - 1u;          // 0 where my run ends, ~0 otherwise
 #pragma unroll
         for (int k = 0; k < CPL; ++k) clear_half<COL & 1>(acc[k][SD][COL >> 1], keep);
     }
 }
 
-template <int DD, int SD, bool HINT>
+template <int DD, int SD, bool HINT, bool DET>
 __device__ __forceinline__ void flush_depth(unsigned long long (&acc)[CPL][DD][2], unsigned mw, unsigned own, unsigned flush,
                                             const int* plp, char* out, uint64_t policy) {
     if (mw & (0xfu << (4 * SD))) {
-        flush_slot<DD, SD, 0, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 1, HINT>(acc, mw, own, flush, plp, out, policy);
-        flush_slot<DD, SD, 2, HINT>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 3, HINT>(acc, mw, own, flush, plp, out, policy);
+        flush_slot<DD, SD, 0, HINT, DET>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 1, HINT, DET>(acc, mw, own, flush, plp, out, policy);
+        flush_slot<DD, SD, 2, HINT, DET>(acc, mw, own, flush, plp, out, policy); flush_slot<DD, SD, 3, HINT, DET>(acc, mw, own, flush, plp, out, policy);
     }
-    if constexpr (SD + 1 < DD) flush_depth<DD, SD + 1, HINT>(acc, mw, own, flush, plp, out, policy);
+    if constexpr (SD + 1 < DD) flush_depth<DD, SD + 1, HINT, DET>(acc, mw, own, flush, plp, out, policy);
 }
 
 // DD depths per unit, a tile is 48 / DD units of one warp: DD 2 is 768 threads, DD 3 512.  The row loop is unrolled twice for DD 3
 // and not at all for DD 2.  Two tiles per SM.
 // HINTS: NCHW output, L2 policies on the head loads and the reductions into the scratch (lift_fwd.cu: lanes)
-template <int DD, bool HALF, bool PLANNED, bool HINTS>
+// DET: the deterministic forward (lift_det.cu) -- planned, no hints; every run's sum is stored to row (tile, k) of P.accum, which
+// holds det_runs_per_tile(h) rows of 64 channels per tile of the launch.
+template <int DD, bool HALF, bool PLANNED, bool HINTS, bool DET>
 __global__ void __launch_bounds__((DPAD / DD) * LPU, 2)
 lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const LiftParams P) {
+    static_assert(!DET || (PLANNED && !HINTS), "the deterministic tile kernel is planned and unhinted");
     constexpr int NU = DPAD / DD;                     // units per tile
     constexpr int NT = NU * LPU;
     constexpr int SLOTS = 4 * DD;
@@ -368,7 +386,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
     // geometry of the tile (the head tile stays in flight meanwhile): the runs of its plan record, or evaluated here
     if (PLANNED) {
         if (tid < COLS_NPAIR) mbar_wait(bar + 1, 0);
-        expand_plan<NT, DD>(L, smem, rec);
+        expand_plan<NT, DD, DET>(L, smem, rec);
     } else {
         unsigned char* touched = P.touched ? P.touched + static_cast<size_t>(frame) * P.pillars : nullptr;
         if (P.grid.pow2[0] && P.grid.pow2[1]) stage_geometry_cols<true, NT, DD>(P, L, smem, w0, touched);
@@ -385,7 +403,9 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
     const float* pp = reinterpret_cast<const float*>(smem + L.off_prob) + unit * DD * WT;
     const float* cp = reinterpret_cast<const float*>(smem + L.off_ctx) + cl * WT;
     const int* plp = reinterpret_cast<const int*>(smem + L.off_pillar) + unit * SLOTS - COLS_NPAIR;          // row h-1
-    char* out = reinterpret_cast<char*>(P.accum + static_cast<size_t>(frame) * P.pillars * P.C + cl * CPL);
+    char* out;
+    if constexpr (DET) out = reinterpret_cast<char*>(P.accum + static_cast<size_t>(blockIdx.x) * det_runs_per_tile(hh) * 64 + cl * CPL);
+    else out = reinterpret_cast<char*>(P.accum + static_cast<size_t>(frame) * P.pillars * P.C + cl * CPL);
     const unsigned* evp = reinterpret_cast<const unsigned*>(smem + L.off_ev) + unit * COLS_EVS + 1;         // row h+1
     const uint64_t keep = HINTS ? l2_evict_last() : 0;   // the scratch accumulator: the layout pass reads these lines next
 
@@ -402,7 +422,7 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
 #pragma unroll UNR
     for (int h = 0; h < hh; ++h, pp += DPAD * WT, cp += 64 * WT, plp += COLS_NPAIR, ++evp) {
         const unsigned ev_next = *evp;                                // the word after the last row stays 0
-        if (mw) flush_depth<DD, 0, HINTS>(acc, mw, own, flush, plp, out, keep);
+        if (mw) flush_depth<DD, 0, HINTS, DET>(acc, mw, own, flush, plp, out, keep);
         ulonglong2 dv[DD];
 #pragma unroll
         for (int dd = 0; dd < DD; ++dd) dv[dd] = *reinterpret_cast<const ulonglong2*>(pp + dd * WT);   // columns (0,1) (2,3)
@@ -430,20 +450,21 @@ lift_forward_cols_kernel(const __grid_constant__ HeadMapsCols head_maps, const L
             const unsigned long long a = acc[k][j >> 2][(j & 3) >> 1];
             v[k] = (j & 1) ? half_of<1>(a) : half_of<0>(a);
         }
-        red_channels_if<HINTS>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u, keep);
+        if constexpr (DET) st_channels_if(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u);
+        else red_channels_if<HINTS>(out + static_cast<size_t>(static_cast<unsigned>(pl)) * (64 * 4), v, pl >= 0 ? 1u : 0u, keep);
     }
 }
 
-template <int DD, bool HALF, bool PLANNED, bool HINTS>
+template <int DD, bool HALF, bool PLANNED, bool HINTS, bool DET>
 static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStream_t stream) {
     constexpr int NU = DPAD / DD, NT = NU * LPU;
     const ColsLayout L(P.hh, P.C, NU);
+    auto kernel = lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS, DET>;
     static OncePerDevice once;                        // zero-initialised (static storage)
-    int rc = once.run([]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    int rc = once.run([kernel]() -> int {
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         // ask for the full shared-memory carve-out (two or three tiles of ~75 KB per SM for the reference shape)
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                              cudaSharedmemCarveoutMaxShared));
+        FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         return FIERY_OK;
     });
     if (rc != FIERY_OK) return rc;
@@ -458,7 +479,7 @@ static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStre
         if (rc != FIERY_OK) return rc;
     }
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
-    lift_forward_cols_kernel<DD, HALF, PLANNED, HINTS><<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
+    kernel<<<static_cast<unsigned>(n_tiles), NT, L.total, stream>>>(maps, P);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -467,8 +488,17 @@ static int launch_forward_cols_t(const LiftParams& P, const void* head, cudaStre
 // measured slower on an H100 than with the plain instructions
 template <int DD, bool HALF, bool PLANNED>
 static int launch_layout_t(const LiftParams& P, const void* head, cudaStream_t stream) {
-    return P.bev_layout == FIERY_BEV_NCHW ? launch_forward_cols_t<DD, HALF, PLANNED, true>(P, head, stream)
-                                          : launch_forward_cols_t<DD, HALF, PLANNED, false>(P, head, stream);
+    return P.bev_layout == FIERY_BEV_NCHW ? launch_forward_cols_t<DD, HALF, PLANNED, true, false>(P, head, stream)
+                                          : launch_forward_cols_t<DD, HALF, PLANNED, false, false>(P, head, stream);
+}
+
+// The deterministic forward's tile kernel (lift_det.cu): P.plan_tiles is required, P.accum receives the runs' partial sums.
+int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t stream) {
+    FIERY_REQUIRE(P.hh <= 32, "feat_h=%d not supported by this build (<= 32)", P.hh);
+    FIERY_REQUIRE(P.C == 64 && P.D <= DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);
+    FIERY_REQUIRE(P.plan_tiles != nullptr, "the deterministic tile kernel needs a plan");
+    return P.head_f16 != nullptr ? launch_forward_cols_t<3, true, true, false, true>(P, head, stream)
+                                 : launch_forward_cols_t<3, false, true, false, true>(P, head, stream);
 }
 
 // Unit shape (DD depths per unit of one warp, 2 channels per lane).  The pooling loop is bound by shared-memory wavefronts (a

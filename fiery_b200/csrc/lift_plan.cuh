@@ -44,6 +44,9 @@ constexpr int PLAN_OFF_RUNS = PLAN_OFF_COUNTS + 16;
 constexpr int PLAN_OFF_STREAMS = PLAN_OFF_RUNS + PLAN_CAP * 4;
 constexpr int PLAN_TILE_BYTES = (PLAN_OFF_STREAMS + PLAN_STREAM_CAP * 4 + 127) & ~127;
 
+// Rows of partial sums a tile of the deterministic forward may store: a (depth, column) pair has at most one run per image row.
+__host__ __device__ inline int det_runs_per_tile(int rows) { return PLAN_PAIRS * rows; }
+
 struct PlanView {
     const unsigned char* tiles;     // tile records of this launch's first frame onwards
     const unsigned char* touched;   // touched map of the same frame onwards (n_frames * pillars bytes)

@@ -19,30 +19,6 @@ __device__ __forceinline__ int run_start(const int64_t* __restrict__ ranks, int6
     return (i > 0 && ranks[i] != ranks[i - 1]) ? 1 : 0;
 }
 
-__device__ __forceinline__ int block_inclusive_scan(int v, int* warp_sums /* >= 32 ints */) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += t;
-    }
-    if (lane == 31) warp_sums[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        int w = (lane < (blockDim.x >> 5)) ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += t;
-        }
-        warp_sums[lane] = w;
-    }
-    __syncthreads();
-    const int base = warp > 0 ? warp_sums[warp - 1] : 0;
-    __syncthreads();
-    return v + base;
-}
-
 __global__ void __launch_bounds__(SCAN_THREADS)
 vs_count_kernel(int64_t n, const int64_t* __restrict__ ranks, int* __restrict__ tile_counts) {
     __shared__ int ws[32];
@@ -131,6 +107,84 @@ __global__ void vs_forward_kernel(int64_t n_rows, int C, int64_t stride, const f
     if (run_ends_here && c < 3) coords_out[static_cast<int64_t>(cur) * 3 + c] = coords[(r1 - 1) * 3 + c];
 }
 
+// ---- deterministic forward ------------------------------------------------------------------------------------------
+// The same walk, but a run that crosses a chunk edge is not combined with atomics: chunk q stores the piece of its first run to
+// edge[q][0] when that run continues from chunk q-1, and the piece of its last run to edge[q][1] when that run starts in chunk q and
+// continues into chunk q+1.  Runs that start and end inside a chunk keep their plain stores.  vs_join_kernel then adds the pieces of
+// every straddling run in chunk order.
+__device__ __forceinline__ int64_t vs_chunk_end(int64_t q, int64_t n_rows) { return min(n_rows, (q + 1) * VS_ROWS); }
+
+__global__ void vs_forward_det_kernel(int64_t n_rows, int C, int64_t stride, const float* __restrict__ feats,
+                                      const int64_t* __restrict__ coords, const int32_t* __restrict__ seg,
+                                      float* __restrict__ sums, int64_t* __restrict__ coords_out, float* __restrict__ edge) {
+    const int c = threadIdx.x;                                             // channel
+    const int64_t chunk = static_cast<int64_t>(blockIdx.x) * blockDim.y + threadIdx.y;
+    const int64_t r0 = chunk * VS_ROWS;
+    if (r0 >= n_rows) return;
+    const int64_t r1 = vs_chunk_end(chunk, n_rows);
+    const bool live = c < C;
+    const int first_seg = seg[r0];
+    const bool open = r0 > 0 && seg[r0 - 1] == first_seg;                 // the first run continues one of the previous chunk
+    float* piece = edge + chunk * 2 * C + c;
+    int cur = first_seg;
+    float acc = 0.f;
+#pragma unroll 8
+    for (int64_t r = r0; r < r1; ++r) {
+        const int s = seg[r];
+        const float x = live ? feats[r * stride + c] : 0.f;
+        if (s != cur) {
+            if (live) {
+                if (cur == first_seg && open) piece[0] = acc;
+                else sums[static_cast<int64_t>(cur) * C + c] = acc;
+            }
+            if (c < 3) coords_out[static_cast<int64_t>(cur) * 3 + c] = coords[(r - 1) * 3 + c];  // last row of the run, geometry.py:295
+            cur = s;
+            acc = 0.f;
+        }
+        acc += x;
+    }
+    const bool run_ends_here = (r1 == n_rows) || (seg[r1] != cur);
+    if (live) {
+        if (cur == first_seg && open) piece[0] = acc;
+        else if (run_ends_here) sums[static_cast<int64_t>(cur) * C + c] = acc;
+        else piece[C] = acc;
+    }
+    if (run_ends_here && c < 3) coords_out[static_cast<int64_t>(cur) * 3 + c] = coords[(r1 - 1) * 3 + c];
+}
+
+// One thread per (chunk, channel): a chunk whose last run starts in it and continues sums that run's pieces -- its own edge[q][1], then
+// edge[j][0] of the chunks j = q+1 .. the chunk where the run ends, in that order.  The end row is found by bisection (seg ascends).
+__global__ void vs_join_kernel(int64_t n_rows, int C, const int32_t* __restrict__ seg, const float* __restrict__ edge,
+                               float* __restrict__ sums) {
+    const int c = threadIdx.x;
+    const int64_t q = static_cast<int64_t>(blockIdx.x) * blockDim.y + threadIdx.y;
+    const int64_t r0 = q * VS_ROWS;
+    if (r0 >= n_rows || c >= C) return;
+    const int64_t r1 = vs_chunk_end(q, n_rows);
+    if (r1 == n_rows) return;
+    const int s = seg[r1 - 1];
+    if (seg[r1] != s) return;                                              // the last run ends in this chunk
+    if (seg[r0] == s && r0 > 0 && seg[r0 - 1] == s) return;                // ... or started before it: a middle piece
+    int64_t lo = r1, hi = n_rows;                                          // first row past the run
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (seg[mid] == s) lo = mid + 1;
+        else hi = mid;
+    }
+    const int64_t last = (lo - 1) / VS_ROWS;
+    float acc = edge[q * 2 * C + C + c];
+    int64_t j = q + 1;
+    for (; j + 4 <= last + 1; j += 4) {                                    // four pieces in flight, added in chunk order
+        float x[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) x[u] = edge[(j + u) * 2 * C + c];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) acc += x[u];
+    }
+    for (; j <= last; ++j) acc += edge[j * 2 * C + c];
+    sums[static_cast<int64_t>(s) * C + c] = acc;
+}
+
 // ---- backward: grad_feats[i] = grad_sums[seg[i]] (geometry.py:305-314) ----------------------------------------------
 __global__ void vs_backward_kernel(int64_t n_rows, int C, const float* __restrict__ grad_sums,
                                    const int32_t* __restrict__ seg, float* __restrict__ grad_feats) {
@@ -192,6 +246,25 @@ int vs_forward(int64_t n_rows, int C, int64_t stride, const float* feats, const 
     const dim3 block(tx, ty);
     vs_forward_kernel<<<static_cast<unsigned>((chunks + ty - 1) / ty), block, 0, stream>>>(n_rows, C, stride, feats, coords,
                                                                                         seg, sums, coords_out);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+size_t vs_det_workspace_bytes(int64_t n_rows, int C) {
+    return static_cast<size_t>((n_rows + VS_ROWS - 1) / VS_ROWS) * 2 * C * sizeof(float);
+}
+
+// Every run is written exactly once (a plain store in its chunk, or by vs_join_kernel), so `sums` needs no zero-fill.
+int vs_forward_det(int64_t n_rows, int C, int64_t stride, const float* feats, const int64_t* coords, const int32_t* seg,
+                   float* sums, int64_t* coords_out, float* edge, cudaStream_t stream) {
+    FIERY_REQUIRE(C <= 1024, "channels=%d exceeds 1024", C);
+    const int tx = ((C < 3 ? 3 : C) + 31) & ~31;
+    const int ty = tx >= 256 ? 1 : 256 / tx;
+    const int64_t chunks = (n_rows + VS_ROWS - 1) / VS_ROWS;
+    const dim3 block(tx, ty);
+    const unsigned grid = static_cast<unsigned>((chunks + ty - 1) / ty);
+    vs_forward_det_kernel<<<grid, block, 0, stream>>>(n_rows, C, stride, feats, coords, seg, sums, coords_out, edge);
+    vs_join_kernel<<<grid, block, 0, stream>>>(n_rows, C, seg, edge, sums);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

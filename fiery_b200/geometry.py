@@ -81,6 +81,18 @@ def _stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _unfilled(shape, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
+    """``torch.empty`` without the NaN fill ``torch.use_deterministic_algorithms(True)`` adds: for workspaces whose contents on entry
+    do not matter and outputs the kernels overwrite completely (a fill of the lift's ~1 GB workspace would cost more than the lift)."""
+    import torch.utils.deterministic as det
+    old = det.fill_uninitialized_memory
+    det.fill_uninitialized_memory = False
+    try:
+        return torch.empty(shape, dtype=dtype, device=device)
+    finally:
+        det.fill_uninitialized_memory = old
+
+
 def _require_cuda(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
         raise _lib.FieryError(f"{name} must be a CUDA tensor: fiery_b200 has no CPU path (got device {t.device})")
@@ -121,10 +133,14 @@ class VoxelsSumming(torch.autograd.Function):
             n_segments = int(n_seg.value)
             sums = torch.empty((n_segments, channels), dtype=torch.float32, device=dev)
             kept = torch.empty((n_segments, 3), dtype=torch.int64, device=dev)
-            _lib.check(lib.fiery_voxels_summing_forward(n_rows, channels, xf.stride(0) if n_rows else channels,
-                                                        xf.data_ptr(), coords.data_ptr(), seg.data_ptr(), n_segments,
-                                                        sums.data_ptr(), kept.data_ptr(), _stream_ptr(dev)),
-                       "fiery_voxels_summing_forward")
+            args = (n_rows, channels, xf.stride(0) if n_rows else channels, xf.data_ptr(), coords.data_ptr(), seg.data_ptr(),
+                    n_segments, sums.data_ptr(), kept.data_ptr())
+            if torch.are_deterministic_algorithms_enabled():     # chunk-edge runs summed in chunk order instead of atomically
+                ws = _unfilled(max(1, int(lib.fiery_voxels_summing_deterministic_workspace_bytes(n_rows, channels))), torch.uint8, dev)
+                _lib.check(lib.fiery_voxels_summing_forward_deterministic(*args, ws.data_ptr(), _stream_ptr(dev)),
+                           "fiery_voxels_summing_forward_deterministic")
+            else:
+                _lib.check(lib.fiery_voxels_summing_forward(*args, _stream_ptr(dev)), "fiery_voxels_summing_forward")
         ctx.save_for_backward(seg)
         ctx.in_dtype = x.dtype
         ctx.channels = channels

@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .geometry import (_require_cuda, _stream_ptr, bev_offset_fp32, calculate_birds_eye_view_parameters, create_frustum,
+from .geometry import (_require_cuda, _stream_ptr, _unfilled, bev_offset_fp32, calculate_birds_eye_view_parameters, create_frustum,
                        split_frustum, z_valid_interval)
 
 # The geometry plan's byte layout (fiery_b200/csrc/lift_plan.cuh): one record per (frame, camera, 4-column tile), then the touched
@@ -398,7 +398,10 @@ class LiftSplat(nn.Module):
                         scratch: Optional[torch.Tensor] = None, plan: Optional[torch.Tensor] = None,
                         warp: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
         """``warp``: (theta (B', 2, 3), copy_mask (B',) uint8) -- the layout pass samples every frame under its map
-        (fiery_lift_forward_warped); NCHW output only."""
+        (fiery_lift_forward_warped); NCHW output only.
+        Under ``torch.use_deterministic_algorithms(True)`` the call runs the bit-reproducible forward
+        (fiery_lift_forward_deterministic: every pillar's runs added in a fixed order, no atomics) in a workspace of its own;
+        ``scratch`` is then unused."""
         _require_cuda(head, "head")
         lib = _lib.load()
         dev = head.device
@@ -417,6 +420,19 @@ class LiftSplat(nn.Module):
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, head.dtype, _lib.BEV_NHWC if nhwc else _lib.BEV_NCHW)
         self._check_plan(plan, desc, dev)
         X, Y, _ = c["dim"]
+        if warp is not None:
+            theta, copy_mask = warp
+            if theta.numel() != B * 6 or copy_mask.numel() != B or theta.dtype != torch.float32 or copy_mask.dtype != torch.uint8:
+                raise ValueError("warp must be (theta (B', 2, 3) float32, copy_mask (B',) uint8) for the B' frames of this call")
+        if torch.are_deterministic_algorithms_enabled():
+            with torch.cuda.device(dev):
+                store = _unfilled((B, X, Y, C) if nhwc else (B, C, X, Y), torch.float32, dev)      # every element is written
+                ws = _unfilled(max(1, int(lib.fiery_lift_deterministic_workspace_bytes(desc))), torch.uint8, dev)
+                _lib.check(lib.fiery_lift_forward_deterministic(
+                    desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(), ws.data_ptr(),
+                    plan.data_ptr() if plan is not None else 0, warp[0].data_ptr() if warp is not None else 0,
+                    warp[1].data_ptr() if warp is not None else 0, _stream_ptr(dev)), "fiery_lift_forward_deterministic")
+            return store.permute(0, 3, 1, 2) if nhwc else store
         pooled = 0
         with torch.cuda.device(dev):
             if nhwc:
@@ -432,9 +448,6 @@ class LiftSplat(nn.Module):
             if warp is None:
                 status = lib.fiery_lift_forward(*args, _stream_ptr(dev))
             else:
-                theta, copy_mask = warp
-                if theta.numel() != B * 6 or copy_mask.numel() != B or theta.dtype != torch.float32 or copy_mask.dtype != torch.uint8:
-                    raise ValueError("warp must be (theta (B', 2, 3) float32, copy_mask (B',) uint8) for the B' frames of this call")
                 status = lib.fiery_lift_forward_warped(*args, theta.data_ptr(), copy_mask.data_ptr(), _stream_ptr(dev))
             if status != 0 and pooled:
                 _scratch.discard(dev, pooled)          # a launch sequence that stopped half way may have left it dirty

@@ -137,6 +137,26 @@ FIERY_API int fiery_lift_forward_warped(const fiery_lift_desc_t* desc, const voi
                                         const float* frustum_u, const float* frustum_v, const float* frustum_d, float* bev_out,
                                         void* scratch, const void* plan, const float* theta, const uint8_t* copy_mask, void* stream);
 
+/*
+ * Bit-reproducible forward lift (what torch.use_deterministic_algorithms(True) selects in the Python layer).  Same descriptors as
+ * fiery_lift_forward: fp32 and fp16 heads, both calibration modes, NCHW and NHWC output, the uniform-depth head.  theta / copy_mask
+ * non-NULL (NCHW only): the warped lift of fiery_lift_forward_warped.  plan: a plan of fiery_lift_plan for this batch, or NULL (the
+ * call then builds a forward-only plan per pass into the workspace).  workspace: fiery_lift_deterministic_workspace_bytes(desc)
+ * bytes; its contents on entry are irrelevant.  bev_out is fully overwritten in both layouts (NHWC needs no zero fill).
+ * Summation order: every pillar of frame f is the fp32 sum of its pillar runs' partial sums (each run's sum is the register chain
+ * the tile kernel computes along the image column), added one after the other in ascending (tile of frame f, run index in the
+ * tile's plan record) order.  The order depends on frame f's geometry only, so a frame's BEV is bit-identical whatever other frames
+ * share the call, however the call is cut into passes, with the caller's plan or the internal one, captured in a graph or not; NCHW
+ * and NHWC hold the same bits, and a warped frame with its copy flag set equals the plain deterministic BEV of that frame.
+ * Frames run in passes bounded like the scratch of fiery_lift_forward (fiery_lift_set_max_chunk_frames applies).  Nothing
+ * synchronises with the host, so the call can be captured in a CUDA graph.
+ */
+FIERY_API size_t fiery_lift_deterministic_workspace_bytes(const fiery_lift_desc_t* desc);
+FIERY_API int fiery_lift_forward_deterministic(const fiery_lift_desc_t* desc, const void* head, const float* calib_a,
+                                               const float* calib_b, const float* frustum_u, const float* frustum_v,
+                                               const float* frustum_d, float* bev_out, void* workspace, const void* plan,
+                                               const float* theta, const uint8_t* copy_mask, void* stream);
+
 /* Number of kernel launches one fiery_lift_forward call with this descriptor issues (NHWC: the tile kernel; NCHW: tile kernel
  * + layout pass per frame group; groups of frames run as concurrent chains on internal streams that are forked from and
  * joined back into `stream` with events, so the call behaves like work queued on `stream` and can be captured in a graph). */
@@ -200,6 +220,13 @@ FIERY_API int fiery_voxels_summing_forward(int64_t n_rows, int32_t channels, int
                                  float* sums_out, int64_t* coords_out, void* stream);
 FIERY_API int fiery_voxels_summing_backward(int64_t n_rows, int32_t channels, const float* grad_sums,
                                   const int32_t* segment_of_row, float* grad_feats, void* stream);
+/* Bit-reproducible fiery_voxels_summing_forward: the same arguments plus a workspace of
+ * fiery_voxels_summing_deterministic_workspace_bytes(n_rows, channels) bytes (contents on entry irrelevant).  A run that crosses the
+ * edge of a 64-row chunk is summed per chunk, and its pieces are added in chunk order (no atomics); sums_out needs no zero fill. */
+FIERY_API size_t fiery_voxels_summing_deterministic_workspace_bytes(int64_t n_rows, int32_t channels);
+FIERY_API int fiery_voxels_summing_forward_deterministic(int64_t n_rows, int32_t channels, int64_t feat_stride, const float* feats,
+                                                         const int64_t* coords, const int32_t* segment_of_row, int64_t n_segments,
+                                                         float* sums_out, int64_t* coords_out, void* workspace, void* stream);
 
 /*
  * BEV feature warping -- the heavy part of warp_features / cumulative_warp_features (fiery/utils/geometry.py:181-253, call
