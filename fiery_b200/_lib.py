@@ -69,6 +69,10 @@ SIGNATURES = {
     "fiery_depth_layer_forward": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_bev_conv_pack_weights": (c_int32, [c_void_p, c_void_p, c_void_p]),
     "fiery_bev_first_conv_forward": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+    "fiery_bev_conv_pack_weights_transposed": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "fiery_bev_first_conv_backward_data": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_bev_first_conv_backward_weight_workspace_bytes": (c_size_t, [c_int32, c_int32, c_int32]),
+    "fiery_bev_first_conv_backward_weight": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

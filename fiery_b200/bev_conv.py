@@ -6,16 +6,22 @@ reference ``state_dict`` entry ``first_conv.weight`` loads unchanged) and runs t
 (fiery_b200/csrc/bev_conv.cu: TF32 operands, fp32 accumulation).  It takes the lift's channel-last BEV directly
 (``LiftSplat(output_layout="channels_last")``), so the lift's NCHW layout pass is not on this path.
 
-Inference op: no backward (training keeps ``nn.Conv2d``; the reference trains this layer under cuDNN).  No CPU path.
+Training: the backward (fiery_b200/csrc/bev_conv_bwd.cu) computes the input and weight gradients on the tensor cores too, on the
+same channel-last layout, bit-reproducibly (no atomics).  ``FirstConv(bn=None)`` -- with or without ``relu`` -- trains through the
+``torch.ops.fiery_b200.first_conv`` operator (fiery_b200/ops.py) whenever grad is enabled; ``install.use_tensor_core_first_conv``
+swaps it into a ``Fiery`` model, leaving ``bn1`` and ``relu`` to the reference's modules.  With ``bn`` given the module folds bn1
+from its running statistics into the kernel's epilogue: that form is for inference only and has no backward.  No CPU path.
 """
 from __future__ import annotations
 
-from typing import Optional
+from collections import OrderedDict
+from typing import Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from . import _lib
+from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.first_conv)
 from .geometry import _require_cuda, _stream_ptr
 
 
@@ -56,16 +62,103 @@ def pack_weight(weight: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def pack_weight_transposed(weight: torch.Tensor) -> torch.Tensor:
+    """(64, 64, 7, 7) conv weight -> (49, 64, 64) = (tap, in, out), TF32-rounded: the B operand of the input gradient (device kernel)."""
+    _require_cuda(weight, "weight")
+    if tuple(weight.shape) != (64, 64, 7, 7):
+        raise ValueError(f"first_conv weight must be (64, 64, 7, 7), got {tuple(weight.shape)}")
+    lib = _lib.load()
+    w = weight.detach().float().contiguous()
+    out = torch.empty((49, 64, 64), dtype=torch.float32, device=w.device)
+    with torch.cuda.device(w.device):
+        _lib.check(lib.fiery_bev_conv_pack_weights_transposed(w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
+                   "fiery_bev_conv_pack_weights_transposed")
+    return out
+
+
+# One cache for both packs: (weight data_ptr, device) -> [version, weight alias, forward pack, transposed pack or None].  The alias
+# keeps the weight's memory alive, so an address in the cache cannot be taken by another tensor while its entry exists; the
+# version counter (shared with every view and the Parameter) changes with each in-place update, e.g. an optimizer step.
+_PACKS: "OrderedDict[tuple, list]" = OrderedDict()
+_PACKS_MAX = 8
+
+
+def packed_weights(weight: torch.Tensor, transposed: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """(forward pack, transposed pack) of ``weight``, each made at most once per weight version; the transposed one only when asked."""
+    key = (weight.data_ptr(), str(weight.device))
+    entry = _PACKS.get(key)
+    if entry is None or entry[0] != weight._version or tuple(entry[1].shape) != tuple(weight.shape):
+        entry = [weight._version, weight.detach(), pack_weight(weight), None]
+        _PACKS[key] = entry
+        while len(_PACKS) > _PACKS_MAX:
+            _PACKS.popitem(last=False)
+    _PACKS.move_to_end(key)
+    if transposed and entry[3] is None:
+        entry[3] = pack_weight_transposed(weight)
+    return entry[2], entry[3]
+
+
+def _channels_last_f32(t: torch.Tensor) -> torch.Tensor:
+    t = t.float() if t.dtype != torch.float32 else t
+    return t if t.permute(0, 2, 3, 1).is_contiguous() else t.contiguous(memory_format=torch.channels_last)
+
+
+def first_conv_backward_data(grad_y: torch.Tensor, packed_weight_t: torch.Tensor, height: int, width: int) -> torch.Tensor:
+    """grad_y (B, 64, Ho, Wo) in any layout (converted to channels-last fp32 once if needed); packed_weight_t (49, 64, 64) from
+    ``pack_weight_transposed``; returns grad_x (B, 64, height, width) fp32 with channels-last strides."""
+    _require_cuda(grad_y, "grad_y")
+    lib = _lib.load()
+    B = grad_y.shape[0]
+    if grad_y.dim() != 4 or grad_y.shape[1] != 64 or tuple(grad_y.shape[2:]) != ((height - 1) // 2 + 1, (width - 1) // 2 + 1):
+        raise ValueError(f"grad_y {tuple(grad_y.shape)} does not match an input of {height}x{width}")
+    g = _channels_last_f32(grad_y)
+    store = torch.empty((B, height, width, 64), dtype=torch.float32, device=g.device)
+    with torch.cuda.device(g.device):
+        _lib.check(lib.fiery_bev_first_conv_backward_data(B, height, width, g.data_ptr(), packed_weight_t.data_ptr(), store.data_ptr(),
+                                                          _stream_ptr(g.device)), "fiery_bev_first_conv_backward_data")
+    return store.permute(0, 3, 1, 2)
+
+
+def backward_weight_workspace_bytes(n_frames: int, height: int, width: int) -> int:
+    """Bytes of device workspace ``first_conv_backward_weight`` uses (host-only answer)."""
+    return int(_lib.load().fiery_bev_first_conv_backward_weight_workspace_bytes(n_frames, height, width))
+
+
+def first_conv_backward_weight(x: torch.Tensor, grad_y: torch.Tensor, workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x (B, 64, H, W), grad_y (B, 64, Ho, Wo), any layout and floating dtype (converted to channels-last fp32 once if needed);
+    returns the weight gradient (64, 64, 7, 7) fp32, bit-reproducible.  ``workspace``: a uint8 device tensor of at least
+    ``backward_weight_workspace_bytes`` bytes to use instead of a fresh one."""
+    _require_cuda(x, "x")
+    lib = _lib.load()
+    if x.dim() != 4 or x.shape[1] != 64:
+        raise ValueError(f"x must be (B, 64, H, W), got {tuple(x.shape)}")
+    B, _, H, W = x.shape
+    if tuple(grad_y.shape) != (B, 64, (H - 1) // 2 + 1, (W - 1) // 2 + 1):
+        raise ValueError(f"grad_y {tuple(grad_y.shape)} does not match x {tuple(x.shape)}")
+    xs, g = _channels_last_f32(x), _channels_last_f32(grad_y)
+    need = backward_weight_workspace_bytes(B, H, W)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+    out = torch.empty((64, 64, 7, 7), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_bev_first_conv_backward_weight(B, H, W, xs.data_ptr(), g.data_ptr(), out.data_ptr(), workspace.data_ptr(),
+                                                            _stream_ptr(x.device)), "fiery_bev_first_conv_backward_weight")
+    return out
+
+
 class FirstConv(nn.Module):
-    """Drop-in for ``Decoder.first_conv`` (+ ``bn1`` + ``relu`` when given) in eval mode.  ``FirstConv.from_decoder(decoder)``
-    adopts the reference module's parameters (shared, not copied)."""
+    """Drop-in for ``Decoder.first_conv`` (+ ``bn1`` + ``relu`` when given).  Without ``bn`` it trains: whenever grad is enabled the
+    forward runs through the ``fiery_b200::first_conv`` operator, whose backward computes the input and weight gradients on the tensor
+    cores, and ``relu`` (if asked) is applied after it by ``torch.relu``; the forward values are those of the fused inference kernel.
+    With ``bn`` (bn1 folded from its running statistics into the epilogue) it is eval-only: ``.train()`` mode raises, and no gradient
+    flows through it.  ``FirstConv.from_decoder(decoder)`` and ``FirstConv.from_conv(conv)`` adopt the reference module's parameters
+    (shared, not copied)."""
 
     def __init__(self, bn: Optional[nn.BatchNorm2d] = None, relu: bool = False):
         super().__init__()
         self.weight = nn.Parameter(torch.empty(64, 64, 7, 7))
         nn.init.kaiming_normal_(self.weight, mode="fan_out", nonlinearity="relu")
         self.bn, self.relu = bn, relu
-        self._packed = None
 
     @classmethod
     def from_decoder(cls, decoder, fuse_bn_relu: bool = True) -> "FirstConv":
@@ -73,11 +166,15 @@ class FirstConv(nn.Module):
         m.weight = decoder.first_conv.weight
         return m
 
+    @classmethod
+    def from_conv(cls, conv: nn.Conv2d) -> "FirstConv":
+        """The trainable form (``bn=None``) of ``Decoder.first_conv`` = ``conv``, sharing its weight Parameter."""
+        m = cls()
+        m.weight = conv.weight
+        return m
+
     def _packed_weight(self) -> torch.Tensor:
-        key = (self.weight.data_ptr(), self.weight._version, str(self.weight.device))
-        if self._packed is None or self._packed[0] != key:
-            self._packed = (key, pack_weight(self.weight))
-        return self._packed[1]
+        return packed_weights(self.weight)[0]
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.training and self.bn is not None:
@@ -89,5 +186,8 @@ class FirstConv(nn.Module):
             bta = self.bn.bias.float() if self.bn.affine else torch.zeros_like(inv)
             scale = g * inv
             shift = bta - self.bn.running_mean.float() * scale
+        if self.bn is None and torch.is_grad_enabled():
+            y = torch.ops.fiery_b200.first_conv(x, self.weight)
+            return torch.relu(y) if self.relu else y
         with torch.no_grad():
             return first_conv_forward(x, self._packed_weight(), scale, shift, self.relu)

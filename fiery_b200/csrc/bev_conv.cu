@@ -18,33 +18,9 @@
 // Operands are TF32 (10-bit mantissa: weights rounded when they are packed, activations read from fp32 by truncation), accumulation
 // fp32 -- the precision cuDNN uses for this layer under torch's default allow_tf32; the parity bar (tests/test_bev_conv_gpu.py) is
 // stated against an fp64 convolution: normwise < 1e-3.
-#include "lift_plan.cuh"
-#include "wgmma.cuh"
+#include "bev_conv.cuh"
 
 namespace fiery {
-
-constexpr int CV_C = 64;                      // input = output channels
-constexpr int CV_TAPS = 49;
-constexpr int CV_TW = 16, CV_TH = 8;          // output patch: 16 x 8 = 128 rows of the accumulator
-constexpr int CV_STAGES = 4;
-constexpr int CV_A_ATOM = 128 * 128;          // 128 rows x 128 bytes (32 fp32 channels), swizzle-128B atom rows
-constexpr int CV_B_ATOM = 64 * 128;           // 64 output channels x 32 input channels
-constexpr int CV_STAGE_BYTES = 2 * CV_A_ATOM + 2 * CV_B_ATOM;      // 48 KB
-constexpr int CV_CONSUMERS = 2;               // warpgroups
-constexpr int CV_PRODUCER_WARP = 4 * CV_CONSUMERS;
-constexpr int CV_THREADS = 128 * CV_CONSUMERS + 32;
-
-struct ConvMaps {
-    CUtensorMap x;       // (C, W, H, B) fp32, box (32, 32, 16, 1), element strides (1, 2, 2, 1), swizzle 128B
-    CUtensorMap w;       // (I, O, tap) fp32, box (32, 64, 1), swizzle 128B
-};
-
-__device__ __forceinline__ void tma_load_3d_sw(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 
 __global__ void __launch_bounds__(CV_THREADS, 1)
 bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restrict__ scale, const float* __restrict__ shift,
@@ -153,22 +129,6 @@ __global__ void pack_conv_weights_kernel(const float* __restrict__ w, float* __r
     packed[i] = __uint_as_float(r);
 }
 
-typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static encode_tiled_fn conv_encode_fn() {
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        cudaFree(nullptr);
-        ctx_bound = true;
-    }
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-        return nullptr;
-    return reinterpret_cast<encode_tiled_fn>(sym);
-}
-
 int launch_pack_conv_weights(const float* w_oihw, float* packed, cudaStream_t stream) {
     const int n = CV_TAPS * CV_C * CV_C;
     pack_conv_weights_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w_oihw, packed);
@@ -187,29 +147,12 @@ int launch_bev_conv(int n_frames, int H, int W, const float* x_nhwc, const float
     if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const int Ho = (H + 2 * 3 - 7) / 2 + 1, Wo = (W + 2 * 3 - 7) / 2 + 1;
     ConvMaps maps;
-    {
-        cuuint64_t dims[4] = {CV_C, static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(n_frames)};
-        cuuint64_t strides[3] = {CV_C * 4ull, static_cast<cuuint64_t>(W) * CV_C * 4ull, static_cast<cuuint64_t>(H) * W * CV_C * 4ull};
-        cuuint32_t box[4] = {32, 2 * CV_TW, 2 * CV_TH, 1};           // traversed with stride 2 along X and Y: 16 x 8 pixels land
-        cuuint32_t estr[4] = {1, 2, 2, 1};
-        CUresult r = fn(&maps.x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x_nhwc), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (conv input) failed with CUresult %d", (int)r);
-    }
-    {
-        cuuint64_t dims[3] = {CV_C, CV_C, CV_TAPS};
-        cuuint64_t strides[2] = {CV_C * 4ull, CV_C * CV_C * 4ull};
-        cuuint32_t box[3] = {32, CV_C, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = fn(&maps.w, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(w_packed), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (conv weights) failed with CUresult %d", (int)r);
-    }
+    int rc = encode_conv_activation_map(fn, &maps.x, x_nhwc, n_frames, H, W, 2 * CV_TW, 2 * CV_TH, 2, 2, "conv input");
+    if (rc == FIERY_OK) rc = encode_conv_weight_map(fn, &maps.w, w_packed, "conv weights");
+    if (rc != FIERY_OK) return rc;
     const int smem = CV_STAGES * CV_STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
     static OncePerDevice once;
-    int rc = once.run([smem]() -> int {
+    rc = once.run([smem]() -> int {
         FIERY_CUDA_CHECK(cudaFuncSetAttribute(bev_conv7x7s2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         return FIERY_OK;
     });

@@ -116,6 +116,11 @@ int launch_warp_theta(int n_seq, int T, int cumulative, const float* flow, float
 int launch_pack_conv_weights(const float* w_oihw, float* packed, cudaStream_t stream);
 int launch_bev_conv(int n_frames, int H, int W, const float* x_nhwc, const float* w_packed, const float* scale, const float* shift,
                     int relu, float* y_nhwc, cudaStream_t stream);
+int launch_pack_conv_weights_transposed(const float* w_oihw, float* packed, cudaStream_t stream);
+int launch_bev_conv_dgrad(int n_frames, int H, int W, const float* gy_nhwc, const float* w_packed_t, float* gx_nhwc, cudaStream_t stream);
+size_t bev_conv_wgrad_workspace_bytes(int n_frames, int H, int W);
+int launch_bev_conv_wgrad(int n_frames, int H, int W, const float* x_nhwc, const float* gy_nhwc, float* dw_oihw, void* workspace,
+                          cudaStream_t stream);
 int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, int dtype, const void* weight_padded, const float* bias,
                        float* head, cudaStream_t stream);
 int vs_plan(int64_t n_rows, const int64_t* ranks, int32_t* seg, int64_t* host_n, cudaStream_t);
@@ -395,6 +400,25 @@ FIERY_API int fiery_bev_first_conv_forward(int32_t n_frames, int32_t height, int
                                            const float* scale, const float* shift, int32_t relu, float* y_nhwc, void* stream) {
     FIERY_REQUIRE(n_frames == 0 || (x_nhwc && packed_weight && y_nhwc), "bev conv: NULL pointer");
     return launch_bev_conv(n_frames, height, width, x_nhwc, packed_weight, scale, shift, relu ? 1 : 0, y_nhwc, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_bev_conv_pack_weights_transposed(const float* weight_oihw, float* packed_out, void* stream) {
+    FIERY_REQUIRE(weight_oihw && packed_out, "bev conv: NULL weight pointer");
+    return launch_pack_conv_weights_transposed(weight_oihw, packed_out, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_bev_first_conv_backward_data(int32_t n_frames, int32_t height, int32_t width, const float* grad_y_nhwc,
+                                                 const float* packed_weight_t, float* grad_x_nhwc, void* stream) {
+    return launch_bev_conv_dgrad(n_frames, height, width, grad_y_nhwc, packed_weight_t, grad_x_nhwc, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_bev_first_conv_backward_weight_workspace_bytes(int32_t n_frames, int32_t height, int32_t width) {
+    return bev_conv_wgrad_workspace_bytes(n_frames, height, width);
+}
+
+FIERY_API int fiery_bev_first_conv_backward_weight(int32_t n_frames, int32_t height, int32_t width, const float* x_nhwc,
+                                                   const float* grad_y_nhwc, float* grad_weight_oihw, void* workspace, void* stream) {
+    return launch_bev_conv_wgrad(n_frames, height, width, x_nhwc, grad_y_nhwc, grad_weight_oihw, workspace, static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API int fiery_depth_layer_forward(int32_t n_images, int32_t pixels, int32_t n_out, const void* feat, int32_t dtype,

@@ -16,6 +16,8 @@ import functools
 import importlib
 import warnings
 
+import torch
+
 from .geometry import VoxelsSumming
 from .lift import calculate_birds_eye_view_features
 from .warp import cumulative_warp_features, warp_features
@@ -105,6 +107,30 @@ def use_tensor_core_depth_layer(model):
                    f"fiery_b200: depth_layer {conv.in_channels}->{conv.out_channels} not covered by the tensor-core kernel; left as is")
         return model
     model.encoder.depth_layer = DepthLayer.from_conv(conv)
+    return model
+
+
+def use_tensor_core_first_conv(model):
+    """Replace ``model.decoder.first_conv`` (``nn.Conv2d(64, 64, 7, stride=2, padding=3, bias=False)``, fiery/models/decoder.py:11) of
+    a ``Fiery`` instance by ``fiery_b200.bev_conv.FirstConv(bn=None)`` sharing the same Parameter (``state_dict`` keys unchanged): the
+    forward and both gradients run on the tensor-core kernels, on the channel-last layout the lift can emit.  ``bn1`` and ``relu``
+    stay the reference's modules, so batch statistics train as before.  Returns the model; a second call does nothing, and a layer
+    the kernels do not cover (e.g. ``in_channels != 64`` when EXTRA_IN_CHANNELS widens the temporal model) is left alone with one
+    warning."""
+    from .bev_conv import FirstConv
+    conv = model.decoder.first_conv
+    if isinstance(conv, FirstConv):
+        return model
+    covered = (isinstance(conv, torch.nn.Conv2d) and conv.in_channels == 64 and conv.out_channels == 64 and conv.kernel_size == (7, 7)
+               and conv.stride == (2, 2) and conv.padding == (3, 3) and conv.dilation == (1, 1) and conv.groups == 1
+               and conv.bias is None and conv.padding_mode == "zeros")
+    if not covered:
+        desc = (f"{conv.in_channels}->{conv.out_channels} k{conv.kernel_size} s{conv.stride}" if isinstance(conv, torch.nn.Conv2d)
+                else type(conv).__name__)
+        _warn_once(("first_conv", desc), f"fiery_b200: first_conv {desc} not covered by the tensor-core kernels (they are built for "
+                                         "Conv2d(64, 64, 7, stride=2, padding=3, bias=False)); left as is")
+        return model
+    model.decoder.first_conv = FirstConv.from_conv(conv)
     return model
 
 

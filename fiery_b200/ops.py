@@ -106,3 +106,75 @@ def _backward(ctx, grad_bev, _grad_plan):
 lift_splat.register_autograd(_backward, setup_context=_setup_context)
 # AMP (baseline.yml PRECISION 16): the reference's softmax / outer product run in fp32 under autocast -> so does the operator
 torch.library.register_autocast("fiery_b200::lift_splat", "cuda", torch.float32)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# The first BEV convolution (Decoder.first_conv, fiery/models/decoder.py:11,59) as dispatcher operators:
+# ``torch.ops.fiery_b200.first_conv`` / ``first_conv_backward`` (fiery_b200/bev_conv.py; kernels in csrc/bev_conv*.cu).
+# Autocast: the operator runs in fp32 (TF32 tensor-core operands, fp32 accumulation) -- under AMP the reference runs this
+# convolution in fp16, so an AMP step computes it at a higher precision than the reference does.
+# ------------------------------------------------------------------------------------------------------------------------------
+def _conv_out(n: int) -> int:
+    return (n - 1) // 2 + 1
+
+
+@torch.library.custom_op("fiery_b200::first_conv", mutates_args=(), device_types="cuda")
+def first_conv(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """Conv2d(64, 64, 7, stride 2, padding 3, no bias): x (B, 64, H, W), any layout -> (B, 64, Ho, Wo) fp32 with channels-last
+    strides.  The weight's TF32 packs are made at most once per weight version (``bev_conv.packed_weights``)."""
+    from .bev_conv import first_conv_forward, packed_weights
+    return first_conv_forward(x, packed_weights(weight)[0])
+
+
+@first_conv.register_fake
+def _(x, weight):
+    B, _, H, W = x.shape
+    return x.new_empty((B, _conv_out(H), _conv_out(W), 64), dtype=torch.float32).permute(0, 3, 1, 2)
+
+
+@torch.library.custom_op("fiery_b200::first_conv_backward", mutates_args=(), device_types="cuda")
+def first_conv_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, need_input: bool,
+                        need_weight: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(grad_x, grad_weight) of ``first_conv``; a gradient that is not asked for is not computed and comes back as an empty tensor.
+    grad_y arriving in another layout (e.g. NCHW-contiguous) is converted to channels-last fp32 once, shared by both gradients.
+    grad_x: x's shape and dtype with channels-last strides (so a ``LiftSplat(output_layout="channels_last")`` upstream takes its
+    NHWC backward route); grad_weight: the weight's shape and dtype, bit-reproducible (no atomics)."""
+    from .bev_conv import _channels_last_f32, first_conv_backward_data, first_conv_backward_weight, packed_weights
+    g = _channels_last_f32(grad_y)
+    H, W = x.shape[2], x.shape[3]
+    grad_x = grad_w = x.new_empty((0,))
+    if need_input:
+        grad_x = first_conv_backward_data(g, packed_weights(weight, transposed=True)[1], H, W)
+        if grad_x.dtype != x.dtype:
+            grad_x = grad_x.to(x.dtype)
+    if need_weight:
+        grad_w = first_conv_backward_weight(x, g)
+        if grad_w.dtype != weight.dtype:
+            grad_w = grad_w.to(weight.dtype)
+    return grad_x, grad_w
+
+
+@first_conv_backward.register_fake
+def _(grad_y, x, weight, need_input, need_weight):
+    B, C, H, W = x.shape
+    grad_x = x.new_empty((B, H, W, C)).permute(0, 3, 1, 2) if need_input else x.new_empty((0,))
+    grad_w = weight.new_empty(weight.shape) if need_weight else x.new_empty((0,))
+    return grad_x, grad_w
+
+
+def _first_conv_setup_context(ctx, inputs, output):
+    x, weight = inputs
+    ctx.save_for_backward(x, weight)
+
+
+def _first_conv_backward(ctx, grad_y):
+    x, weight = ctx.saved_tensors
+    need_input, need_weight = bool(ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1])
+    if not (need_input or need_weight):
+        return None, None
+    grad_x, grad_w = torch.ops.fiery_b200.first_conv_backward(grad_y, x, weight, need_input, need_weight)
+    return (grad_x if need_input else None), (grad_w if need_weight else None)
+
+
+first_conv.register_autograd(_first_conv_backward, setup_context=_first_conv_setup_context)
+torch.library.register_autocast("fiery_b200::first_conv", "cuda", torch.float32)

@@ -20,6 +20,8 @@
  *       replaces Encoder.depth_layer (the head tensor's producer)  fiery/models/encoder.py:36,96   [SURVEY.md section 8f, next-3]
  *   fiery_bev_first_conv_forward
  *       replaces Decoder.first_conv (+ bn1 + relu in eval mode)  fiery/models/decoder.py:11,59-61   [SURVEY.md section 8f, next-2]
+ *   fiery_bev_first_conv_backward_data / _weight
+ *       the backward of Decoder.first_conv (what cuDNN runs for the reference's training step)
  *   fiery_warp_features_forward / _backward, fiery_warp_theta
  *       replace affine_grid + grid_sample inside warp_features  fiery/utils/geometry.py:219-220 (called from
  *       cumulative_warp_features geometry.py:225-253, call site fiery.py:143)   [SURVEY.md section 8f, next-1]
@@ -267,6 +269,31 @@ FIERY_API int fiery_warp_theta(int32_t n_sequences, int32_t T, int32_t cumulativ
 FIERY_API int fiery_bev_conv_pack_weights(const float* weight_oihw, float* packed_out, void* stream);
 FIERY_API int fiery_bev_first_conv_forward(int32_t n_frames, int32_t height, int32_t width, const float* x_nhwc, const float* packed_weight,
                                            const float* scale, const float* shift, int32_t relu, float* y_nhwc, void* stream);
+
+/*
+ * Backward of fiery_bev_first_conv_forward without the optional affine / relu (wgmma, TF32 operands, fp32 accumulation); the
+ * same shapes: x_nhwc / grad_x_nhwc (n_frames, height, width, 64) fp32, grad_y_nhwc (n_frames, Ho, Wo, 64) fp32 with
+ * Ho = (height - 1) / 2 + 1, Wo likewise.  Pointers 16-byte aligned.
+ *
+ * fiery_bev_conv_pack_weights_transposed: the module's (64, 64, 7, 7) weight -> (49, 64, 64) = (tap r*7+s, in, out), rounded to
+ * TF32 (nearest, ties away).
+ * fiery_bev_first_conv_backward_data: grad_x = the input gradient (the transposed convolution of grad_y), fully overwritten (no
+ * zero fill needed).  Each element is the fp32 accumulation of its taps' products in a fixed order (no atomics): bit-reproducible.
+ * fiery_bev_first_conv_backward_weight: grad_weight_oihw (64, 64, 7, 7) fp32 = the weight gradient, fully overwritten (zeros when
+ * n_frames == 0).  workspace: fiery_bev_first_conv_backward_weight_workspace_bytes(n_frames, height, width) bytes (0 when
+ * n_frames == 0 or the shape is invalid; at most 18 x 49 x 64 x 64 x 4 bytes = 13.8 MiB); its contents on entry are irrelevant.
+ * Summation order: the output pixels are cut into 16 x 8 tiles, numbered frame by frame in row-major tile order, and the tiles
+ * into c = min(tiles, 18) chunks, chunk k holding tiles [k * tiles / c, (k + 1) * tiles / c).  A chunk's partial is the tensor
+ * core's fp32 accumulation over its tiles in ascending order, 8 pixels per MMA; grad_weight is the fp32 sum of the c partials in
+ * ascending chunk order.  The order depends on (n_frames, height, width) only, not on the device or the stream, so the result is
+ * bit-reproducible and the call can be captured in a CUDA graph.  No host synchronisation.
+ */
+FIERY_API int fiery_bev_conv_pack_weights_transposed(const float* weight_oihw, float* packed_out, void* stream);
+FIERY_API int fiery_bev_first_conv_backward_data(int32_t n_frames, int32_t height, int32_t width, const float* grad_y_nhwc,
+                                                 const float* packed_weight_t, float* grad_x_nhwc, void* stream);
+FIERY_API size_t fiery_bev_first_conv_backward_weight_workspace_bytes(int32_t n_frames, int32_t height, int32_t width);
+FIERY_API int fiery_bev_first_conv_backward_weight(int32_t n_frames, int32_t height, int32_t width, const float* x_nhwc,
+                                                   const float* grad_y_nhwc, float* grad_weight_oihw, void* workspace, void* stream);
 
 /*
  * Encoder.depth_layer on the tensor cores -- the 1x1 convolution 128 -> D + C that produces the head tensor
