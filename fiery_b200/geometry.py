@@ -77,6 +77,7 @@ def z_valid_interval(resolution_z: float, dim_z: int) -> Tuple[np.float32, np.fl
     return np.float32(lo), np.float32(hi)
 
 
+@torch.compiler.disable          # the raw handle exists on eager streams only: a C-ABI call breaks a torch.compile graph here
 def _stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 

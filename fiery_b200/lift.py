@@ -40,6 +40,12 @@ def _plan_touched_offset(n_frames: int, n_cameras: int, feat_w: int) -> int:
     return n_frames * n_cameras * ((feat_w + 3) // 4) * _PLAN_TILE_BYTES
 
 
+def _plan_bytes(n_frames, n_cameras, feat_w: int, pillars: int):
+    """fiery_lift_plan_bytes: the tile records, then the touched maps rounded up to 128 bytes (0 for 0 frames).  Integer arithmetic
+    only, so ``n_frames`` / ``n_cameras`` may be SymInts (the operator's fake implementation sizes the plan it returns with it)."""
+    return _plan_touched_offset(n_frames, n_cameras, feat_w) + (n_frames * pillars + 127) // 128 * 128
+
+
 _TORCH_TO_DTYPE = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16}
 
 # Half-precision head tensors (AMP, baseline.yml PRECISION 16): False (default) = the tensor is widened to fp32 on the device
@@ -164,6 +170,7 @@ class LiftSplat(nn.Module):
         return tuple((p.data_ptr(), p._version, str(p.device), tuple(p.shape))
                      for p in (self.frustum, self.bev_resolution, self.bev_start_position, self.bev_dimension))
 
+    @torch.compiler.disable      # host bookkeeping (parameters read back with numpy): runs eagerly, never compiled into a graph
     def _constants(self, device: torch.device):
         c = self._consts
         key = self._param_key()
@@ -314,6 +321,8 @@ class LiftSplat(nn.Module):
         pillars that receive a point.  Diagnostic (bench.py uses it for the per-kernel algorithmic bytes); synchronises."""
         c = self._constants(plan.device)
         X, Y, _ = c["dim"]
+        if plan.numel() != max(1, _plan_bytes(n_frames, n_cameras, c["w"], X * Y)):
+            raise ValueError(f"plan holds {plan.numel()} bytes, not those of {n_frames} frames of {n_cameras} cameras")
         t0 = _plan_touched_offset(n_frames, n_cameras, c["w"])
         records = plan[:t0].view(t0 // _PLAN_TILE_BYTES, _PLAN_TILE_BYTES)
         counts = records[:, _PLAN_OFF_COUNTS:_PLAN_OFF_COUNTS + 8].contiguous().view(torch.int32)

@@ -20,15 +20,17 @@ from typing import Optional, Tuple
 
 import torch
 
+from .lift import _plan_bytes
 from .warp import _warp_adjoint
 
-_REGISTRY = {}          # handle -> (weakref to the LiftSplat module, (C, X, Y, channels_last) as python values for the fake impl)
+_REGISTRY = {}          # handle -> (weakref to the LiftSplat module, (C, X, Y, feat_w, channels_last) as python values for the fakes)
 
 
 def register_module(module, device: torch.device) -> int:
     handle = id(module)
-    X, Y, _ = module._constants(device)["dim"]                      # cached host-side integers: no device sync here
-    meta = (int(module.encoder_out_channels), int(X), int(Y), module.output_layout == "channels_last")
+    c = module._constants(device)                                    # cached host-side integers: no device sync here
+    X, Y, _ = c["dim"]
+    meta = (int(module.encoder_out_channels), int(X), int(Y), int(c["w"]), module.output_layout == "channels_last")
     entry = _REGISTRY.get(handle)
     if entry is None or entry[0]() is not module or entry[1] != meta:
         _REGISTRY[handle] = (weakref.ref(module, lambda _r, h=handle: _REGISTRY.pop(h, None)), meta)
@@ -64,11 +66,15 @@ def lift_splat(head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.T
 
 @lift_splat.register_fake
 def _(head, intrinsics, extrinsics, plan, handle, make_plan, theta=None, copy_mask=None):
-    C, X, Y, channels_last = _REGISTRY[handle][1]                   # python values only: nothing here touches a real tensor
-    B = intrinsics.shape[0]
+    # python values only: nothing here touches a real tensor.  Under dynamic shapes the handle may arrive as a SymInt: int()
+    # specialises the graph on it (it names one module)
+    C, X, Y, feat_w, channels_last = _REGISTRY[int(handle)][1]
+    B, n = intrinsics.shape[:2]
     bev = head.new_empty((B, X, Y, C), dtype=torch.float32).permute(0, 3, 1, 2) if channels_last and theta is None \
         else head.new_empty((B, C, X, Y), dtype=torch.float32)
-    return bev, head.new_empty((0,), dtype=torch.uint8)
+    # the plan made here (fiery_lift_plan_bytes bytes; 0 for B' = 0, where the real op makes none), else an empty tensor
+    plan_bytes = _plan_bytes(B, n, feat_w, X * Y) if plan is None and make_plan else 0
+    return bev, head.new_empty((plan_bytes,), dtype=torch.uint8)
 
 
 @torch.library.custom_op("fiery_b200::lift_splat_backward", mutates_args=(), device_types="cuda")
@@ -87,7 +93,7 @@ def lift_splat_backward(head: torch.Tensor, intrinsics: torch.Tensor, extrinsics
 
 @lift_splat_backward.register_fake
 def _(head, intrinsics, extrinsics, grad_bev, plan, handle, theta=None, copy_mask=None):
-    return torch.empty_like(head)
+    return head.new_empty(head.shape)                                # NCHW-contiguous whatever the head's layout, like the op
 
 
 def _setup_context(ctx, inputs, output):
@@ -142,7 +148,7 @@ def first_conv_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Ten
     from .bev_conv import _channels_last_f32, first_conv_backward_data, first_conv_backward_weight, packed_weights
     g = _channels_last_f32(grad_y)
     H, W = x.shape[2], x.shape[3]
-    grad_x = grad_w = x.new_empty((0,))
+    grad_x, grad_w = x.new_empty((0,)), x.new_empty((0,))         # two tensors: an operator's outputs may not alias each other
     if need_input:
         grad_x = first_conv_backward_data(g, packed_weights(weight, transposed=True)[1], H, W)
         if grad_x.dtype != x.dtype:
