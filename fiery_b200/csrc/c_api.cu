@@ -92,23 +92,21 @@ int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels
     return FIERY_OK;
 }
 
-// launchers defined next to their kernels
-int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* scratch, const void* plan,
-                        const float* warp_theta, const unsigned char* warp_copy,
-                        cudaStream_t);
-int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* workspace, const void* plan,
-                            const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream);
-size_t lift_det_workspace_bytes(const LiftParams& P);
-int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
-int lift_chunk_frames(const LiftParams& P);
-size_t lift_scratch_bytes(const LiftParams& P);
-void lift_set_max_chunk_frames(int n);
-void lift_set_timer(LaunchTimer* t);
-int lift_forward_launches(const LiftParams& P);
-size_t lift_backward_relayout_bytes(const LiftParams& P);
-int launch_lift_backward(const LiftParams& P, const void* head, int head_dtype, float* workspace, const void* plan, cudaStream_t);
-int launch_point_indices(const LiftParams& P, int64_t* idx_out, uint8_t* valid_out, int32_t* pillar_out, cudaStream_t);
-int launch_compose(int n, const float* K, const float* E, float* combined, float* translation, cudaStream_t);
+// Head shapes the lift's kernels are built for.  The plan needs rows and depth bins that fit a tile record; the forward and backward
+// tile kernels also need 64 channels and a 16-byte row pitch for their tensor maps.  The entry points check the shape once, after
+// their 0-frame return; the launchers behind them rely on it.
+int check_lift_geometry(const LiftParams& P) {
+    FIERY_REQUIRE(P.hh >= 1 && P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
+    FIERY_REQUIRE(P.D >= 1 && P.D <= DPAD, "depth_bins=%d not supported by this build (1..48)", P.D);
+    return FIERY_OK;
+}
+static int check_lift_tile_shape(const LiftParams& P) {
+    FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
+    FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
+    return check_lift_geometry(P);
+}
+
+// launchers defined next to their kernels (the lift's: lift_plan.cuh)
 int launch_warp(int forward, int n_maps, int C, int H, int W, const float* a, long long a_stride, const float* theta,
                 const unsigned char* copy_mask, float* b, long long b_stride, int nearest, cudaStream_t stream);
 int launch_warp_theta(int n_seq, int T, int cumulative, const float* flow, float ex, float ey, float* theta,
@@ -131,6 +129,18 @@ size_t vs_det_workspace_bytes(int64_t n_rows, int channels);
 int vs_forward_det(int64_t n_rows, int channels, int64_t feat_stride, const float* feats, const int64_t* coords, const int32_t* seg,
                    float* sums, int64_t* coords_out, float* edge, cudaStream_t);
 
+// shape-only parameters for the size queries (no pointers); false for a descriptor they answer 0 for
+static bool shape_params(const fiery_lift_desc_t* d, LiftParams& P) {
+    if (!d || d->n_frames < 0 || d->n_cameras < 1 || d->feat_w < 1 || d->bev_x < 1 || d->bev_y < 1) return false;
+    P = LiftParams{};
+    P.n_frames = d->n_frames; P.n_cameras = d->n_cameras; P.C = d->channels; P.D = d->depth_bins;
+    P.hh = d->feat_h; P.ww = d->feat_w;
+    P.n_wtiles = (d->feat_w + WT - 1) / WT;
+    P.bev_layout = d->bev_layout;
+    P.pillars = static_cast<long long>(d->bev_x) * d->bev_y;
+    return true;
+}
+
 static int make_params(const fiery_lift_desc_t* d, const float* calib_a, const float* calib_b, const float* fu,
                        const float* fv, const float* fd, LiftParams& P) {
     FIERY_REQUIRE(d != nullptr, "desc is NULL");
@@ -146,18 +156,33 @@ static int make_params(const fiery_lift_desc_t* d, const float* calib_a, const f
     FIERY_REQUIRE(d->n_frames == 0 || (calib_a && calib_b), "calibration pointer is NULL");
     FIERY_REQUIRE(fu && fv && fd, "frustum pointer is NULL");
     for (int a = 0; a < 3; ++a) FIERY_REQUIRE(d->bev_resolution[a] > 0.f, "bev_resolution[%d] must be positive", a);
-    P.n_frames = d->n_frames; P.n_cameras = d->n_cameras; P.frame0 = 0;
-    P.D = d->depth_bins; P.C = d->channels; P.hh = d->feat_h; P.ww = d->feat_w;
-    P.n_wtiles = (d->feat_w + WT - 1) / WT;
+    shape_params(d, P);                              // accepts every descriptor that passed the checks above
     P.use_depth = d->use_depth_distribution ? 1 : 0;
     P.head_channels = d->channels + (P.use_depth ? d->depth_bins : 0);
     P.calib_mode = d->calib_mode;
     P.calib_a = calib_a; P.calib_b = calib_b; P.fu = fu; P.fv = fv; P.fd = fd;
-    P.accum = nullptr; P.touched = nullptr; P.plan_tiles = nullptr; P.grad_bev = nullptr; P.grad_head = nullptr; P.head_f16 = nullptr;
-    P.bev_layout = d->bev_layout;
-    P.pillars = static_cast<long long>(d->bev_x) * d->bev_y;
     P.grid = make_grid_params(*d);
     return FIERY_OK;
+}
+
+// The body of the three forward entry points: `launch` is the default or the deterministic launcher, `buffer` its scratch or
+// workspace; `warped` (fiery_lift_forward_warped) requires theta and copy_mask, the others take both or neither.
+static int lift_forward(decltype(&launch_lift_forward) launch, const fiery_lift_desc_t* desc, const void* head, const float* calib_a,
+                        const float* calib_b, const float* fu, const float* fv, const float* fd, float* bev_out, void* buffer,
+                        const void* plan, const float* theta, const uint8_t* copy_mask, bool warped, void* stream) {
+    LiftParams P;
+    int rc = make_params(desc, calib_a, calib_b, fu, fv, fd, P);
+    if (rc != FIERY_OK) return rc;
+    if (P.n_frames == 0) return FIERY_OK;
+    if (warped) FIERY_REQUIRE(head && bev_out && theta && copy_mask, "head / bev_out / theta / copy_mask is NULL");
+    FIERY_REQUIRE(head && bev_out, "head / bev_out is NULL");
+    FIERY_REQUIRE((theta == nullptr) == (copy_mask == nullptr), "theta and copy_mask go together (the warped lift) or are both NULL");
+    FIERY_REQUIRE(!theta || desc->bev_layout == FIERY_BEV_NCHW, "the warped lift writes the NCHW layout only");
+    FIERY_REQUIRE(desc->head_dtype == FIERY_DTYPE_F32 || desc->head_dtype == FIERY_DTYPE_F16, "head dtype %d not supported (fp32 / fp16)",
+                  desc->head_dtype);
+    rc = check_lift_tile_shape(P);
+    if (rc != FIERY_OK) return rc;
+    return launch(P, head, desc->head_dtype, bev_out, buffer, plan, theta, copy_mask, static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace fiery
@@ -169,18 +194,6 @@ extern "C" {
 FIERY_API int fiery_abi_version(void) { return FIERY_B200_ABI_VERSION; }
 
 FIERY_API const char* fiery_last_error(void) { return g_last_error; }
-
-// shape-only parameters for the size queries (no pointers)
-static bool shape_params(const fiery_lift_desc_t* d, LiftParams& P) {
-    if (!d || d->n_frames < 0 || d->n_cameras < 1 || d->feat_w < 1 || d->bev_x < 1 || d->bev_y < 1) return false;
-    P = LiftParams{};
-    P.n_frames = d->n_frames; P.n_cameras = d->n_cameras; P.C = d->channels; P.D = d->depth_bins;
-    P.hh = d->feat_h; P.ww = d->feat_w;
-    P.n_wtiles = (d->feat_w + WT - 1) / WT;
-    P.bev_layout = d->bev_layout;
-    P.pillars = static_cast<long long>(d->bev_x) * d->bev_y;
-    return true;
-}
 
 FIERY_API size_t fiery_lift_plan_bytes(const fiery_lift_desc_t* d) {
     LiftParams P;
@@ -225,24 +238,15 @@ FIERY_API size_t fiery_lift_workspace_bytes(const fiery_lift_desc_t* d) {
 FIERY_API int fiery_lift_forward(const fiery_lift_desc_t* desc, const void* head, const float* calib_a, const float* calib_b,
                        const float* frustum_u, const float* frustum_v, const float* frustum_d, float* bev_out,
                        void* scratch, const void* plan, void* stream) {
-    LiftParams P;
-    int rc = make_params(desc, calib_a, calib_b, frustum_u, frustum_v, frustum_d, P);
-    if (rc != FIERY_OK) return rc;
-    if (P.n_frames == 0) return FIERY_OK;
-    FIERY_REQUIRE(head && bev_out, "head / bev_out is NULL");
-    return launch_lift_forward(P, head, desc->head_dtype, bev_out, scratch, plan, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    return lift_forward(launch_lift_forward, desc, head, calib_a, calib_b, frustum_u, frustum_v, frustum_d, bev_out, scratch, plan,
+                        nullptr, nullptr, false, stream);
 }
 
 FIERY_API int fiery_lift_forward_warped(const fiery_lift_desc_t* desc, const void* head, const float* calib_a, const float* calib_b,
                                         const float* frustum_u, const float* frustum_v, const float* frustum_d, float* bev_out,
                                         void* scratch, const void* plan, const float* theta, const uint8_t* copy_mask, void* stream) {
-    LiftParams P;
-    int rc = make_params(desc, calib_a, calib_b, frustum_u, frustum_v, frustum_d, P);
-    if (rc != FIERY_OK) return rc;
-    if (P.n_frames == 0) return FIERY_OK;
-    FIERY_REQUIRE(head && bev_out && theta && copy_mask, "head / bev_out / theta / copy_mask is NULL");
-    FIERY_REQUIRE(desc->bev_layout == FIERY_BEV_NCHW, "the warped lift writes the NCHW layout only");
-    return launch_lift_forward(P, head, desc->head_dtype, bev_out, scratch, plan, theta, copy_mask, static_cast<cudaStream_t>(stream));
+    return lift_forward(launch_lift_forward, desc, head, calib_a, calib_b, frustum_u, frustum_v, frustum_d, bev_out, scratch, plan,
+                        theta, copy_mask, true, stream);
 }
 
 FIERY_API size_t fiery_lift_deterministic_workspace_bytes(const fiery_lift_desc_t* d) {
@@ -255,14 +259,8 @@ FIERY_API int fiery_lift_forward_deterministic(const fiery_lift_desc_t* desc, co
                                                const float* calib_b, const float* frustum_u, const float* frustum_v,
                                                const float* frustum_d, float* bev_out, void* workspace, const void* plan,
                                                const float* theta, const uint8_t* copy_mask, void* stream) {
-    LiftParams P;
-    int rc = make_params(desc, calib_a, calib_b, frustum_u, frustum_v, frustum_d, P);
-    if (rc != FIERY_OK) return rc;
-    if (P.n_frames == 0) return FIERY_OK;
-    FIERY_REQUIRE(head && bev_out, "head / bev_out is NULL");
-    FIERY_REQUIRE((theta == nullptr) == (copy_mask == nullptr), "theta and copy_mask go together (the warped lift) or are both NULL");
-    FIERY_REQUIRE(!theta || desc->bev_layout == FIERY_BEV_NCHW, "the warped lift writes the NCHW layout only");
-    return launch_lift_forward_det(P, head, desc->head_dtype, bev_out, workspace, plan, theta, copy_mask, static_cast<cudaStream_t>(stream));
+    return lift_forward(launch_lift_forward_det, desc, head, calib_a, calib_b, frustum_u, frustum_v, frustum_d, bev_out, workspace,
+                        plan, theta, copy_mask, false, stream);
 }
 
 FIERY_API int fiery_lift_forward_timed(const fiery_lift_desc_t* desc, const void* head, const float* calib_a, const float* calib_b,
@@ -300,7 +298,10 @@ FIERY_API int fiery_lift_backward(const fiery_lift_desc_t* desc, const void* hea
     P.grad_head = static_cast<float*>(grad_head);
     FIERY_REQUIRE(workspace != nullptr || (desc->bev_layout == FIERY_BEV_NHWC && plan != nullptr),
                   "backward needs the workspace of fiery_lift_workspace_bytes() (NCHW grad_bev re-layout and/or the geometry plan)");
-    return launch_lift_backward(P, head, desc->head_dtype, workspace, plan, static_cast<cudaStream_t>(stream));
+    FIERY_REQUIRE(desc->head_dtype == FIERY_DTYPE_F32, "head dtype %d not supported by this build (fp32 only)", desc->head_dtype);
+    rc = check_lift_tile_shape(P);
+    if (rc != FIERY_OK) return rc;
+    return launch_lift_backward(P, head, workspace, plan, static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API int fiery_lift_point_indices(const fiery_lift_desc_t* desc, const float* calib_a, const float* calib_b,

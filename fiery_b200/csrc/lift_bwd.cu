@@ -308,18 +308,11 @@ nchw_to_nhwc_kernel(const float* __restrict__ src, float* __restrict__ dst, cons
     }
 }
 
-int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
-
 size_t lift_backward_relayout_bytes(const LiftParams& P) {
     return P.bev_layout == FIERY_BEV_NCHW ? static_cast<size_t>(P.n_frames) * P.pillars * P.C * sizeof(float) : 0;
 }
 
-int launch_lift_backward(const LiftParams& P, const void* head, int head_dtype, float* workspace, const void* plan, cudaStream_t stream) {
-    FIERY_REQUIRE(head_dtype == FIERY_DTYPE_F32, "head dtype %d not supported by this build (fp32 only)", head_dtype);
-    FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
-    FIERY_REQUIRE(P.D >= 1 && P.D <= DPAD, "depth_bins=%d not supported by this build (1..48)", P.D);
-    FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
-    FIERY_REQUIRE(P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
+int launch_lift_backward(const LiftParams& P, const void* head, float* workspace, const void* plan, cudaStream_t stream) {
     HeadMapsCols hm, gm;
     int rc = encode_head_maps_cols(&hm, head, P, BW_CH);
     if (rc != FIERY_OK) return rc;

@@ -302,7 +302,7 @@ __global__ void compose_calibration_kernel(int n, const float* __restrict__ K, c
 static std::atomic<int> g_max_chunk_frames{0};       // fiery_lift_set_max_chunk_frames (test hook: forces the multi-pass path)
 void lift_set_max_chunk_frames(int n) { g_max_chunk_frames.store(n > 0 ? n : 0); }
 
-int lift_chunk_frames(const LiftParams& P) {
+static int lift_chunk_frames(const LiftParams& P) {
     const long long per_frame = P.pillars * P.C * 4 + P.pillars;
     long long c = (1ll << 30) / (per_frame > 0 ? per_frame : 1);
     const int forced = g_max_chunk_frames.load();
@@ -310,9 +310,6 @@ int lift_chunk_frames(const LiftParams& P) {
     if (c > P.n_frames) c = P.n_frames;
     return static_cast<int>(c < 1 ? 1 : c);
 }
-
-int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream);
-int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels, int n_frames, int box_pillars);
 
 // Side streams and fork/join events of the forward chains: created once per host thread and device (thread_local, so concurrent
 // callers never share or race on them), reused by every call -- nothing is created or destroyed on the launch path.
@@ -430,19 +427,45 @@ static inline void timer_end(cudaStream_t st) {
     }
 }
 
+// The NCHW layout pass of both forward paths: the warped pass when a warp is given, else the TMA pass when the output has a 16-byte
+// row pitch, else the fallback pass.
+struct LayoutPass {
+    const float* warp_theta;
+    const unsigned char* warp_copy;
+    bool tma;                                       // the TMA pass's output map needs a 16-byte row pitch
+    CUtensorMap bev_map;
+};
+static int prepare_layout_pass(LayoutPass* L, const LiftParams& P, float* bev_out, const float* warp_theta,
+                               const unsigned char* warp_copy) {
+    *L = LayoutPass{warp_theta, warp_copy, P.pillars % 4 == 0, {}};
+    if (P.bev_layout != FIERY_BEV_NCHW || !L->tma || warp_theta) return FIERY_OK;
+    return encode_bev_map(&L->bev_map, bev_out, P.pillars, P.C, P.n_frames, FT_P);
+}
+
+// output frames frame0 .. frame0 + n_frames - 1 from their accumulator rows and marks
+static void launch_layout_pass(const LayoutPass& L, const LiftParams& P, float* accum, unsigned char* marks, float* bev_out, int frame0,
+                               int n_frames, int clear_marks, int last_in_lane, cudaStream_t st) {
+    if (L.warp_theta) {
+        const int tpf = static_cast<int>((P.pillars + FW_P - 1) / FW_P);
+        finalize_warp_kernel<<<static_cast<unsigned>(tpf) * n_frames, FW_THREADS, 0, st>>>(
+            accum, marks, bev_out, P.pillars, P.grid.X, P.grid.Y, tpf, frame0, L.warp_theta, L.warp_copy);
+    } else if (L.tma) {
+        const int tpf = static_cast<int>((P.pillars + FT_P - 1) / FT_P);
+        finalize_tma_kernel<<<static_cast<unsigned>(tpf) * n_frames, FT_THREADS, 0, st>>>(
+            L.bev_map, accum, marks, P.pillars, tpf, frame0, clear_marks, last_in_lane);
+    } else {
+        const int bpf = static_cast<int>((P.pillars + FIN_THREADS - 1) / FIN_THREADS);
+        finalize_nchw_kernel<<<static_cast<unsigned>(bpf) * n_frames, FIN_THREADS, 0, st>>>(
+            accum, marks, bev_out + static_cast<size_t>(frame0) * P.C * P.pillars, P.pillars, bpf, clear_marks);
+    }
+}
+
 // warp_theta != NULL: the layout pass samples every frame under its (2, 3) affine map (frames flagged in warp_copy pass through) --
 // the lift followed by cumulative_warp_features in one chain; NCHW output only
 int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* scratch, const void* plan,
                         const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream) {
-    FIERY_REQUIRE(head_dtype == FIERY_DTYPE_F32 || head_dtype == FIERY_DTYPE_F16, "head dtype %d not supported (fp32 / fp16)", head_dtype);
-    FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
-    FIERY_REQUIRE(P.D >= 1 && P.D <= 48, "depth_bins=%d not supported by this build (1..48)", P.D);
-    FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
-    FIERY_REQUIRE(P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
     const bool nchw = P.bev_layout == FIERY_BEV_NCHW;
-    FIERY_REQUIRE(!warp_theta || nchw, "the warped lift writes the NCHW layout only");
     FIERY_REQUIRE(scratch != nullptr || !nchw, "NCHW output needs the zeroed scratch buffer of fiery_lift_scratch_bytes()");
-    int rc = FIERY_OK;
     LiftParams Q = P;
     Q.head_f16 = head_dtype == FIERY_DTYPE_F16 ? head : nullptr;
     // lift into a channel-last accumulator (NHWC: the caller's zero-filled output itself), then the layout pass for NCHW; several
@@ -451,12 +474,9 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
     float* accum = static_cast<float*>(scratch);    // [accumulator floats of the lanes][one mark byte per pillar]
     unsigned char* scratch_marks =
         nchw ? reinterpret_cast<unsigned char*>(accum + static_cast<size_t>(scratch_frames(P)) * P.pillars * P.C) : nullptr;
-    const bool tma_pass = P.pillars % 4 == 0;      // the output map needs a 16-byte row pitch
-    CUtensorMap bev_map;
-    if (nchw && tma_pass && !warp_theta) {
-        rc = encode_bev_map(&bev_map, bev_out, P.pillars, P.C, P.n_frames, FT_P);
-        if (rc != FIERY_OK) return rc;
-    }
+    LayoutPass pass;
+    int rc = prepare_layout_pass(&pass, P, bev_out, warp_theta, warp_copy);
+    if (rc != FIERY_OK) return rc;
     ChainResources* res = nullptr;
     for (int f0 = 0; f0 < P.n_frames; f0 += chunk) {
         const int nf = (P.n_frames - f0 < chunk) ? P.n_frames - f0 : chunk;
@@ -498,21 +518,11 @@ int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, f
             if (rc != FIERY_OK) return rc;
             if (nchw) {
                 timer_begin(st, 2);
+                launch_layout_pass(pass, P, Q.accum, marks, bev_out, Q.frame0, Q.n_frames, plan ? 0 : 1, last_in_lane ? 1 : 0, st);
                 if (warp_theta) {
-                    const int tpf = static_cast<int>((P.pillars + FW_P - 1) / FW_P);
-                    finalize_warp_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FW_THREADS, 0, st>>>(
-                        Q.accum, marks, bev_out, P.pillars, P.grid.X, P.grid.Y, tpf, Q.frame0, warp_theta, warp_copy);
                     const long long n = P.pillars * Q.n_frames;
                     clear_touched_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(Q.accum, marks, n, plan ? 0 : 1,
                                                                                                  last_in_lane ? 1 : 0);
-                } else if (tma_pass) {
-                    const int tpf = static_cast<int>((P.pillars + FT_P - 1) / FT_P);
-                    finalize_tma_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FT_THREADS, 0, st>>>(
-                        bev_map, Q.accum, marks, P.pillars, tpf, Q.frame0, plan ? 0 : 1, last_in_lane ? 1 : 0);
-                } else {
-                    const int bpf = static_cast<int>((P.pillars + FIN_THREADS - 1) / FIN_THREADS);
-                    finalize_nchw_kernel<<<static_cast<unsigned>(bpf) * Q.n_frames, FIN_THREADS, 0, st>>>(
-                        Q.accum, marks, bev_out + static_cast<size_t>(Q.frame0) * P.C * P.pillars, P.pillars, bpf, plan ? 0 : 1);
                 }
                 timer_end(st);
                 FIERY_CUDA_CHECK(cudaGetLastError());
@@ -561,20 +571,9 @@ static DetLayout det_layout(const LiftParams& P) {
 
 size_t lift_det_workspace_bytes(const LiftParams& P) { return P.n_frames > 0 ? det_layout(P).total : 0; }
 
-int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t stream);
-int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
-int launch_det_reduce(const LiftParams& P, int nf, const unsigned char* tiles, const float* partials, int* start, int* cursor,
-                      int* lists, float* out, int zero_empty, cudaStream_t stream);
-
 int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* workspace, const void* plan,
                             const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream) {
-    FIERY_REQUIRE(head_dtype == FIERY_DTYPE_F32 || head_dtype == FIERY_DTYPE_F16, "head dtype %d not supported (fp32 / fp16)", head_dtype);
-    FIERY_REQUIRE(P.C == 64, "channels=%d not supported by this build (C must be 64)", P.C);
-    FIERY_REQUIRE(P.D >= 1 && P.D <= 48, "depth_bins=%d not supported by this build (1..48)", P.D);
-    FIERY_REQUIRE(P.ww % 4 == 0, "feat_w=%d must be a multiple of 4 (TMA row pitch must be 16-byte aligned)", P.ww);
-    FIERY_REQUIRE(P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
     const bool nchw = P.bev_layout == FIERY_BEV_NCHW;
-    FIERY_REQUIRE(!warp_theta || nchw, "the warped lift writes the NCHW layout only");
     FIERY_REQUIRE(workspace != nullptr, "the deterministic forward needs the workspace of fiery_lift_deterministic_workspace_bytes()");
     const DetLayout W = det_layout(P);
     unsigned char* ws = static_cast<unsigned char*>(workspace);
@@ -583,12 +582,9 @@ int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtyp
     int* start = reinterpret_cast<int*>(ws + W.start);
     int* cursor = reinterpret_cast<int*>(ws + W.cursor);
     int* lists = reinterpret_cast<int*>(ws + W.lists);
-    const bool tma_pass = P.pillars % 4 == 0;
-    CUtensorMap bev_map;
-    if (nchw && tma_pass && !warp_theta) {
-        const int rc = encode_bev_map(&bev_map, bev_out, P.pillars, P.C, P.n_frames, FT_P);
-        if (rc != FIERY_OK) return rc;
-    }
+    LayoutPass pass;
+    int rc = prepare_layout_pass(&pass, P, bev_out, warp_theta, warp_copy);
+    if (rc != FIERY_OK) return rc;
     LiftParams Q = P;
     Q.head_f16 = head_dtype == FIERY_DTYPE_F16 ? head : nullptr;
     Q.touched = nullptr;
@@ -603,13 +599,13 @@ int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtyp
         } else {                                     // a forward-only plan of this pass's frames (no backward streams)
             const PlanView v = plan_view(ws + W.plan, Q.n_frames, P.n_cameras, P.n_wtiles, P.pillars, 0);
             FIERY_CUDA_CHECK(cudaMemsetAsync(const_cast<unsigned char*>(v.touched), 0, static_cast<size_t>(Q.n_frames) * P.pillars, stream));
-            const int rc = launch_lift_plan(Q, const_cast<unsigned char*>(v.tiles), const_cast<unsigned char*>(v.touched), 0, stream);
+            rc = launch_lift_plan(Q, const_cast<unsigned char*>(v.tiles), const_cast<unsigned char*>(v.touched), 0, stream);
             if (rc != FIERY_OK) return rc;
             Q.plan_tiles = v.tiles;
             marks = v.touched;
         }
         Q.accum = partials;
-        int rc = launch_forward_cols_det(Q, head, stream);
+        rc = launch_forward_cols_det(Q, head, stream);
         if (rc != FIERY_OK) return rc;
         float* out = nchw ? accum : bev_out + static_cast<size_t>(f0) * P.pillars * P.C;
         rc = launch_det_reduce(Q, Q.n_frames, Q.plan_tiles, partials, start, cursor, lists, out, nchw ? 0 : 1, stream);
@@ -617,20 +613,7 @@ int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtyp
         if (!nchw) continue;
         // the layout passes of the default path, unchanged; they read exactly the marked rows, which the reduction has written.  The
         // workspace needs no restoring, so marks are never cleared and the accumulator's rows need not be re-zeroed after the warp.
-        unsigned char* m = const_cast<unsigned char*>(marks);
-        if (warp_theta) {
-            const int tpf = static_cast<int>((P.pillars + FW_P - 1) / FW_P);
-            finalize_warp_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FW_THREADS, 0, stream>>>(
-                accum, m, bev_out, P.pillars, P.grid.X, P.grid.Y, tpf, f0, warp_theta, warp_copy);
-        } else if (tma_pass) {
-            const int tpf = static_cast<int>((P.pillars + FT_P - 1) / FT_P);
-            finalize_tma_kernel<<<static_cast<unsigned>(tpf) * Q.n_frames, FT_THREADS, 0, stream>>>(
-                bev_map, accum, m, P.pillars, tpf, f0, 0, 1);
-        } else {
-            const int bpf = static_cast<int>((P.pillars + FIN_THREADS - 1) / FIN_THREADS);
-            finalize_nchw_kernel<<<static_cast<unsigned>(bpf) * Q.n_frames, FIN_THREADS, 0, stream>>>(
-                accum, m, bev_out + static_cast<size_t>(f0) * P.C * P.pillars, P.pillars, bpf, 0);
-        }
+        launch_layout_pass(pass, P, accum, const_cast<unsigned char*>(marks), bev_out, f0, Q.n_frames, 0, 1, stream);
         FIERY_CUDA_CHECK(cudaGetLastError());
     }
     return FIERY_OK;

@@ -494,8 +494,6 @@ static int launch_layout_t(const LiftParams& P, const void* head, cudaStream_t s
 
 // The deterministic forward's tile kernel (lift_det.cu): P.plan_tiles is required, P.accum receives the runs' partial sums.
 int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t stream) {
-    FIERY_REQUIRE(P.hh <= 32, "feat_h=%d not supported by this build (<= 32)", P.hh);
-    FIERY_REQUIRE(P.C == 64 && P.D <= DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);
     FIERY_REQUIRE(P.plan_tiles != nullptr, "the deterministic tile kernel needs a plan");
     return P.head_f16 != nullptr ? launch_forward_cols_t<3, true, true, false, true>(P, head, stream)
                                  : launch_forward_cols_t<3, false, true, false, true>(P, head, stream);
@@ -508,8 +506,6 @@ int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t 
 //     loop not unrolled) while tiles run alone on an SM, i.e. when the last wave is at most half full;
 //   * geometry from a plan: DD = 3 always.
 int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream) {
-    FIERY_REQUIRE(P.hh <= 32, "feat_h=%d not supported by this build (<= 32)", P.hh);
-    FIERY_REQUIRE(P.C == 64 && P.D <= DPAD, "column kernel: C=%d D=%d not supported", P.C, P.D);
     const bool half = P.head_f16 != nullptr;
     if (P.plan_tiles != nullptr)
         return half ? launch_layout_t<3, true, true>(P, head, stream) : launch_layout_t<3, false, true>(P, head, stream);

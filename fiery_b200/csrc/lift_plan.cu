@@ -154,8 +154,8 @@ lift_plan_kernel(const LiftParams P, unsigned char* __restrict__ tiles, unsigned
 }
 
 int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream) {
-    FIERY_REQUIRE(P.hh >= 1 && P.hh <= PLAN_MAX_ROWS, "feat_h=%d not supported by this build (<= %d)", P.hh, PLAN_MAX_ROWS);
-    FIERY_REQUIRE(P.D >= 1 && P.D <= 48, "depth_bins=%d not supported by this build (1..48)", P.D);
+    int rc = check_lift_geometry(P);
+    if (rc != FIERY_OK) return rc;
     const long long n_tiles = static_cast<long long>(P.n_frames) * P.n_cameras * P.n_wtiles;
     if (n_tiles == 0) return FIERY_OK;
     if (P.grid.pow2[0] && P.grid.pow2[1])

@@ -97,4 +97,27 @@ struct LaunchTimer {
 // first row of row group rg (rg may be PLAN_RG: one past the last row)
 __host__ __device__ __forceinline__ int plan_group_row(int rows, int rg) { return (rows * rg) / PLAN_RG; }
 
+// ---- host side of the lift, defined in c_api.cu and next to the kernels ------------------------------------------------------------
+int check_lift_geometry(const LiftParams& P);      // rows and depth bins of a plan's tile record
+int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels, int n_frames, int box_pillars);
+int launch_lift_plan(const LiftParams& P, unsigned char* tiles, unsigned char* touched, int want_streams, cudaStream_t stream);
+int launch_forward_cols(const LiftParams& P, const void* head, cudaStream_t stream);
+int launch_forward_cols_det(const LiftParams& P, const void* head, cudaStream_t stream);
+int launch_det_reduce(const LiftParams& P, int nf, const unsigned char* tiles, const float* partials, int* start, int* cursor,
+                      int* lists, float* out, int zero_empty, cudaStream_t stream);
+// the two forward launchers take the same arguments: c_api.cu calls both through one pointer type
+int launch_lift_forward(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* scratch, const void* plan,
+                        const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream);
+int launch_lift_forward_det(const LiftParams& P, const void* head, int head_dtype, float* bev_out, void* workspace, const void* plan,
+                            const float* warp_theta, const unsigned char* warp_copy, cudaStream_t stream);
+size_t lift_scratch_bytes(const LiftParams& P);
+size_t lift_det_workspace_bytes(const LiftParams& P);
+int lift_forward_launches(const LiftParams& P);
+void lift_set_max_chunk_frames(int n);
+void lift_set_timer(LaunchTimer* t);
+int launch_point_indices(const LiftParams& P, int64_t* idx_out, uint8_t* valid_out, int32_t* pillar_out, cudaStream_t stream);
+int launch_compose(int n, const float* K, const float* E, float* combined, float* translation, cudaStream_t stream);
+size_t lift_backward_relayout_bytes(const LiftParams& P);
+int launch_lift_backward(const LiftParams& P, const void* head, float* workspace, const void* plan, cudaStream_t stream);
+
 }  // namespace fiery

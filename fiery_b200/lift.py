@@ -225,12 +225,12 @@ class LiftSplat(nn.Module):
 
     @staticmethod
     def _check_plan(plan: Optional[torch.Tensor], desc: _lib.LiftDesc, dev: torch.device) -> None:
-        """A caller-owned plan must be the buffer ``plan()`` makes for this call's (B', n): exactly fiery_lift_plan_bytes(desc)
-        bytes of uint8 on ``dev`` (one byte for B' = 0).  The kernels find the touched maps at an offset computed from this call's
-        frame count, so a plan of another batch would be read at the wrong place, not merely out of range."""
+        """A caller-owned plan must be the buffer ``plan()`` makes for this call's (B', n): exactly ``_plan_bytes`` bytes of uint8
+        on ``dev`` (one byte for B' = 0).  The kernels find the touched maps at an offset computed from this call's frame count, so a
+        plan of another batch would be read at the wrong place, not merely out of range."""
         if plan is None:
             return
-        want = max(1, int(_lib.load().fiery_lift_plan_bytes(desc)))
+        want = max(1, _plan_bytes(desc.n_frames, desc.n_cameras, desc.feat_w, desc.bev_x * desc.bev_y))
         if plan.dtype != torch.uint8 or plan.device != dev or plan.numel() != want:
             raise ValueError("plan was made for another batch shape: rebuild it with LiftSplat.plan(intrinsics, extrinsics)")
 
@@ -279,7 +279,8 @@ class LiftSplat(nn.Module):
         lib = _lib.load()
         dev = intrinsics.device
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, _lib.BEV_NCHW)
-        buf = torch.empty(max(1, int(lib.fiery_lift_plan_bytes(desc))), dtype=torch.uint8, device=dev)
+        buf = torch.empty(max(1, _plan_bytes(desc.n_frames, desc.n_cameras, desc.feat_w, desc.bev_x * desc.bev_y)), dtype=torch.uint8,
+                          device=dev)
         with torch.cuda.device(dev):
             _lib.check(lib.fiery_lift_plan(desc, *(t.data_ptr() for t in geo), buf.data_ptr(), _stream_ptr(dev)), "fiery_lift_plan")
         return buf
@@ -433,35 +434,29 @@ class LiftSplat(nn.Module):
             theta, copy_mask = warp
             if theta.numel() != B * 6 or copy_mask.numel() != B or theta.dtype != torch.float32 or copy_mask.dtype != torch.uint8:
                 raise ValueError("warp must be (theta (B', 2, 3) float32, copy_mask (B',) uint8) for the B' frames of this call")
-        if torch.are_deterministic_algorithms_enabled():
-            with torch.cuda.device(dev):
-                store = _unfilled((B, X, Y, C) if nhwc else (B, C, X, Y), torch.float32, dev)      # every element is written
-                ws = _unfilled(max(1, int(lib.fiery_lift_deterministic_workspace_bytes(desc))), torch.uint8, dev)
-                _lib.check(lib.fiery_lift_forward_deterministic(
-                    desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(), ws.data_ptr(),
-                    plan.data_ptr() if plan is not None else 0, warp[0].data_ptr() if warp is not None else 0,
-                    warp[1].data_ptr() if warp is not None else 0, _stream_ptr(dev)), "fiery_lift_forward_deterministic")
-            return store.permute(0, 3, 1, 2) if nhwc else store
+        warp_ptrs = (theta.data_ptr(), copy_mask.data_ptr()) if warp is not None else (0, 0)
+        shape = (B, X, Y, C) if nhwc else (B, C, X, Y)
         pooled = 0
         with torch.cuda.device(dev):
-            if nhwc:
-                store = torch.zeros((B, X, Y, C), dtype=torch.float32, device=dev)
-                out = store.permute(0, 3, 1, 2)
+            if torch.are_deterministic_algorithms_enabled():
+                entry, extra = "fiery_lift_forward_deterministic", warp_ptrs
+                store = _unfilled(shape, torch.float32, dev)                      # every element is written
+                buf = _unfilled(max(1, int(lib.fiery_lift_deterministic_workspace_bytes(desc))), torch.uint8, dev)
             else:
-                store = out = torch.empty((B, C, X, Y), dtype=torch.float32, device=dev)
-            if scratch is None and B and not nhwc:
-                pooled = int(lib.fiery_lift_scratch_bytes(desc))
-                scratch = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
-            args = (desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(),
-                    scratch.data_ptr() if (B and scratch is not None) else 0, plan.data_ptr() if plan is not None else 0)
-            if warp is None:
-                status = lib.fiery_lift_forward(*args, _stream_ptr(dev))
-            else:
-                status = lib.fiery_lift_forward_warped(*args, theta.data_ptr(), copy_mask.data_ptr(), _stream_ptr(dev))
+                entry, extra = ("fiery_lift_forward_warped", warp_ptrs) if warp is not None else ("fiery_lift_forward", ())
+                # NHWC: the tile kernels reduce into the output itself, so it starts zeroed
+                store = (torch.zeros if nhwc else torch.empty)(shape, dtype=torch.float32, device=dev)
+                buf = scratch
+                if buf is None and B and not nhwc:
+                    pooled = int(lib.fiery_lift_scratch_bytes(desc))
+                    buf = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
+            status = getattr(lib, entry)(desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(),
+                                         buf.data_ptr() if (B and buf is not None) else 0, plan.data_ptr() if plan is not None else 0,
+                                         *extra, _stream_ptr(dev))
             if status != 0 and pooled:
                 _scratch.discard(dev, pooled)          # a launch sequence that stopped half way may have left it dirty
-            _lib.check(status, "fiery_lift_forward_warped" if warp is not None else "fiery_lift_forward")
-        return out
+            _lib.check(status, entry)
+        return store.permute(0, 3, 1, 2) if nhwc else store
 
     def _launch_backward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
                          grad_bev: torch.Tensor, plan: Optional[torch.Tensor] = None) -> torch.Tensor:
