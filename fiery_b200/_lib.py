@@ -34,6 +34,16 @@ class LiftDesc(ctypes.Structure):
     ]
 
 
+class TemporalEntryDesc(ctypes.Structure):
+    """Mirror of ``fiery_temporal_entry_desc_t``."""
+
+    _fields_ = [
+        ("batch", c_int32), ("frames", c_int32), ("pixels", c_int32), ("in_channels", c_int32), ("extra_channels", c_int32),
+        ("n_segments", c_int32), ("seg_channels", c_int32 * 4),
+        ("in_stride_b", c_int64), ("in_stride_t", c_int64), ("in_stride_c", c_int64),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/fiery_b200.h declares
 SIGNATURES = {
     "fiery_abi_version": (c_int32, []),
@@ -73,6 +83,13 @@ SIGNATURES = {
     "fiery_bev_first_conv_backward_data": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_bev_first_conv_backward_weight_workspace_bytes": (c_size_t, [c_int32, c_int32, c_int32]),
     "fiery_bev_first_conv_backward_weight": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_temporal_entry_packed_bytes": (c_size_t, [POINTER(TemporalEntryDesc)]),
+    "fiery_temporal_entry_pack_weights": (c_int32, [POINTER(TemporalEntryDesc), c_void_p, c_void_p, c_void_p]),
+    "fiery_temporal_entry_forward": (c_int32, [POINTER(TemporalEntryDesc), c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
+    "fiery_temporal_entry_backward_data": (c_int32, [POINTER(TemporalEntryDesc), POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
+    "fiery_temporal_entry_backward_weight_workspace_bytes": (c_size_t, [POINTER(TemporalEntryDesc)]),
+    "fiery_temporal_entry_backward_weight": (c_int32, [POINTER(TemporalEntryDesc), c_void_p, c_void_p, POINTER(c_void_p), c_void_p,
+                                                       c_void_p, c_void_p]),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

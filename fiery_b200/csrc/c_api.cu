@@ -121,6 +121,15 @@ int launch_bev_conv_wgrad(int n_frames, int H, int W, const float* x_nhwc, const
                           cudaStream_t stream);
 int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, int dtype, const void* weight_padded, const float* bias,
                        float* head, cudaStream_t stream);
+size_t temporal_entry_packed_bytes(const fiery_temporal_entry_desc_t* d);
+int launch_temporal_entry_pack(const fiery_temporal_entry_desc_t* d, const float* w, float* packed, cudaStream_t stream);
+int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
+                                  float* const* out, cudaStream_t stream);
+int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, float* gx,
+                                cudaStream_t stream);
+size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d);
+int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
+                                float* gw, void* workspace, cudaStream_t stream);
 int vs_plan(int64_t n_rows, const int64_t* ranks, int32_t* seg, int64_t* host_n, cudaStream_t);
 int vs_forward(int64_t n_rows, int channels, int64_t feat_stride, const float* feats, const int64_t* coords,
                const int32_t* seg, int64_t n_seg, float* sums, int64_t* coords_out, cudaStream_t);
@@ -426,6 +435,90 @@ FIERY_API int fiery_depth_layer_forward(int32_t n_images, int32_t pixels, int32_
                                         const void* weight_padded, const float* bias, float* head_out, void* stream) {
     FIERY_REQUIRE(n_images == 0 || (feat && weight_padded && head_out), "depth layer: NULL pointer");
     return launch_depth_layer(n_images, pixels, n_out, feat, dtype, weight_padded, bias, head_out, static_cast<cudaStream_t>(stream));
+}
+
+// The temporal entry's shape limits, one place for every entry point.  The messages name the field.
+static int check_temporal_entry_desc(const fiery_temporal_entry_desc_t* d) {
+    FIERY_REQUIRE(d, "temporal entry: NULL desc");
+    FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0, "temporal entry: batch = %d, frames = %d must be >= 0", d->batch, d->frames);
+    FIERY_REQUIRE(d->in_channels >= 1 && d->in_channels <= 128, "temporal entry: in_channels K = %d must be in 1..128", d->in_channels);
+    FIERY_REQUIRE(d->extra_channels >= 0 && d->extra_channels <= 8, "temporal entry: extra_channels E = %d must be in 0..8",
+                  d->extra_channels);
+    FIERY_REQUIRE(d->n_segments >= 1 && d->n_segments <= 4, "temporal entry: n_segments = %d must be in 1..4", d->n_segments);
+    int n_out = 0, n_pad = 0;
+    for (int q = 0; q < d->n_segments; ++q) {
+        FIERY_REQUIRE(d->seg_channels[q] >= 1 && d->seg_channels[q] <= 256, "temporal entry: seg_channels[%d] = %d must be in 1..256", q,
+                      d->seg_channels[q]);
+        n_out += d->seg_channels[q];
+        n_pad += (d->seg_channels[q] + 7) / 8 * 8;
+    }
+    FIERY_REQUIRE(n_out <= 256, "temporal entry: N_out = %d output channels (sum of seg_channels) must be <= 256", n_out);
+    FIERY_REQUIRE(n_pad <= 256, "temporal entry: N_out with each segment rounded up to 8 channels = %d must be <= 256", n_pad);
+    FIERY_REQUIRE(d->pixels >= 1 && d->pixels % 4 == 0, "temporal entry: pixels X*Y = %d must be a positive multiple of 4 (16-byte TMA pitch)",
+                  d->pixels);
+    FIERY_REQUIRE(d->in_stride_b >= 0 && d->in_stride_t >= 0 && d->in_stride_c >= 0 && d->in_stride_b % 4 == 0 && d->in_stride_t % 4 == 0 &&
+                  d->in_stride_c % 4 == 0, "temporal entry: input strides (%lld, %lld, %lld) must be non-negative multiples of 4 elements",
+                  (long long)d->in_stride_b, (long long)d->in_stride_t, (long long)d->in_stride_c);
+    return FIERY_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+FIERY_API size_t fiery_temporal_entry_packed_bytes(const fiery_temporal_entry_desc_t* desc) {
+    if (check_temporal_entry_desc(desc) != FIERY_OK) return 0;
+    return temporal_entry_packed_bytes(desc);
+}
+
+FIERY_API int fiery_temporal_entry_pack_weights(const fiery_temporal_entry_desc_t* desc, const float* weight, void* packed, void* stream) {
+    const int rc = check_temporal_entry_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(weight && packed, "temporal entry: NULL weight pointer");
+    FIERY_REQUIRE(aligned16(packed), "temporal entry: packed weights must be 16-byte aligned");
+    return launch_temporal_entry_pack(desc, weight, static_cast<float*>(packed), static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_temporal_entry_forward(const fiery_temporal_entry_desc_t* desc, const float* x, const float* extra, const void* packed,
+                                           float* const* out, void* stream) {
+    const int rc = check_temporal_entry_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if (desc->batch == 0 || desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(x && packed && out && (extra || desc->extra_channels == 0), "temporal entry: NULL pointer");
+    FIERY_REQUIRE(aligned16(x) && aligned16(packed), "temporal entry: pointers must be 16-byte aligned");
+    for (int q = 0; q < desc->n_segments; ++q) FIERY_REQUIRE(out[q] && aligned16(out[q]), "temporal entry: out[%d] is NULL or misaligned", q);
+    return launch_temporal_entry_forward(desc, x, desc->extra_channels ? extra : nullptr, static_cast<const float*>(packed), out,
+                                         static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_temporal_entry_backward_data(const fiery_temporal_entry_desc_t* desc, const float* const* grad_out, const void* packed,
+                                                 float* grad_x, void* stream) {
+    const int rc = check_temporal_entry_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if (desc->batch == 0 || desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(grad_out && packed && grad_x, "temporal entry: NULL pointer");
+    FIERY_REQUIRE(aligned16(packed) && aligned16(grad_x), "temporal entry: pointers must be 16-byte aligned");
+    for (int q = 0; q < desc->n_segments; ++q)
+        FIERY_REQUIRE(grad_out[q] && aligned16(grad_out[q]), "temporal entry: grad_out[%d] is NULL or misaligned", q);
+    return launch_temporal_entry_dgrad(desc, grad_out, static_cast<const float*>(packed), grad_x, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_temporal_entry_backward_weight_workspace_bytes(const fiery_temporal_entry_desc_t* desc) {
+    if (check_temporal_entry_desc(desc) != FIERY_OK) return 0;
+    return temporal_entry_wgrad_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_temporal_entry_backward_weight(const fiery_temporal_entry_desc_t* desc, const float* x, const float* extra,
+                                                   const float* const* grad_out, float* grad_w, void* workspace, void* stream) {
+    const int rc = check_temporal_entry_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_w, "temporal entry: NULL grad_w");
+    if (desc->batch > 0 && desc->frames > 0) {
+        FIERY_REQUIRE(x && grad_out && workspace && (extra || desc->extra_channels == 0), "temporal entry: NULL pointer");
+        FIERY_REQUIRE(aligned16(x) && aligned16(workspace), "temporal entry: pointers must be 16-byte aligned");
+        for (int q = 0; q < desc->n_segments; ++q)
+            FIERY_REQUIRE(grad_out[q] && aligned16(grad_out[q]), "temporal entry: grad_out[%d] is NULL or misaligned", q);
+    }
+    return launch_temporal_entry_wgrad(desc, x, desc->extra_channels ? extra : nullptr, grad_out, grad_w, workspace,
+                                       static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -134,6 +134,31 @@ def use_tensor_core_first_conv(model):
     return model
 
 
+def use_tensor_core_temporal_model(model):
+    """Replace every covered ``TemporalBlock`` in ``model.temporal_model.model`` (fiery/models/temporal_model.py:27-45) of a ``Fiery``
+    instance by ``fiery_b200.temporal.TensorCoreTemporalBlock``, which adopts the block's children (``state_dict`` keys unchanged) and
+    runs its four 1x1x1 input convolutions as one tensor-core GEMM, forward and backward.  Returns the model; a second call does
+    nothing.  A ``TemporalModelIdentity`` (the static configs) is left alone, and so are blocks the kernels do not cover (wrong
+    kernel size or bias, shapes outside the limits, an X*Y the TMA cannot take), with one warning."""
+    from .temporal import TensorCoreTemporalBlock, block_reason
+    blocks = getattr(model.temporal_model, "model", None)
+    if blocks is None:
+        return model
+    skipped = []
+    for i, block in enumerate(blocks):
+        if isinstance(block, TensorCoreTemporalBlock) or type(block).__name__ != "TemporalBlock":
+            continue
+        reason = block_reason(block)
+        if reason is None:
+            blocks[i] = TensorCoreTemporalBlock(block)
+        else:
+            skipped.append(f"block {i}: {reason}")
+    if skipped:
+        _warn_once(("temporal", tuple(skipped)), "fiery_b200: TemporalBlock(s) not covered by the tensor-core kernels, left as is: "
+                   + "; ".join(skipped))
+    return model
+
+
 def uninstall():
     if not _saved:
         return

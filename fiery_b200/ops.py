@@ -16,7 +16,7 @@ constants (a registry of weak references; the constants are tiny host-derived te
 from __future__ import annotations
 
 import weakref
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 
@@ -184,3 +184,72 @@ def _first_conv_backward(ctx, grad_y):
 
 first_conv.register_autograd(_first_conv_backward, setup_context=_first_conv_setup_context)
 torch.library.register_autocast("fiery_b200::first_conv", "cuda", torch.float32)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# The temporal block's 1x1x1 input projections (TemporalBlock, fiery/layers/temporal.py:218-281) as dispatcher operators:
+# ``torch.ops.fiery_b200.temporal_entry`` / ``temporal_entry_backward`` (fiery_b200/temporal.py; kernels in csrc/temporal_entry.cu).
+# Autocast: the operator runs in fp32 (TF32 tensor-core operands, fp32 accumulation), as first_conv does; under AMP the reference runs
+# these convolutions in fp16.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::temporal_entry", mutates_args=(), device_types="cuda")
+def temporal_entry(x: torch.Tensor, weights: List[torch.Tensor], extra: Optional[torch.Tensor]) -> List[torch.Tensor]:
+    """x (b, K, s, X, Y), any strides; weights: 1..4 Conv3d weights (C_q, K + E, 1, 1, 1); extra (b, s, E) per-frame channels that
+    are constant over the map (E = 0: None).  Returns one contiguous (b, C_q, s, X, Y) fp32 tensor per weight: the 1x1x1 convolution
+    of ``cat([x, extra broadcast over the map], 1)``.  The weights' pack is made at most once per weight version."""
+    from .temporal import entry_forward
+    return entry_forward(x, weights, extra)
+
+
+@temporal_entry.register_fake
+def _(x, weights, extra):
+    b, _, s, h, w = x.shape
+    return [x.new_empty((b, wt.shape[0], s, h, w), dtype=torch.float32) for wt in weights]
+
+
+@torch.library.custom_op("fiery_b200::temporal_entry_backward", mutates_args=(), device_types="cuda")
+def temporal_entry_backward(grads: List[torch.Tensor], x: torch.Tensor, weights: List[torch.Tensor], extra: Optional[torch.Tensor],
+                            need_input: bool, need_weight: bool) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+    """(grad_x, grad_weights) of ``temporal_entry``; a gradient that is not asked for is not computed and comes back empty.
+    grad_x: x's shape and dtype, with x's strides where the kernels read x as it lies (``temporal.input_strides``); grad_weights: each
+    weight's shape and dtype, bit-reproducible (no atomics).  extra gets no gradient."""
+    from .temporal import entry_backward_data, entry_backward_weight
+    grad_x = x.new_empty((0,))
+    grad_w = [wt.new_empty((0,)) for wt in weights]
+    if need_input:
+        grad_x = entry_backward_data(grads, x, weights)
+        if grad_x.dtype != x.dtype:
+            grad_x = grad_x.to(x.dtype)
+    if need_weight:
+        grad_w = [g if g.dtype == wt.dtype else g.to(wt.dtype) for g, wt in zip(entry_backward_weight(grads, x, weights, extra), weights)]
+    return grad_x, grad_w
+
+
+@temporal_entry_backward.register_fake
+def _(grads, x, weights, extra, need_input, need_weight):
+    from .temporal import input_strides
+    grad_x = x.new_empty_strided(tuple(x.shape), input_strides(tuple(x.shape), x.stride())) if need_input else x.new_empty((0,))
+    grad_w = [wt.new_empty(wt.shape) if need_weight else wt.new_empty((0,)) for wt in weights]
+    return grad_x, grad_w
+
+
+def _temporal_entry_setup_context(ctx, inputs, output):
+    x, weights, extra = inputs
+    ctx.n_weights = len(weights)
+    ctx.save_for_backward(x, extra, *weights)
+
+
+def _temporal_entry_backward(ctx, grads):
+    x, extra, *weights = ctx.saved_tensors
+    # a tensor-list input's needs_input_grad is a list, and its gradient must be a list of the same length
+    need_input, need_w = bool(ctx.needs_input_grad[0]), [bool(n) for n in ctx.needs_input_grad[1]]
+    if not (need_input or any(need_w)):
+        return None, [None] * len(weights), None
+    grads = [g if g is not None else torch.zeros((x.shape[0], wt.shape[0], *x.shape[2:]), dtype=torch.float32, device=x.device)
+             for g, wt in zip(grads, weights)]
+    grad_x, grad_w = torch.ops.fiery_b200.temporal_entry_backward(grads, x, weights, extra, need_input, any(need_w))
+    return (grad_x if need_input else None), [g if n else None for g, n in zip(grad_w, need_w)], None
+
+
+temporal_entry.register_autograd(_temporal_entry_backward, setup_context=_temporal_entry_setup_context)
+torch.library.register_autocast("fiery_b200::temporal_entry", "cuda", torch.float32)

@@ -1,0 +1,362 @@
+"""The temporal block's input projections on the tensor cores (fiery/layers/temporal.py:218-281).
+
+A reference ``TemporalBlock`` applies four 1x1x1 ``Conv3d`` to the same input -- ``convolution_paths[0][0].conv``,
+``convolution_paths[1][0].conv``, ``convolution_paths[2].conv`` (each in -> in / 2) and ``projection[0]`` (in -> out, when the block
+changes the channel count) -- so they are one GEMM over the input's pixel planes.  ``torch.ops.fiery_b200.temporal_entry``
+(fiery_b200/ops.py; kernels in csrc/temporal_entry.cu) computes it: it reads the input as it lies (the permuted view
+``TemporalModel.forward`` makes, or a contiguous NCDHW tensor) and writes each conv's output as its own contiguous
+(b, C, s, X, Y) tensor, the layout ``BatchNorm3d`` and the causal convolutions take.  Both gradients run on the tensor cores too;
+the weight gradient is bit-reproducible.
+
+``TensorCoreTemporalBlock.from_block(block)`` adopts the reference block's children under the same names (``state_dict`` keys are
+unchanged) and replaces only those four convolutions; ``install.use_tensor_core_temporal_model`` swaps it into a model.
+
+``temporal_model_forward(temporal_model, bev, future_egomotion)`` is the folded form of fiery.py:148-158: the egopose channels
+are constant over the map, so instead of concatenating them to the BEV (a 70-channel copy) the first block's GEMM takes the 64-channel
+BEV and the egopose enters as a per-(frame, output channel) bias; its pyramid pooling is computed from the BEV's spatial means and the
+egopose itself.  No CPU path.
+"""
+from __future__ import annotations
+
+import warnings
+from collections import OrderedDict
+from typing import List, Optional, Sequence, Tuple
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+
+from . import _lib
+from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.temporal_entry)
+from .geometry import _require_cuda, _stream_ptr
+
+MAX_IN_CHANNELS, MAX_OUT_CHANNELS, MAX_EXTRA_CHANNELS = 128, 256, 8
+_warned_pixels = set()
+
+
+def _round8(n: int) -> int:
+    return (n + 7) // 8 * 8
+
+
+def unsupported_reason(in_channels: int, seg_channels: Sequence[int], extra_channels: int = 0,
+                       pixels: Optional[int] = None) -> Optional[str]:
+    """None if the kernels take these shapes, else the reason (the limits of include/fiery_b200.h)."""
+    if not 1 <= in_channels <= MAX_IN_CHANNELS:
+        return f"in_channels K = {in_channels} (the kernels take 1..{MAX_IN_CHANNELS})"
+    if not 0 <= extra_channels <= MAX_EXTRA_CHANNELS:
+        return f"extra_channels E = {extra_channels} (the kernels take 0..{MAX_EXTRA_CHANNELS})"
+    if not 1 <= len(seg_channels) <= 4:
+        return f"{len(seg_channels)} convolutions (the kernels take 1..4)"
+    if sum(seg_channels) > MAX_OUT_CHANNELS or sum(_round8(c) for c in seg_channels) > MAX_OUT_CHANNELS:
+        return f"N_out = {sum(seg_channels)} output channels {tuple(seg_channels)} (the kernels take <= {MAX_OUT_CHANNELS})"
+    if pixels is not None and pixels % 4:
+        return f"X*Y = {pixels} pixels (the kernels need a multiple of 4: 16-byte TMA pitch)"
+    return None
+
+
+def _desc(x: torch.Tensor, seg_channels: Sequence[int], extra_channels: int) -> _lib.TemporalEntryDesc:
+    b, k, s, h, w = x.shape
+    d = _lib.TemporalEntryDesc()
+    d.batch, d.frames, d.pixels, d.in_channels, d.extra_channels = b, s, h * w, k, extra_channels
+    d.n_segments = len(seg_channels)
+    for i, c in enumerate(seg_channels):
+        d.seg_channels[i] = int(c)
+    d.in_stride_b, d.in_stride_c, d.in_stride_t = x.stride(0), x.stride(1), x.stride(2)
+    return d
+
+
+def _takes_as_is(shape, stride) -> bool:
+    """The kernels read (b, K, s, X, Y) as it lies when the pixel planes are contiguous, every other stride is a multiple of 4
+    elements (16-byte TMA pitch) and no two elements share an address: the input gradient is written with these strides, so an
+    expanded (stride-0) or otherwise overlapping input is read from a contiguous copy instead."""
+    _, _, _, h, w = shape
+    if not ((stride[4] == 1 or w == 1) and (stride[3] == w or h == 1) and all(st % 4 == 0 for st in stride[:3])):
+        return False
+    # non-overlapping: with the dimensions of size > 1 sorted by stride, each stride covers the extent of the one before it
+    dims = sorted((st, n) for st, n in zip(stride, shape) if n > 1)
+    extent = 1
+    for st, n in dims:
+        if st < extent:
+            return False
+        extent = st * n
+    return True
+
+
+def input_strides(shape, stride) -> Tuple[int, ...]:
+    """Strides of the tensor the kernels read for an input of this shape / stride: its own, or those of a contiguous copy.  The input
+    gradient comes back with these strides."""
+    if _takes_as_is(shape, stride):
+        return tuple(stride)
+    b, k, s, h, w = shape
+    return (k * s * h * w, s * h * w, h * w, w, 1)
+
+
+def _entry_input(x: torch.Tensor) -> torch.Tensor:
+    x = x.float() if x.dtype != torch.float32 else x
+    return x if _takes_as_is(x.shape, x.stride()) else x.contiguous()
+
+
+def _stacked(weights: Sequence[torch.Tensor]) -> torch.Tensor:
+    return torch.cat([w.detach().float().reshape(w.shape[0], -1) for w in weights], 0).contiguous()
+
+
+# (device, weights' data_ptrs, in_channels) -> [versions, weight aliases, pack].  The aliases keep the weights' memory alive, so an
+# address in the cache cannot be taken by another tensor while its entry exists; a version counter changes with each in-place update
+# (an optimizer step), so a pack is made at most once per weight version.
+_PACKS: "OrderedDict[tuple, list]" = OrderedDict()
+_PACKS_MAX = 16
+
+
+def packed_weights(weights: Sequence[torch.Tensor], in_channels: int) -> torch.Tensor:
+    """The device pack of the stacked weights (fiery_temporal_entry_pack_weights), made at most once per weight version."""
+    key = (str(weights[0].device), in_channels) + tuple(w.data_ptr() for w in weights)
+    versions = tuple(w._version for w in weights)
+    entry = _PACKS.get(key)
+    if entry is None or entry[0] != versions or any(tuple(a.shape) != tuple(w.shape) for a, w in zip(entry[1], weights)):
+        entry = [versions, [w.detach() for w in weights], pack_weights(weights, in_channels)]
+        _PACKS[key] = entry
+        while len(_PACKS) > _PACKS_MAX:
+            _PACKS.popitem(last=False)
+    _PACKS.move_to_end(key)
+    return entry[2]
+
+
+def pack_weights(weights: Sequence[torch.Tensor], in_channels: int) -> torch.Tensor:
+    """(C_q, K + E, 1, 1, 1) conv weights -> the uint8 device pack the three kernels take."""
+    _require_cuda(weights[0], "weight")
+    lib = _lib.load()
+    w = _stacked(weights)
+    seg = [int(t.shape[0]) for t in weights]
+    d = _desc(torch.empty((0, in_channels, 0, 1, 4)), seg, w.shape[1] - in_channels)
+    n = int(lib.fiery_temporal_entry_packed_bytes(d))
+    if n == 0:
+        raise _lib.FieryError(f"temporal entry: weights {[tuple(t.shape) for t in weights]} with K = {in_channels} are not supported: "
+                              f"{unsupported_reason(in_channels, seg, w.shape[1] - in_channels)}")
+    out = torch.empty(n, dtype=torch.uint8, device=w.device)
+    with torch.cuda.device(w.device):
+        _lib.check(lib.fiery_temporal_entry_pack_weights(d, w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
+                   "fiery_temporal_entry_pack_weights")
+    return out
+
+
+def _extra_f32(extra: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    return None if extra is None else extra.detach().float().contiguous()
+
+
+def _ptrs(ts: Sequence[torch.Tensor]):
+    arr = (_lib.c_void_p * 4)()
+    for i, t in enumerate(ts):
+        arr[i] = t.data_ptr()
+    return arr
+
+
+def entry_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], extra: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+    """x (b, K, s, X, Y) any float dtype and strides; weights: 1..4 tensors (C_q, K + E, 1, 1, 1); extra: (b, s, E) or None.  Returns
+    the C_q-channel outputs, each a contiguous (b, C_q, s, X, Y) fp32 tensor."""
+    _require_cuda(x, "x")
+    lib = _lib.load()
+    xs = _entry_input(x)
+    b, K, s, h, w = xs.shape
+    seg = [int(t.shape[0]) for t in weights]
+    E = int(weights[0].shape[1]) - K
+    reason = unsupported_reason(K, seg, E, h * w)
+    if reason is not None:
+        raise _lib.FieryError(f"temporal entry: {reason}")
+    outs = [torch.empty((b, c, s, h, w), dtype=torch.float32, device=x.device) for c in seg]
+    e = _extra_f32(extra) if E else None
+    if E and (e is None or tuple(e.shape) != (b, s, E)):
+        raise ValueError(f"extra must be ({b}, {s}, {E}) for weights with {K + E} input channels and x with {K}")
+    packed = packed_weights(weights, K)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_temporal_entry_forward(_desc(xs, seg, E), xs.data_ptr(), e.data_ptr() if e is not None else 0,
+                                                    packed.data_ptr(), _ptrs(outs), _stream_ptr(x.device)),
+                   "fiery_temporal_entry_forward")
+    return outs
+
+
+def _grads_f32(grads: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+    return [g.float().contiguous() for g in grads]
+
+
+def entry_backward_data(grads: Sequence[torch.Tensor], x: torch.Tensor, weights: Sequence[torch.Tensor]) -> torch.Tensor:
+    """The input gradient: x's shape in fp32, with ``input_strides(x)``."""
+    lib = _lib.load()
+    b, K, s, h, w = x.shape
+    seg = [int(t.shape[0]) for t in weights]
+    E = int(weights[0].shape[1]) - K
+    gs = _grads_f32(grads)
+    gx = torch.empty_strided(tuple(x.shape), input_strides(x.shape, x.stride()), dtype=torch.float32, device=x.device)
+    packed = packed_weights(weights, K)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_temporal_entry_backward_data(_desc(gx, seg, E), _ptrs(gs), packed.data_ptr(), gx.data_ptr(),
+                                                          _stream_ptr(x.device)), "fiery_temporal_entry_backward_data")
+    return gx
+
+
+def backward_weight_workspace_bytes(x_shape, seg_channels: Sequence[int], extra_channels: int = 0) -> int:
+    """Bytes of device workspace the weight gradient uses (host-only answer; 0 for 0 frames or unsupported shapes)."""
+    b, k, s, h, w = x_shape
+    return int(_lib.load().fiery_temporal_entry_backward_weight_workspace_bytes(
+        _desc(torch.empty((b, k, s, h, w), device="meta"), seg_channels, extra_channels)))
+
+
+def entry_backward_weight(grads: Sequence[torch.Tensor], x: torch.Tensor, weights: Sequence[torch.Tensor],
+                          extra: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+    """The weight gradients, each of its weight's shape in fp32; bit-reproducible (fixed summation order, no atomics)."""
+    lib = _lib.load()
+    xs = _entry_input(x)
+    K = xs.shape[1]
+    seg = [int(t.shape[0]) for t in weights]
+    E = int(weights[0].shape[1]) - K
+    gs = _grads_f32(grads)
+    e = _extra_f32(extra) if E else None
+    d = _desc(xs, seg, E)
+    need = int(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d))
+    ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+    gw = torch.empty((sum(seg), K + E), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_temporal_entry_backward_weight(d, xs.data_ptr(), e.data_ptr() if e is not None else 0, _ptrs(gs),
+                                                            gw.data_ptr(), ws.data_ptr(), _stream_ptr(x.device)),
+                   "fiery_temporal_entry_backward_weight")
+    return [g.reshape(t.shape).clone() for g, t in zip(gw.split(seg, 0), weights)]     # separate tensors: operator outputs may not alias
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# module
+# ------------------------------------------------------------------------------------------------------------------------------
+def _is_1x1x1(conv) -> bool:
+    return (isinstance(conv, nn.Conv3d) and conv.kernel_size == (1, 1, 1) and conv.stride == (1, 1, 1) and conv.padding == (0, 0, 0)
+            and conv.dilation == (1, 1, 1) and conv.groups == 1 and conv.bias is None)
+
+
+def block_pixels(block) -> Optional[int]:
+    """X*Y of the maps the block is built for (its pyramid pooling's kernel covers the whole map), or None if it has none."""
+    pp = getattr(block, "pyramid_pooling", None) if getattr(block, "use_pyramid_pooling", False) else None
+    if pp is None:
+        return None
+    k = pp.features[0].avgpool.kernel_size
+    return int(k[1]) * int(k[2])
+
+
+def block_reason(block) -> Optional[str]:
+    """None if ``block`` (a reference TemporalBlock) is covered by the kernels, else the reason."""
+    try:
+        paths = block.convolution_paths
+        convs = [paths[0][0].conv, paths[1][0].conv, paths[2].conv]
+        if block.projection is not None:
+            convs.append(block.projection[0])
+    except (AttributeError, IndexError, TypeError):
+        return f"{type(block).__name__} does not have the TemporalBlock structure"
+    for c in convs:
+        if not _is_1x1x1(c):
+            return f"{c} is not a bias-free 1x1x1 Conv3d"
+    if len({c.in_channels for c in convs}) != 1:
+        return "the 1x1x1 convolutions take different inputs"
+    return unsupported_reason(convs[0].in_channels, [c.out_channels for c in convs], 0, block_pixels(block))
+
+
+class TensorCoreTemporalBlock(nn.Module):
+    """Drop-in for a reference ``TemporalBlock`` whose four 1x1x1 input convolutions run as one tensor-core GEMM
+    (``torch.ops.fiery_b200.temporal_entry``).  It holds the reference block's children under the same names (``state_dict`` keys
+    are unchanged) and looks them up at call time, so ``SyncBatchNorm.convert_sync_batchnorm`` works before or after the swap.  The
+    norms, activations, causal convolutions, pyramid pooling, aggregation and projection BN are the block's own modules."""
+
+    def __init__(self, block):
+        super().__init__()
+        for name in ("in_channels", "half_channels", "out_channels", "kernels", "use_pyramid_pooling"):
+            setattr(self, name, getattr(block, name))
+        self.convolution_paths = block.convolution_paths
+        if block.use_pyramid_pooling:
+            self.pyramid_pooling = block.pyramid_pooling
+        self.aggregation = block.aggregation
+        self.projection = block.projection
+
+    @classmethod
+    def from_block(cls, block) -> "TensorCoreTemporalBlock":
+        reason = block_reason(block)
+        if reason is not None:
+            raise ValueError(f"TemporalBlock not covered by the tensor-core kernels: {reason}")
+        return cls(block)
+
+    def _entry_convs(self):
+        p = self.convolution_paths
+        convs = [p[0][0].conv, p[1][0].conv, p[2].conv]
+        return convs + [self.projection[0]] if self.projection is not None else convs
+
+    def _tail(self, x: torch.Tensor, ys: Sequence[torch.Tensor], pooled: Optional[torch.Tensor]) -> torch.Tensor:
+        """Everything after the four convolutions (temporal.py:268-281); ``x`` is the block input the skip adds when there is no
+        projection."""
+        p = self.convolution_paths
+        paths = []
+        for i in range(3):
+            entry = p[i][0] if i < 2 else p[i]
+            y = entry.activation(entry.norm(ys[i]))
+            paths.append(p[i][1](y) if i < 2 else y)
+        x_residual = torch.cat(paths, dim=1)
+        if pooled is not None:
+            x_residual = torch.cat([x_residual, pooled], dim=1)
+        x_residual = self.aggregation(x_residual)
+        skip = self.projection[1](ys[3]) if self.projection is not None else x
+        return skip + x_residual
+
+    def forward(self, *inputs):
+        (x,) = inputs
+        convs = self._entry_convs()
+        pixels = x.shape[3] * x.shape[4]
+        if pixels % 4:
+            # only a block without pyramid pooling reaches this: install() checks the map size through its pooling kernel
+            if pixels not in _warned_pixels:
+                _warned_pixels.add(pixels)
+                warnings.warn(f"fiery_b200: TemporalBlock input of X*Y = {pixels} pixels is not covered by the tensor-core kernels "
+                              "(they need a multiple of 4); its 1x1x1 convolutions run as the reference's Conv3d", RuntimeWarning,
+                              stacklevel=2)
+            ys = [c(x) for c in convs]
+        else:
+            ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in convs], None)
+        pooled = self.pyramid_pooling(x) if self.use_pyramid_pooling else None
+        return self._tail(x, ys, pooled)
+
+    def forward_folded(self, x: torch.Tensor, extra: torch.Tensor) -> torch.Tensor:
+        """The block on the input ``cat([x, extra broadcast over the map], channel)`` without building it: x (b, K, s, X, Y), extra
+        (b, s, E) constant per frame (the egopose).  The block must have no skip without projection (its input is the concat)."""
+        if self.projection is None:
+            raise ValueError("the folded form needs a block with a projection: the skip would add the concatenated input")
+        ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in self._entry_convs()], extra)
+        pooled = None
+        if self.use_pyramid_pooling:
+            means = torch.cat([x.float().mean(dim=(3, 4)), extra.float().permute(0, 2, 1)], dim=1)
+            pooled = _pyramid_from_means(self.pyramid_pooling, means, x.shape[3], x.shape[4])
+        return self._tail(x, ys, pooled)
+
+
+def _pyramid_from_means(pp, means: torch.Tensor, h: int, w: int) -> torch.Tensor:
+    """PyramidSpatioTemporalPooling (temporal.py:152-178) for pool sizes that cover the whole (h, w) map, from the input's per-frame
+    spatial means (b, C, s): the spatial average is the mean itself, the temporal window (2, padding 1, not counting the pad) and
+    the 1x1x1 conv / bn / relu run on (b, C, s + 1, 1, 1), and the bilinear upsampling of a 1x1 map is a broadcast."""
+    b, _, s = means.shape
+    out = []
+    for f in pp.features:
+        k = tuple(f.avgpool.kernel_size)
+        if k[1:] != (h, w):
+            raise ValueError(f"pyramid pooling kernel {k} does not cover the {h}x{w} map; the folded form needs one that does")
+        pooled = F.avg_pool3d(means[..., None, None], (2, 1, 1), stride=1, padding=(1, 0, 0), count_include_pad=False)
+        y = f.conv_bn_relu(pooled)[:, :, :-1]
+        out.append(y.expand(b, y.shape[1], s, h, w))
+    return torch.cat(out, 1)
+
+
+def temporal_model_forward(temporal_model, bev: torch.Tensor, future_egomotion: torch.Tensor) -> torch.Tensor:
+    """fiery.py:148-158 (egopose concat + ``self.temporal_model(x)``) without the concat: bev (b, s, C, X, Y) the warped BEV,
+    future_egomotion (b, s, E).  The egopose fed at frame t is zeros at t = 0 and ``future_egomotion[:, t - 1]`` after that, as in the
+    reference.  The first block must be a ``TensorCoreTemporalBlock`` (``install.use_tensor_core_temporal_model``)."""
+    blocks = temporal_model.model
+    first = blocks[0]
+    if not isinstance(first, TensorCoreTemporalBlock):
+        raise TypeError("temporal_model_forward needs the first block swapped: call install.use_tensor_core_temporal_model(model)")
+    b, s = bev.shape[:2]
+    extra = torch.cat([torch.zeros_like(future_egomotion[:, :1]), future_egomotion[:, :s - 1]], dim=1)
+    x = first.forward_folded(bev.permute(0, 2, 1, 3, 4), extra)
+    for m in list(blocks)[1:]:
+        x = m(x)
+    x = x.permute(0, 2, 1, 3, 4).contiguous()
+    return x[:, (temporal_model.receptive_field - 1):]

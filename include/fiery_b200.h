@@ -305,6 +305,52 @@ FIERY_API int fiery_bev_first_conv_backward_weight(int32_t n_frames, int32_t hei
 FIERY_API int fiery_depth_layer_forward(int32_t n_images, int32_t pixels, int32_t n_out, const void* feat, int32_t dtype,
                                         const void* weight_padded, const float* bias, float* head_out, void* stream);
 
+/*
+ * The temporal block's 1x1x1 input projections as one GEMM (TemporalBlock, fiery/layers/temporal.py:218-281): the paths'
+ * conv_1x1x1_norm_activated convolutions and the projection's Conv3d read the same block input, so their n_segments (<= 4) weights,
+ * stacked along the output channel, are one matrix W (N_out, K + E), N_out = sum of seg_channels, row-major fp32.  wgmma, TF32
+ * operands, fp32 accumulation; W is rounded to TF32 (nearest, ties away) when packed, activations are truncated by the tensor core.
+ *
+ * x: the block input, element (b, t, k, p) at x[b * in_stride_b + t * in_stride_t + k * in_stride_c + p], p < pixels = X*Y, so the
+ * permuted concat (b, K, s, X, Y) of a (b, s, K, X, Y) tensor and a contiguous (b, K, s, X, Y) tensor are both read as they lie.
+ * extra: NULL (E = 0) or (batch, frames, E) fp32 channels that are constant over the map (the egopose): they enter the forward as the
+ * bias sum_j W[o, K + j] * extra[b, t, j], computed in fp32.
+ * out[q] / grad_out[q]: segment q's (batch, seg_channels[q], frames, X, Y) fp32, contiguous.
+ * Limits (rejected with a message naming the field): 1 <= K <= 128; N_out <= 256, also with every segment rounded up to 8 channels;
+ * 0 <= E <= 8; pixels % 4 == 0; the strides multiples of 4 elements; pointers 16-byte aligned.  batch * frames == 0 is a no-op (the
+ * weight gradient is then zero).
+ *
+ * fiery_temporal_entry_packed_bytes / fiery_temporal_entry_pack_weights: the device pack of W that the three calls take.
+ * fiery_temporal_entry_forward: out[q] fully overwritten.
+ * fiery_temporal_entry_backward_data: grad_x (the K input channels, written with x's strides) = sum_q W_q^T grad_out[q].
+ * fiery_temporal_entry_backward_weight: grad_w (N_out, K + E) = sum over frames and pixels of grad_out x^T (columns K + j: of the
+ * extra channel j), fully overwritten.  workspace: fiery_temporal_entry_backward_weight_workspace_bytes(desc) bytes (0 for 0 frames),
+ * contents irrelevant.  Summation order: the frames' pixels are cut into 64-pixel tiles, numbered frame by frame (b, then t), and the
+ * tiles into c = min(tiles, 128) chunks, chunk i holding tiles [i * tiles / c, (i + 1) * tiles / c); a chunk's partial is the tensor
+ * core's fp32 accumulation over its tiles in ascending order, and grad_w the fp32 sum of the partials in ascending chunk order.  The
+ * order depends on (batch * frames, pixels) only: bit-reproducible, graph-capturable, no host synchronisation.
+ */
+typedef struct {
+    int32_t batch;
+    int32_t frames;
+    int32_t pixels;
+    int32_t in_channels;          /* K */
+    int32_t extra_channels;       /* E */
+    int32_t n_segments;
+    int32_t seg_channels[4];
+    int64_t in_stride_b, in_stride_t, in_stride_c;   /* elements */
+} fiery_temporal_entry_desc_t;
+
+FIERY_API size_t fiery_temporal_entry_packed_bytes(const fiery_temporal_entry_desc_t* desc);
+FIERY_API int fiery_temporal_entry_pack_weights(const fiery_temporal_entry_desc_t* desc, const float* weight, void* packed, void* stream);
+FIERY_API int fiery_temporal_entry_forward(const fiery_temporal_entry_desc_t* desc, const float* x, const float* extra, const void* packed,
+                                           float* const* out, void* stream);
+FIERY_API int fiery_temporal_entry_backward_data(const fiery_temporal_entry_desc_t* desc, const float* const* grad_out, const void* packed,
+                                                 float* grad_x, void* stream);
+FIERY_API size_t fiery_temporal_entry_backward_weight_workspace_bytes(const fiery_temporal_entry_desc_t* desc);
+FIERY_API int fiery_temporal_entry_backward_weight(const fiery_temporal_entry_desc_t* desc, const float* x, const float* extra,
+                                                   const float* const* grad_out, float* grad_w, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
