@@ -44,6 +44,15 @@ class TemporalEntryDesc(ctypes.Structure):
     ]
 
 
+class CausalConv3dDesc(ctypes.Structure):
+    """Mirror of ``fiery_causal_conv3d_desc_t``."""
+
+    _fields_ = [
+        ("batch", c_int32), ("frames", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("in_channels", c_int32),
+        ("out_channels", c_int32), ("kt", c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/fiery_b200.h declares
 SIGNATURES = {
     "fiery_abi_version": (c_int32, []),
@@ -90,6 +99,12 @@ SIGNATURES = {
     "fiery_temporal_entry_backward_weight_workspace_bytes": (c_size_t, [POINTER(TemporalEntryDesc)]),
     "fiery_temporal_entry_backward_weight": (c_int32, [POINTER(TemporalEntryDesc), c_void_p, c_void_p, POINTER(c_void_p), c_void_p,
                                                        c_void_p, c_void_p]),
+    "fiery_causal_conv3d_packed_bytes": (c_size_t, [POINTER(CausalConv3dDesc)]),
+    "fiery_causal_conv3d_pack_weights": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p]),
+    "fiery_causal_conv3d_forward": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_causal_conv3d_backward_data": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_causal_conv3d_backward_weight_workspace_bytes": (c_size_t, [POINTER(CausalConv3dDesc)]),
+    "fiery_causal_conv3d_backward_weight": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

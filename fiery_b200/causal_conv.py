@@ -1,0 +1,186 @@
+"""The temporal model's causal convolutions on the tensor cores (``CausalConv3d``, fiery/layers/temporal.py:65-85).
+
+A reference ``CausalConv3d`` is a zero pad (``kt - 1`` frames in front, one pixel around the map), a bias-free ``Conv3d`` with kernel
+(kt, 3, 3), a ``BatchNorm3d`` and a ``ReLU``.  ``torch.ops.fiery_b200.causal_conv3d`` (fiery_b200/ops.py; kernels in
+csrc/causal_conv.cu) computes the pad and the convolution in one pass over a contiguous (b, C, s, X, Y) tensor, without a padded
+copy; both gradients run on the tensor cores too, and the weight gradient is bit-reproducible.
+
+``TensorCoreCausalConv3d.from_module(m)`` adopts the reference module's children under the same names (``state_dict`` keys are
+unchanged) and replaces only the pad and the convolution; BatchNorm and ReLU stay the reference's own modules, so batch statistics
+train as before.  ``install.use_tensor_core_causal_convs`` swaps it into a model.  No CPU path.
+"""
+from __future__ import annotations
+
+import warnings
+from typing import Optional
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.causal_conv3d)
+from .geometry import _require_cuda, _stream_ptr
+from .temporal import packed_weights
+
+MAX_CHANNELS = 64
+_warned_widths = set()
+
+
+def unsupported_reason(in_channels: int, out_channels: int, kt: int, grid_y: Optional[int] = None) -> Optional[str]:
+    """None if the kernels take these shapes, else the reason (the limits of include/fiery_b200.h)."""
+    if not 1 <= in_channels <= MAX_CHANNELS:
+        return f"in_channels = {in_channels} (the kernels take 1..{MAX_CHANNELS})"
+    if not 1 <= out_channels <= MAX_CHANNELS:
+        return f"out_channels = {out_channels} (the kernels take 1..{MAX_CHANNELS})"
+    if kt not in (1, 2):
+        return f"kernel ({kt}, 3, 3) (the kernels take kt = 1 or 2)"
+    if grid_y is not None and grid_y % 4:
+        return f"Y = {grid_y} map columns (the kernels need a multiple of 4: 16-byte TMA row pitch)"
+    return None
+
+
+def _desc(shape, out_channels: int, kt: int) -> _lib.CausalConv3dDesc:
+    b, c, s, h, w = shape
+    d = _lib.CausalConv3dDesc()
+    d.batch, d.frames, d.grid_x, d.grid_y, d.in_channels, d.out_channels, d.kt = b, s, h, w, c, out_channels, kt
+    return d
+
+
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    """a contiguous fp32 tensor: the layout the kernels read"""
+    return t.float().contiguous() if t.dtype != torch.float32 else t.contiguous()
+
+
+def pack_weights(weights, in_channels: int) -> torch.Tensor:
+    """[(C_out, C_in, kt, 3, 3) weight] -> the uint8 device pack the forward and the input gradient take."""
+    (weight,) = weights
+    _require_cuda(weight, "weight")
+    lib = _lib.load()
+    w = _f32(weight.detach())
+    c_out, c_in, kt = int(w.shape[0]), int(w.shape[1]), int(w.shape[2])
+    d = _desc((0, c_in, 0, 1, 4), c_out, kt)
+    n = int(lib.fiery_causal_conv3d_packed_bytes(d))
+    if n == 0 or tuple(w.shape[3:]) != (3, 3):
+        raise _lib.FieryError(f"causal conv: weight {tuple(w.shape)} is not supported: "
+                              f"{unsupported_reason(c_in, c_out, kt) or 'kernel must be (kt, 3, 3)'}")
+    out = torch.empty(n, dtype=torch.uint8, device=w.device)
+    with torch.cuda.device(w.device):
+        _lib.check(lib.fiery_causal_conv3d_pack_weights(d, w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
+                   "fiery_causal_conv3d_pack_weights")
+    return out
+
+
+def _packed(weight: torch.Tensor) -> torch.Tensor:
+    return packed_weights([weight], int(weight.shape[1]), pack=pack_weights)
+
+
+def _check(x_shape, weight: torch.Tensor) -> int:
+    c_out, c_in, kt = int(weight.shape[0]), int(weight.shape[1]), int(weight.shape[2])
+    if x_shape[1] != c_in or tuple(weight.shape[3:]) != (3, 3):
+        raise ValueError(f"causal conv: x {tuple(x_shape)} and weight {tuple(weight.shape)} do not match")
+    reason = unsupported_reason(c_in, c_out, kt, int(x_shape[4]))
+    if reason is not None:
+        raise _lib.FieryError(f"causal conv: {reason}")
+    return kt
+
+
+def conv_forward(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """x (b, C_in, s, X, Y) any float dtype and strides; weight (C_out, C_in, kt, 3, 3).  Returns the contiguous fp32
+    (b, C_out, s, X, Y) output of the causal pad + Conv3d."""
+    _require_cuda(x, "x")
+    lib = _lib.load()
+    kt = _check(x.shape, weight)
+    xs = _f32(x)
+    b, _, s, h, w = xs.shape
+    y = torch.empty((b, weight.shape[0], s, h, w), dtype=torch.float32, device=x.device)
+    packed = _packed(weight)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_causal_conv3d_forward(_desc(xs.shape, int(weight.shape[0]), kt), xs.data_ptr(), packed.data_ptr(),
+                                                   y.data_ptr(), _stream_ptr(x.device)), "fiery_causal_conv3d_forward")
+    return y
+
+
+def conv_backward_data(grad_y: torch.Tensor, x_shape, weight: torch.Tensor) -> torch.Tensor:
+    """The input gradient: a contiguous fp32 tensor of x's shape."""
+    lib = _lib.load()
+    kt = _check(x_shape, weight)
+    g = _f32(grad_y)
+    gx = torch.empty(tuple(x_shape), dtype=torch.float32, device=g.device)
+    packed = _packed(weight)
+    with torch.cuda.device(g.device):
+        _lib.check(lib.fiery_causal_conv3d_backward_data(_desc(tuple(x_shape), int(weight.shape[0]), kt), g.data_ptr(),
+                                                         packed.data_ptr(), gx.data_ptr(), _stream_ptr(g.device)),
+                   "fiery_causal_conv3d_backward_data")
+    return gx
+
+
+def backward_weight_workspace_bytes(x_shape, out_channels: int, kt: int) -> int:
+    """Bytes of device workspace the weight gradient uses (host-only answer; 0 for 0 frames or unsupported shapes)."""
+    return int(_lib.load().fiery_causal_conv3d_backward_weight_workspace_bytes(_desc(tuple(x_shape), out_channels, kt)))
+
+
+def conv_backward_weight(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """The weight gradient, fp32 of the weight's shape; bit-reproducible (fixed summation order, no atomics)."""
+    lib = _lib.load()
+    kt = _check(x.shape, weight)
+    xs, g = _f32(x), _f32(grad_y)
+    d = _desc(xs.shape, int(weight.shape[0]), kt)
+    need = int(lib.fiery_causal_conv3d_backward_weight_workspace_bytes(d))
+    ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+    gw = torch.empty(tuple(weight.shape), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.fiery_causal_conv3d_backward_weight(d, xs.data_ptr(), g.data_ptr(), gw.data_ptr(), ws.data_ptr(),
+                                                           _stream_ptr(x.device)), "fiery_causal_conv3d_backward_weight")
+    return gw
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# module
+# ------------------------------------------------------------------------------------------------------------------------------
+def module_reason(m) -> Optional[str]:
+    """None if ``m`` (a reference CausalConv3d) is covered by the kernels, else the reason.  The map width is checked at call time."""
+    pad, conv = getattr(m, "pad", None), getattr(m, "conv", None)
+    if not isinstance(conv, nn.Conv3d) or not isinstance(pad, nn.ConstantPad3d):
+        return f"{type(m).__name__} does not have the CausalConv3d structure"
+    kt = conv.kernel_size[0]
+    if not (conv.kernel_size[1:] == (3, 3) and conv.stride == (1, 1, 1) and conv.padding == (0, 0, 0) and conv.dilation == (1, 1, 1)
+            and conv.groups == 1 and conv.bias is None and conv.padding_mode == "zeros"):
+        return f"{conv} is not a bias-free (kt, 3, 3) Conv3d with stride 1 and dilation 1"
+    if tuple(pad.padding) != (1, 1, 1, 1, kt - 1, 0) or pad.value != 0:
+        return f"pad {tuple(pad.padding)} is not the causal zero pad of a ({kt}, 3, 3) kernel"
+    return unsupported_reason(conv.in_channels, conv.out_channels, kt)
+
+
+class TensorCoreCausalConv3d(nn.Module):
+    """Drop-in for a reference ``CausalConv3d`` whose pad and convolution run on the tensor cores
+    (``torch.ops.fiery_b200.causal_conv3d``).  It holds the reference module's ``pad``, ``conv``, ``norm`` and ``activation`` under the
+    same names (``state_dict`` keys are unchanged, the Parameters are shared) and looks them up at call time, so
+    ``SyncBatchNorm.convert_sync_batchnorm`` works before or after the swap.  A map whose width Y is not a multiple of 4 runs the
+    reference's pad and Conv3d, with one warning."""
+
+    def __init__(self, m):
+        super().__init__()
+        self.pad = m.pad
+        self.conv = m.conv
+        self.norm = m.norm
+        self.activation = m.activation
+
+    @classmethod
+    def from_module(cls, m) -> "TensorCoreCausalConv3d":
+        reason = module_reason(m)
+        if reason is not None:
+            raise ValueError(f"CausalConv3d not covered by the tensor-core kernels: {reason}")
+        return cls(m)
+
+    def forward(self, *inputs):
+        (x,) = inputs
+        width = x.shape[4]
+        if width % 4:
+            if width not in _warned_widths:
+                _warned_widths.add(width)
+                warnings.warn(f"fiery_b200: CausalConv3d input of Y = {width} map columns is not covered by the tensor-core kernels "
+                              "(they need a multiple of 4); it runs as the reference's pad and Conv3d", RuntimeWarning, stacklevel=2)
+            y = self.conv(self.pad(x))
+        else:
+            y = torch.ops.fiery_b200.causal_conv3d(x, self.conv.weight)
+        return self.activation(self.norm(y))

@@ -130,6 +130,13 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
 size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d);
 int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
                                 float* gw, void* workspace, cudaStream_t stream);
+size_t causal_conv_packed_bytes(const fiery_causal_conv3d_desc_t* d);
+int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w, float* packed, cudaStream_t stream);
+int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
+int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
+size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d);
+int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const float* gy, float* gw, void* workspace,
+                             cudaStream_t stream);
 int vs_plan(int64_t n_rows, const int64_t* ranks, int32_t* seg, int64_t* host_n, cudaStream_t);
 int vs_forward(int64_t n_rows, int channels, int64_t feat_stride, const float* feats, const int64_t* coords,
                const int32_t* seg, int64_t n_seg, float* sums, int64_t* coords_out, cudaStream_t);
@@ -519,6 +526,68 @@ FIERY_API int fiery_temporal_entry_backward_weight(const fiery_temporal_entry_de
     }
     return launch_temporal_entry_wgrad(desc, x, desc->extra_channels ? extra : nullptr, grad_out, grad_w, workspace,
                                        static_cast<cudaStream_t>(stream));
+}
+
+// The causal convolution's shape limits, one place for every entry point.  The messages name the field.
+static int check_causal_conv_desc(const fiery_causal_conv3d_desc_t* d) {
+    FIERY_REQUIRE(d, "causal conv: NULL desc");
+    FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0, "causal conv: batch = %d, frames = %d must be >= 0", d->batch, d->frames);
+    FIERY_REQUIRE(d->in_channels >= 1 && d->in_channels <= 64, "causal conv: in_channels = %d must be in 1..64", d->in_channels);
+    FIERY_REQUIRE(d->out_channels >= 1 && d->out_channels <= 64, "causal conv: out_channels = %d must be in 1..64", d->out_channels);
+    FIERY_REQUIRE(d->kt == 1 || d->kt == 2, "causal conv: kt = %d must be 1 or 2 (kernel (kt, 3, 3))", d->kt);
+    FIERY_REQUIRE(d->grid_x >= 1, "causal conv: grid_x = %d must be >= 1", d->grid_x);
+    FIERY_REQUIRE(d->grid_y >= 1 && d->grid_y % 4 == 0, "causal conv: grid_y = %d must be a positive multiple of 4 (16-byte TMA row pitch)",
+                  d->grid_y);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_causal_conv3d_packed_bytes(const fiery_causal_conv3d_desc_t* desc) {
+    if (check_causal_conv_desc(desc) != FIERY_OK) return 0;
+    return causal_conv_packed_bytes(desc);
+}
+
+FIERY_API int fiery_causal_conv3d_pack_weights(const fiery_causal_conv3d_desc_t* desc, const float* weight, void* packed, void* stream) {
+    const int rc = check_causal_conv_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(weight && packed, "causal conv: NULL weight pointer");
+    FIERY_REQUIRE(aligned16(packed), "causal conv: packed weights must be 16-byte aligned");
+    return launch_causal_conv_pack(desc, weight, static_cast<float*>(packed), static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_causal_conv3d_forward(const fiery_causal_conv3d_desc_t* desc, const float* x, const void* packed, float* y, void* stream) {
+    const int rc = check_causal_conv_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if (desc->batch == 0 || desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(x && packed && y, "causal conv: NULL pointer");
+    FIERY_REQUIRE(aligned16(x) && aligned16(packed) && aligned16(y), "causal conv: pointers must be 16-byte aligned");
+    return launch_causal_conv_forward(desc, x, static_cast<const float*>(packed), y, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_causal_conv3d_backward_data(const fiery_causal_conv3d_desc_t* desc, const float* grad_y, const void* packed,
+                                                float* grad_x, void* stream) {
+    const int rc = check_causal_conv_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if (desc->batch == 0 || desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(grad_y && packed && grad_x, "causal conv: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_y) && aligned16(packed) && aligned16(grad_x), "causal conv: pointers must be 16-byte aligned");
+    return launch_causal_conv_dgrad(desc, grad_y, static_cast<const float*>(packed), grad_x, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_causal_conv3d_backward_weight_workspace_bytes(const fiery_causal_conv3d_desc_t* desc) {
+    if (check_causal_conv_desc(desc) != FIERY_OK) return 0;
+    return causal_conv_wgrad_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc_t* desc, const float* x, const float* grad_y,
+                                                  float* grad_w, void* workspace, void* stream) {
+    const int rc = check_causal_conv_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_w, "causal conv: NULL grad_w");
+    if (desc->batch > 0 && desc->frames > 0) {
+        FIERY_REQUIRE(x && grad_y && workspace, "causal conv: NULL pointer");
+        FIERY_REQUIRE(aligned16(x) && aligned16(grad_y) && aligned16(workspace), "causal conv: pointers must be 16-byte aligned");
+    }
+    return launch_causal_conv_wgrad(desc, x, grad_y, grad_w, workspace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,0 +1,471 @@
+// The temporal model's causal convolutions (CausalConv3d, fiery/layers/temporal.py:65-85): a zero pad of (kt - 1) frames in front and
+// one pixel around the map, then a bias-free Conv3d with kernel (kt, 3, 3), kt in {1, 2}, on a contiguous fp32 (b, C, s, X, Y) tensor:
+//
+//   y[o, t, p]  = sum_{tau, dy, dx, i} W[o, i, tau, dy, dx] * x[i, t + tau - (kt - 1), p + (dy - 1, dx - 1)]
+//   gx[i, t, p] = sum_{tau, dy, dx, o} W[o, i, tau, dy, dx] * gy[o, t + (kt - 1) - tau, p - (dy - 1, dx - 1)]
+//   gW[o, i, tau, dy, dx] = sum_{b, t, p} gy[o, t, p] * x[i, t + tau - (kt - 1), p + (dy - 1, dx - 1)]
+//
+// All three run on the tensor cores: wgmma, TF32 operands, fp32 accumulation.  Weights are rounded to TF32 (cvt.rna) when packed, and
+// every register A operand (the forward's x, the input gradient's gy, the weight gradient's x) is rounded the same way as it is read
+// out of shared memory: nearest rounding halves the error of the tensor core's own truncation, which the weight gradient's
+// shared-memory gy operand still gets.  No padded copy of the input exists:
+// every load is a TMA box at shifted coordinates, and the TMA's zero fill for coordinates outside the tensor is the padding -- the
+// spatial ring, frame -1 in the forward and frame s in the input gradient.
+//
+// Forward and input gradient: one kernel.  The input gradient is the forward's convolution on gy with the weights transposed in
+// (o, i), the spatial taps mirrored and the time taps reading forward (frames t .. t + kt - 1) instead of back, so the two differ only
+// in the pack they read and a frame offset.  One CTA per output tile of 8 rows x 16 columns (128 pixels, two consumer warpgroups of
+// 4 x 16 pixels).  The producer warp loads the kt halo tiles (Kpad channels x 10 x 28 pixels, no swizzle) once and streams the 9 kt
+// taps' weight slices (N x Kpad, K-major, 128-byte swizzle) through a ring.  Each tap's MMAs read the pixel tile out of the halo tile
+// at the tap's shift as the register A operand: the halo's 28-column rows make a channel plane 280 floats = 24 banks apart, so the
+// 4 channels x 8 consecutive pixels of a fragment load hit 32 different banks.  N = the output channels rounded up to 8
+// (wgmma_tf32_rs<N>, wgmma.cuh).  Each accumulator row of a warp is 8 consecutive pixels of one map row, so the fragments are stored
+// straight to the (b, C, s, X, Y) output: every warp store fills whole 32-byte sectors.
+//
+// Weight gradient: D (input channels, one m64 block) x (output channels rounded up to 8) = sum over pixels of x_tap gy^T.  Tiles are
+// 32-pixel runs of one map row; CTA (chunk, (tau, dy)) owns the three taps dx = 0, 1, 2.  The gy run is the K-major shared-memory B
+// operand; the x run of the tap's frame and row is loaded once, 4 columns early and 44 wide, and read as the register A operand at
+// each dx's shift (im2col from shared memory; 44-float rows put a fragment's 8 channels x 4 pixels on 32 banks).  The summation order
+// is wgrad_chunks.cuh's: bit-reproducible, no atomics.
+#include "bev_conv.cuh"
+#include "wgrad_chunks.cuh"
+
+namespace fiery {
+
+constexpr int CC_TX = 8, CC_TY = 16;               // output tile: rows x columns of the map
+// Every TMA box starts on a 16-byte boundary of the contiguous map row: the column padding comes from a box that starts 4 columns
+// early (zero fill at column -4 .. -1), and the MMA operands are read from it at the tap's shift.
+constexpr int CC_HX = CC_TX + 2, CC_HY = 28;       // halo box: rows x0 - 1 .. x0 + 8, columns y0 - 4 .. y0 + 23 (y0 - 1 .. y0 + 16 used)
+constexpr int CC_HY_OFF = 3;                       // halo column of input column y0 + c + dx - 1 is c + dx + CC_HY_OFF
+constexpr int CC_PLANE = CC_HX * CC_HY;            // floats per channel of a halo tile: 280 = 24 banks apart
+constexpr int CC_WSTAGES = 4;                      // weight-slice ring
+constexpr int CC_FWD_THREADS = 2 * 128 + 32;
+constexpr int CC_WG_PX = 32;                       // weight gradient: pixels per tile
+constexpr int CC_WG_STAGES = 4;
+constexpr int CC_WG_XP = 44;                       // weight gradient x tile: columns 32 run - 4 .. 32 run + 39, 44 = 12 banks apart
+constexpr int CC_WG_X_BYTES = 64 * CC_WG_XP * 4;   // 64 input-channel rows (zero past C_in): 11 KB, a multiple of 1024
+constexpr int CC_SMEM_SLACK = 1024 + 256;
+
+__host__ __device__ __forceinline__ int cc_round8(int v) { return (v + 7) / 8 * 8; }
+
+struct CcShape {
+    int batch, frames, X, Y, cin, cout, kt, taps;
+};
+
+static CcShape cc_shape(const fiery_causal_conv3d_desc_t* d) {
+    return CcShape{d->batch, d->frames, d->grid_x, d->grid_y, d->in_channels, d->out_channels, d->kt, 9 * d->kt};
+}
+
+// One direction's pack: (taps, ka, n, 32) floats -- tap j's B operand is ka 128-byte-swizzle atoms of n K-major rows x 32 k.
+struct CcPackDir {
+    int n, kpad, ka;
+    size_t floats;
+};
+static CcPackDir cc_pack_dir(int n_channels, int k_channels, int taps) {
+    CcPackDir p;
+    p.n = cc_round8(n_channels);
+    p.kpad = cc_round8(k_channels);
+    p.ka = (p.kpad + 31) / 32;
+    p.floats = static_cast<size_t>(taps) * p.ka * p.n * 32;
+    return p;
+}
+
+// the forward pack F (rows o, k = i), then the input gradient's T (rows i, k = o; time taps reversed, spatial taps mirrored)
+size_t causal_conv_packed_bytes(const fiery_causal_conv3d_desc_t* d) {
+    const CcShape s = cc_shape(d);
+    return (cc_pack_dir(s.cout, s.cin, s.taps).floats + cc_pack_dir(s.cin, s.cout, s.taps).floats) * sizeof(float);
+}
+
+__global__ void causal_conv_pack_kernel(CcShape s, CcPackDir f, CcPackDir t, const float* __restrict__ w, float* __restrict__ packed) {
+    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const bool fwd = i < f.floats;
+    if (!fwd && i >= f.floats + t.floats) return;
+    const CcPackDir& p = fwd ? f : t;
+    const size_t j = fwd ? i : i - f.floats;
+    const int k = static_cast<int>(j % 32), n = static_cast<int>(j / 32 % p.n), a = static_cast<int>(j / 32 / p.n % p.ka);
+    const int tap = static_cast<int>(j / 32 / p.n / p.ka);
+    const int c = 32 * a + k;
+    const int jt = tap / 9, ay = tap / 3 % 3, ax = tap % 3;
+    float v = 0.f;
+    if (fwd) {
+        if (n < s.cout && c < s.cin) v = __uint_as_float(to_tf32(w[((static_cast<size_t>(n) * s.cin + c) * s.kt + jt) * 9 + ay * 3 + ax]));
+    } else if (n < s.cin && c < s.cout) {
+        v = __uint_as_float(to_tf32(w[((static_cast<size_t>(c) * s.cin + n) * s.kt + (s.kt - 1 - jt)) * 9 + (2 - ay) * 3 + (2 - ax)]));
+    }
+    packed[i] = v;
+}
+
+int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w, float* packed, cudaStream_t stream) {
+    const CcShape s = cc_shape(d);
+    const CcPackDir f = cc_pack_dir(s.cout, s.cin, s.taps), t = cc_pack_dir(s.cin, s.cout, s.taps);
+    const size_t n = f.floats + t.floats;
+    causal_conv_pack_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(s, f, t, w, packed);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+__device__ __forceinline__ void cc_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// forward and input gradient
+// ------------------------------------------------------------------------------------------------------------------------------
+struct CcFwdMaps {
+    CUtensorMap x;                                 // input (Y, X, s, C, b), box (20, 10, 1, kpad, 1), no swizzle
+    CUtensorMap w;                                 // pack (32, n, taps * ka), box (32, n, 1), swizzle 128B
+};
+struct CcFwdLaunch {
+    int frames, X, Y, kpad, ka, n_out, kt, t_off, tiles_x, tiles_y;
+};
+
+template <int N>
+__global__ void __launch_bounds__(CC_FWD_THREADS, 1)
+causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch L, float* __restrict__ out) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    const int w_bytes = L.ka * N * 128;
+    const int x_floats = L.kpad * CC_PLANE;
+    const int taps = 9 * L.kt;
+    unsigned char* s_w = smem;
+    const float* s_x = reinterpret_cast<const float*>(s_w + CC_WSTAGES * w_bytes);
+    uint64_t* x_full = reinterpret_cast<uint64_t*>(const_cast<float*>(s_x) + L.kt * x_floats);
+    uint64_t* full = x_full + 1;
+    uint64_t* empty = full + CC_WSTAGES;
+
+    int tile = blockIdx.x;
+    const int ty = tile % L.tiles_y;
+    tile /= L.tiles_y;
+    const int tx = tile % L.tiles_x;
+    const int f = tile / L.tiles_x, b = f / L.frames, t = f % L.frames;
+    const int x0 = tx * CC_TX, y0 = ty * CC_TY;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == 8 && lane == 0) {
+        tma_prefetch_desc(&maps.x);
+        tma_prefetch_desc(&maps.w);
+        mbar_init(x_full, 1);
+        for (int i = 0; i < CC_WSTAGES; ++i) {
+            mbar_init(full + i, 1);
+            mbar_init(empty + i, 8);                   // one arrival per consumer warp
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {                               // ===== TMA producer: the halo tiles, then the taps' weight slices =====
+            mbar_arrive_expect_tx(x_full, L.kt * x_floats * 4);
+            for (int jt = 0; jt < L.kt; ++jt)
+                tma_load_5d(const_cast<float*>(s_x) + jt * x_floats, &maps.x, x_full, y0 - 4, x0 - 1, t + jt + L.t_off, 0, b);
+            for (int j = 0; j < taps; ++j) {
+                const int st = j % CC_WSTAGES, use = j / CC_WSTAGES;
+                if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
+                mbar_arrive_expect_tx(full + st, w_bytes);
+                for (int a = 0; a < L.ka; ++a) tma_load_3d_sw(s_w + st * w_bytes + a * N * 128, &maps.w, full + st, 0, 0, j * L.ka + a);
+            }
+        }
+        return;
+    }
+
+    // ===== consumers: warp w of warpgroup g owns tile row 4g + w; accumulator rows 16w + lane/4 (+ 8) = columns lane/4 (+ 8) =====
+    const int row = 4 * (warp >> 2) + (warp & 3);
+    const int col = lane >> 2, kq = lane & 3;
+    const int nks = L.kpad / 8;
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    mbar_wait(x_full, 0);
+#pragma unroll 1
+    for (int j = 0; j < taps; ++j) {
+        const int st = j % CC_WSTAGES, use = j / CC_WSTAGES;
+        const int jt = j / 9, ay = j / 3 % 3, ax = j % 3;
+        const float* h = s_x + jt * x_floats + (row + ay) * CC_HY + col + ax + CC_HY_OFF + kq * CC_PLANE;
+        const uint32_t wb = smem_addr(s_w + st * w_bytes);
+        mbar_wait(full + st, use & 1);
+#pragma unroll 1
+        for (int a = 0; a < L.ka; ++a) {               // 32 channels (4 k-steps) at a time
+            uint32_t fr[4][4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float* hk = h + (32 * a + 8 * k) * CC_PLANE;
+                const bool on = 4 * a + k < nks;
+                fr[k][0] = on ? to_tf32(hk[0]) : 0u;
+                fr[k][1] = on ? to_tf32(hk[8]) : 0u;
+                fr[k][2] = on ? to_tf32(hk[4 * CC_PLANE]) : 0u;
+                fr[k][3] = on ? to_tf32(hk[4 * CC_PLANE + 8]) : 0u;
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                if (4 * a + k < nks) wgmma_tf32_rs<N>(acc, fr[k], gmma_desc_sw128(wb + a * N * 128 + k * 32, 16, 1024));
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        wgmma_fence_operands(acc);
+        __syncwarp();
+        if (lane == 0) cc_arrive(empty + st);          // this warp is done with the slice
+    }
+
+    const int gx = x0 + row;
+    if (gx >= L.X) return;
+    const size_t plane = static_cast<size_t>(L.X) * L.Y;
+#pragma unroll
+    for (int jn = 0; jn < N / 8; ++jn)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int c = 8 * jn + 2 * kq + e;
+            if (c >= L.n_out) continue;
+            float* dst = out + ((static_cast<size_t>(b) * L.n_out + c) * L.frames + t) * plane + static_cast<size_t>(gx) * L.Y + y0 + col;
+            if (y0 + col < L.Y) dst[0] = acc[4 * jn + e];
+            if (y0 + col + 8 < L.Y) dst[8] = acc[4 * jn + 2 + e];
+        }
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// weight gradient
+// ------------------------------------------------------------------------------------------------------------------------------
+struct CcWgradMaps {
+    CUtensorMap gy;                                // (Y, X, s, C_out, b), box (32, 1, 1, NO, 1), swizzle 128B
+    CUtensorMap x;                                 // (Y, X, s, C_in, b), box (44, 1, 1, 64, 1), no swizzle
+};
+
+static long long cc_wgrad_tiles(const CcShape& s) {
+    return static_cast<long long>(s.batch) * s.frames * s.X * ((s.Y + CC_WG_PX - 1) / CC_WG_PX);
+}
+static size_t cc_partial_floats(const CcShape& s) { return static_cast<size_t>(s.taps) * s.cout * s.cin; }
+
+size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d) {
+    const CcShape s = cc_shape(d);
+    return static_cast<size_t>(wgrad_chunks(cc_wgrad_tiles(s))) * cc_partial_floats(s) * sizeof(float);
+}
+
+// grid (chunks, 3 kt): CTA (chunk, tau * 3 + dy) accumulates the taps (tau, dy, 0..2) over its chunk's tiles as D (input channels x
+// NO output channels) = x_tap gy^T.  Per tile the stage holds the x row run of frame t + tau - (kt - 1), row x + dy - 1 (64 channel rows
+// of 44 columns, read as the register A operand at column offset dx + 3) and the gy run (NO K-major rows of 32 pixels, the B operand).
+// Thread 0 issues the loads: at iteration i, after the barrier that ends the MMAs on tile i - 1, tile i + stages - 1 into that tile's
+// stage.
+template <int NO>
+__global__ void __launch_bounds__(128, 1)
+causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, float* __restrict__ partial, int n_tiles) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    constexpr int STAGE_BYTES = CC_WG_X_BYTES + NO * 128;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + CC_WG_STAGES * STAGE_BYTES);
+    const int tau = blockIdx.y / 3, dy = blockIdx.y % 3;
+    const int t0 = static_cast<int>(static_cast<long long>(blockIdx.x) * n_tiles / gridDim.x);
+    const int t1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * n_tiles / gridDim.x);
+    const int runs = (s.Y + CC_WG_PX - 1) / CC_WG_PX;
+
+    auto load = [&](int i) {                       // tile t0 + i = ((b * s + t) * X + x) * runs + run, into stage i % stages
+        int t = t0 + i;
+        const int run = t % runs;
+        t /= runs;
+        const int x = t % s.X, f = t / s.X, b = f / s.frames, tt = f % s.frames;
+        unsigned char* dst = smem + (i % CC_WG_STAGES) * STAGE_BYTES;
+        uint64_t* bar = full + i % CC_WG_STAGES;
+        mbar_arrive_expect_tx(bar, STAGE_BYTES);
+        tma_load_5d(dst, &maps.x, bar, CC_WG_PX * run - 4, x + dy - 1, tt + tau - (s.kt - 1), 0, b);
+        tma_load_5d(dst + CC_WG_X_BYTES, &maps.gy, bar, CC_WG_PX * run, x, tt, 0, b);
+    };
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&maps.gy);
+        tma_prefetch_desc(&maps.x);
+        for (int i = 0; i < CC_WG_STAGES; ++i) mbar_init(full + i, 1);
+        fence_mbar_init();
+        for (int i = 0; i < CC_WG_STAGES - 1 && t0 + i < t1; ++i) load(i);
+    }
+    __syncthreads();
+
+    const int w4 = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int ra = 16 * w4 + (lane >> 2), kq = lane & 3;   // A fragment: channel rows ra, ra + 8; pixel columns kq, kq + 4
+    float acc[3][NO / 2];
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx)
+#pragma unroll
+        for (int i = 0; i < NO / 2; ++i) acc[dx][i] = 0.f;
+
+    for (int i = 0; t0 + i < t1; ++i) {
+        __syncthreads();                           // every warp is done with tile i - 1: its stage may be refilled
+        if (threadIdx.x == 0 && t0 + i + CC_WG_STAGES - 1 < t1) load(i + CC_WG_STAGES - 1);
+        const int st = i % CC_WG_STAGES;
+        mbar_wait(full + st, (i / CC_WG_STAGES) & 1);
+        const float* xs = reinterpret_cast<const float*>(smem + st * STAGE_BYTES) + ra * CC_WG_XP + kq + 3;
+        const uint32_t g_addr = smem_addr(smem + st * STAGE_BYTES + CC_WG_X_BYTES);
+        uint32_t a[CC_WG_PX / 8][3][4];
+#pragma unroll
+        for (int ks = 0; ks < CC_WG_PX / 8; ++ks)
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+                const float* p = xs + 8 * ks + dx;
+                a[ks][dx][0] = to_tf32(p[0]);
+                a[ks][dx][1] = to_tf32(p[8 * CC_WG_XP]);
+                a[ks][dx][2] = to_tf32(p[4]);
+                a[ks][dx][3] = to_tf32(p[8 * CC_WG_XP + 4]);
+            }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < CC_WG_PX / 8; ++ks) {
+            const uint64_t db = gmma_desc_sw128(g_addr + 32 * ks, 16, 1024);
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) wgmma_tf32_rs<NO>(acc[dx], a[ks][dx], db);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) wgmma_fence_operands(acc[dx]);
+    }
+
+    // this chunk's partial: accumulator (row = input channel ci, column = output channel o) of tap (tau, dy, dx) ->
+    // partial[chunk][tap][o][ci]
+    const size_t n_oi = static_cast<size_t>(s.cout) * s.cin;
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx) {
+        float* dst = partial + (static_cast<size_t>(blockIdx.x) * s.taps + 9 * tau + 3 * dy + dx) * n_oi;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int ci = ra + 8 * half;
+            if (ci >= s.cin) continue;
+#pragma unroll
+            for (int jn = 0; jn < NO / 8; ++jn)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int o = 8 * jn + 2 * kq + e;
+                    if (o < s.cout) dst[static_cast<size_t>(o) * s.cin + ci] = acc[dx][4 * jn + 2 * half + e];
+                }
+        }
+    }
+}
+
+// grad_w (C_out, C_in, kt, 3, 3) = sum of the chunks' partials in ascending chunk order (zeros when there are none)
+__global__ void causal_conv_wgrad_reduce_kernel(const CcShape s, const float* __restrict__ partial, int n_chunks, float* __restrict__ gw) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s.cout * s.cin * s.taps) return;
+    const int tap = i % s.taps, oi = i / s.taps;     // oi = o * cin + ci
+    const size_t stride = static_cast<size_t>(s.taps) * s.cout * s.cin;
+    const size_t off = static_cast<size_t>(tap) * s.cout * s.cin + oi;
+    float acc = 0.f;
+    for (int c = 0; c < n_chunks; ++c) acc += partial[c * stride + off];
+    gw[i] = acc;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// host
+// ------------------------------------------------------------------------------------------------------------------------------
+static int cc_encode(encode_tiled_fn fn, CUtensorMap* map, const float* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+                     const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* what) {
+    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<float*>(base), dims, strides_bytes, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (causal conv %s) failed with CUresult %d", what, (int)r);
+    return FIERY_OK;
+}
+
+// a contiguous (b, C, s, X, Y) activation as the 5-D map (Y, X, s, C, b)
+static int cc_encode_activation(encode_tiled_fn fn, CUtensorMap* map, const CcShape& s, const float* t, int channels, cuuint32_t box_y,
+                                cuuint32_t box_x, cuuint32_t box_c, CUtensorMapSwizzle swizzle, const char* what) {
+    const cuuint64_t Y = s.Y, X = s.X, S = s.frames, C = channels;
+    cuuint64_t dims[5] = {Y, X, S, C, static_cast<cuuint64_t>(s.batch)};
+    cuuint64_t strides[4] = {Y * 4, X * Y * 4, S * X * Y * 4, C * S * X * Y * 4};
+    cuuint32_t box[5] = {box_y, box_x, 1, box_c, 1};
+    return cc_encode(fn, map, t, 5, dims, strides, box, swizzle, what);
+}
+
+static int cc_sm_attr(const void* kernel, int smem) {
+    FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    return FIERY_OK;
+}
+
+// forward (dgrad = 0): x (C_in channels) -> y (C_out) with pack F; input gradient (dgrad = 1): gy (C_out) -> gx (C_in) with pack T
+static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const float* in, const float* packed, float* out, cudaStream_t stream) {
+    const CcShape s = cc_shape(d);
+    const CcPackDir f = cc_pack_dir(s.cout, s.cin, s.taps);
+    const CcPackDir p = dgrad ? cc_pack_dir(s.cin, s.cout, s.taps) : f;
+    const float* w = dgrad ? packed + f.floats : packed;
+    encode_tiled_fn fn = conv_encode_fn();
+    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    CcFwdMaps maps;
+    int rc = cc_encode_activation(fn, &maps.x, s, in, dgrad ? s.cout : s.cin, CC_HY, CC_HX, static_cast<cuuint32_t>(p.kpad),
+                                  CU_TENSOR_MAP_SWIZZLE_NONE, dgrad ? "output gradient" : "input");
+    if (rc != FIERY_OK) return rc;
+    {
+        cuuint64_t dims[3] = {32, static_cast<cuuint64_t>(p.n), static_cast<cuuint64_t>(s.taps) * p.ka};
+        cuuint64_t strides[2] = {128, static_cast<cuuint64_t>(p.n) * 128};
+        cuuint32_t box[3] = {32, static_cast<cuuint32_t>(p.n), 1};
+        if ((rc = cc_encode(fn, &maps.w, w, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) != FIERY_OK) return rc;
+    }
+    CcFwdLaunch L;
+    L.frames = s.frames;
+    L.X = s.X;
+    L.Y = s.Y;
+    L.kpad = p.kpad;
+    L.ka = p.ka;
+    L.n_out = dgrad ? s.cin : s.cout;
+    L.kt = s.kt;
+    L.t_off = dgrad ? 0 : -(s.kt - 1);
+    L.tiles_x = (s.X + CC_TX - 1) / CC_TX;
+    L.tiles_y = (s.Y + CC_TY - 1) / CC_TY;
+    const long long n_tiles = static_cast<long long>(s.batch) * s.frames * L.tiles_x * L.tiles_y;
+    FIERY_REQUIRE(n_tiles < (1ll << 31), "causal conv: too many pixel tiles");
+    const int smem = CC_WSTAGES * p.ka * p.n * 128 + s.kt * p.kpad * CC_PLANE * 4 + CC_SMEM_SLACK;
+    switch (p.n) {
+#define CC_FWD_CASE(N)                                                                                                             \
+    case N:                                                                                                                        \
+        if ((rc = cc_sm_attr(reinterpret_cast<const void*>(causal_conv_fwd_kernel<N>), smem)) != FIERY_OK) return rc;             \
+        causal_conv_fwd_kernel<N><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L, out);                 \
+        break;
+        CC_FWD_CASE(8) CC_FWD_CASE(16) CC_FWD_CASE(24) CC_FWD_CASE(32) CC_FWD_CASE(40) CC_FWD_CASE(48) CC_FWD_CASE(56) CC_FWD_CASE(64)
+#undef CC_FWD_CASE
+        default: return set_error(FIERY_E_INVALID, "causal conv: %d channels padded to %d", L.n_out, p.n);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream) {
+    return cc_launch_conv(d, 0, x, packed, y, stream);
+}
+
+int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream) {
+    return cc_launch_conv(d, 1, gy, packed, gx, stream);
+}
+
+int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const float* gy, float* gw, void* workspace,
+                             cudaStream_t stream) {
+    const CcShape s = cc_shape(d);
+    const long long tiles = cc_wgrad_tiles(s);
+    const int n_chunks = wgrad_chunks(tiles);
+    float* partial = static_cast<float*>(workspace);
+    if (n_chunks > 0) {
+        FIERY_REQUIRE(tiles < (1ll << 31), "causal conv: too many pixel tiles");
+        encode_tiled_fn fn = conv_encode_fn();
+        if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+        const int no = cc_round8(s.cout);
+        CcWgradMaps maps;
+        int rc = cc_encode_activation(fn, &maps.gy, s, gy, s.cout, CC_WG_PX, 1, static_cast<cuuint32_t>(no), CU_TENSOR_MAP_SWIZZLE_128B,
+                                      "output gradient");
+        if (rc == FIERY_OK)
+            rc = cc_encode_activation(fn, &maps.x, s, x, s.cin, CC_WG_XP, 1, 64, CU_TENSOR_MAP_SWIZZLE_NONE, "input");
+        if (rc != FIERY_OK) return rc;
+        const int smem = CC_WG_STAGES * (CC_WG_X_BYTES + no * 128) + CC_SMEM_SLACK;
+        const dim3 grid(static_cast<unsigned>(n_chunks), static_cast<unsigned>(3 * s.kt));
+        switch (no) {
+#define CC_WG_CASE(N)                                                                                                              \
+    case N:                                                                                                                        \
+        if ((rc = cc_sm_attr(reinterpret_cast<const void*>(causal_conv_wgrad_kernel<N>), smem)) != FIERY_OK) return rc;           \
+        causal_conv_wgrad_kernel<N><<<grid, 128, smem, stream>>>(maps, s, partial, static_cast<int>(tiles));                        \
+        break;
+            CC_WG_CASE(8) CC_WG_CASE(16) CC_WG_CASE(24) CC_WG_CASE(32) CC_WG_CASE(40) CC_WG_CASE(48) CC_WG_CASE(56) CC_WG_CASE(64)
+#undef CC_WG_CASE
+            default: return set_error(FIERY_E_INVALID, "causal conv: out_channels padded to %d", no);
+        }
+        FIERY_CUDA_CHECK(cudaGetLastError());
+    }
+    const int n_red = s.cout * s.cin * s.taps;
+    causal_conv_wgrad_reduce_kernel<<<(n_red + 255) / 256, 256, 0, stream>>>(s, partial, n_chunks, gw);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+}  // namespace fiery

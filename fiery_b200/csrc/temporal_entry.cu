@@ -26,6 +26,7 @@
 // same MMAs.  The 64-pixel tiles are cut into chunks whose boundaries depend on (frames, X*Y) only; each chunk stores its partial and a
 // reduce kernel adds the partials in ascending chunk order: bit-reproducible, no atomics.
 #include "bev_conv.cuh"
+#include "wgrad_chunks.cuh"
 
 namespace fiery {
 
@@ -36,7 +37,6 @@ constexpr int TE_STG_PITCH = 66;                   // staging row pitch (floats)
 constexpr int TE_STG_FLOATS = 32 * TE_STG_PITCH;   // 32 channels x 64 pixels
 constexpr int TE_SMEM_MAX = 232448;                // sm_90 opt-in shared memory per block
 constexpr int TE_SMEM_SLACK = 1024 + 256;          // alignment + barriers
-constexpr int TE_WG_MAX_CHUNKS = 128;              // weight-gradient chunks (fixed: the summation order is device independent)
 constexpr int TE_ROW_TABLE_BYTES = 2 * 256 * (8 + 4);   // forward: per warpgroup and padded output row, destination + bias
 
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
@@ -452,10 +452,7 @@ struct TeWgradMaps {
 static long long te_bwd_tiles(int n_frames, int pixels) {
     return static_cast<long long>(n_frames) * ((pixels + TE_BWD_PX - 1) / TE_BWD_PX);
 }
-static int te_wgrad_chunks(int n_frames, int pixels) {
-    const long long t = te_bwd_tiles(n_frames, pixels);
-    return static_cast<int>(t < TE_WG_MAX_CHUNKS ? t : TE_WG_MAX_CHUNKS);
-}
+static int te_wgrad_chunks(int n_frames, int pixels) { return wgrad_chunks(te_bwd_tiles(n_frames, pixels)); }
 // partial: (Nrows = round64(Npad)) x (Kx = round64(K + E)) floats per chunk
 static size_t te_partial_floats(const TeShape& s) {
     return static_cast<size_t>(round_up(s.Npad, 64)) * round_up(s.K + s.E, 64);

@@ -159,6 +159,43 @@ def use_tensor_core_temporal_model(model):
     return model
 
 
+def use_tensor_core_causal_convs(model):
+    """Replace every covered ``CausalConv3d`` under ``model.temporal_model.model`` of a ``Fiery`` instance -- ``convolution_paths[0][1]``
+    and ``[1][1]`` of each ``TemporalBlock`` or ``TensorCoreTemporalBlock``, and ``layers.conv`` of each ``Bottleneck3D``
+    (INBETWEEN_LAYERS > 0) -- by ``fiery_b200.causal_conv.TensorCoreCausalConv3d``, which adopts the module's children
+    (``state_dict`` keys unchanged) and runs its pad and (kt, 3, 3) convolution on the tensor cores, forward and backward.  Works before
+    or after ``use_tensor_core_temporal_model``.  Returns the model; a second call does nothing, and modules the kernels do not cover
+    (more than 64 channels, another kernel size, a bias) are left alone with one warning."""
+    from .causal_conv import TensorCoreCausalConv3d, module_reason
+    blocks = getattr(model.temporal_model, "model", None)
+    if blocks is None:
+        return model
+    skipped = []
+    for i, block in enumerate(blocks):
+        kind = type(block).__name__
+        if kind in ("TemporalBlock", "TensorCoreTemporalBlock"):
+            slots = [(block.convolution_paths[p], 1, f"block {i} path {p}") for p in (0, 1)]
+        elif kind == "Bottleneck3D":
+            slots = [(block.layers, "conv", f"block {i} bottleneck")]
+        else:
+            continue
+        for parent, key, where in slots:
+            m = parent[key] if isinstance(key, int) else getattr(parent, key)
+            if isinstance(m, TensorCoreCausalConv3d):
+                continue
+            reason = module_reason(m)
+            if reason is not None:
+                skipped.append(f"{where}: {reason}")
+            elif isinstance(key, int):
+                parent[key] = TensorCoreCausalConv3d(m)
+            else:
+                setattr(parent, key, TensorCoreCausalConv3d(m))
+    if skipped:
+        _warn_once(("causal", tuple(skipped)), "fiery_b200: CausalConv3d module(s) not covered by the tensor-core kernels, left as is: "
+                   + "; ".join(skipped))
+    return model
+
+
 def uninstall():
     if not _saved:
         return

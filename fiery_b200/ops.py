@@ -253,3 +253,66 @@ def _temporal_entry_backward(ctx, grads):
 
 temporal_entry.register_autograd(_temporal_entry_backward, setup_context=_temporal_entry_setup_context)
 torch.library.register_autocast("fiery_b200::temporal_entry", "cuda", torch.float32)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# The temporal model's causal convolution (CausalConv3d's pad + Conv3d, fiery/layers/temporal.py:65-85) as dispatcher operators:
+# ``torch.ops.fiery_b200.causal_conv3d`` / ``causal_conv3d_backward`` (fiery_b200/causal_conv.py; kernels in csrc/causal_conv.cu).
+# Autocast: the operator runs in fp32 (TF32 tensor-core operands, fp32 accumulation), as temporal_entry does.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::causal_conv3d", mutates_args=(), device_types="cuda")
+def causal_conv3d(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """x (b, C_in, s, X, Y), Y % 4 == 0; weight (C_out, C_in, kt, 3, 3), kt 1 or 2.  Returns the contiguous (b, C_out, s, X, Y) fp32
+    ``Conv3d(ConstantPad3d((1, 1, 1, 1, kt - 1, 0))(x))``.  A non-contiguous or 16-bit x is read from a contiguous fp32 copy; the
+    weight's pack is made at most once per weight version."""
+    from .causal_conv import conv_forward
+    return conv_forward(x, weight)
+
+
+@causal_conv3d.register_fake
+def _(x, weight):
+    b, _, s, h, w = x.shape
+    return x.new_empty((b, weight.shape[0], s, h, w), dtype=torch.float32)
+
+
+@torch.library.custom_op("fiery_b200::causal_conv3d_backward", mutates_args=(), device_types="cuda")
+def causal_conv3d_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, need_input: bool,
+                           need_weight: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(grad_x, grad_weight) of ``causal_conv3d``; a gradient that is not asked for is not computed and comes back empty.  grad_x: x's
+    shape and dtype, contiguous; grad_weight: the weight's shape and dtype, bit-reproducible (no atomics)."""
+    from .causal_conv import conv_backward_data, conv_backward_weight
+    grad_x, grad_w = x.new_empty((0,)), weight.new_empty((0,))
+    if need_input:
+        grad_x = conv_backward_data(grad_y, tuple(x.shape), weight)
+        if grad_x.dtype != x.dtype:
+            grad_x = grad_x.to(x.dtype)
+    if need_weight:
+        grad_w = conv_backward_weight(grad_y, x, weight)
+        if grad_w.dtype != weight.dtype:
+            grad_w = grad_w.to(weight.dtype)
+    return grad_x, grad_w
+
+
+@causal_conv3d_backward.register_fake
+def _(grad_y, x, weight, need_input, need_weight):
+    grad_x = x.new_empty(x.shape) if need_input else x.new_empty((0,))
+    grad_w = weight.new_empty(weight.shape) if need_weight else weight.new_empty((0,))
+    return grad_x, grad_w
+
+
+def _causal_conv3d_setup_context(ctx, inputs, output):
+    x, weight = inputs
+    ctx.save_for_backward(x, weight)
+
+
+def _causal_conv3d_backward(ctx, grad_y):
+    x, weight = ctx.saved_tensors
+    need_input, need_weight = bool(ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1])
+    if not (need_input or need_weight):
+        return None, None
+    grad_x, grad_w = torch.ops.fiery_b200.causal_conv3d_backward(grad_y, x, weight, need_input, need_weight)
+    return (grad_x if need_input else None), (grad_w if need_weight else None)
+
+
+causal_conv3d.register_autograd(_causal_conv3d_backward, setup_context=_causal_conv3d_setup_context)
+torch.library.register_autocast("fiery_b200::causal_conv3d", "cuda", torch.float32)

@@ -100,20 +100,22 @@ def _stacked(weights: Sequence[torch.Tensor]) -> torch.Tensor:
     return torch.cat([w.detach().float().reshape(w.shape[0], -1) for w in weights], 0).contiguous()
 
 
-# (device, weights' data_ptrs, in_channels) -> [versions, weight aliases, pack].  The aliases keep the weights' memory alive, so an
-# address in the cache cannot be taken by another tensor while its entry exists; a version counter changes with each in-place update
-# (an optimizer step), so a pack is made at most once per weight version.
+# (pack function, device, in_channels, weights' data_ptrs) -> [versions, weight aliases, pack].  The aliases keep the weights' memory
+# alive, so an address in the cache cannot be taken by another tensor while its entry exists; a version counter changes with each
+# in-place update (an optimizer step), so a pack is made at most once per weight version.
 _PACKS: "OrderedDict[tuple, list]" = OrderedDict()
 _PACKS_MAX = 16
 
 
-def packed_weights(weights: Sequence[torch.Tensor], in_channels: int) -> torch.Tensor:
-    """The device pack of the stacked weights (fiery_temporal_entry_pack_weights), made at most once per weight version."""
-    key = (str(weights[0].device), in_channels) + tuple(w.data_ptr() for w in weights)
+def packed_weights(weights: Sequence[torch.Tensor], in_channels: int, pack=None) -> torch.Tensor:
+    """The device pack ``pack(weights, in_channels)`` (default: the temporal entry's, fiery_temporal_entry_pack_weights), made at
+    most once per weight version.  The causal convolution (fiery_b200/causal_conv.py) keeps its packs here too."""
+    pack = pack_weights if pack is None else pack
+    key = (pack, str(weights[0].device), in_channels) + tuple(w.data_ptr() for w in weights)
     versions = tuple(w._version for w in weights)
     entry = _PACKS.get(key)
     if entry is None or entry[0] != versions or any(tuple(a.shape) != tuple(w.shape) for a, w in zip(entry[1], weights)):
-        entry = [versions, [w.detach() for w in weights], pack_weights(weights, in_channels)]
+        entry = [versions, [w.detach() for w in weights], pack(weights, in_channels)]
         _PACKS[key] = entry
         while len(_PACKS) > _PACKS_MAX:
             _PACKS.popitem(last=False)

@@ -351,6 +351,51 @@ FIERY_API size_t fiery_temporal_entry_backward_weight_workspace_bytes(const fier
 FIERY_API int fiery_temporal_entry_backward_weight(const fiery_temporal_entry_desc_t* desc, const float* x, const float* extra,
                                                    const float* const* grad_out, float* grad_w, void* workspace, void* stream);
 
+/*
+ * The temporal model's causal convolution (CausalConv3d, fiery/layers/temporal.py:65-85) without its BatchNorm and ReLU: a zero pad of
+ * kt - 1 frames in front and one pixel around the map, then a bias-free Conv3d with kernel (kt, 3, 3), stride 1, dilation 1:
+ *   y[b, o, t, p] = sum_{i, tau, dy, dx} W[o, i, tau, dy, dx] * x[b, i, t + tau - (kt - 1), p + (dy - 1, dx - 1)]
+ * (terms outside the tensor are zero).  wgmma, TF32 operands, fp32 accumulation; W is rounded to TF32 (nearest, ties away) when
+ * packed, and so are x in the forward and the weight gradient and grad_y in backward_data; grad_y in the weight gradient is
+ * truncated by the tensor core.
+ *
+ * x / grad_x: (batch, in_channels, frames, grid_x, grid_y) fp32, contiguous; y / grad_y: (batch, out_channels, frames, grid_x, grid_y)
+ * fp32, contiguous; weight / grad_w: (out_channels, in_channels, kt, 3, 3) fp32, contiguous.
+ * Limits (rejected with FIERY_E_INVALID and a message naming the field): 1 <= in_channels, out_channels <= 64; kt 1 or 2; grid_x >= 1;
+ * grid_y a positive multiple of 4 (16-byte TMA row pitch); pointers 16-byte aligned.  batch * frames == 0 is a no-op (the weight
+ * gradient is then zero).
+ *
+ * fiery_causal_conv3d_packed_bytes / fiery_causal_conv3d_pack_weights: the device pack of W that forward and backward_data take.
+ * fiery_causal_conv3d_forward: y fully overwritten.
+ * fiery_causal_conv3d_backward_data: grad_x = the adjoint of the forward applied to grad_y, fully overwritten.
+ * fiery_causal_conv3d_backward_weight: grad_w[o, i, tau, dy, dx] = sum over batch, frames and pixels of grad_y[b, o, t, p] *
+ * x[b, i, t + tau - (kt - 1), p + (dy - 1, dx - 1)], fully overwritten.  workspace: fiery_causal_conv3d_backward_weight_workspace_bytes
+ * (desc) bytes (0 for 0 frames), contents irrelevant.  Summation order: the pixels are cut into tiles of 32 consecutive grid_y
+ * positions of one map row, numbered (b, t, x, run) with the run fastest, and the tiles into c = min(tiles, 128) chunks, chunk i
+ * holding tiles [i * tiles / c, (i + 1) * tiles / c); a chunk's partial is the tensor core's fp32 accumulation over its tiles in
+ * ascending order, and grad_w the fp32 sum of the partials in ascending chunk order.  The order depends on the shape only:
+ * bit-reproducible, graph-capturable, no host synchronisation.
+ */
+typedef struct {
+    int32_t batch;
+    int32_t frames;
+    int32_t grid_x;               /* X: map rows */
+    int32_t grid_y;               /* Y: map columns, contiguous */
+    int32_t in_channels;
+    int32_t out_channels;
+    int32_t kt;                   /* time taps: 2 for the (2, 3, 3) convolution, 1 for (1, 3, 3) */
+} fiery_causal_conv3d_desc_t;
+
+FIERY_API size_t fiery_causal_conv3d_packed_bytes(const fiery_causal_conv3d_desc_t* desc);
+FIERY_API int fiery_causal_conv3d_pack_weights(const fiery_causal_conv3d_desc_t* desc, const float* weight, void* packed, void* stream);
+FIERY_API int fiery_causal_conv3d_forward(const fiery_causal_conv3d_desc_t* desc, const float* x, const void* packed, float* y,
+                                          void* stream);
+FIERY_API int fiery_causal_conv3d_backward_data(const fiery_causal_conv3d_desc_t* desc, const float* grad_y, const void* packed,
+                                                float* grad_x, void* stream);
+FIERY_API size_t fiery_causal_conv3d_backward_weight_workspace_bytes(const fiery_causal_conv3d_desc_t* desc);
+FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc_t* desc, const float* x, const float* grad_y,
+                                                  float* grad_w, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
