@@ -112,7 +112,7 @@ __device__ __forceinline__ void cc_arrive(uint64_t* bar) {
 // forward and input gradient
 // ------------------------------------------------------------------------------------------------------------------------------
 struct CcFwdMaps {
-    CUtensorMap x;                                 // input (Y, X, s, C, b), box (20, 10, 1, kpad, 1), no swizzle
+    CUtensorMap x;                                 // input (Y, X, s, C, b), box (28, 10, 1, kpad, 1) = CC_HY x CC_HX, no swizzle
     CUtensorMap w;                                 // pack (32, n, taps * ka), box (32, n, 1), swizzle 128B
 };
 struct CcFwdLaunch {
