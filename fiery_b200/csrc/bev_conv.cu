@@ -60,8 +60,8 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
                 // input patch of this tap: pixels (2*oy + r - 3, 2*ox + s - 3); negative / too large coordinates read as zero
                 tma_load_4d(a, &maps.x, full + st, 0, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
                 tma_load_4d(a + CV_A_ATOM, &maps.x, full + st, 32, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
-                tma_load_3d_sw(bw, &maps.w, full + st, 0, 0, it);
-                tma_load_3d_sw(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, it);
+                tma_load_3d(bw, &maps.w, full + st, 0, 0, it);
+                tma_load_3d(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, it);
             }
         }
         return;
@@ -82,14 +82,14 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
         for (int atom = 0; atom < 2; ++atom) {
 #pragma unroll
             for (int k = 0; k < 4; ++k)               // 8 TF32 values (32 bytes) per MMA along K
-                wgmma_m64n64k8_tf32_ss(acc, gmma_desc_sw128(a_addr + atom * CV_A_ATOM + 32 * k, 16, 1024),
-                                       gmma_desc_sw128(b_addr + atom * CV_B_ATOM + 32 * k, 16, 1024));
+                wgmma_tf32_ss<64>(acc, gmma_desc_sw128(a_addr + atom * CV_A_ATOM + 32 * k, 16, 1024),
+                                  gmma_desc_sw128(b_addr + atom * CV_B_ATOM + 32 * k, 16, 1024));
         }
         wgmma_commit();
         if (it > 0) {                                 // the previous tap's MMAs are complete: its stage may be refilled
             wgmma_wait<1>();
             __syncwarp();
-            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + (it - 1) % CV_STAGES)) : "memory");
+            if (lane == 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
         }
     }
     wgmma_wait<0>();
@@ -124,9 +124,7 @@ __global__ void pack_conv_weights_kernel(const float* __restrict__ w, float* __r
     const int in = i % CV_C, out = (i / CV_C) % CV_C, tap = i / (CV_C * CV_C);
     // rounded to TF32 (nearest, ties away) here, once per weight update: the tensor core would otherwise TRUNCATE the low mantissa
     // bits of an fp32 operand.  (The activations stay as the lift wrote them -- a rounding pass over 82 MB is not worth 1.5e-4.)
-    unsigned r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(w[(static_cast<size_t>(out) * CV_C + in) * CV_TAPS + tap]));
-    packed[i] = __uint_as_float(r);
+    packed[i] = __uint_as_float(to_tf32(w[(static_cast<size_t>(out) * CV_C + in) * CV_TAPS + tap]));
 }
 
 int launch_pack_conv_weights(const float* w_oihw, float* packed, cudaStream_t stream) {
@@ -143,19 +141,14 @@ int launch_bev_conv(int n_frames, int H, int W, const float* x_nhwc, const float
     FIERY_REQUIRE((scale == nullptr) == (shift == nullptr), "bev conv: scale and shift go together");
     FIERY_REQUIRE((reinterpret_cast<uintptr_t>(x_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_packed) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(y_nhwc) & 15) == 0, "bev conv: pointers must be 16-byte aligned");
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const int Ho = (H + 2 * 3 - 7) / 2 + 1, Wo = (W + 2 * 3 - 7) / 2 + 1;
     ConvMaps maps;
-    int rc = encode_conv_activation_map(fn, &maps.x, x_nhwc, n_frames, H, W, 2 * CV_TW, 2 * CV_TH, 2, 2, "conv input");
-    if (rc == FIERY_OK) rc = encode_conv_weight_map(fn, &maps.w, w_packed, "conv weights");
+    int rc = encode_conv_activation_map(&maps.x, x_nhwc, n_frames, H, W, 2 * CV_TW, 2 * CV_TH, 2, 2, "conv input");
+    if (rc == FIERY_OK) rc = encode_conv_weight_map(&maps.w, w_packed, "conv weights");
     if (rc != FIERY_OK) return rc;
     const int smem = CV_STAGES * CV_STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
     static OncePerDevice once;
-    rc = once.run([smem]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(bev_conv7x7s2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        return FIERY_OK;
-    });
+    rc = once.run([smem]() { return set_dynamic_smem(bev_conv7x7s2_kernel, smem); });
     if (rc != FIERY_OK) return rc;
     const int tiles_x = (Wo + CV_TW - 1) / CV_TW, tiles_y = (Ho + CV_TH - 1) / CV_TH;
     bev_conv7x7s2_kernel<<<static_cast<unsigned>(n_frames * tiles_x * tiles_y), CV_THREADS, smem, stream>>>(maps, scale, shift, relu, y_nhwc,

@@ -1,7 +1,6 @@
 // Constants and host helpers shared by the first BEV convolution's forward (bev_conv.cu) and backward (bev_conv_bwd.cu):
 // Conv2d(64, 64, kernel_size=7, stride=2, padding=3, bias=False) on channel-last fp32 tensors, wgmma TF32.
 #pragma once
-#include "lift_plan.cuh"
 #include "wgmma.cuh"
 
 namespace fiery {
@@ -22,62 +21,25 @@ struct ConvMaps {
     CUtensorMap w;       // (I, O, tap) fp32, box (32, 64, 1), swizzle 128B
 };
 
-__device__ __forceinline__ void tma_load_3d_sw(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-
-// fp32 -> TF32, round to nearest with ties away from zero (the tensor core itself truncates an fp32 operand's low mantissa bits)
-__device__ __forceinline__ uint32_t to_tf32(float v) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return r;
-}
-
-typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-inline encode_tiled_fn conv_encode_fn() {
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        cudaFree(nullptr);
-        ctx_bound = true;
-    }
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-        return nullptr;
-    return reinterpret_cast<encode_tiled_fn>(sym);
-}
-
 // A channel-last fp32 activation (n_frames, H, W, 64) as a 4-D map (C, W, H, B): box (32, box_w, box_h, 1) traversed with element
 // strides (1, stride_w, stride_h, 1), 128-byte swizzle; coordinates outside the tensor read as zero (the convolution's padding)
-inline int encode_conv_activation_map(encode_tiled_fn fn, CUtensorMap* map, const float* t, int n_frames, int H, int W, int box_w,
-                                      int box_h, int stride_w, int stride_h, const char* what) {
+inline int encode_conv_activation_map(CUtensorMap* map, const float* t, int n_frames, int H, int W, int box_w, int box_h, int stride_w,
+                                      int stride_h, const char* what) {
     cuuint64_t dims[4] = {CV_C, static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(n_frames)};
     cuuint64_t strides[3] = {CV_C * 4ull, static_cast<cuuint64_t>(W) * CV_C * 4ull, static_cast<cuuint64_t>(H) * W * CV_C * 4ull};
     cuuint32_t box[4] = {32, static_cast<cuuint32_t>(box_w), static_cast<cuuint32_t>(box_h), 1};
     cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride_w), static_cast<cuuint32_t>(stride_h), 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(t), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (%s) failed with CUresult %d", what, (int)r);
-    return FIERY_OK;
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, t, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 // A packed weight (tap, N rows, 64 K) fp32 as a 3-D map, box (32, 64, 1): one tap's K-major B operand, half the K range per load
-inline int encode_conv_weight_map(encode_tiled_fn fn, CUtensorMap* map, const float* packed, const char* what) {
+inline int encode_conv_weight_map(CUtensorMap* map, const float* packed, const char* what) {
     cuuint64_t dims[3] = {CV_C, CV_C, CV_TAPS};
     cuuint64_t strides[2] = {CV_C * 4ull, CV_C * CV_C * 4ull};
     cuuint32_t box[3] = {32, CV_C, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(packed), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (%s) failed with CUresult %d", what, (int)r);
-    return FIERY_OK;
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, packed, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 inline int conv_out_size(int n) { return (n + 2 * 3 - 7) / 2 + 1; }

@@ -77,8 +77,8 @@ bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restr
                 mbar_arrive_expect_tx(full + st, CV_STAGE_BYTES);
                 tma_load_4d(a, &maps.x, full + st, 0, qx0 + dx, qy0 + dy, b);
                 tma_load_4d(a + CV_A_ATOM, &maps.x, full + st, 32, qx0 + dx, qy0 + dy, b);
-                tma_load_3d_sw(bw, &maps.w, full + st, 0, 0, r * 7 + s);
-                tma_load_3d_sw(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, r * 7 + s);
+                tma_load_3d(bw, &maps.w, full + st, 0, 0, r * 7 + s);
+                tma_load_3d(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, r * 7 + s);
             }
         }
         return;
@@ -103,20 +103,20 @@ bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restr
             for (int atom = 0; atom < 2; ++atom) {
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk)
-                    wgmma_m64n64k8_tf32_ss(acc, gmma_desc_sw128(a_addr + atom * CV_A_ATOM + 32 * kk, 16, 1024),
-                                           gmma_desc_sw128(b_addr + atom * CV_B_ATOM + 32 * kk, 16, 1024));
+                    wgmma_tf32_ss<64>(acc, gmma_desc_sw128(a_addr + atom * CV_A_ATOM + 32 * kk, 16, 1024),
+                                      gmma_desc_sw128(b_addr + atom * CV_B_ATOM + 32 * kk, 16, 1024));
             }
             wgmma_commit();
             // the previous tap's MMAs are complete: its stage may be refilled (a phase's first tap waits for nothing)
             wgmma_wait<1>();
             __syncwarp();
-            if (lane == 0 && k > 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + (it - 1) % CV_STAGES)) : "memory");
+            if (lane == 0 && k > 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
         }
         // the phase's last tap: drain, store the phase's pixels (2 q_y + p_y, 2 q_x + p_x), restart the accumulator
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
         __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + (it - 1) % CV_STAGES)) : "memory");
+        if (lane == 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
         const int cq = 2 * (lane & 3);
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -156,19 +156,14 @@ int launch_bev_conv_dgrad(int n_frames, int H, int W, const float* gy_nhwc, cons
     FIERY_REQUIRE(gy_nhwc && w_packed_t && gx_nhwc, "bev conv backward: NULL pointer");
     FIERY_REQUIRE((reinterpret_cast<uintptr_t>(gy_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_packed_t) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(gx_nhwc) & 15) == 0, "bev conv backward: pointers must be 16-byte aligned");
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const int Ho = conv_out_size(H), Wo = conv_out_size(W);
     ConvMaps maps;
-    int rc = encode_conv_activation_map(fn, &maps.x, gy_nhwc, n_frames, Ho, Wo, CV_TW, CV_TH, 1, 1, "conv output gradient");
-    if (rc == FIERY_OK) rc = encode_conv_weight_map(fn, &maps.w, w_packed_t, "transposed conv weights");
+    int rc = encode_conv_activation_map(&maps.x, gy_nhwc, n_frames, Ho, Wo, CV_TW, CV_TH, 1, 1, "conv output gradient");
+    if (rc == FIERY_OK) rc = encode_conv_weight_map(&maps.w, w_packed_t, "transposed conv weights");
     if (rc != FIERY_OK) return rc;
     const int smem = CV_STAGES * CV_STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
     static OncePerDevice once;
-    rc = once.run([smem]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(bev_conv7x7s2_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        return FIERY_OK;
-    });
+    rc = once.run([smem]() { return set_dynamic_smem(bev_conv7x7s2_dgrad_kernel, smem); });
     if (rc != FIERY_OK) return rc;
     const int tiles_x = (Wo + CV_TW - 1) / CV_TW, tiles_y = (Ho + CV_TH - 1) / CV_TH;     // tiles of q: q < ceil(H / 2) = Ho
     bev_conv7x7s2_dgrad_kernel<<<static_cast<unsigned>(n_frames * tiles_x * tiles_y), CV_THREADS, smem, stream>>>(maps, gx_nhwc, H, W,
@@ -283,7 +278,7 @@ __device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned 
 #pragma unroll
                 for (int ks = 0; ks < 2; ++ks) {
                     const int k = 2 * kg + ks;
-                    wgmma_m64n64k8_tf32_rs(acc[t], a[t][ks], gmma_desc_sw128(b_addr + (k >> 2) * WG_B_ATOM + 32 * (k & 3), 16, 1024));
+                    wgmma_tf32_rs<64>(acc[t], a[t][ks], gmma_desc_sw128(b_addr + (k >> 2) * WG_B_ATOM + 32 * (k & 3), 16, 1024));
                 }
             wgmma_commit();
             wgmma_wait<0>();
@@ -360,19 +355,14 @@ int launch_bev_conv_wgrad(int n_frames, int H, int W, const float* x_nhwc, const
     FIERY_REQUIRE(x_nhwc && gy_nhwc && workspace, "bev conv backward: NULL pointer");
     FIERY_REQUIRE((reinterpret_cast<uintptr_t>(x_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(gy_nhwc) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "bev conv backward: pointers must be 16-byte aligned");
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const int Ho = conv_out_size(H), Wo = conv_out_size(W);
     FIERY_REQUIRE(wgrad_tiles(n_frames, H, W) < (1ll << 31), "bev conv backward: too many pixels");
     CUtensorMap xmap;
-    int rc = encode_conv_activation_map(fn, &xmap, x_nhwc, n_frames, H, W, WG_WIN_W, 2 * CV_TH, 1, 2, "conv input window");
+    int rc = encode_conv_activation_map(&xmap, x_nhwc, n_frames, H, W, WG_WIN_W, 2 * CV_TH, 1, 2, "conv input window");
     if (rc != FIERY_OK) return rc;
     const int smem = WG_STAGES * WG_X_STAGE + 2 * WG_B_BYTES + 1024 /* alignment slack */ + 64 /* barriers */;
     static OncePerDevice once;
-    rc = once.run([smem]() -> int {
-        FIERY_CUDA_CHECK(cudaFuncSetAttribute(bev_conv7x7s2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        return FIERY_OK;
-    });
+    rc = once.run([smem]() { return set_dynamic_smem(bev_conv7x7s2_wgrad_kernel, smem); });
     if (rc != FIERY_OK) return rc;
     const int tiles_x = (Wo + CV_TW - 1) / CV_TW, tiles_y = (Ho + CV_TH - 1) / CV_TH;
     float* partial = static_cast<float*>(workspace);

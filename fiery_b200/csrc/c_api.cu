@@ -17,12 +17,9 @@ int set_error(int code, const char* fmt, ...) {
     return code;
 }
 
-// ---- TMA descriptor: head tensor viewed as (channels_total = images*head_channels, h, w), innermost w ------------------
-typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static encode_tiled_fn get_encode_fn() {
+int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                      const cuuint64_t* strides_bytes, const cuuint32_t* box, const cuuint32_t* elem_strides,
+                      CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2_promotion, const char* what) {
     // cuTensorMapEncodeTiled is a driver call and needs a current context; a thread that has made no runtime call yet
     // (e.g. the autograd engine's worker on its first backward) has none, so bind the primary context once per thread.
     static thread_local bool ctx_bound = false;
@@ -30,21 +27,25 @@ static encode_tiled_fn get_encode_fn() {
         cudaFree(nullptr);
         ctx_bound = true;
     }
-    static encode_tiled_fn fn = nullptr;
-    if (fn) return fn;
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-        return nullptr;
-    fn = reinterpret_cast<encode_tiled_fn>(sym);
-    return fn;
+    static const auto encode = []() -> decltype(&cuTensorMapEncodeTiled) {
+        void* sym = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            return nullptr;
+        return reinterpret_cast<decltype(&cuTensorMapEncodeTiled)>(sym);
+    }();
+    if (!encode) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    static const cuuint32_t unit[5] = {1, 1, 1, 1, 1};
+    const CUresult r = encode(map, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), dims, strides_bytes, box,
+                              elem_strides ? elem_strides : unit, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2_promotion,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (%s) failed with CUresult %d", what, (int)r);
+    return FIERY_OK;
 }
 
 // Tensor maps of the lift's tile kernels (lift_tile.cuh: HeadMapsCols)
 int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams& P, int channels_per_lane) {
-    encode_tiled_fn fn = get_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const size_t es = 4;
     // the image coordinate of a tile is absolute (frame0 * n_cameras + ...): the map spans every image up to this launch's last
     const cuuint64_t ww = P.ww, hh = P.hh, n_images = static_cast<cuuint64_t>(P.frame0 + P.n_frames) * P.n_cameras;
@@ -53,15 +54,13 @@ int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams
                   "head tensor (or its context slice) is not 16-byte aligned");
     const int cpl = channels_per_lane;
     FIERY_REQUIRE(cpl >= 1 && P.C % cpl == 0 && P.C / cpl <= 256 && hh <= 256, "column kernel: unsupported head shape");
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     if (P.use_depth) {
         cuuint64_t dims[4] = {ww, static_cast<cuuint64_t>(P.D), hh, n_images};
         cuuint64_t strides[3] = {plane, ww * es, image};
         cuuint32_t box[4] = {WT, 48, static_cast<cuuint32_t>(hh), 1};
-        CUresult r = fn(&maps->depth, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(head), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (depth, 4-D) failed with CUresult %d", (int)r);
+        const int rc = encode_tensor_map(&maps->depth, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, head, dims, strides, box, nullptr,
+                                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "depth, 4-D");
+        if (rc != FIERY_OK) return rc;
     } else {
         memset(&maps->depth, 0, sizeof(CUtensorMap));
     }
@@ -69,27 +68,19 @@ int encode_head_maps_cols(HeadMapsCols* maps, const void* head, const LiftParams
     cuuint64_t dims[5] = {ww, static_cast<cuuint64_t>(P.C / cpl), static_cast<cuuint64_t>(cpl), hh, n_images};
     cuuint64_t strides[4] = {cpl * plane, plane, ww * es, image};
     cuuint32_t box[5] = {WT, static_cast<cuuint32_t>(P.C / cpl), static_cast<cuuint32_t>(cpl), static_cast<cuuint32_t>(hh), 1};
-    CUresult r = fn(&maps->ctx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<char*>(ctx_base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (context, 5-D) failed with CUresult %d", (int)r);
-    return FIERY_OK;
+    return encode_tensor_map(&maps->ctx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, ctx_base, dims, strides, box, nullptr,
+                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "context, 5-D");
 }
 
 // NCHW output (frames, C, X*Y) as a 3-D map, innermost the pillar axis; the layout pass stores (box_pillars x C) blocks into it
 int encode_bev_map(CUtensorMap* map, float* bev, long long pillars, int channels, int n_frames, int box_pillars) {
-    encode_tiled_fn fn = get_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     FIERY_REQUIRE((reinterpret_cast<uintptr_t>(bev) & 15) == 0 && pillars % 4 == 0, "BEV output is not 16-byte aligned / pitched");
     FIERY_REQUIRE(channels <= 256 && box_pillars <= 256, "BEV map: box too large");
     cuuint64_t dims[3] = {static_cast<cuuint64_t>(pillars), static_cast<cuuint64_t>(channels), static_cast<cuuint64_t>(n_frames)};
     cuuint64_t strides[2] = {static_cast<cuuint64_t>(pillars) * 4, static_cast<cuuint64_t>(pillars) * channels * 4};
     cuuint32_t box[3] = {static_cast<cuuint32_t>(box_pillars), static_cast<cuuint32_t>(channels), 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, bev, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (BEV output) failed with CUresult %d", (int)r);
-    return FIERY_OK;
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, bev, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                             CU_TENSOR_MAP_L2_PROMOTION_NONE, "BEV output");
 }
 
 // Head shapes the lift's kernels are built for.  The plan needs rows and depth bins that fit a tile record; the forward and backward

@@ -27,7 +27,7 @@
 // operand; the x run of the tap's frame and row is loaded once, 4 columns early and 44 wide, and read as the register A operand at
 // each dx's shift (im2col from shared memory; 44-float rows put a fragment's 8 channels x 4 pixels on 32 banks).  The summation order
 // is wgrad_chunks.cuh's: bit-reproducible, no atomics.
-#include "bev_conv.cuh"
+#include "wgmma.cuh"
 #include "wgrad_chunks.cuh"
 
 namespace fiery {
@@ -104,10 +104,6 @@ int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w,
     return FIERY_OK;
 }
 
-__device__ __forceinline__ void cc_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-
 // ------------------------------------------------------------------------------------------------------------------------------
 // forward and input gradient
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -162,7 +158,7 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
                 const int st = j % CC_WSTAGES, use = j / CC_WSTAGES;
                 if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
                 mbar_arrive_expect_tx(full + st, w_bytes);
-                for (int a = 0; a < L.ka; ++a) tma_load_3d_sw(s_w + st * w_bytes + a * N * 128, &maps.w, full + st, 0, 0, j * L.ka + a);
+                for (int a = 0; a < L.ka; ++a) tma_load_3d(s_w + st * w_bytes + a * N * 128, &maps.w, full + st, 0, 0, j * L.ka + a);
             }
         }
         return;
@@ -204,7 +200,7 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
         }
         wgmma_fence_operands(acc);
         __syncwarp();
-        if (lane == 0) cc_arrive(empty + st);          // this warp is done with the slice
+        if (lane == 0) mbar_arrive(empty + st);        // this warp is done with the slice
     }
 
     const int gx = x0 + row;
@@ -353,28 +349,15 @@ __global__ void causal_conv_wgrad_reduce_kernel(const CcShape s, const float* __
 // ------------------------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------------------------
-static int cc_encode(encode_tiled_fn fn, CUtensorMap* map, const float* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                     const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* what) {
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<float*>(base), dims, strides_bytes, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (causal conv %s) failed with CUresult %d", what, (int)r);
-    return FIERY_OK;
-}
-
 // a contiguous (b, C, s, X, Y) activation as the 5-D map (Y, X, s, C, b)
-static int cc_encode_activation(encode_tiled_fn fn, CUtensorMap* map, const CcShape& s, const float* t, int channels, cuuint32_t box_y,
-                                cuuint32_t box_x, cuuint32_t box_c, CUtensorMapSwizzle swizzle, const char* what) {
+static int cc_encode_activation(CUtensorMap* map, const CcShape& s, const float* t, int channels, cuuint32_t box_y, cuuint32_t box_x,
+                                cuuint32_t box_c, CUtensorMapSwizzle swizzle, const char* what) {
     const cuuint64_t Y = s.Y, X = s.X, S = s.frames, C = channels;
     cuuint64_t dims[5] = {Y, X, S, C, static_cast<cuuint64_t>(s.batch)};
     cuuint64_t strides[4] = {Y * 4, X * Y * 4, S * X * Y * 4, C * S * X * Y * 4};
     cuuint32_t box[5] = {box_y, box_x, 1, box_c, 1};
-    return cc_encode(fn, map, t, 5, dims, strides, box, swizzle, what);
-}
-
-static int cc_sm_attr(const void* kernel, int smem) {
-    FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    return FIERY_OK;
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, t, dims, strides, box, nullptr, swizzle,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 // forward (dgrad = 0): x (C_in channels) -> y (C_out) with pack F; input gradient (dgrad = 1): gy (C_out) -> gx (C_in) with pack T
@@ -383,17 +366,17 @@ static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const 
     const CcPackDir f = cc_pack_dir(s.cout, s.cin, s.taps);
     const CcPackDir p = dgrad ? cc_pack_dir(s.cin, s.cout, s.taps) : f;
     const float* w = dgrad ? packed + f.floats : packed;
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     CcFwdMaps maps;
-    int rc = cc_encode_activation(fn, &maps.x, s, in, dgrad ? s.cout : s.cin, CC_HY, CC_HX, static_cast<cuuint32_t>(p.kpad),
-                                  CU_TENSOR_MAP_SWIZZLE_NONE, dgrad ? "output gradient" : "input");
+    int rc = cc_encode_activation(&maps.x, s, in, dgrad ? s.cout : s.cin, CC_HY, CC_HX, static_cast<cuuint32_t>(p.kpad),
+                                  CU_TENSOR_MAP_SWIZZLE_NONE, dgrad ? "causal conv output gradient" : "causal conv input");
     if (rc != FIERY_OK) return rc;
     {
         cuuint64_t dims[3] = {32, static_cast<cuuint64_t>(p.n), static_cast<cuuint64_t>(s.taps) * p.ka};
         cuuint64_t strides[2] = {128, static_cast<cuuint64_t>(p.n) * 128};
         cuuint32_t box[3] = {32, static_cast<cuuint32_t>(p.n), 1};
-        if ((rc = cc_encode(fn, &maps.w, w, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) != FIERY_OK) return rc;
+        if ((rc = encode_tensor_map(&maps.w, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, w, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "causal conv weights")) != FIERY_OK)
+            return rc;
     }
     CcFwdLaunch L;
     L.frames = s.frames;
@@ -412,7 +395,7 @@ static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const 
     switch (p.n) {
 #define CC_FWD_CASE(N)                                                                                                             \
     case N:                                                                                                                        \
-        if ((rc = cc_sm_attr(reinterpret_cast<const void*>(causal_conv_fwd_kernel<N>), smem)) != FIERY_OK) return rc;             \
+        if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<N>, smem)) != FIERY_OK) return rc;                                       \
         causal_conv_fwd_kernel<N><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L, out);                 \
         break;
         CC_FWD_CASE(8) CC_FWD_CASE(16) CC_FWD_CASE(24) CC_FWD_CASE(32) CC_FWD_CASE(40) CC_FWD_CASE(48) CC_FWD_CASE(56) CC_FWD_CASE(64)
@@ -439,21 +422,19 @@ int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x
     float* partial = static_cast<float*>(workspace);
     if (n_chunks > 0) {
         FIERY_REQUIRE(tiles < (1ll << 31), "causal conv: too many pixel tiles");
-        encode_tiled_fn fn = conv_encode_fn();
-        if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
         const int no = cc_round8(s.cout);
         CcWgradMaps maps;
-        int rc = cc_encode_activation(fn, &maps.gy, s, gy, s.cout, CC_WG_PX, 1, static_cast<cuuint32_t>(no), CU_TENSOR_MAP_SWIZZLE_128B,
-                                      "output gradient");
+        int rc = cc_encode_activation(&maps.gy, s, gy, s.cout, CC_WG_PX, 1, static_cast<cuuint32_t>(no), CU_TENSOR_MAP_SWIZZLE_128B,
+                                      "causal conv output gradient");
         if (rc == FIERY_OK)
-            rc = cc_encode_activation(fn, &maps.x, s, x, s.cin, CC_WG_XP, 1, 64, CU_TENSOR_MAP_SWIZZLE_NONE, "input");
+            rc = cc_encode_activation(&maps.x, s, x, s.cin, CC_WG_XP, 1, 64, CU_TENSOR_MAP_SWIZZLE_NONE, "causal conv input");
         if (rc != FIERY_OK) return rc;
         const int smem = CC_WG_STAGES * (CC_WG_X_BYTES + no * 128) + CC_SMEM_SLACK;
         const dim3 grid(static_cast<unsigned>(n_chunks), static_cast<unsigned>(3 * s.kt));
         switch (no) {
 #define CC_WG_CASE(N)                                                                                                              \
     case N:                                                                                                                        \
-        if ((rc = cc_sm_attr(reinterpret_cast<const void*>(causal_conv_wgrad_kernel<N>), smem)) != FIERY_OK) return rc;           \
+        if ((rc = set_dynamic_smem(causal_conv_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                     \
         causal_conv_wgrad_kernel<N><<<grid, 128, smem, stream>>>(maps, s, partial, static_cast<int>(tiles));                        \
         break;
             CC_WG_CASE(8) CC_WG_CASE(16) CC_WG_CASE(24) CC_WG_CASE(32) CC_WG_CASE(40) CC_WG_CASE(48) CC_WG_CASE(56) CC_WG_CASE(64)

@@ -1,4 +1,4 @@
-// Shared device helpers: mbarrier / TMA / L2-policy PTX wrappers for sm_90a, error plumbing.
+// Shared helpers: mbarrier / TMA / L2-policy PTX wrappers for sm_90a, error plumbing, TMA descriptors and kernel launch set-up.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <atomic>
+#include <mutex>
 #include "../../include/fiery_b200.h"
 
 namespace fiery {
@@ -28,6 +30,50 @@ int set_error(int code, const char* fmt, ...);
         if (!(cond)) return ::fiery::set_error(FIERY_E_INVALID, __VA_ARGS__); \
     } while (0)
 
+// cuTensorMapEncodeTiled (definition in c_api.cu) without interleave and with FLOAT_OOB_FILL_NONE: coordinates outside the tensor
+// read as zero, which the convolutions use as their padding.  elem_strides: nullptr for all 1.  A failure is reported through
+// set_error, naming the map by `what`.
+int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                      const cuuint64_t* strides_bytes, const cuuint32_t* box, const cuuint32_t* elem_strides,
+                      CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2_promotion, const char* what);
+
+// ------------------------------------------------------------------------------------------------------------
+// host-side launch set-up
+// ------------------------------------------------------------------------------------------------------------
+// One-time per-device set-up of a kernel (function attributes are per device), safe when several host threads call in.
+struct OncePerDevice {
+    std::atomic<int> done[64];
+    std::mutex mu;
+    template <typename F>
+    int run(F&& configure) {
+        int dev = 0;
+        FIERY_CUDA_CHECK(cudaGetDevice(&dev));
+        std::atomic<int>& flag = done[dev & 63];
+        if (flag.load(std::memory_order_acquire)) return FIERY_OK;
+        std::lock_guard<std::mutex> lock(mu);
+        if (flag.load(std::memory_order_relaxed)) return FIERY_OK;
+        const int rc = configure();
+        if (rc == FIERY_OK) flag.store(1, std::memory_order_release);
+        return rc;
+    }
+};
+
+template <typename Kernel>
+int set_dynamic_smem(Kernel kernel, int bytes) {
+    FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    return FIERY_OK;
+}
+
+// Persistent grid: at most one CTA per SM of the current device, the n_tiles (>= 1) tiles spread evenly over them.
+inline int persistent_grid(long long n_tiles, unsigned* grid) {
+    int dev = 0, sms = 0;
+    FIERY_CUDA_CHECK(cudaGetDevice(&dev));
+    FIERY_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const long long waves = (n_tiles + sms - 1) / sms;
+    *grid = static_cast<unsigned>((n_tiles + waves - 1) / waves);
+    return FIERY_OK;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------------------------
@@ -46,6 +92,10 @@ __device__ __forceinline__ void fence_mbar_init() {
 
 __device__ __forceinline__ void fence_proxy_async() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -102,7 +152,11 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
                  ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)), "l"(policy) : "memory");
 }
 
-// 3-D tiled TMA load global -> shared, completion signalled on an mbarrier (SASS: UTMALDG)
+// 2-D and 3-D tiled TMA loads global -> shared, completion signalled on an mbarrier (SASS: UTMALDG)
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+                 ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1) : "memory");
+}
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"

@@ -17,7 +17,6 @@
 //                feat^T x W^T: the weight matrix is the K-major B operand as it lies, the feature tile is the A operand, read from
 //                shared memory into registers.  Warpgroup g owns pixel rows 64g .. 64g + 63, in the order dl_pixel() gives them
 //                (conflict-free fragment loads from the swizzled tile).
-#include "lift_plan.cuh"
 #include "wgmma.cuh"
 
 namespace fiery {
@@ -33,14 +32,6 @@ struct DepthLayerMaps {
     CUtensorMap w;        // (K, M) padded weights, box (128 bytes of K, 128 rows), swizzle 128B
     CUtensorMap feat;     // (pixels, K, images), box (128 bytes of pixels, 128 channels, 1), swizzle 128B
 };
-
-__device__ __forceinline__ void tma_load_2d_sw(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
 
 template <int ES>
 struct DlShape {
@@ -99,7 +90,7 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
         if (lane == 0) {                               // ===== TMA producer: weights once, then this CTA's feature tiles =====
             mbar_arrive_expect_tx(w_full, S::W_BYTES);
 #pragma unroll
-            for (int a = 0; a < S::ATOMS; ++a) tma_load_2d_sw(s_w + a * S::W_ATOM, &maps.w, w_full, a * S::EPR, 0);
+            for (int a = 0; a < S::ATOMS; ++a) tma_load_2d(s_w + a * S::W_ATOM, &maps.w, w_full, a * S::EPR, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
                 const int st = it % S::STAGES, use = it / S::STAGES;
@@ -197,22 +188,6 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
     }
 }
 
-typedef CUresult (*dl_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static dl_encode_fn dl_encoder() {
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        cudaFree(nullptr);
-        ctx_bound = true;
-    }
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-        return nullptr;
-    return reinterpret_cast<dl_encode_fn>(sym);
-}
-
 // dtype: 0 fp32 (TF32 math), 1 fp16, 2 bf16 -- of BOTH the feature map and the padded weight matrix
 int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, int dtype, const void* weight_padded, const float* bias,
                        float* head, cudaStream_t stream) {
@@ -225,8 +200,6 @@ int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, in
                   "depth layer: h*w = %d must give a 16-byte row pitch (and a multiple of 4)", pixels);
     FIERY_REQUIRE((reinterpret_cast<uintptr_t>(feat) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight_padded) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(head) & 15) == 0, "depth layer: pointers must be 16-byte aligned");
-    dl_encode_fn fn = dl_encoder();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const CUtensorMapDataType dt = dtype == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     const cuuint32_t epr = 128 / es;
     DepthLayerMaps maps;
@@ -234,39 +207,30 @@ int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, in
         cuuint64_t dims[2] = {DL_K, DL_M};
         cuuint64_t strides[1] = {static_cast<cuuint64_t>(DL_K) * es};
         cuuint32_t box[2] = {epr, DL_M};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = fn(&maps.w, dt, 2, const_cast<void*>(weight_padded), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (depth layer weights) failed with CUresult %d", (int)r);
+        const int rc = encode_tensor_map(&maps.w, dt, 2, weight_padded, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "depth layer weights");
+        if (rc != FIERY_OK) return rc;
     }
     {
         cuuint64_t dims[3] = {static_cast<cuuint64_t>(pixels), DL_K, static_cast<cuuint64_t>(n_images)};
         cuuint64_t strides[2] = {static_cast<cuuint64_t>(pixels) * es, static_cast<cuuint64_t>(pixels) * DL_K * es};
         cuuint32_t box[3] = {epr, DL_K, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = fn(&maps.feat, dt, 3, const_cast<void*>(feat), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (feature map) failed with CUresult %d", (int)r);
+        const int rc = encode_tensor_map(&maps.feat, dt, 3, feat, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "feature map");
+        if (rc != FIERY_OK) return rc;
     }
     static OncePerDevice once;
-    static int n_sm[64];
     int rc = once.run([]() -> int {
         FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<2>::SMEM));
         FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<2>::SMEM));
         FIERY_CUDA_CHECK(cudaFuncSetAttribute(depth_layer_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlShape<4>::SMEM));
-        int dev = 0;
-        FIERY_CUDA_CHECK(cudaGetDevice(&dev));
-        FIERY_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev));
         return FIERY_OK;
     });
     if (rc != FIERY_OK) return rc;
-    int dev = 0;
-    FIERY_CUDA_CHECK(cudaGetDevice(&dev));
     const int tiles_per_image = (pixels + DL_N - 1) / DL_N;
     const int n_tiles = n_images * tiles_per_image;
-    const int sms = n_sm[dev & 63];
-    const int waves = (n_tiles + sms - 1) / sms;                       // one persistent CTA per SM, the tiles spread evenly over them
-    const unsigned grid = static_cast<unsigned>((n_tiles + waves - 1) / waves);
+    unsigned grid = 0;
+    if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     if (dtype == 0)
         depth_layer_kernel<4, false><<<grid, DL_THREADS, DlShape<4>::SMEM, stream>>>(maps, bias, head, n_out, pixels, tiles_per_image, n_tiles);
     else if (dtype == 1)

@@ -21,9 +21,6 @@
 //           runs that start inside the group -- exactly the sequence of gradient rows thread (rg, column) of the backward
 //           kernel gathers for its slot j -- and ends with two -1 entries (the kernel prefetches two entries ahead).
 #pragma once
-#include <atomic>
-#include <mutex>
-
 #include "lift_tile.cuh"
 
 namespace fiery {
@@ -66,24 +63,6 @@ __host__ __device__ inline PlanView plan_view(const void* plan, long long n_fram
     v.touched = base + static_cast<size_t>(n_frames_total) * n_cameras * n_wtiles * PLAN_TILE_BYTES + static_cast<size_t>(frame0) * pillars;
     return v;
 }
-
-// One-time per-device set-up of a kernel (function attributes are per device), safe when several host threads call in.
-struct OncePerDevice {
-    std::atomic<int> done[64];
-    std::mutex mu;
-    template <typename F>
-    int run(F&& configure) {
-        int dev = 0;
-        FIERY_CUDA_CHECK(cudaGetDevice(&dev));
-        std::atomic<int>& flag = done[dev & 63];
-        if (flag.load(std::memory_order_acquire)) return FIERY_OK;
-        std::lock_guard<std::mutex> lock(mu);
-        if (flag.load(std::memory_order_relaxed)) return FIERY_OK;
-        const int rc = configure();
-        if (rc == FIERY_OK) flag.store(1, std::memory_order_release);
-        return rc;
-    }
-};
 
 // Event pairs around the kernel launches of one forward call (fiery_lift_forward_timed): kind 0 = plan kernel, 1 = tile kernel,
 // 2 = layout pass.

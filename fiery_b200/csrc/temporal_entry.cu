@@ -25,7 +25,7 @@
 // operands.  With E > 0 the egopose is written into the input tile's rows K .. K + E - 1 (TF32-rounded) so its columns come out of the
 // same MMAs.  The 64-pixel tiles are cut into chunks whose boundaries depend on (frames, X*Y) only; each chunk stores its partial and a
 // reduce kernel adds the partials in ascending chunk order: bit-reproducible, no atomics.
-#include "bev_conv.cuh"
+#include "wgmma.cuh"
 #include "wgrad_chunks.cuh"
 
 namespace fiery {
@@ -137,9 +137,6 @@ int launch_temporal_entry_pack(const fiery_temporal_entry_desc_t* d, const float
 // ------------------------------------------------------------------------------------------------------------------------------
 // shared device helpers
 // ------------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void te_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
 __device__ __forceinline__ void te_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // accumulator row r (0..127) -> pixel of the tile: rows 64g .. 64g + 63 map to pixels 64g .. 64g + 63, and the 8 rows one fragment
@@ -172,7 +169,7 @@ __device__ __forceinline__ void te_mma_group(float (&acc)[NC][32], const unsigne
 #pragma unroll
     for (int k = 0; k < 4; ++k)
 #pragma unroll
-        for (int c = 0; c < NC; ++c) wgmma_m64n64k8_tf32_rs(acc[c], a[k], gmma_desc_sw128(b_atom + c * 64 * 128 + k * 32, 16, 1024));
+        for (int c = 0; c < NC; ++c) wgmma_tf32_rs<64>(acc[c], a[k], gmma_desc_sw128(b_atom + c * 64 * 128 + k * 32, 16, 1024));
     wgmma_commit();
     wgmma_wait<0>();
 }
@@ -267,7 +264,7 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
     if (warp == 8) {
         if (lane == 0) {                               // ===== TMA producer: weights once, then this CTA's input tiles =====
             mbar_arrive_expect_tx(w_full, (k32 / 32) * w_atom);
-            for (int a = 0; a < k32 / 32; ++a) tma_load_3d_sw(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
+            for (int a = 0; a < k32 / 32; ++a) tma_load_3d(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
                 const int st = it % stages, use = it / stages;
@@ -308,7 +305,7 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
 #pragma unroll
         for (int c = 0; c < NCH; ++c) wgmma_fence_operands(acc[c]);
         __syncwarp();
-        if (lane == 0) te_arrive(empty + st);          // this warp's part of the tile has been read
+        if (lane == 0) mbar_arrive(empty + st);        // this warp's part of the tile has been read
 
         const int pbase = p0 + 64 * g;
         const int n_valid = s.pixels - pbase;
@@ -390,7 +387,7 @@ temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeSh
     if (warp == 4) {
         if (lane == 0) {
             mbar_arrive_expect_tx(w_full, (npad32 / 32) * w_atom);
-            for (int a = 0; a < npad32 / 32; ++a) tma_load_3d_sw(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
+            for (int a = 0; a < npad32 / 32; ++a) tma_load_3d(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
                 const int st = it % stages, use = it / stages;
@@ -425,7 +422,7 @@ temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeSh
 #pragma unroll
         for (int c = 0; c < NCHK; ++c) wgmma_fence_operands(acc[c]);
         __syncwarp();
-        if (lane == 0) te_arrive(empty + st);
+        if (lane == 0) mbar_arrive(empty + st);
 
         float* base = gx + static_cast<size_t>(b) * s.sb + static_cast<size_t>(tt) * s.st + p0;
 #pragma unroll
@@ -530,7 +527,7 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
             const uint64_t da = gmma_desc_sw128(g_addr + blk * rows * 128 + 32 * kk, 16, 1024);
 #pragma unroll
             for (int c = 0; c < NC; ++c)
-                wgmma_m64n64k8_tf32_ss(acc[c], da, gmma_desc_sw128(x_addr + blk * xrows * 128 + c * 64 * 128 + 32 * kk, 16, 1024));
+                wgmma_tf32_ss<64>(acc[c], da, gmma_desc_sw128(x_addr + blk * xrows * 128 + c * 64 * 128 + 32 * kk, 16, 1024));
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -572,50 +569,36 @@ __global__ void temporal_entry_wgrad_reduce_kernel(const TeShape s, const float*
 // ------------------------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------------------------
-static int te_encode(encode_tiled_fn fn, CUtensorMap* map, const float* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                     const cuuint32_t* box, const char* what) {
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<float*>(base), dims, strides_bytes, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled (temporal entry %s) failed with CUresult %d", what, (int)r);
-    return FIERY_OK;
-}
-
 // the block input (b, t, channel, X*Y) with its strides; box (32 pixels, Kpad channels)
-static int te_encode_input(encode_tiled_fn fn, CUtensorMap* map, const TeShape& s, const float* x) {
+static int te_encode_input(CUtensorMap* map, const TeShape& s, const float* x) {
     cuuint64_t dims[4] = {static_cast<cuuint64_t>(s.pixels), static_cast<cuuint64_t>(s.K), static_cast<cuuint64_t>(s.frames),
                           static_cast<cuuint64_t>(s.batch)};
     cuuint64_t strides[3] = {static_cast<cuuint64_t>(s.sc) * 4, static_cast<cuuint64_t>(s.st) * 4, static_cast<cuuint64_t>(s.sb) * 4};
     cuuint32_t box[4] = {32, static_cast<cuuint32_t>(s.Kpad), 1, 1};
-    return te_encode(fn, map, x, 4, dims, strides, box, "input");
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "temporal entry input");
 }
 
-static int te_encode_grads(encode_tiled_fn fn, TeGradMaps* maps, const TeShape& s, const float* const* gy) {
+static int te_encode_grads(TeGradMaps* maps, const TeShape& s, const float* const* gy) {
     for (int q = 0; q < s.n_seg; ++q) {
         const cuuint64_t C = static_cast<cuuint64_t>(s.seg_ch[q]), P = static_cast<cuuint64_t>(s.pixels), S = static_cast<cuuint64_t>(s.frames);
         cuuint64_t dims[4] = {P, S, C, static_cast<cuuint64_t>(s.batch)};
         cuuint64_t strides[3] = {P * 4, S * P * 4, C * S * P * 4};
         const int box_rows = q + 1 < s.n_seg ? round_up(s.seg_ch[q], 8) : s.Npad32 - s.seg_off[q];
         cuuint32_t box[4] = {32, 1, static_cast<cuuint32_t>(box_rows), 1};
-        const int rc = te_encode(fn, &maps->gy[q], gy[q], 4, dims, strides, box, "output gradient");
+        const int rc = encode_tensor_map(&maps->gy[q], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, gy[q], dims, strides, box, nullptr,
+                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "temporal entry output gradient");
         if (rc != FIERY_OK) return rc;
     }
     return FIERY_OK;
 }
 
-static int te_encode_pack(encode_tiled_fn fn, CUtensorMap* map, const float* base, int cols, int rows, const char* what) {
+static int te_encode_pack(CUtensorMap* map, const float* base, int cols, int rows, const char* what) {
     cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), 1};
     cuuint64_t strides[2] = {static_cast<cuuint64_t>(cols) * 4, static_cast<cuuint64_t>(cols) * rows * 4};
     cuuint32_t box[3] = {32, static_cast<cuuint32_t>(rows), 1};
-    return te_encode(fn, map, base, 3, dims, strides, box, what);
-}
-
-static int te_sm_count(int* n) {
-    int dev = 0;
-    FIERY_CUDA_CHECK(cudaGetDevice(&dev));
-    FIERY_CUDA_CHECK(cudaDeviceGetAttribute(n, cudaDevAttrMultiProcessorCount, dev));
-    return FIERY_OK;
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 static int te_stages(int fixed_bytes, int stage_bytes) {
@@ -623,27 +606,13 @@ static int te_stages(int fixed_bytes, int stage_bytes) {
     return n < 4 ? n : 4;
 }
 
-// persistent grid: at most one CTA per SM, the tiles spread evenly over them
-static unsigned te_grid(long long n_tiles, int sms) {
-    const long long waves = (n_tiles + sms - 1) / sms;
-    return static_cast<unsigned>((n_tiles + waves - 1) / waves);
-}
-
-template <typename K>
-static int te_set_smem(K kernel, int smem) {
-    FIERY_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    return FIERY_OK;
-}
-
 int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
                                   float* const* out, cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const TePack p = te_pack_layout(s);
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     TeFwdMaps maps;
-    int rc = te_encode_pack(fn, &maps.w, packed, p.k32, p.nch * 64, "forward weights");
-    if (rc == FIERY_OK) rc = te_encode_input(fn, &maps.x, s, x);
+    int rc = te_encode_pack(&maps.w, packed, p.k32, p.nch * 64, "temporal entry forward weights");
+    if (rc == FIERY_OK) rc = te_encode_input(&maps.x, s, x);
     if (rc != FIERY_OK) return rc;
     TeOut o{};
     for (int q = 0; q < s.n_seg; ++q) o.p[q] = out[q];
@@ -653,14 +622,13 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
     const int tiles_per_frame = (s.pixels + TE_FWD_PX - 1) / TE_FWD_PX;
     const long long n_tiles = static_cast<long long>(s.batch) * s.frames * tiles_per_frame;
     FIERY_REQUIRE(n_tiles < (1ll << 31), "temporal entry: too many pixel tiles");
-    int sms = 0;
-    if ((rc = te_sm_count(&sms)) != FIERY_OK) return rc;
-    const unsigned grid = te_grid(n_tiles, sms);
+    unsigned grid = 0;
+    if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     const float* we = packed + p.f_floats + p.t_floats;
     switch (p.nch) {
 #define TE_FWD_CASE(N)                                                                                                              \
     case N:                                                                                                                         \
-        if ((rc = te_set_smem(temporal_entry_fwd_kernel<N>, smem)) != FIERY_OK) return rc;                                          \
+        if ((rc = set_dynamic_smem(temporal_entry_fwd_kernel<N>, smem)) != FIERY_OK) return rc;                                     \
         temporal_entry_fwd_kernel<N><<<grid, TE_FWD_THREADS, smem, stream>>>(maps, s, extra, we, o, stages, tiles_per_frame,       \
                                                                              static_cast<int>(n_tiles));                           \
         break;
@@ -676,11 +644,9 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
                                 cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const TePack p = te_pack_layout(s);
-    encode_tiled_fn fn = conv_encode_fn();
-    if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     TeDgradMaps maps;
-    int rc = te_encode_pack(fn, &maps.w, packed + p.f_floats, p.npad32, p.nchk * 64, "transposed weights");
-    if (rc == FIERY_OK) rc = te_encode_grads(fn, &maps.g, s, gy);
+    int rc = te_encode_pack(&maps.w, packed + p.f_floats, p.npad32, p.nchk * 64, "temporal entry transposed weights");
+    if (rc == FIERY_OK) rc = te_encode_grads(&maps.g, s, gy);
     if (rc != FIERY_OK) return rc;
     const int rows = round_up(s.Npad, 64);
     const int fixed = static_cast<int>(p.t_floats * 4) + TE_STG_FLOATS * 4;
@@ -689,14 +655,13 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
     const int tiles_per_frame = (s.pixels + TE_BWD_PX - 1) / TE_BWD_PX;
     const long long n_tiles = te_bwd_tiles(s.batch * s.frames, s.pixels);
     FIERY_REQUIRE(n_tiles < (1ll << 31), "temporal entry: too many pixel tiles");
-    int sms = 0;
-    if ((rc = te_sm_count(&sms)) != FIERY_OK) return rc;
-    const unsigned grid = te_grid(n_tiles, sms);
+    unsigned grid = 0;
+    if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     if (p.nchk == 1) {
-        if ((rc = te_set_smem(temporal_entry_dgrad_kernel<1>, smem)) != FIERY_OK) return rc;
+        if ((rc = set_dynamic_smem(temporal_entry_dgrad_kernel<1>, smem)) != FIERY_OK) return rc;
         temporal_entry_dgrad_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, static_cast<int>(n_tiles));
     } else {
-        if ((rc = te_set_smem(temporal_entry_dgrad_kernel<2>, smem)) != FIERY_OK) return rc;
+        if ((rc = set_dynamic_smem(temporal_entry_dgrad_kernel<2>, smem)) != FIERY_OK) return rc;
         temporal_entry_dgrad_kernel<2><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, static_cast<int>(n_tiles));
     }
     FIERY_CUDA_CHECK(cudaGetLastError());
@@ -711,11 +676,9 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
     const int n_red = s.n_out * (s.K + s.E);
     float* partial = static_cast<float*>(workspace);
     if (n_chunks > 0) {
-        encode_tiled_fn fn = conv_encode_fn();
-        if (!fn) return set_error(FIERY_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
         TeWgradMaps maps;
-        int rc = te_encode_input(fn, &maps.x, s, x);
-        if (rc == FIERY_OK) rc = te_encode_grads(fn, &maps.g, s, gy);
+        int rc = te_encode_input(&maps.x, s, x);
+        if (rc == FIERY_OK) rc = te_encode_grads(&maps.g, s, gy);
         if (rc != FIERY_OK) return rc;
         const int rows = round_up(s.Npad, 64), nc = round_up(s.K + s.E, 64) / 64;
         const int stage_bytes = 2 * (rows + 64 * nc) * 128;
@@ -728,7 +691,7 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
         switch (nc) {
 #define TE_WG_CASE(N)                                                                                                              \
     case N:                                                                                                                        \
-        if ((rc = te_set_smem(temporal_entry_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                       \
+        if ((rc = set_dynamic_smem(temporal_entry_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                  \
         temporal_entry_wgrad_kernel<N><<<n_chunks, threads, smem, stream>>>(maps, s, extra, partial, stages, tiles_per_frame, n_tiles); \
         break;
             TE_WG_CASE(1) TE_WG_CASE(2) TE_WG_CASE(3)

@@ -10,6 +10,13 @@
 
 namespace fiery {
 
+// fp32 -> TF32, round to nearest with ties away from zero (the tensor core itself truncates an fp32 operand's low mantissa bits)
+__device__ __forceinline__ uint32_t to_tf32(float v) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+    return r;
+}
+
 // Shared-memory matrix descriptor, 128-byte swizzle (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B).  K-major operand: rows
 // of 128 bytes along K, 8-row groups SBO = 1024 bytes apart, LBO unused.  MN-major operand (16-bit types only): 128-byte rows along
 // M/N, one k each; 8 consecutive k = one 1024-byte atom, SBO = stride between k-groups of 8, LBO = stride between 128-byte blocks
@@ -65,27 +72,6 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32_rs(float (&d)[64], const ui
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db)
         : "memory");
 }
-// D (64 x 64) += A (64 x 8 TF32, registers, fragment as for wgmma_m64n128k8_tf32_rs) * B (8 x 64 TF32, K-major, shared)
-__device__ __forceinline__ void wgmma_m64n64k8_tf32_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db)
-        : "memory");
-}
-// D (64 x 64) += A (64 x 8 TF32, K-major, shared) * B (8 x 64 TF32, K-major, shared)
-__device__ __forceinline__ void wgmma_m64n64k8_tf32_ss(float (&d)[32], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "%32, %33, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db)
-        : "memory");
-}
-
 // m64nNk8 TF32 for every N = 8, 16, ..., 64 (the causal convolution's N is its channel count rounded up to 8).  d: the N/2
 // accumulator floats of the fragment above; rs: A from registers as for wgmma_m64n128k8_tf32_rs; ss: A K-major in shared memory.
 template <int N> __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db);
