@@ -1,13 +1,17 @@
-"""ctypes binding of libfiery_b200.so (C ABI: include/fiery_b200.h).
+"""ctypes binding of libfiery_b200.so (C ABI: include/fiery_b200.h), the one helper every launch goes through (``call``) and the
+cache of the tensor-core layers' weight packs (``packed``).
 
 There is no fallback: if the shared library is missing or a call fails this module raises.  Build it in-tree with
 ``python -m fiery_b200.build`` (the built ``.so`` travels with the repo snapshot to the GPU box).
 """
 from __future__ import annotations
 
+import collections
 import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
+
+import torch
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libfiery_b200.so")
 ABI_VERSION = 2
@@ -139,3 +143,52 @@ def check(status: int, what: str) -> None:
     if status != 0:
         msg = load().fiery_last_error()
         raise FieryError(f"{what} failed ({status}): {msg.decode() if msg else 'no message'}")
+
+
+@torch.compiler.disable          # the raw handle exists on eager streams only: a C-ABI call breaks a torch.compile graph here
+def _stream_ptr(device: torch.device) -> int:
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _require_cuda(t: torch.Tensor, name: str) -> None:
+    if not t.is_cuda:
+        raise FieryError(f"{name} must be a CUDA tensor: fiery_b200 has no CPU path (got device {t.device})")
+
+
+def call(entry: str, device: torch.device, *args) -> None:
+    """``lib.<entry>(*args, stream)`` with ``device`` current and its current stream as the last argument; raises ``FieryError``
+    under the entry's name if the call fails."""
+    with torch.cuda.device(device):
+        check(getattr(load(), entry)(*args, _stream_ptr(device)), entry)
+
+
+def f32(t: torch.Tensor) -> torch.Tensor:
+    """A contiguous fp32 tensor: the layout the kernels read."""
+    return t.float().contiguous() if t.dtype != torch.float32 else t.contiguous()
+
+
+# (pack function, args, device, the weights' data_ptrs) -> (the weights' versions, aliases of the weights, pack).  The aliases keep the
+# weights' memory alive, so no other tensor can take an address in the cache while its entry exists; a weight's version counter
+# (shared with its views, its aliases and the Parameter) changes with each in-place update, e.g. an optimizer step or a checkpoint
+# load.  One training step of a model with every layer swapped uses one pack per DepthLayer operand dtype, two for FirstConv (the
+# transposed one for the input gradient), three per TemporalBlock (its entry and two causal convolutions) and one per Bottleneck3D:
+# 15 for the four temporal blocks of a 5-frame receptive field.  The bound leaves room for in-between layers (up to four per block
+# there) without a step ever evicting a pack it uses again.
+_PACK_CACHE_SIZE = 32
+_pack_cache: "collections.OrderedDict[tuple, tuple]" = collections.OrderedDict()
+
+
+@torch.compiler.disable          # host bookkeeping on data_ptr and _version: runs eagerly, never compiled into a graph
+def packed(pack, weights, *args):
+    """``pack(weights, *args)``, made at most once per version of ``weights`` (a tensor or a list of tensors)."""
+    ws = (weights,) if isinstance(weights, torch.Tensor) else tuple(weights)
+    key = (pack, args, ws[0].device) + tuple(w.data_ptr() for w in ws)
+    versions = tuple(w._version for w in ws)
+    entry = _pack_cache.get(key)
+    if entry is None or entry[0] != versions or any(a.shape != w.shape for a, w in zip(entry[1], ws)):
+        entry = (versions, [w.detach() for w in ws], pack(weights, *args))
+        _pack_cache[key] = entry
+        while len(_pack_cache) > _PACK_CACHE_SIZE:
+            _pack_cache.popitem(last=False)
+    _pack_cache.move_to_end(key)
+    return entry[2]

@@ -8,21 +8,21 @@ reference ``state_dict`` entry ``first_conv.weight`` loads unchanged) and runs t
 
 Training: the backward (fiery_b200/csrc/bev_conv_bwd.cu) computes the input and weight gradients on the tensor cores too, on the
 same channel-last layout, bit-reproducibly (no atomics).  ``FirstConv(bn=None)`` -- with or without ``relu`` -- trains through the
-``torch.ops.fiery_b200.first_conv`` operator (fiery_b200/ops.py) whenever grad is enabled; ``install.use_tensor_core_first_conv``
-swaps it into a ``Fiery`` model, leaving ``bn1`` and ``relu`` to the reference's modules.  With ``bn`` given the module folds bn1
-from its running statistics into the kernel's epilogue: that form is for inference only and has no backward.  No CPU path.
+``torch.ops.fiery_b200.first_conv`` operator (registered below through fiery_b200/ops.py) whenever grad is enabled;
+``install.use_tensor_core_first_conv`` swaps it into a ``Fiery`` model, leaving ``bn1`` and ``relu`` to the reference's modules.
+With ``bn`` given the module folds bn1 from its running statistics into the kernel's epilogue: that form is for inference only and
+has no backward.  No CPU path.
 """
 from __future__ import annotations
 
-from collections import OrderedDict
-from typing import Optional, Tuple
+from typing import Optional
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.first_conv)
-from .geometry import _require_cuda, _stream_ptr
+from ._lib import _require_cuda
+from .ops import _register_conv
 
 
 def first_conv_forward(x: torch.Tensor, packed_weight: torch.Tensor, scale: Optional[torch.Tensor] = None,
@@ -30,7 +30,6 @@ def first_conv_forward(x: torch.Tensor, packed_weight: torch.Tensor, scale: Opti
     """x: (B, 64, H, W) fp32 with channels-last strides (physical (B, H, W, 64)); packed_weight (49, 64, 64) from ``pack_weight``;
     returns (B, 64, Ho, Wo) fp32, channels-last strides, ``relu(conv(x) * scale + shift)`` (scale/shift/relu optional)."""
     _require_cuda(x, "x")
-    lib = _lib.load()
     if x.dim() != 4 or x.shape[1] != 64:
         raise ValueError(f"x must be (B, 64, H, W), got {tuple(x.shape)}")
     B, C, H, W = x.shape
@@ -41,11 +40,8 @@ def first_conv_forward(x: torch.Tensor, packed_weight: torch.Tensor, scale: Opti
     store = torch.empty((B, Ho, Wo, 64), dtype=torch.float32, device=x.device)
     sc = scale.float().contiguous() if scale is not None else None
     sh = shift.float().contiguous() if shift is not None else None
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_bev_first_conv_forward(B, H, W, xs.data_ptr(), packed_weight.data_ptr(),
-                                                    sc.data_ptr() if sc is not None else 0, sh.data_ptr() if sh is not None else 0,
-                                                    1 if relu else 0, store.data_ptr(), _stream_ptr(x.device)),
-                   "fiery_bev_first_conv_forward")
+    _lib.call("fiery_bev_first_conv_forward", x.device, B, H, W, xs.data_ptr(), packed_weight.data_ptr(),
+              sc.data_ptr() if sc is not None else 0, sh.data_ptr() if sh is not None else 0, 1 if relu else 0, store.data_ptr())
     return store.permute(0, 3, 1, 2)
 
 
@@ -54,11 +50,9 @@ def pack_weight(weight: torch.Tensor) -> torch.Tensor:
     _require_cuda(weight, "weight")
     if tuple(weight.shape) != (64, 64, 7, 7):
         raise ValueError(f"first_conv weight must be (64, 64, 7, 7), got {tuple(weight.shape)}")
-    lib = _lib.load()
     w = weight.detach().float().contiguous()
     out = torch.empty((49, 64, 64), dtype=torch.float32, device=w.device)
-    with torch.cuda.device(w.device):
-        _lib.check(lib.fiery_bev_conv_pack_weights(w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)), "fiery_bev_conv_pack_weights")
+    _lib.call("fiery_bev_conv_pack_weights", w.device, w.data_ptr(), out.data_ptr())
     return out
 
 
@@ -67,35 +61,10 @@ def pack_weight_transposed(weight: torch.Tensor) -> torch.Tensor:
     _require_cuda(weight, "weight")
     if tuple(weight.shape) != (64, 64, 7, 7):
         raise ValueError(f"first_conv weight must be (64, 64, 7, 7), got {tuple(weight.shape)}")
-    lib = _lib.load()
     w = weight.detach().float().contiguous()
     out = torch.empty((49, 64, 64), dtype=torch.float32, device=w.device)
-    with torch.cuda.device(w.device):
-        _lib.check(lib.fiery_bev_conv_pack_weights_transposed(w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
-                   "fiery_bev_conv_pack_weights_transposed")
+    _lib.call("fiery_bev_conv_pack_weights_transposed", w.device, w.data_ptr(), out.data_ptr())
     return out
-
-
-# One cache for both packs: (weight data_ptr, device) -> [version, weight alias, forward pack, transposed pack or None].  The alias
-# keeps the weight's memory alive, so an address in the cache cannot be taken by another tensor while its entry exists; the
-# version counter (shared with every view and the Parameter) changes with each in-place update, e.g. an optimizer step.
-_PACKS: "OrderedDict[tuple, list]" = OrderedDict()
-_PACKS_MAX = 8
-
-
-def packed_weights(weight: torch.Tensor, transposed: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-    """(forward pack, transposed pack) of ``weight``, each made at most once per weight version; the transposed one only when asked."""
-    key = (weight.data_ptr(), str(weight.device))
-    entry = _PACKS.get(key)
-    if entry is None or entry[0] != weight._version or tuple(entry[1].shape) != tuple(weight.shape):
-        entry = [weight._version, weight.detach(), pack_weight(weight), None]
-        _PACKS[key] = entry
-        while len(_PACKS) > _PACKS_MAX:
-            _PACKS.popitem(last=False)
-    _PACKS.move_to_end(key)
-    if transposed and entry[3] is None:
-        entry[3] = pack_weight_transposed(weight)
-    return entry[2], entry[3]
 
 
 def _channels_last_f32(t: torch.Tensor) -> torch.Tensor:
@@ -107,15 +76,13 @@ def first_conv_backward_data(grad_y: torch.Tensor, packed_weight_t: torch.Tensor
     """grad_y (B, 64, Ho, Wo) in any layout (converted to channels-last fp32 once if needed); packed_weight_t (49, 64, 64) from
     ``pack_weight_transposed``; returns grad_x (B, 64, height, width) fp32 with channels-last strides."""
     _require_cuda(grad_y, "grad_y")
-    lib = _lib.load()
     B = grad_y.shape[0]
     if grad_y.dim() != 4 or grad_y.shape[1] != 64 or tuple(grad_y.shape[2:]) != ((height - 1) // 2 + 1, (width - 1) // 2 + 1):
         raise ValueError(f"grad_y {tuple(grad_y.shape)} does not match an input of {height}x{width}")
     g = _channels_last_f32(grad_y)
     store = torch.empty((B, height, width, 64), dtype=torch.float32, device=g.device)
-    with torch.cuda.device(g.device):
-        _lib.check(lib.fiery_bev_first_conv_backward_data(B, height, width, g.data_ptr(), packed_weight_t.data_ptr(), store.data_ptr(),
-                                                          _stream_ptr(g.device)), "fiery_bev_first_conv_backward_data")
+    _lib.call("fiery_bev_first_conv_backward_data", g.device, B, height, width, g.data_ptr(), packed_weight_t.data_ptr(),
+              store.data_ptr())
     return store.permute(0, 3, 1, 2)
 
 
@@ -129,7 +96,6 @@ def first_conv_backward_weight(x: torch.Tensor, grad_y: torch.Tensor, workspace:
     returns the weight gradient (64, 64, 7, 7) fp32, bit-reproducible.  ``workspace``: a uint8 device tensor of at least
     ``backward_weight_workspace_bytes`` bytes to use instead of a fresh one."""
     _require_cuda(x, "x")
-    lib = _lib.load()
     if x.dim() != 4 or x.shape[1] != 64:
         raise ValueError(f"x must be (B, 64, H, W), got {tuple(x.shape)}")
     B, _, H, W = x.shape
@@ -140,10 +106,25 @@ def first_conv_backward_weight(x: torch.Tensor, grad_y: torch.Tensor, workspace:
     if workspace is None or workspace.numel() < need:
         workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
     out = torch.empty((64, 64, 7, 7), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_bev_first_conv_backward_weight(B, H, W, xs.data_ptr(), g.data_ptr(), out.data_ptr(), workspace.data_ptr(),
-                                                            _stream_ptr(x.device)), "fiery_bev_first_conv_backward_weight")
+    _lib.call("fiery_bev_first_conv_backward_weight", x.device, B, H, W, xs.data_ptr(), g.data_ptr(), out.data_ptr(),
+              workspace.data_ptr())
     return out
+
+
+# ``torch.ops.fiery_b200.first_conv(x, weight)``: x (B, 64, H, W), any layout and floating dtype -> (B, 64, Ho, Wo) fp32 with
+# channels-last strides.  ``first_conv_backward``: grad_x of x's shape and dtype with channels-last strides (so a
+# ``LiftSplat(output_layout="channels_last")`` upstream takes its NHWC backward route); grad_weight bit-reproducible (no atomics).
+# grad_y is converted to channels-last fp32 once, shared by both gradients.  The weight's packs come from ``_lib.packed``, the
+# transposed one only when the input gradient is asked for.
+_register_conv(
+    "first_conv",
+    forward=lambda x, weight: first_conv_forward(x, _lib.packed(pack_weight, weight)),
+    grad_layout=_channels_last_f32,
+    grad_input=lambda g, x, weight: first_conv_backward_data(g, _lib.packed(pack_weight_transposed, weight), x.shape[2], x.shape[3]),
+    grad_weight=lambda g, x, weight: first_conv_backward_weight(x, g),
+    fake_output=lambda x, weight: x.new_empty((x.shape[0], (x.shape[2] - 1) // 2 + 1, (x.shape[3] - 1) // 2 + 1, 64),
+                                              dtype=torch.float32).permute(0, 3, 1, 2),
+    fake_grad_input=lambda x: x.new_empty((x.shape[0], x.shape[2], x.shape[3], x.shape[1])).permute(0, 3, 1, 2))
 
 
 class FirstConv(nn.Module):
@@ -173,9 +154,6 @@ class FirstConv(nn.Module):
         m.weight = conv.weight
         return m
 
-    def _packed_weight(self) -> torch.Tensor:
-        return packed_weights(self.weight)[0]
-
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.training and self.bn is not None:
             raise RuntimeError("FirstConv folds bn1 with its running statistics: call .eval() (training keeps nn.Conv2d + BatchNorm2d)")
@@ -190,4 +168,4 @@ class FirstConv(nn.Module):
             y = torch.ops.fiery_b200.first_conv(x, self.weight)
             return torch.relu(y) if self.relu else y
         with torch.no_grad():
-            return first_conv_forward(x, self._packed_weight(), scale, shift, self.relu)
+            return first_conv_forward(x, _lib.packed(pack_weight, self.weight), scale, shift, self.relu)

@@ -1,9 +1,9 @@
 """The temporal model's causal convolutions on the tensor cores (``CausalConv3d``, fiery/layers/temporal.py:65-85).
 
 A reference ``CausalConv3d`` is a zero pad (``kt - 1`` frames in front, one pixel around the map), a bias-free ``Conv3d`` with kernel
-(kt, 3, 3), a ``BatchNorm3d`` and a ``ReLU``.  ``torch.ops.fiery_b200.causal_conv3d`` (fiery_b200/ops.py; kernels in
-csrc/causal_conv.cu) computes the pad and the convolution in one pass over a contiguous (b, C, s, X, Y) tensor, without a padded
-copy; both gradients run on the tensor cores too, and the weight gradient is bit-reproducible.
+(kt, 3, 3), a ``BatchNorm3d`` and a ``ReLU``.  ``torch.ops.fiery_b200.causal_conv3d`` (registered below through fiery_b200/ops.py;
+kernels in csrc/causal_conv.cu) computes the pad and the convolution in one pass over a contiguous (b, C, s, X, Y) tensor, without a
+padded copy; both gradients run on the tensor cores too, and the weight gradient is bit-reproducible.
 
 ``TensorCoreCausalConv3d.from_module(m)`` adopts the reference module's children under the same names (``state_dict`` keys are
 unchanged) and replaces only the pad and the convolution; BatchNorm and ReLU stay the reference's own modules, so batch statistics
@@ -18,9 +18,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.causal_conv3d)
-from .geometry import _require_cuda, _stream_ptr
-from .temporal import packed_weights
+from ._lib import _require_cuda, f32
+from .ops import _register_conv
 
 MAX_CHANNELS = 64
 _warned_widths = set()
@@ -46,17 +45,12 @@ def _desc(shape, out_channels: int, kt: int) -> _lib.CausalConv3dDesc:
     return d
 
 
-def _f32(t: torch.Tensor) -> torch.Tensor:
-    """a contiguous fp32 tensor: the layout the kernels read"""
-    return t.float().contiguous() if t.dtype != torch.float32 else t.contiguous()
-
-
 def pack_weights(weights, in_channels: int) -> torch.Tensor:
     """[(C_out, C_in, kt, 3, 3) weight] -> the uint8 device pack the forward and the input gradient take."""
     (weight,) = weights
     _require_cuda(weight, "weight")
     lib = _lib.load()
-    w = _f32(weight.detach())
+    w = f32(weight.detach())
     c_out, c_in, kt = int(w.shape[0]), int(w.shape[1]), int(w.shape[2])
     d = _desc((0, c_in, 0, 1, 4), c_out, kt)
     n = int(lib.fiery_causal_conv3d_packed_bytes(d))
@@ -64,14 +58,12 @@ def pack_weights(weights, in_channels: int) -> torch.Tensor:
         raise _lib.FieryError(f"causal conv: weight {tuple(w.shape)} is not supported: "
                               f"{unsupported_reason(c_in, c_out, kt) or 'kernel must be (kt, 3, 3)'}")
     out = torch.empty(n, dtype=torch.uint8, device=w.device)
-    with torch.cuda.device(w.device):
-        _lib.check(lib.fiery_causal_conv3d_pack_weights(d, w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
-                   "fiery_causal_conv3d_pack_weights")
+    _lib.call("fiery_causal_conv3d_pack_weights", w.device, d, w.data_ptr(), out.data_ptr())
     return out
 
 
 def _packed(weight: torch.Tensor) -> torch.Tensor:
-    return packed_weights([weight], int(weight.shape[1]), pack=pack_weights)
+    return _lib.packed(pack_weights, [weight], int(weight.shape[1]))
 
 
 def _check(x_shape, weight: torch.Tensor) -> int:
@@ -88,29 +80,24 @@ def conv_forward(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     """x (b, C_in, s, X, Y) any float dtype and strides; weight (C_out, C_in, kt, 3, 3).  Returns the contiguous fp32
     (b, C_out, s, X, Y) output of the causal pad + Conv3d."""
     _require_cuda(x, "x")
-    lib = _lib.load()
     kt = _check(x.shape, weight)
-    xs = _f32(x)
+    xs = f32(x)
     b, _, s, h, w = xs.shape
     y = torch.empty((b, weight.shape[0], s, h, w), dtype=torch.float32, device=x.device)
     packed = _packed(weight)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_causal_conv3d_forward(_desc(xs.shape, int(weight.shape[0]), kt), xs.data_ptr(), packed.data_ptr(),
-                                                   y.data_ptr(), _stream_ptr(x.device)), "fiery_causal_conv3d_forward")
+    _lib.call("fiery_causal_conv3d_forward", x.device, _desc(xs.shape, int(weight.shape[0]), kt), xs.data_ptr(), packed.data_ptr(),
+              y.data_ptr())
     return y
 
 
 def conv_backward_data(grad_y: torch.Tensor, x_shape, weight: torch.Tensor) -> torch.Tensor:
     """The input gradient: a contiguous fp32 tensor of x's shape."""
-    lib = _lib.load()
     kt = _check(x_shape, weight)
-    g = _f32(grad_y)
+    g = f32(grad_y)
     gx = torch.empty(tuple(x_shape), dtype=torch.float32, device=g.device)
     packed = _packed(weight)
-    with torch.cuda.device(g.device):
-        _lib.check(lib.fiery_causal_conv3d_backward_data(_desc(tuple(x_shape), int(weight.shape[0]), kt), g.data_ptr(),
-                                                         packed.data_ptr(), gx.data_ptr(), _stream_ptr(g.device)),
-                   "fiery_causal_conv3d_backward_data")
+    _lib.call("fiery_causal_conv3d_backward_data", g.device, _desc(tuple(x_shape), int(weight.shape[0]), kt), g.data_ptr(),
+              packed.data_ptr(), gx.data_ptr())
     return gx
 
 
@@ -123,15 +110,27 @@ def conv_backward_weight(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Te
     """The weight gradient, fp32 of the weight's shape; bit-reproducible (fixed summation order, no atomics)."""
     lib = _lib.load()
     kt = _check(x.shape, weight)
-    xs, g = _f32(x), _f32(grad_y)
+    xs, g = f32(x), f32(grad_y)
     d = _desc(xs.shape, int(weight.shape[0]), kt)
     need = int(lib.fiery_causal_conv3d_backward_weight_workspace_bytes(d))
     ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
     gw = torch.empty(tuple(weight.shape), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_causal_conv3d_backward_weight(d, xs.data_ptr(), g.data_ptr(), gw.data_ptr(), ws.data_ptr(),
-                                                           _stream_ptr(x.device)), "fiery_causal_conv3d_backward_weight")
+    _lib.call("fiery_causal_conv3d_backward_weight", x.device, d, xs.data_ptr(), g.data_ptr(), gw.data_ptr(), ws.data_ptr())
     return gw
+
+
+# ``torch.ops.fiery_b200.causal_conv3d(x, weight)``: x (b, C_in, s, X, Y), Y % 4 == 0; weight (C_out, C_in, kt, 3, 3), kt 1 or 2 ->
+# the contiguous (b, C_out, s, X, Y) fp32 ``Conv3d(ConstantPad3d((1, 1, 1, 1, kt - 1, 0))(x))``; a non-contiguous or 16-bit x is read
+# from a contiguous fp32 copy.  ``causal_conv3d_backward``: grad_x of x's shape and dtype, contiguous; grad_weight bit-reproducible
+# (no atomics).  The gradients are looked up by name when the operator runs, so a wrapper put in their place sees every launch.
+_register_conv(
+    "causal_conv3d",
+    forward=conv_forward,
+    grad_layout=f32,
+    grad_input=lambda g, x, weight: conv_backward_data(g, tuple(x.shape), weight),
+    grad_weight=lambda g, x, weight: conv_backward_weight(g, x, weight),
+    fake_output=lambda x, weight: x.new_empty((x.shape[0], weight.shape[0], *x.shape[2:]), dtype=torch.float32),
+    fake_grad_input=lambda x: x.new_empty(x.shape))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

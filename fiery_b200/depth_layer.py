@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .geometry import _require_cuda, _stream_ptr
+from ._lib import _require_cuda
 
 _DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
@@ -32,12 +32,11 @@ def pack_weight(weight: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
 
 def depth_layer_forward(feat: torch.Tensor, weight: torch.Tensor, bias, packed: torch.Tensor = None) -> torch.Tensor:
     """feat (N, 128, h, w) fp32 / fp16 / bf16 contiguous; weight (n_out, 128, 1, 1); bias (n_out,) or None -> (N, n_out, h, w) fp32.
-    ``packed``: ``pack_weight(weight, feat.dtype)`` made earlier (the module caches it per weight version)."""
+    ``packed``: ``pack_weight(weight, feat.dtype)`` made earlier (the module takes it from ``_lib.packed``)."""
     _require_cuda(feat, "feat")
     if feat.dim() != 4 or feat.shape[1] != 128 or feat.dtype not in _DTYPE_CODE:
         raise ValueError(f"feat must be (N, 128, h, w) in fp32 / fp16 / bf16, got {tuple(feat.shape)} {feat.dtype}")
     n_out = weight.shape[0]
-    lib = _lib.load()
     x = feat.contiguous()
     N, _, h, w = x.shape
     wp = packed if packed is not None else pack_weight(weight, x.dtype)
@@ -47,10 +46,8 @@ def depth_layer_forward(feat: torch.Tensor, weight: torch.Tensor, bias, packed: 
     if bias is not None:
         b = bias if (bias.dtype == torch.float32 and bias.is_contiguous()) else bias.detach().float().contiguous()
     out = torch.empty((N, n_out, h, w), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_depth_layer_forward(N, h * w, n_out, x.data_ptr(), _DTYPE_CODE[x.dtype], wp.data_ptr(),
-                                                 b.data_ptr() if b is not None else 0, out.data_ptr(), _stream_ptr(x.device)),
-                   "fiery_depth_layer_forward")
+    _lib.call("fiery_depth_layer_forward", x.device, N, h * w, n_out, x.data_ptr(), _DTYPE_CODE[x.dtype], wp.data_ptr(),
+              b.data_ptr() if b is not None else 0, out.data_ptr())
     return out
 
 
@@ -92,15 +89,9 @@ class DepthLayer(nn.Module):
             raise ValueError("the tensor-core kernel is built for 128 input channels and <= 128 outputs (encoder.py:33-36)")
         conv = nn.Conv2d(in_channels, out_channels, kernel_size=1, padding=0, bias=bias)      # the reference's initialisation
         self.weight, self.bias = conv.weight, conv.bias
-        self._packed = {}                                  # dtype -> (weight version, data_ptr, packed operand)
 
     def _packed_weight(self, dtype):
-        key = (self.weight._version, self.weight.data_ptr(), self.weight.device)
-        hit = self._packed.get(dtype)
-        if hit is None or hit[0] != key:
-            hit = (key, pack_weight(self.weight, dtype))   # re-made after every optimizer step (64 KB)
-            self._packed[dtype] = hit
-        return hit[1]
+        return _lib.packed(pack_weight, self.weight, dtype)        # re-made after every optimizer step (64 KB)
 
     @classmethod
     def from_conv(cls, conv: nn.Conv2d) -> "DepthLayer":

@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import _require_cuda, _stream_ptr  # noqa: F401  (_stream_ptr: bench.py, tools/ and tests import it from here)
 
 
 def calculate_birds_eye_view_parameters(x_bounds: Sequence[float], y_bounds: Sequence[float], z_bounds: Sequence[float]):
@@ -77,11 +78,6 @@ def z_valid_interval(resolution_z: float, dim_z: int) -> Tuple[np.float32, np.fl
     return np.float32(lo), np.float32(hi)
 
 
-@torch.compiler.disable          # the raw handle exists on eager streams only: a C-ABI call breaks a torch.compile graph here
-def _stream_ptr(device: torch.device) -> int:
-    return torch.cuda.current_stream(device).cuda_stream
-
-
 def _unfilled(shape, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
     """``torch.empty`` without the NaN fill ``torch.use_deterministic_algorithms(True)`` adds: for workspaces whose contents on entry
     do not matter and outputs the kernels overwrite completely (a fill of the lift's ~1 GB workspace would cost more than the lift)."""
@@ -92,11 +88,6 @@ def _unfilled(shape, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
         return torch.empty(shape, dtype=dtype, device=device)
     finally:
         det.fill_uninitialized_memory = old
-
-
-def _require_cuda(t: torch.Tensor, name: str) -> None:
-    if not t.is_cuda:
-        raise _lib.FieryError(f"{name} must be a CUDA tensor: fiery_b200 has no CPU path (got device {t.device})")
 
 
 class VoxelsSumming(torch.autograd.Function):
@@ -125,23 +116,19 @@ class VoxelsSumming(torch.autograd.Function):
         coords = geometry.to(torch.int64).contiguous()
         rk = ranks.to(torch.int64).contiguous()
         dev = x.device
-        with torch.cuda.device(dev):
-            seg = torch.empty(n_rows, dtype=torch.int32, device=dev)
-            n_seg = ctypes.c_int64(0)
-            _lib.check(lib.fiery_voxels_summing_plan(n_rows, rk.data_ptr(), seg.data_ptr(), ctypes.byref(n_seg),
-                                                     _stream_ptr(dev)),
-                       "fiery_voxels_summing_plan")
-            n_segments = int(n_seg.value)
-            sums = torch.empty((n_segments, channels), dtype=torch.float32, device=dev)
-            kept = torch.empty((n_segments, 3), dtype=torch.int64, device=dev)
-            args = (n_rows, channels, xf.stride(0) if n_rows else channels, xf.data_ptr(), coords.data_ptr(), seg.data_ptr(),
-                    n_segments, sums.data_ptr(), kept.data_ptr())
-            if torch.are_deterministic_algorithms_enabled():     # chunk-edge runs summed in chunk order instead of atomically
-                ws = _unfilled(max(1, int(lib.fiery_voxels_summing_deterministic_workspace_bytes(n_rows, channels))), torch.uint8, dev)
-                _lib.check(lib.fiery_voxels_summing_forward_deterministic(*args, ws.data_ptr(), _stream_ptr(dev)),
-                           "fiery_voxels_summing_forward_deterministic")
-            else:
-                _lib.check(lib.fiery_voxels_summing_forward(*args, _stream_ptr(dev)), "fiery_voxels_summing_forward")
+        seg = torch.empty(n_rows, dtype=torch.int32, device=dev)
+        n_seg = ctypes.c_int64(0)
+        _lib.call("fiery_voxels_summing_plan", dev, n_rows, rk.data_ptr(), seg.data_ptr(), ctypes.byref(n_seg))
+        n_segments = int(n_seg.value)
+        sums = torch.empty((n_segments, channels), dtype=torch.float32, device=dev)
+        kept = torch.empty((n_segments, 3), dtype=torch.int64, device=dev)
+        args = (n_rows, channels, xf.stride(0) if n_rows else channels, xf.data_ptr(), coords.data_ptr(), seg.data_ptr(),
+                n_segments, sums.data_ptr(), kept.data_ptr())
+        if torch.are_deterministic_algorithms_enabled():     # chunk-edge runs summed in chunk order instead of atomically
+            ws = _unfilled(max(1, int(lib.fiery_voxels_summing_deterministic_workspace_bytes(n_rows, channels))), torch.uint8, dev)
+            _lib.call("fiery_voxels_summing_forward_deterministic", dev, *args, ws.data_ptr())
+        else:
+            _lib.call("fiery_voxels_summing_forward", dev, *args)
         ctx.save_for_backward(seg)
         ctx.in_dtype = x.dtype
         ctx.channels = channels
@@ -151,12 +138,8 @@ class VoxelsSumming(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_x, grad_geometry):
         (seg,) = ctx.saved_tensors
-        lib = _lib.load()
         n_rows, channels = seg.shape[0], ctx.channels
         g = grad_x.float().contiguous()
-        dev = g.device
-        out = torch.empty((n_rows, channels), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.fiery_voxels_summing_backward(n_rows, channels, g.data_ptr(), seg.data_ptr(), out.data_ptr(),
-                                                         _stream_ptr(dev)), "fiery_voxels_summing_backward")
+        out = torch.empty((n_rows, channels), dtype=torch.float32, device=g.device)
+        _lib.call("fiery_voxels_summing_backward", g.device, n_rows, channels, g.data_ptr(), seg.data_ptr(), out.data_ptr())
         return out.to(ctx.in_dtype), None, None

@@ -25,8 +25,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .geometry import (_require_cuda, _stream_ptr, _unfilled, bev_offset_fp32, calculate_birds_eye_view_parameters, create_frustum,
-                       split_frustum, z_valid_interval)
+from ._lib import _require_cuda
+from .geometry import _unfilled, bev_offset_fp32, calculate_birds_eye_view_parameters, create_frustum, split_frustum, z_valid_interval
 
 # The geometry plan's byte layout (fiery_b200/csrc/lift_plan.cuh): one record per (frame, camera, 4-column tile), then the touched
 # maps (one byte per frame and pillar).  A record holds mask[192] u32, off[192] u16, soff[64] u16, the counts (n_runs, n_stream) u32
@@ -276,35 +276,30 @@ class LiftSplat(nn.Module):
         of its own (B', n) (``ValueError``); a plan of the same size made by another module, BEV grid or frustum, or for other
         calibrations, cannot be detected and gives a wrong BEV."""
         _require_cuda(intrinsics, "intrinsics")
-        lib = _lib.load()
         dev = intrinsics.device
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, _lib.BEV_NCHW)
         buf = torch.empty(max(1, _plan_bytes(desc.n_frames, desc.n_cameras, desc.feat_w, desc.bev_x * desc.bev_y)), dtype=torch.uint8,
                           device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.fiery_lift_plan(desc, *(t.data_ptr() for t in geo), buf.data_ptr(), _stream_ptr(dev)), "fiery_lift_plan")
+        _lib.call("fiery_lift_plan", dev, desc, *(t.data_ptr() for t in geo), buf.data_ptr())
         return buf
 
     def point_indices(self, intrinsics: torch.Tensor, extrinsics: torch.Tensor):
         """Integer voxel coordinates of every frustum point, as the reference computes them at fiery.py:236-256.
         Returns (idx (B', N, 3) int64, valid (B', N) bool, pillar (B', N) int32 [rank, or -1 if masked])."""
         _require_cuda(intrinsics, "intrinsics")
-        lib = _lib.load()
         dev = intrinsics.device
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, _lib.BEV_NCHW)
         B, N = desc.n_frames, desc.n_cameras * desc.depth_bins * desc.feat_h * desc.feat_w
         idx = torch.empty((B, N, 3), dtype=torch.int64, device=dev)
         valid = torch.empty((B, N), dtype=torch.uint8, device=dev)
         pillar = torch.empty((B, N), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.fiery_lift_point_indices(desc, *(t.data_ptr() for t in geo), idx.data_ptr(), valid.data_ptr(),
-                                                    pillar.data_ptr(), _stream_ptr(dev)), "fiery_lift_point_indices")
+        _lib.call("fiery_lift_point_indices", dev, desc, *(t.data_ptr() for t in geo), idx.data_ptr(), valid.data_ptr(),
+                  pillar.data_ptr())
         return idx, valid.bool(), pillar
 
     def compose_calibration(self, intrinsics: torch.Tensor, extrinsics: torch.Tensor):
         """combined = R @ inverse(K) and translation (fiery.py:196,203) from the device kernel."""
         _require_cuda(intrinsics, "intrinsics")
-        lib = _lib.load()
         dev = intrinsics.device
         K = intrinsics.float().contiguous()
         E = extrinsics.float().contiguous()
@@ -312,9 +307,7 @@ class LiftSplat(nn.Module):
         n = int(np.prod(lead)) if len(lead) else 1
         comb = torch.empty(lead + (3, 3), dtype=torch.float32, device=dev)
         trans = torch.empty(lead + (3,), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.fiery_compose_calibration(n, K.data_ptr(), E.data_ptr(), comb.data_ptr(), trans.data_ptr(),
-                                                     _stream_ptr(dev)), "fiery_compose_calibration")
+        _lib.call("fiery_compose_calibration", dev, n, K.data_ptr(), E.data_ptr(), comb.data_ptr(), trans.data_ptr())
         return comb, trans
 
     def plan_summary(self, plan: torch.Tensor, n_frames: int, n_cameras: int) -> Dict[str, int]:
@@ -437,31 +430,30 @@ class LiftSplat(nn.Module):
         warp_ptrs = (theta.data_ptr(), copy_mask.data_ptr()) if warp is not None else (0, 0)
         shape = (B, X, Y, C) if nhwc else (B, C, X, Y)
         pooled = 0
-        with torch.cuda.device(dev):
-            if torch.are_deterministic_algorithms_enabled():
-                entry, extra = "fiery_lift_forward_deterministic", warp_ptrs
-                store = _unfilled(shape, torch.float32, dev)                      # every element is written
-                buf = _unfilled(max(1, int(lib.fiery_lift_deterministic_workspace_bytes(desc))), torch.uint8, dev)
-            else:
-                entry, extra = ("fiery_lift_forward_warped", warp_ptrs) if warp is not None else ("fiery_lift_forward", ())
-                # NHWC: the tile kernels reduce into the output itself, so it starts zeroed
-                store = (torch.zeros if nhwc else torch.empty)(shape, dtype=torch.float32, device=dev)
-                buf = scratch
-                if buf is None and B and not nhwc:
-                    pooled = int(lib.fiery_lift_scratch_bytes(desc))
-                    buf = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
-            status = getattr(lib, entry)(desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(),
-                                         buf.data_ptr() if (B and buf is not None) else 0, plan.data_ptr() if plan is not None else 0,
-                                         *extra, _stream_ptr(dev))
-            if status != 0 and pooled:
+        if torch.are_deterministic_algorithms_enabled():
+            entry, extra = "fiery_lift_forward_deterministic", warp_ptrs
+            store = _unfilled(shape, torch.float32, dev)                      # every element is written
+            buf = _unfilled(max(1, int(lib.fiery_lift_deterministic_workspace_bytes(desc))), torch.uint8, dev)
+        else:
+            entry, extra = ("fiery_lift_forward_warped", warp_ptrs) if warp is not None else ("fiery_lift_forward", ())
+            # NHWC: the tile kernels reduce into the output itself, so it starts zeroed
+            store = (torch.zeros if nhwc else torch.empty)(shape, dtype=torch.float32, device=dev)
+            buf = scratch
+            if buf is None and B and not nhwc:
+                pooled = int(lib.fiery_lift_scratch_bytes(desc))
+                buf = _scratch.get(dev, pooled)            # zero-filled once; the kernels leave it zeroed again
+        try:
+            _lib.call(entry, dev, desc, head.data_ptr(), *(t.data_ptr() for t in geo), store.data_ptr(),
+                      buf.data_ptr() if (B and buf is not None) else 0, plan.data_ptr() if plan is not None else 0, *extra)
+        except _lib.FieryError:
+            if pooled:
                 _scratch.discard(dev, pooled)          # a launch sequence that stopped half way may have left it dirty
-            _lib.check(status, entry)
+            raise
         return store.permute(0, 3, 1, 2) if nhwc else store
 
     def _launch_backward(self, head: torch.Tensor, intrinsics: torch.Tensor, extrinsics: torch.Tensor,
                          grad_bev: torch.Tensor, plan: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Gradient of the BEV w.r.t. ``head``, in ``head``'s dtype; the backward kernel reads the head widened to fp32."""
-        lib = _lib.load()
         dev = head.device
         h32 = head.float().contiguous()
         g = grad_bev.float()
@@ -473,14 +465,11 @@ class LiftSplat(nn.Module):
         desc, geo = self._abi_args(dev, intrinsics, extrinsics, torch.float32, layout)
         self._check_plan(plan, desc, dev)
         grad_head = torch.empty_like(h32)
-        with torch.cuda.device(dev):
-            ws = None
-            if plan is None or layout == _lib.BEV_NCHW:        # re-layout of an NCHW gradient and/or room for the plan records
-                ws = torch.empty(max(1, int(lib.fiery_lift_workspace_bytes(desc)) // 4), dtype=torch.float32, device=dev)
-            _lib.check(lib.fiery_lift_backward(desc, h32.data_ptr(), *(t.data_ptr() for t in geo), g.data_ptr(), grad_head.data_ptr(),
-                                               ws.data_ptr() if ws is not None else 0,
-                                               plan.data_ptr() if plan is not None else 0, _stream_ptr(dev)),
-                       "fiery_lift_backward")
+        ws = None
+        if plan is None or layout == _lib.BEV_NCHW:        # re-layout of an NCHW gradient and/or room for the plan records
+            ws = torch.empty(max(1, int(_lib.load().fiery_lift_workspace_bytes(desc)) // 4), dtype=torch.float32, device=dev)
+        _lib.call("fiery_lift_backward", dev, desc, h32.data_ptr(), *(t.data_ptr() for t in geo), g.data_ptr(), grad_head.data_ptr(),
+                  ws.data_ptr() if ws is not None else 0, plan.data_ptr() if plan is not None else 0)
         return grad_head.to(head.dtype)
 
 

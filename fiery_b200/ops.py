@@ -12,6 +12,9 @@ geometry plan that the forward and the backward share.
 
 The operators take plain tensors plus an integer ``handle`` naming the ``LiftSplat`` module that holds the frustum / BEV-grid
 constants (a registry of weak references; the constants are tiny host-derived tensors, not operator inputs).
+
+The tensor-core layers' operators follow: ``temporal_entry`` here, and ``first_conv`` and ``causal_conv3d``, which their layer modules
+(fiery_b200/bev_conv.py, fiery_b200/causal_conv.py) register through ``_register_conv``.  Importing this module registers them all.
 """
 from __future__ import annotations
 
@@ -115,75 +118,57 @@ torch.library.register_autocast("fiery_b200::lift_splat", "cuda", torch.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# The first BEV convolution (Decoder.first_conv, fiery/models/decoder.py:11,59) as dispatcher operators:
-# ``torch.ops.fiery_b200.first_conv`` / ``first_conv_backward`` (fiery_b200/bev_conv.py; kernels in csrc/bev_conv*.cu).
-# Autocast: the operator runs in fp32 (TF32 tensor-core operands, fp32 accumulation) -- under AMP the reference runs this
-# convolution in fp16, so an AMP step computes it at a higher precision than the reference does.
+# Convolutions of one input by one weight as dispatcher operators ``fiery_b200::<name>`` / ``<name>_backward``, each registered by
+# its layer module with the forward, the two gradients and the fake shapes: ``first_conv`` (Decoder.first_conv,
+# fiery/models/decoder.py:11,59; fiery_b200/bev_conv.py) and ``causal_conv3d`` (CausalConv3d's pad + Conv3d,
+# fiery/layers/temporal.py:65-85; fiery_b200/causal_conv.py).
+# Autocast: the operators run in fp32 (TF32 tensor-core operands, fp32 accumulation) -- under AMP the reference runs these
+# convolutions in fp16, so an AMP step computes them at a higher precision than the reference does.
 # ------------------------------------------------------------------------------------------------------------------------------
-def _conv_out(n: int) -> int:
-    return (n - 1) // 2 + 1
+def _cast_back(grad: Optional[torch.Tensor], like: torch.Tensor) -> torch.Tensor:
+    """``grad`` in the dtype of the tensor it is the gradient of; a gradient that was not asked for (None) comes back as an empty
+    tensor (an operator returns tensors)."""
+    if grad is None:
+        return like.new_empty((0,))
+    return grad if grad.dtype == like.dtype else grad.to(like.dtype)
 
 
-@torch.library.custom_op("fiery_b200::first_conv", mutates_args=(), device_types="cuda")
-def first_conv(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
-    """Conv2d(64, 64, 7, stride 2, padding 3, no bias): x (B, 64, H, W), any layout -> (B, 64, Ho, Wo) fp32 with channels-last
-    strides.  The weight's TF32 packs are made at most once per weight version (``bev_conv.packed_weights``)."""
-    from .bev_conv import first_conv_forward, packed_weights
-    return first_conv_forward(x, packed_weights(weight)[0])
+def _register_conv(name: str, forward, grad_layout, grad_input, grad_weight, fake_output, fake_grad_input) -> None:
+    """``fiery_b200::<name>(x, weight) = forward(x, weight)`` and ``<name>_backward(grad_y, x, weight, need_input, need_weight)
+    -> (grad_x, grad_weight)``: grad_y is converted once by ``grad_layout`` and shared by ``grad_input(g, x, weight)`` and
+    ``grad_weight(g, x, weight)``; only the gradients asked for are computed, in x's and the weight's dtype.  The fakes take their
+    shapes and strides from ``fake_output(x, weight)`` and ``fake_grad_input(x)``; the weight gradient has the weight's shape."""
+    @torch.library.custom_op(f"fiery_b200::{name}", mutates_args=(), device_types="cuda")
+    def op(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+        return forward(x, weight)
 
+    op.register_fake(fake_output)
 
-@first_conv.register_fake
-def _(x, weight):
-    B, _, H, W = x.shape
-    return x.new_empty((B, _conv_out(H), _conv_out(W), 64), dtype=torch.float32).permute(0, 3, 1, 2)
+    @torch.library.custom_op(f"fiery_b200::{name}_backward", mutates_args=(), device_types="cuda")
+    def backward_op(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, need_input: bool,
+                    need_weight: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+        g = grad_layout(grad_y)
+        return (_cast_back(grad_input(g, x, weight) if need_input else None, x),
+                _cast_back(grad_weight(g, x, weight) if need_weight else None, weight))
 
+    @backward_op.register_fake
+    def _(grad_y, x, weight, need_input, need_weight):
+        return (fake_grad_input(x) if need_input else x.new_empty((0,)),
+                weight.new_empty(weight.shape) if need_weight else weight.new_empty((0,)))
 
-@torch.library.custom_op("fiery_b200::first_conv_backward", mutates_args=(), device_types="cuda")
-def first_conv_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, need_input: bool,
-                        need_weight: bool) -> Tuple[torch.Tensor, torch.Tensor]:
-    """(grad_x, grad_weight) of ``first_conv``; a gradient that is not asked for is not computed and comes back as an empty tensor.
-    grad_y arriving in another layout (e.g. NCHW-contiguous) is converted to channels-last fp32 once, shared by both gradients.
-    grad_x: x's shape and dtype with channels-last strides (so a ``LiftSplat(output_layout="channels_last")`` upstream takes its
-    NHWC backward route); grad_weight: the weight's shape and dtype, bit-reproducible (no atomics)."""
-    from .bev_conv import _channels_last_f32, first_conv_backward_data, first_conv_backward_weight, packed_weights
-    g = _channels_last_f32(grad_y)
-    H, W = x.shape[2], x.shape[3]
-    grad_x, grad_w = x.new_empty((0,)), x.new_empty((0,))         # two tensors: an operator's outputs may not alias each other
-    if need_input:
-        grad_x = first_conv_backward_data(g, packed_weights(weight, transposed=True)[1], H, W)
-        if grad_x.dtype != x.dtype:
-            grad_x = grad_x.to(x.dtype)
-    if need_weight:
-        grad_w = first_conv_backward_weight(x, g)
-        if grad_w.dtype != weight.dtype:
-            grad_w = grad_w.to(weight.dtype)
-    return grad_x, grad_w
+    def setup_context(ctx, inputs, output):
+        ctx.save_for_backward(*inputs)
 
+    def backward(ctx, grad_y):
+        x, weight = ctx.saved_tensors
+        need_input, need_weight = bool(ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1])
+        if not (need_input or need_weight):
+            return None, None
+        grad_x, grad_w = backward_op(grad_y, x, weight, need_input, need_weight)
+        return (grad_x if need_input else None), (grad_w if need_weight else None)
 
-@first_conv_backward.register_fake
-def _(grad_y, x, weight, need_input, need_weight):
-    B, C, H, W = x.shape
-    grad_x = x.new_empty((B, H, W, C)).permute(0, 3, 1, 2) if need_input else x.new_empty((0,))
-    grad_w = weight.new_empty(weight.shape) if need_weight else x.new_empty((0,))
-    return grad_x, grad_w
-
-
-def _first_conv_setup_context(ctx, inputs, output):
-    x, weight = inputs
-    ctx.save_for_backward(x, weight)
-
-
-def _first_conv_backward(ctx, grad_y):
-    x, weight = ctx.saved_tensors
-    need_input, need_weight = bool(ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1])
-    if not (need_input or need_weight):
-        return None, None
-    grad_x, grad_w = torch.ops.fiery_b200.first_conv_backward(grad_y, x, weight, need_input, need_weight)
-    return (grad_x if need_input else None), (grad_w if need_weight else None)
-
-
-first_conv.register_autograd(_first_conv_backward, setup_context=_first_conv_setup_context)
-torch.library.register_autocast("fiery_b200::first_conv", "cuda", torch.float32)
+    op.register_autograd(backward, setup_context=setup_context)
+    torch.library.register_autocast(f"fiery_b200::{name}", "cuda", torch.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -214,15 +199,9 @@ def temporal_entry_backward(grads: List[torch.Tensor], x: torch.Tensor, weights:
     grad_x: x's shape and dtype, with x's strides where the kernels read x as it lies (``temporal.input_strides``); grad_weights: each
     weight's shape and dtype, bit-reproducible (no atomics).  extra gets no gradient."""
     from .temporal import entry_backward_data, entry_backward_weight
-    grad_x = x.new_empty((0,))
-    grad_w = [wt.new_empty((0,)) for wt in weights]
-    if need_input:
-        grad_x = entry_backward_data(grads, x, weights)
-        if grad_x.dtype != x.dtype:
-            grad_x = grad_x.to(x.dtype)
-    if need_weight:
-        grad_w = [g if g.dtype == wt.dtype else g.to(wt.dtype) for g, wt in zip(entry_backward_weight(grads, x, weights, extra), weights)]
-    return grad_x, grad_w
+    grad_x = _cast_back(entry_backward_data(grads, x, weights) if need_input else None, x)
+    grad_w = entry_backward_weight(grads, x, weights, extra) if need_weight else [None] * len(weights)
+    return grad_x, [_cast_back(g, wt) for g, wt in zip(grad_w, weights)]
 
 
 @temporal_entry_backward.register_fake
@@ -255,64 +234,4 @@ temporal_entry.register_autograd(_temporal_entry_backward, setup_context=_tempor
 torch.library.register_autocast("fiery_b200::temporal_entry", "cuda", torch.float32)
 
 
-# ------------------------------------------------------------------------------------------------------------------------------
-# The temporal model's causal convolution (CausalConv3d's pad + Conv3d, fiery/layers/temporal.py:65-85) as dispatcher operators:
-# ``torch.ops.fiery_b200.causal_conv3d`` / ``causal_conv3d_backward`` (fiery_b200/causal_conv.py; kernels in csrc/causal_conv.cu).
-# Autocast: the operator runs in fp32 (TF32 tensor-core operands, fp32 accumulation), as temporal_entry does.
-# ------------------------------------------------------------------------------------------------------------------------------
-@torch.library.custom_op("fiery_b200::causal_conv3d", mutates_args=(), device_types="cuda")
-def causal_conv3d(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
-    """x (b, C_in, s, X, Y), Y % 4 == 0; weight (C_out, C_in, kt, 3, 3), kt 1 or 2.  Returns the contiguous (b, C_out, s, X, Y) fp32
-    ``Conv3d(ConstantPad3d((1, 1, 1, 1, kt - 1, 0))(x))``.  A non-contiguous or 16-bit x is read from a contiguous fp32 copy; the
-    weight's pack is made at most once per weight version."""
-    from .causal_conv import conv_forward
-    return conv_forward(x, weight)
-
-
-@causal_conv3d.register_fake
-def _(x, weight):
-    b, _, s, h, w = x.shape
-    return x.new_empty((b, weight.shape[0], s, h, w), dtype=torch.float32)
-
-
-@torch.library.custom_op("fiery_b200::causal_conv3d_backward", mutates_args=(), device_types="cuda")
-def causal_conv3d_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, need_input: bool,
-                           need_weight: bool) -> Tuple[torch.Tensor, torch.Tensor]:
-    """(grad_x, grad_weight) of ``causal_conv3d``; a gradient that is not asked for is not computed and comes back empty.  grad_x: x's
-    shape and dtype, contiguous; grad_weight: the weight's shape and dtype, bit-reproducible (no atomics)."""
-    from .causal_conv import conv_backward_data, conv_backward_weight
-    grad_x, grad_w = x.new_empty((0,)), weight.new_empty((0,))
-    if need_input:
-        grad_x = conv_backward_data(grad_y, tuple(x.shape), weight)
-        if grad_x.dtype != x.dtype:
-            grad_x = grad_x.to(x.dtype)
-    if need_weight:
-        grad_w = conv_backward_weight(grad_y, x, weight)
-        if grad_w.dtype != weight.dtype:
-            grad_w = grad_w.to(weight.dtype)
-    return grad_x, grad_w
-
-
-@causal_conv3d_backward.register_fake
-def _(grad_y, x, weight, need_input, need_weight):
-    grad_x = x.new_empty(x.shape) if need_input else x.new_empty((0,))
-    grad_w = weight.new_empty(weight.shape) if need_weight else weight.new_empty((0,))
-    return grad_x, grad_w
-
-
-def _causal_conv3d_setup_context(ctx, inputs, output):
-    x, weight = inputs
-    ctx.save_for_backward(x, weight)
-
-
-def _causal_conv3d_backward(ctx, grad_y):
-    x, weight = ctx.saved_tensors
-    need_input, need_weight = bool(ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1])
-    if not (need_input or need_weight):
-        return None, None
-    grad_x, grad_w = torch.ops.fiery_b200.causal_conv3d_backward(grad_y, x, weight, need_input, need_weight)
-    return (grad_x if need_input else None), (grad_w if need_weight else None)
-
-
-causal_conv3d.register_autograd(_causal_conv3d_backward, setup_context=_causal_conv3d_setup_context)
-torch.library.register_autocast("fiery_b200::causal_conv3d", "cuda", torch.float32)
+from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

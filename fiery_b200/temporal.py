@@ -19,7 +19,6 @@ egopose itself.  No CPU path.
 from __future__ import annotations
 
 import warnings
-from collections import OrderedDict
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -28,7 +27,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.temporal_entry)
-from .geometry import _require_cuda, _stream_ptr
+from ._lib import _require_cuda, f32
 
 MAX_IN_CHANNELS, MAX_OUT_CHANNELS, MAX_EXTRA_CHANNELS = 128, 256, 8
 _warned_pixels = set()
@@ -100,29 +99,6 @@ def _stacked(weights: Sequence[torch.Tensor]) -> torch.Tensor:
     return torch.cat([w.detach().float().reshape(w.shape[0], -1) for w in weights], 0).contiguous()
 
 
-# (pack function, device, in_channels, weights' data_ptrs) -> [versions, weight aliases, pack].  The aliases keep the weights' memory
-# alive, so an address in the cache cannot be taken by another tensor while its entry exists; a version counter changes with each
-# in-place update (an optimizer step), so a pack is made at most once per weight version.
-_PACKS: "OrderedDict[tuple, list]" = OrderedDict()
-_PACKS_MAX = 16
-
-
-def packed_weights(weights: Sequence[torch.Tensor], in_channels: int, pack=None) -> torch.Tensor:
-    """The device pack ``pack(weights, in_channels)`` (default: the temporal entry's, fiery_temporal_entry_pack_weights), made at
-    most once per weight version.  The causal convolution (fiery_b200/causal_conv.py) keeps its packs here too."""
-    pack = pack_weights if pack is None else pack
-    key = (pack, str(weights[0].device), in_channels) + tuple(w.data_ptr() for w in weights)
-    versions = tuple(w._version for w in weights)
-    entry = _PACKS.get(key)
-    if entry is None or entry[0] != versions or any(tuple(a.shape) != tuple(w.shape) for a, w in zip(entry[1], weights)):
-        entry = [versions, [w.detach() for w in weights], pack(weights, in_channels)]
-        _PACKS[key] = entry
-        while len(_PACKS) > _PACKS_MAX:
-            _PACKS.popitem(last=False)
-    _PACKS.move_to_end(key)
-    return entry[2]
-
-
 def pack_weights(weights: Sequence[torch.Tensor], in_channels: int) -> torch.Tensor:
     """(C_q, K + E, 1, 1, 1) conv weights -> the uint8 device pack the three kernels take."""
     _require_cuda(weights[0], "weight")
@@ -135,14 +111,8 @@ def pack_weights(weights: Sequence[torch.Tensor], in_channels: int) -> torch.Ten
         raise _lib.FieryError(f"temporal entry: weights {[tuple(t.shape) for t in weights]} with K = {in_channels} are not supported: "
                               f"{unsupported_reason(in_channels, seg, w.shape[1] - in_channels)}")
     out = torch.empty(n, dtype=torch.uint8, device=w.device)
-    with torch.cuda.device(w.device):
-        _lib.check(lib.fiery_temporal_entry_pack_weights(d, w.data_ptr(), out.data_ptr(), _stream_ptr(w.device)),
-                   "fiery_temporal_entry_pack_weights")
+    _lib.call("fiery_temporal_entry_pack_weights", w.device, d, w.data_ptr(), out.data_ptr())
     return out
-
-
-def _extra_f32(extra: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    return None if extra is None else extra.detach().float().contiguous()
 
 
 def _ptrs(ts: Sequence[torch.Tensor]):
@@ -156,7 +126,6 @@ def entry_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], extra: Optio
     """x (b, K, s, X, Y) any float dtype and strides; weights: 1..4 tensors (C_q, K + E, 1, 1, 1); extra: (b, s, E) or None.  Returns
     the C_q-channel outputs, each a contiguous (b, C_q, s, X, Y) fp32 tensor."""
     _require_cuda(x, "x")
-    lib = _lib.load()
     xs = _entry_input(x)
     b, K, s, h, w = xs.shape
     seg = [int(t.shape[0]) for t in weights]
@@ -165,33 +134,24 @@ def entry_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], extra: Optio
     if reason is not None:
         raise _lib.FieryError(f"temporal entry: {reason}")
     outs = [torch.empty((b, c, s, h, w), dtype=torch.float32, device=x.device) for c in seg]
-    e = _extra_f32(extra) if E else None
+    e = f32(extra.detach()) if E and extra is not None else None
     if E and (e is None or tuple(e.shape) != (b, s, E)):
         raise ValueError(f"extra must be ({b}, {s}, {E}) for weights with {K + E} input channels and x with {K}")
-    packed = packed_weights(weights, K)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_temporal_entry_forward(_desc(xs, seg, E), xs.data_ptr(), e.data_ptr() if e is not None else 0,
-                                                    packed.data_ptr(), _ptrs(outs), _stream_ptr(x.device)),
-                   "fiery_temporal_entry_forward")
+    packed = _lib.packed(pack_weights, weights, K)
+    _lib.call("fiery_temporal_entry_forward", x.device, _desc(xs, seg, E), xs.data_ptr(), e.data_ptr() if e is not None else 0,
+              packed.data_ptr(), _ptrs(outs))
     return outs
-
-
-def _grads_f32(grads: Sequence[torch.Tensor]) -> List[torch.Tensor]:
-    return [g.float().contiguous() for g in grads]
 
 
 def entry_backward_data(grads: Sequence[torch.Tensor], x: torch.Tensor, weights: Sequence[torch.Tensor]) -> torch.Tensor:
     """The input gradient: x's shape in fp32, with ``input_strides(x)``."""
-    lib = _lib.load()
     b, K, s, h, w = x.shape
     seg = [int(t.shape[0]) for t in weights]
     E = int(weights[0].shape[1]) - K
-    gs = _grads_f32(grads)
+    gs = [f32(g) for g in grads]
     gx = torch.empty_strided(tuple(x.shape), input_strides(x.shape, x.stride()), dtype=torch.float32, device=x.device)
-    packed = packed_weights(weights, K)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_temporal_entry_backward_data(_desc(gx, seg, E), _ptrs(gs), packed.data_ptr(), gx.data_ptr(),
-                                                          _stream_ptr(x.device)), "fiery_temporal_entry_backward_data")
+    packed = _lib.packed(pack_weights, weights, K)
+    _lib.call("fiery_temporal_entry_backward_data", x.device, _desc(gx, seg, E), _ptrs(gs), packed.data_ptr(), gx.data_ptr())
     return gx
 
 
@@ -210,16 +170,14 @@ def entry_backward_weight(grads: Sequence[torch.Tensor], x: torch.Tensor, weight
     K = xs.shape[1]
     seg = [int(t.shape[0]) for t in weights]
     E = int(weights[0].shape[1]) - K
-    gs = _grads_f32(grads)
-    e = _extra_f32(extra) if E else None
+    gs = [f32(g) for g in grads]
+    e = f32(extra.detach()) if E and extra is not None else None
     d = _desc(xs, seg, E)
     need = int(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d))
     ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
     gw = torch.empty((sum(seg), K + E), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.fiery_temporal_entry_backward_weight(d, xs.data_ptr(), e.data_ptr() if e is not None else 0, _ptrs(gs),
-                                                            gw.data_ptr(), ws.data_ptr(), _stream_ptr(x.device)),
-                   "fiery_temporal_entry_backward_weight")
+    _lib.call("fiery_temporal_entry_backward_weight", x.device, d, xs.data_ptr(), e.data_ptr() if e is not None else 0, _ptrs(gs),
+              gw.data_ptr(), ws.data_ptr())
     return [g.reshape(t.shape).clone() for g, t in zip(gw.split(seg, 0), weights)]     # separate tensors: operator outputs may not alias
 
 

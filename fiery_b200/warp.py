@@ -16,7 +16,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from .geometry import _require_cuda, _stream_ptr
+from ._lib import _require_cuda
 
 
 def _mode_flag(mode: str) -> int:
@@ -41,15 +41,12 @@ class _WarpMaps(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, theta, copy_mask, nearest: int):
         _require_cuda(x, "x")
-        lib = _lib.load()
         n, C, H, W = x.shape
         xs = _dense_maps(x)
         th = theta.detach().float().contiguous()
         out = torch.empty((n, C, H, W), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(lib.fiery_warp_features_forward(n, C, H, W, xs.data_ptr(), xs.stride(0) if n else 0, th.data_ptr(),
-                                                       copy_mask.data_ptr() if copy_mask is not None else 0, out.data_ptr(),
-                                                       C * H * W, nearest, _stream_ptr(x.device)), "fiery_warp_features_forward")
+        _lib.call("fiery_warp_features_forward", x.device, n, C, H, W, xs.data_ptr(), xs.stride(0) if n else 0, th.data_ptr(),
+                  copy_mask.data_ptr() if copy_mask is not None else 0, out.data_ptr(), C * H * W, nearest)
         ctx.save_for_backward(th, copy_mask)
         ctx.nearest, ctx.dtype = nearest, x.dtype
         return out
@@ -64,30 +61,24 @@ def _warp_adjoint(grad_out: torch.Tensor, theta: torch.Tensor, copy_mask, neares
     """Gradient (n, C, H, W) float32 of the maps sampled under theta (n, 2, 3) float32 w.r.t. their sources, for the upstream
     gradient ``grad_out`` (n, C, H, W); maps flagged in ``copy_mask`` (n,) uint8 or None pass it through (the gather adjoint,
     fiery_warp_features_backward).  Used by ``_WarpMaps`` and by the warped lift's backward (fiery_b200/ops.py)."""
-    lib = _lib.load()
     n, C, H, W = grad_out.shape
     g = _dense_maps(grad_out)
     grad_x = torch.empty((n, C, H, W), dtype=torch.float32, device=g.device)       # overwritten by the gather adjoint
-    with torch.cuda.device(g.device):
-        _lib.check(lib.fiery_warp_features_backward(n, C, H, W, g.data_ptr(), g.stride(0) if n else 0, theta.data_ptr(),
-                                                    copy_mask.data_ptr() if copy_mask is not None else 0, grad_x.data_ptr(),
-                                                    C * H * W, nearest, _stream_ptr(g.device)), "fiery_warp_features_backward")
+    _lib.call("fiery_warp_features_backward", g.device, n, C, H, W, g.data_ptr(), g.stride(0) if n else 0, theta.data_ptr(),
+              copy_mask.data_ptr() if copy_mask is not None else 0, grad_x.data_ptr(), C * H * W, nearest)
     return grad_x
 
 
 def _device_theta(flow: torch.Tensor, spatial_extent, cumulative: bool):
     """theta (n, 2, 3) and copy mask (n,) for ``flow`` (b, 6) or, cumulative, (b, T, 6): fiery_warp_theta."""
     _require_cuda(flow, "flow")
-    lib = _lib.load()
     f = flow.detach().float().contiguous()
     b = f.shape[0]
     T = f.shape[1] if cumulative else 1
     theta = torch.empty((b * T, 2, 3), dtype=torch.float32, device=f.device)
     mask = torch.empty((b * T,), dtype=torch.uint8, device=f.device) if cumulative else None
-    with torch.cuda.device(f.device):
-        _lib.check(lib.fiery_warp_theta(b, T, 1 if cumulative else 0, f.data_ptr(), float(spatial_extent[0]),
-                                        float(spatial_extent[1]), theta.data_ptr(), mask.data_ptr() if cumulative else 0,
-                                        _stream_ptr(f.device)), "fiery_warp_theta")
+    _lib.call("fiery_warp_theta", f.device, b, T, 1 if cumulative else 0, f.data_ptr(), float(spatial_extent[0]),
+              float(spatial_extent[1]), theta.data_ptr(), mask.data_ptr() if cumulative else 0)
     return theta, mask
 
 
