@@ -25,11 +25,8 @@ namespace fiery {
 __global__ void __launch_bounds__(CV_THREADS, 1)
 bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restrict__ scale, const float* __restrict__ shift,
                      int relu, float* __restrict__ y, int Ho, int Wo, int tiles_x, int tiles_y) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // the dynamic window is only guaranteed 16-byte aligned: align to the 1024 bytes the swizzle atoms need
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + CV_STAGES * CV_STAGE_BYTES);
-    uint64_t* empty = full + CV_STAGES;
+    unsigned char* smem = dynamic_smem_1024();
+    const MbarRing ring(reinterpret_cast<uint64_t*>(smem + CV_STAGES * CV_STAGE_BYTES), CV_STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
@@ -40,28 +37,23 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
     if (warp == CV_PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w);
-        for (int s = 0; s < CV_STAGES; ++s) {
-            mbar_init(full + s, 1);
-            mbar_init(empty + s, 4 * CV_CONSUMERS);   // one arrival per consumer warp
-        }
-        fence_mbar_init();
+        ring.init(4 * CV_CONSUMERS);
     }
     __syncthreads();
 
     if (warp == CV_PRODUCER_WARP) {
         if (lane == 0) {                              // ===== TMA producer =====
             for (int it = 0; it < CV_TAPS; ++it) {
-                const int st = it % CV_STAGES;
-                if (it >= CV_STAGES) mbar_wait(empty + st, ((it / CV_STAGES) - 1) & 1);
+                const int st = ring.produce(it, CV_STAGE_BYTES);
+                uint64_t* full = ring.full + st;
                 unsigned char* a = smem + st * CV_STAGE_BYTES;
                 unsigned char* bw = a + 2 * CV_A_ATOM;
                 const int r = it / 7, s = it % 7;
-                mbar_arrive_expect_tx(full + st, CV_STAGE_BYTES);
                 // input patch of this tap: pixels (2*oy + r - 3, 2*ox + s - 3); negative / too large coordinates read as zero
-                tma_load_4d(a, &maps.x, full + st, 0, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
-                tma_load_4d(a + CV_A_ATOM, &maps.x, full + st, 32, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
-                tma_load_3d(bw, &maps.w, full + st, 0, 0, it);
-                tma_load_3d(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, it);
+                tma_load_4d(a, &maps.x, full, 0, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
+                tma_load_4d(a + CV_A_ATOM, &maps.x, full, 32, 2 * ox0 + s - 3, 2 * oy0 + r - 3, b);
+                tma_load_3d(bw, &maps.w, full, 0, 0, it);
+                tma_load_3d(bw + CV_B_ATOM, &maps.w, full, 32, 0, it);
             }
         }
         return;
@@ -74,8 +66,7 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
     for (int i = 0; i < CV_C / 2; ++i) acc[i] = 0.f;
     wgmma_fence();
     for (int it = 0; it < CV_TAPS; ++it) {
-        const int st = it % CV_STAGES;
-        mbar_wait(full + st, (it / CV_STAGES) & 1);
+        const int st = ring.consume(it);
         const uint32_t a_addr = smem_addr(smem + st * CV_STAGE_BYTES) + g * 64 * 128;
         const uint32_t b_addr = smem_addr(smem + st * CV_STAGE_BYTES) + 2 * CV_A_ATOM;
 #pragma unroll
@@ -88,8 +79,7 @@ bev_conv7x7s2_kernel(const __grid_constant__ ConvMaps maps, const float* __restr
         wgmma_commit();
         if (it > 0) {                                 // the previous tap's MMAs are complete: its stage may be refilled
             wgmma_wait<1>();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
+            ring.release(it - 1);
         }
     }
     wgmma_wait<0>();
@@ -136,11 +126,6 @@ int launch_pack_conv_weights(const float* w_oihw, float* packed, cudaStream_t st
 
 int launch_bev_conv(int n_frames, int H, int W, const float* x_nhwc, const float* w_packed, const float* scale, const float* shift,
                     int relu, float* y_nhwc, cudaStream_t stream) {
-    FIERY_REQUIRE(n_frames >= 0 && H >= 1 && W >= 1, "bev conv: bad shape %d x %d x %d", n_frames, H, W);
-    if (n_frames == 0) return FIERY_OK;
-    FIERY_REQUIRE((scale == nullptr) == (shift == nullptr), "bev conv: scale and shift go together");
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(x_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_packed) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(y_nhwc) & 15) == 0, "bev conv: pointers must be 16-byte aligned");
     const int Ho = (H + 2 * 3 - 7) / 2 + 1, Wo = (W + 2 * 3 - 7) / 2 + 1;
     ConvMaps maps;
     int rc = encode_conv_activation_map(&maps.x, x_nhwc, n_frames, H, W, 2 * CV_TW, 2 * CV_TH, 2, 2, "conv input");

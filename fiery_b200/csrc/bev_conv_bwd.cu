@@ -22,6 +22,7 @@
 // Operand rounding: the packed weights (both packs) and, in wgrad, both operands are rounded to TF32 (cvt.rna) on their way to
 // the tensor core; dgrad's grad_y operand is read from fp32 by the tensor core, which truncates it -- as the forward does with x.
 #include "bev_conv.cuh"
+#include "wgrad_chunks.cuh"
 
 namespace fiery {
 
@@ -42,10 +43,8 @@ __device__ __forceinline__ void dgrad_item(int it, int& ph, int& r, int& s) {
 // maps.x: grad_y (64, Wo, Ho, B), box (32, 16, 8, 1), element strides 1;  maps.w: the transposed pack (tap, in, out)
 __global__ void __launch_bounds__(CV_THREADS, 1)
 bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restrict__ gx, int H, int W, int tiles_x, int tiles_y) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + CV_STAGES * CV_STAGE_BYTES);
-    uint64_t* empty = full + CV_STAGES;
+    unsigned char* smem = dynamic_smem_1024();
+    const MbarRing ring(reinterpret_cast<uint64_t*>(smem + CV_STAGES * CV_STAGE_BYTES), CV_STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
@@ -56,29 +55,24 @@ bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restr
     if (warp == CV_PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w);
-        for (int s = 0; s < CV_STAGES; ++s) {
-            mbar_init(full + s, 1);
-            mbar_init(empty + s, 4 * CV_CONSUMERS);
-        }
-        fence_mbar_init();
+        ring.init(4 * CV_CONSUMERS);
     }
     __syncthreads();
 
     if (warp == CV_PRODUCER_WARP) {
         if (lane == 0) {                              // ===== TMA producer =====
             for (int it = 0; it < CV_TAPS; ++it) {
-                const int st = it % CV_STAGES;
-                if (it >= CV_STAGES) mbar_wait(empty + st, ((it / CV_STAGES) - 1) & 1);
+                const int st = ring.produce(it, CV_STAGE_BYTES);
+                uint64_t* full = ring.full + st;
                 unsigned char* a = smem + st * CV_STAGE_BYTES;
                 unsigned char* bw = a + 2 * CV_A_ATOM;
                 int ph, r, s;
                 dgrad_item(it, ph, r, s);
                 const int dy = ((ph >> 1) + 3 - r) / 2, dx = ((ph & 1) + 3 - s) / 2;     // -1 .. 2
-                mbar_arrive_expect_tx(full + st, CV_STAGE_BYTES);
-                tma_load_4d(a, &maps.x, full + st, 0, qx0 + dx, qy0 + dy, b);
-                tma_load_4d(a + CV_A_ATOM, &maps.x, full + st, 32, qx0 + dx, qy0 + dy, b);
-                tma_load_3d(bw, &maps.w, full + st, 0, 0, r * 7 + s);
-                tma_load_3d(bw + CV_B_ATOM, &maps.w, full + st, 32, 0, r * 7 + s);
+                tma_load_4d(a, &maps.x, full, 0, qx0 + dx, qy0 + dy, b);
+                tma_load_4d(a + CV_A_ATOM, &maps.x, full, 32, qx0 + dx, qy0 + dy, b);
+                tma_load_3d(bw, &maps.w, full, 0, 0, r * 7 + s);
+                tma_load_3d(bw + CV_B_ATOM, &maps.w, full, 32, 0, r * 7 + s);
             }
         }
         return;
@@ -95,8 +89,7 @@ bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restr
         const int n = ph == 0 ? DG_PHASE_END0 : ph == 1 ? DG_PHASE_END1 - DG_PHASE_END0 : ph == 2 ? DG_PHASE_END2 - DG_PHASE_END1
                                                                                               : CV_TAPS - DG_PHASE_END2;
         for (int k = 0; k < n; ++k, ++it) {
-            const int st = it % CV_STAGES;
-            mbar_wait(full + st, (it / CV_STAGES) & 1);
+            const int st = ring.consume(it);
             const uint32_t a_addr = smem_addr(smem + st * CV_STAGE_BYTES) + g * 64 * 128;
             const uint32_t b_addr = smem_addr(smem + st * CV_STAGE_BYTES) + 2 * CV_A_ATOM;
 #pragma unroll
@@ -109,14 +102,15 @@ bev_conv7x7s2_dgrad_kernel(const __grid_constant__ ConvMaps maps, float* __restr
             wgmma_commit();
             // the previous tap's MMAs are complete: its stage may be refilled (a phase's first tap waits for nothing)
             wgmma_wait<1>();
+            // open-coded release: a phase's first tap has no stage to release, and `if (k > 0) ring.release(it - 1)` would put the
+            // warp sync under a branch in this loop (0.4% slower on an H100); here every tap syncs and only the arrival is conditional
             __syncwarp();
-            if (lane == 0 && k > 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
+            if (lane == 0 && k > 0) mbar_arrive(ring.empty + (it - 1) % CV_STAGES);
         }
         // the phase's last tap: drain, store the phase's pixels (2 q_y + p_y, 2 q_x + p_x), restart the accumulator
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + (it - 1) % CV_STAGES);
+        ring.release(it - 1);
         const int cq = 2 * (lane & 3);
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -151,11 +145,6 @@ int launch_pack_conv_weights_transposed(const float* w_oihw, float* packed, cuda
 }
 
 int launch_bev_conv_dgrad(int n_frames, int H, int W, const float* gy_nhwc, const float* w_packed_t, float* gx_nhwc, cudaStream_t stream) {
-    FIERY_REQUIRE(n_frames >= 0 && H >= 1 && W >= 1, "bev conv backward: bad shape %d x %d x %d", n_frames, H, W);
-    if (n_frames == 0) return FIERY_OK;
-    FIERY_REQUIRE(gy_nhwc && w_packed_t && gx_nhwc, "bev conv backward: NULL pointer");
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(gy_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_packed_t) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(gx_nhwc) & 15) == 0, "bev conv backward: pointers must be 16-byte aligned");
     const int Ho = conv_out_size(H), Wo = conv_out_size(W);
     ConvMaps maps;
     int rc = encode_conv_activation_map(&maps.x, gy_nhwc, n_frames, Ho, Wo, CV_TW, CV_TH, 1, 1, "conv output gradient");
@@ -182,7 +171,7 @@ constexpr int WG_STAGES = 2;
 constexpr int WG_B_ATOM = CV_C * 128;                 // 64 output channels x 32 pixels (K-major, swizzle 128B)
 constexpr int WG_B_BYTES = 4 * WG_B_ATOM;             // the tile's 128 pixels
 constexpr int WG_KSTEPS = CV_TW * CV_TH / 8;          // 16 MMAs of k = 8 pixels per tile and tap
-constexpr int WG_MAX_CHUNKS = 18;                     // pixel chunks (x 7 tap rows = 126 CTAs); workspace <= 18 x 784 KB
+constexpr int CV_WG_MAX_CHUNKS = 18;                  // pixel chunks (x 7 tap rows = 126 CTAs); workspace <= 18 x 784 KB
 constexpr int WG_THREADS = 128 * CV_CONSUMERS;         // two warpgroups, no producer warp
 constexpr size_t WG_PARTIAL_FLOATS = static_cast<size_t>(CV_TAPS) * CV_C * CV_C;
 
@@ -191,28 +180,24 @@ static long long wgrad_tiles(int n_frames, int H, int W) {
     return static_cast<long long>(n_frames) * ((Wo + CV_TW - 1) / CV_TW) * ((Ho + CV_TH - 1) / CV_TH);
 }
 
-int bev_conv_wgrad_chunks(int n_frames, int H, int W) {
-    const long long t = wgrad_tiles(n_frames, H, W);
-    return static_cast<int>(t < WG_MAX_CHUNKS ? t : WG_MAX_CHUNKS);
-}
-
 size_t bev_conv_wgrad_workspace_bytes(int n_frames, int H, int W) {
     if (n_frames < 0 || H < 1 || W < 1) return 0;
-    return static_cast<size_t>(bev_conv_wgrad_chunks(n_frames, H, W)) * WG_PARTIAL_FLOATS * sizeof(float);
+    return static_cast<size_t>(wgrad_chunks(wgrad_tiles(n_frames, H, W), CV_WG_MAX_CHUNKS)) * WG_PARTIAL_FLOATS * sizeof(float);
+}
+
+// the x window of pixel tile `tile` (both channel halves) into the stage of iteration it
+__device__ __forceinline__ void wgrad_load_window(const CUtensorMap* xmap, unsigned char* xs, const MbarRing& ring, int r, int tile, int it,
+                                                  int tiles_x, int tiles_y) {
+    const int b = tile / (tiles_x * tiles_y), ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
+    const int st = ring.arm(it, WG_X_STAGE);
+    unsigned char* a = xs + st * WG_X_STAGE;
+    tma_load_4d(a, xmap, ring.full + st, 0, 2 * tx * CV_TW - 3, 2 * ty * CV_TH + r - 3, b);
+    tma_load_4d(a + WG_WIN_ATOM, xmap, ring.full + st, 32, 2 * tx * CV_TW - 3, 2 * ty * CV_TH + r - 3, b);
 }
 
 // One warpgroup's NS taps (s0 .. s0 + NS - 1 of row r) over the chunk's pixel tiles
-__device__ __forceinline__ void wgrad_load_window(const CUtensorMap* xmap, unsigned char* xs, uint64_t* full, int r, int tile, int it,
-                                                  int tiles_x, int tiles_y) {
-    const int b = tile / (tiles_x * tiles_y), ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
-    unsigned char* a = xs + (it % WG_STAGES) * WG_X_STAGE;
-    mbar_arrive_expect_tx(full + it % WG_STAGES, WG_X_STAGE);
-    tma_load_4d(a, xmap, full + it % WG_STAGES, 0, 2 * tx * CV_TW - 3, 2 * ty * CV_TH + r - 3, b);
-    tma_load_4d(a + WG_WIN_ATOM, xmap, full + it % WG_STAGES, 32, 2 * tx * CV_TW - 3, 2 * ty * CV_TH + r - 3, b);
-}
-
 template <int NS>
-__device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned char* xs, unsigned char* bs, uint64_t* full,
+__device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned char* xs, unsigned char* bs, const MbarRing& ring,
                                               const float* __restrict__ gy, float* __restrict__ partial, int r, int s0, int t0, int t1,
                                               int Ho, int Wo, int tiles_x, int tiles_y) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wq = warp & 3;
@@ -223,7 +208,7 @@ __device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned 
         for (int i = 0; i < 32; ++i) acc[t][i] = 0.f;
 
     for (int tile = t0; tile < t1; ++tile) {
-        const int it = tile - t0, st = it % WG_STAGES;
+        const int it = tile - t0;
         const int b = tile / (tiles_x * tiles_y), ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
         const int oy0 = ty * CV_TH, ox0 = tx * CV_TW;
         unsigned char* bt = bs + (it & 1) * WG_B_BYTES;
@@ -249,11 +234,11 @@ __device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned 
             }
         }
         fence_proxy_async();                          // generic-proxy stores -> visible to the tensor core's async proxy
-        asm volatile("bar.sync 1, %0;" ::"n"(WG_THREADS) : "memory");   // both warpgroups (their code paths differ: named barrier)
+        named_barrier(1, WG_THREADS);                 // both warpgroups (their code paths differ: named barrier)
         // every warp has finished tile it - 1: its x stage may be refilled with the next tile's window
-        if (threadIdx.x == 0 && tile + 1 < t1) wgrad_load_window(xmap, xs, full, r, tile + 1, it + 1, tiles_x, tiles_y);
+        if (threadIdx.x == 0 && tile + 1 < t1) wgrad_load_window(xmap, xs, ring, r, tile + 1, it + 1, tiles_x, tiles_y);
 
-        mbar_wait(full + st, (it / WG_STAGES) & 1);
+        const int st = ring.consume(it);
         const unsigned char* xw = xs + st * WG_X_STAGE;
         const uint32_t b_addr = smem_addr(bt);
 #pragma unroll 1
@@ -310,11 +295,9 @@ __device__ __forceinline__ void wgrad_consume(const CUtensorMap* xmap, unsigned 
 __global__ void __launch_bounds__(WG_THREADS, 1)
 bev_conv7x7s2_wgrad_kernel(const __grid_constant__ CUtensorMap xmap, const float* __restrict__ gy, float* __restrict__ partial, int Ho,
                            int Wo, int tiles_x, int tiles_y, int n_tiles) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    unsigned char* xs = smem;
-    unsigned char* bs = smem + WG_STAGES * WG_X_STAGE;
-    uint64_t* full = reinterpret_cast<uint64_t*>(bs + 2 * WG_B_BYTES);
+    unsigned char* xs = dynamic_smem_1024();
+    unsigned char* bs = xs + WG_STAGES * WG_X_STAGE;
+    const MbarRing ring(reinterpret_cast<uint64_t*>(bs + 2 * WG_B_BYTES), WG_STAGES);
 
     const int r = blockIdx.x;
     const int t0 = static_cast<int>(static_cast<long long>(blockIdx.y) * n_tiles / gridDim.y);
@@ -322,56 +305,41 @@ bev_conv7x7s2_wgrad_kernel(const __grid_constant__ CUtensorMap xmap, const float
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&xmap);
-        for (int s = 0; s < WG_STAGES; ++s) mbar_init(full + s, 1);
-        fence_mbar_init();
-        wgrad_load_window(&xmap, xs, full, r, t0, 0, tiles_x, tiles_y);
+        ring.init(0);
+        wgrad_load_window(&xmap, xs, ring, r, t0, 0, tiles_x, tiles_y);
     }
     __syncthreads();
-    if (threadIdx.x < 128) wgrad_consume<4>(&xmap, xs, bs, full, gy, partial, r, 0, t0, t1, Ho, Wo, tiles_x, tiles_y);
-    else wgrad_consume<3>(&xmap, xs, bs, full, gy, partial, r, 4, t0, t1, Ho, Wo, tiles_x, tiles_y);
+    if (threadIdx.x < 128) wgrad_consume<4>(&xmap, xs, bs, ring, gy, partial, r, 0, t0, t1, Ho, Wo, tiles_x, tiles_y);
+    else wgrad_consume<3>(&xmap, xs, bs, ring, gy, partial, r, 4, t0, t1, Ho, Wo, tiles_x, tiles_y);
 }
 
-// dw (OIHW) = sum of the chunks' partials in ascending chunk order (zeros when there are none)
-__global__ void bev_conv7x7s2_wgrad_reduce_kernel(const float* __restrict__ partial, int n_chunks, float* __restrict__ dw) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= static_cast<int>(WG_PARTIAL_FLOATS)) return;
-    float s = 0.f;
-    for (int c = 0; c < n_chunks; ++c) s += partial[c * WG_PARTIAL_FLOATS + i];
-    dw[i] = s;
-}
+// a chunk's partial is laid out as dw (OIHW)
+struct CvWgradOffset {
+    __device__ size_t operator()(int i) const { return i; }
+};
 
 int launch_bev_conv_wgrad(int n_frames, int H, int W, const float* x_nhwc, const float* gy_nhwc, float* dw_oihw, void* workspace,
                           cudaStream_t stream) {
-    FIERY_REQUIRE(n_frames >= 0 && H >= 1 && W >= 1, "bev conv backward: bad shape %d x %d x %d", n_frames, H, W);
-    FIERY_REQUIRE(dw_oihw, "bev conv backward: NULL grad_weight");
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(dw_oihw) & 15) == 0, "bev conv backward: pointers must be 16-byte aligned");
-    const int n_chunks = bev_conv_wgrad_chunks(n_frames, H, W);
-    const int n_red = static_cast<int>(WG_PARTIAL_FLOATS);
-    if (n_chunks == 0) {
-        bev_conv7x7s2_wgrad_reduce_kernel<<<(n_red + 255) / 256, 256, 0, stream>>>(nullptr, 0, dw_oihw);
-        FIERY_CUDA_CHECK(cudaGetLastError());
-        return FIERY_OK;
-    }
-    FIERY_REQUIRE(x_nhwc && gy_nhwc && workspace, "bev conv backward: NULL pointer");
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(x_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(gy_nhwc) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "bev conv backward: pointers must be 16-byte aligned");
-    const int Ho = conv_out_size(H), Wo = conv_out_size(W);
-    FIERY_REQUIRE(wgrad_tiles(n_frames, H, W) < (1ll << 31), "bev conv backward: too many pixels");
-    CUtensorMap xmap;
-    int rc = encode_conv_activation_map(&xmap, x_nhwc, n_frames, H, W, WG_WIN_W, 2 * CV_TH, 1, 2, "conv input window");
-    if (rc != FIERY_OK) return rc;
-    const int smem = WG_STAGES * WG_X_STAGE + 2 * WG_B_BYTES + 1024 /* alignment slack */ + 64 /* barriers */;
-    static OncePerDevice once;
-    rc = once.run([smem]() { return set_dynamic_smem(bev_conv7x7s2_wgrad_kernel, smem); });
-    if (rc != FIERY_OK) return rc;
-    const int tiles_x = (Wo + CV_TW - 1) / CV_TW, tiles_y = (Ho + CV_TH - 1) / CV_TH;
+    const long long tiles = wgrad_tiles(n_frames, H, W);
+    const int n_chunks = wgrad_chunks(tiles, CV_WG_MAX_CHUNKS);
     float* partial = static_cast<float*>(workspace);
-    bev_conv7x7s2_wgrad_kernel<<<dim3(7, n_chunks), WG_THREADS, smem, stream>>>(xmap, gy_nhwc, partial, Ho, Wo, tiles_x, tiles_y,
-                                                                               static_cast<int>(wgrad_tiles(n_frames, H, W)));
-    FIERY_CUDA_CHECK(cudaGetLastError());
-    bev_conv7x7s2_wgrad_reduce_kernel<<<(n_red + 255) / 256, 256, 0, stream>>>(partial, n_chunks, dw_oihw);
-    FIERY_CUDA_CHECK(cudaGetLastError());
-    return FIERY_OK;
+    if (n_chunks > 0) {
+        FIERY_REQUIRE(tiles < (1ll << 31), "bev conv backward: too many pixels");
+        CUtensorMap xmap;
+        int rc = encode_conv_activation_map(&xmap, x_nhwc, n_frames, H, W, WG_WIN_W, 2 * CV_TH, 1, 2, "conv input window");
+        if (rc != FIERY_OK) return rc;
+        const int smem = WG_STAGES * WG_X_STAGE + 2 * WG_B_BYTES + 1024 /* alignment slack */ + 64 /* barriers */;
+        static OncePerDevice once;
+        rc = once.run([smem]() { return set_dynamic_smem(bev_conv7x7s2_wgrad_kernel, smem); });
+        if (rc != FIERY_OK) return rc;
+        const int Ho = conv_out_size(H), Wo = conv_out_size(W);
+        const int tiles_x = (Wo + CV_TW - 1) / CV_TW, tiles_y = (Ho + CV_TH - 1) / CV_TH;
+        bev_conv7x7s2_wgrad_kernel<<<dim3(7, n_chunks), WG_THREADS, smem, stream>>>(xmap, gy_nhwc, partial, Ho, Wo, tiles_x, tiles_y,
+                                                                                   static_cast<int>(tiles));
+        FIERY_CUDA_CHECK(cudaGetLastError());
+    }
+    return launch_wgrad_reduce(partial, n_chunks, WG_PARTIAL_FLOATS, static_cast<int>(WG_PARTIAL_FLOATS), CvWgradOffset{}, dw_oihw,
+                               stream);
 }
 
 }  // namespace fiery

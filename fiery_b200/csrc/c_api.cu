@@ -399,6 +399,8 @@ FIERY_API int fiery_warp_theta(int32_t n_sequences, int32_t T, int32_t cumulativ
                              static_cast<cudaStream_t>(stream));
 }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 FIERY_API int fiery_bev_conv_pack_weights(const float* weight_oihw, float* packed_out, void* stream) {
     FIERY_REQUIRE(weight_oihw && packed_out, "bev conv: NULL weight pointer");
     return launch_pack_conv_weights(weight_oihw, packed_out, static_cast<cudaStream_t>(stream));
@@ -407,6 +409,10 @@ FIERY_API int fiery_bev_conv_pack_weights(const float* weight_oihw, float* packe
 FIERY_API int fiery_bev_first_conv_forward(int32_t n_frames, int32_t height, int32_t width, const float* x_nhwc, const float* packed_weight,
                                            const float* scale, const float* shift, int32_t relu, float* y_nhwc, void* stream) {
     FIERY_REQUIRE(n_frames == 0 || (x_nhwc && packed_weight && y_nhwc), "bev conv: NULL pointer");
+    FIERY_REQUIRE(n_frames >= 0 && height >= 1 && width >= 1, "bev conv: bad shape %d x %d x %d", n_frames, height, width);
+    if (n_frames == 0) return FIERY_OK;
+    FIERY_REQUIRE((scale == nullptr) == (shift == nullptr), "bev conv: scale and shift go together");
+    FIERY_REQUIRE(aligned16(x_nhwc) && aligned16(packed_weight) && aligned16(y_nhwc), "bev conv: pointers must be 16-byte aligned");
     return launch_bev_conv(n_frames, height, width, x_nhwc, packed_weight, scale, shift, relu ? 1 : 0, y_nhwc, static_cast<cudaStream_t>(stream));
 }
 
@@ -417,6 +423,11 @@ FIERY_API int fiery_bev_conv_pack_weights_transposed(const float* weight_oihw, f
 
 FIERY_API int fiery_bev_first_conv_backward_data(int32_t n_frames, int32_t height, int32_t width, const float* grad_y_nhwc,
                                                  const float* packed_weight_t, float* grad_x_nhwc, void* stream) {
+    FIERY_REQUIRE(n_frames >= 0 && height >= 1 && width >= 1, "bev conv backward: bad shape %d x %d x %d", n_frames, height, width);
+    if (n_frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(grad_y_nhwc && packed_weight_t && grad_x_nhwc, "bev conv backward: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_y_nhwc) && aligned16(packed_weight_t) && aligned16(grad_x_nhwc),
+                  "bev conv backward: pointers must be 16-byte aligned");
     return launch_bev_conv_dgrad(n_frames, height, width, grad_y_nhwc, packed_weight_t, grad_x_nhwc, static_cast<cudaStream_t>(stream));
 }
 
@@ -426,12 +437,27 @@ FIERY_API size_t fiery_bev_first_conv_backward_weight_workspace_bytes(int32_t n_
 
 FIERY_API int fiery_bev_first_conv_backward_weight(int32_t n_frames, int32_t height, int32_t width, const float* x_nhwc,
                                                    const float* grad_y_nhwc, float* grad_weight_oihw, void* workspace, void* stream) {
+    FIERY_REQUIRE(n_frames >= 0 && height >= 1 && width >= 1, "bev conv backward: bad shape %d x %d x %d", n_frames, height, width);
+    FIERY_REQUIRE(grad_weight_oihw, "bev conv backward: NULL grad_weight");
+    FIERY_REQUIRE(aligned16(grad_weight_oihw), "bev conv backward: pointers must be 16-byte aligned");
+    if (n_frames > 0) {
+        FIERY_REQUIRE(x_nhwc && grad_y_nhwc && workspace, "bev conv backward: NULL pointer");
+        FIERY_REQUIRE(aligned16(x_nhwc) && aligned16(grad_y_nhwc) && aligned16(workspace), "bev conv backward: pointers must be 16-byte aligned");
+    }
     return launch_bev_conv_wgrad(n_frames, height, width, x_nhwc, grad_y_nhwc, grad_weight_oihw, workspace, static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API int fiery_depth_layer_forward(int32_t n_images, int32_t pixels, int32_t n_out, const void* feat, int32_t dtype,
                                         const void* weight_padded, const float* bias, float* head_out, void* stream) {
     FIERY_REQUIRE(n_images == 0 || (feat && weight_padded && head_out), "depth layer: NULL pointer");
+    // 128 = DL_M (depth_layer.cu): the rows of the padded weight matrix
+    FIERY_REQUIRE(n_images >= 0 && pixels >= 1 && n_out >= 1 && n_out <= 128, "depth layer: bad shape (%d images, %d pixels, %d outputs)",
+                  n_images, pixels, n_out);
+    FIERY_REQUIRE(dtype >= 0 && dtype <= 2, "depth layer: dtype %d not supported (0 fp32, 1 fp16, 2 bf16)", dtype);
+    if (n_images == 0) return FIERY_OK;
+    FIERY_REQUIRE((static_cast<long long>(pixels) * (dtype == 0 ? 4 : 2)) % 16 == 0 && pixels % 4 == 0,
+                  "depth layer: h*w = %d must give a 16-byte row pitch (and a multiple of 4)", pixels);
+    FIERY_REQUIRE(aligned16(feat) && aligned16(weight_padded) && aligned16(head_out), "depth layer: pointers must be 16-byte aligned");
     return launch_depth_layer(n_images, pixels, n_out, feat, dtype, weight_padded, bias, head_out, static_cast<cudaStream_t>(stream));
 }
 
@@ -459,8 +485,6 @@ static int check_temporal_entry_desc(const fiery_temporal_entry_desc_t* d) {
                   (long long)d->in_stride_b, (long long)d->in_stride_t, (long long)d->in_stride_c);
     return FIERY_OK;
 }
-
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 FIERY_API size_t fiery_temporal_entry_packed_bytes(const fiery_temporal_entry_desc_t* desc) {
     if (check_temporal_entry_desc(desc) != FIERY_OK) return 0;

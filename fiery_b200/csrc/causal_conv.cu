@@ -118,16 +118,13 @@ struct CcFwdLaunch {
 template <int N>
 __global__ void __launch_bounds__(CC_FWD_THREADS, 1)
 causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch L, float* __restrict__ out) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     const int w_bytes = L.ka * N * 128;
     const int x_floats = L.kpad * CC_PLANE;
     const int taps = 9 * L.kt;
-    unsigned char* s_w = smem;
+    unsigned char* s_w = dynamic_smem_1024();
     const float* s_x = reinterpret_cast<const float*>(s_w + CC_WSTAGES * w_bytes);
     uint64_t* x_full = reinterpret_cast<uint64_t*>(const_cast<float*>(s_x) + L.kt * x_floats);
-    uint64_t* full = x_full + 1;
-    uint64_t* empty = full + CC_WSTAGES;
+    const MbarRing ring(x_full + 1, CC_WSTAGES);
 
     int tile = blockIdx.x;
     const int ty = tile % L.tiles_y;
@@ -140,12 +137,8 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w);
-        mbar_init(x_full, 1);
-        for (int i = 0; i < CC_WSTAGES; ++i) {
-            mbar_init(full + i, 1);
-            mbar_init(empty + i, 8);                   // one arrival per consumer warp
-        }
-        fence_mbar_init();
+        mbar_init(x_full, 1);                          // published to the async proxy by the fence in ring.init
+        ring.init(8);
     }
     __syncthreads();
 
@@ -155,10 +148,8 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
             for (int jt = 0; jt < L.kt; ++jt)
                 tma_load_5d(const_cast<float*>(s_x) + jt * x_floats, &maps.x, x_full, y0 - 4, x0 - 1, t + jt + L.t_off, 0, b);
             for (int j = 0; j < taps; ++j) {
-                const int st = j % CC_WSTAGES, use = j / CC_WSTAGES;
-                if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
-                mbar_arrive_expect_tx(full + st, w_bytes);
-                for (int a = 0; a < L.ka; ++a) tma_load_3d(s_w + st * w_bytes + a * N * 128, &maps.w, full + st, 0, 0, j * L.ka + a);
+                const int st = ring.produce(j, w_bytes);
+                for (int a = 0; a < L.ka; ++a) tma_load_3d(s_w + st * w_bytes + a * N * 128, &maps.w, ring.full + st, 0, 0, j * L.ka + a);
             }
         }
         return;
@@ -174,11 +165,9 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
     mbar_wait(x_full, 0);
 #pragma unroll 1
     for (int j = 0; j < taps; ++j) {
-        const int st = j % CC_WSTAGES, use = j / CC_WSTAGES;
         const int jt = j / 9, ay = j / 3 % 3, ax = j % 3;
         const float* h = s_x + jt * x_floats + (row + ay) * CC_HY + col + ax + CC_HY_OFF + kq * CC_PLANE;
-        const uint32_t wb = smem_addr(s_w + st * w_bytes);
-        mbar_wait(full + st, use & 1);
+        const uint32_t wb = smem_addr(s_w + ring.consume(j) * w_bytes);
 #pragma unroll 1
         for (int a = 0; a < L.ka; ++a) {               // 32 channels (4 k-steps) at a time
             uint32_t fr[4][4];
@@ -199,8 +188,7 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
             wgmma_wait<0>();
         }
         wgmma_fence_operands(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + st);        // this warp is done with the slice
+        ring.release(j);                               // this warp is done with the slice
     }
 
     const int gx = x0 + row;
@@ -233,7 +221,7 @@ static size_t cc_partial_floats(const CcShape& s) { return static_cast<size_t>(s
 
 size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d) {
     const CcShape s = cc_shape(d);
-    return static_cast<size_t>(wgrad_chunks(cc_wgrad_tiles(s))) * cc_partial_floats(s) * sizeof(float);
+    return static_cast<size_t>(wgrad_chunks(cc_wgrad_tiles(s), WG_MAX_CHUNKS)) * cc_partial_floats(s) * sizeof(float);
 }
 
 // grid (chunks, 3 kt): CTA (chunk, tau * 3 + dy) accumulates the taps (tau, dy, 0..2) over its chunk's tiles as D (input channels x
@@ -244,10 +232,9 @@ size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d) {
 template <int NO>
 __global__ void __launch_bounds__(128, 1)
 causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, float* __restrict__ partial, int n_tiles) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    unsigned char* smem = dynamic_smem_1024();
     constexpr int STAGE_BYTES = CC_WG_X_BYTES + NO * 128;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + CC_WG_STAGES * STAGE_BYTES);
+    const MbarRing ring(reinterpret_cast<uint64_t*>(smem + CC_WG_STAGES * STAGE_BYTES), CC_WG_STAGES);
     const int tau = blockIdx.y / 3, dy = blockIdx.y % 3;
     const int t0 = static_cast<int>(static_cast<long long>(blockIdx.x) * n_tiles / gridDim.x);
     const int t1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * n_tiles / gridDim.x);
@@ -258,9 +245,9 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
         const int run = t % runs;
         t /= runs;
         const int x = t % s.X, f = t / s.X, b = f / s.frames, tt = f % s.frames;
-        unsigned char* dst = smem + (i % CC_WG_STAGES) * STAGE_BYTES;
-        uint64_t* bar = full + i % CC_WG_STAGES;
-        mbar_arrive_expect_tx(bar, STAGE_BYTES);
+        const int st = ring.arm(i, STAGE_BYTES);
+        unsigned char* dst = smem + st * STAGE_BYTES;
+        uint64_t* bar = ring.full + st;
         tma_load_5d(dst, &maps.x, bar, CC_WG_PX * run - 4, x + dy - 1, tt + tau - (s.kt - 1), 0, b);
         tma_load_5d(dst + CC_WG_X_BYTES, &maps.gy, bar, CC_WG_PX * run, x, tt, 0, b);
     };
@@ -268,8 +255,7 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&maps.gy);
         tma_prefetch_desc(&maps.x);
-        for (int i = 0; i < CC_WG_STAGES; ++i) mbar_init(full + i, 1);
-        fence_mbar_init();
+        ring.init(0);
         for (int i = 0; i < CC_WG_STAGES - 1 && t0 + i < t1; ++i) load(i);
     }
     __syncthreads();
@@ -285,8 +271,7 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
     for (int i = 0; t0 + i < t1; ++i) {
         __syncthreads();                           // every warp is done with tile i - 1: its stage may be refilled
         if (threadIdx.x == 0 && t0 + i + CC_WG_STAGES - 1 < t1) load(i + CC_WG_STAGES - 1);
-        const int st = i % CC_WG_STAGES;
-        mbar_wait(full + st, (i / CC_WG_STAGES) & 1);
+        const int st = ring.consume(i);
         const float* xs = reinterpret_cast<const float*>(smem + st * STAGE_BYTES) + ra * CC_WG_XP + kq + 3;
         const uint32_t g_addr = smem_addr(smem + st * STAGE_BYTES + CC_WG_X_BYTES);
         uint32_t a[CC_WG_PX / 8][3][4];
@@ -334,17 +319,14 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
     }
 }
 
-// grad_w (C_out, C_in, kt, 3, 3) = sum of the chunks' partials in ascending chunk order (zeros when there are none)
-__global__ void causal_conv_wgrad_reduce_kernel(const CcShape s, const float* __restrict__ partial, int n_chunks, float* __restrict__ gw) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= s.cout * s.cin * s.taps) return;
-    const int tap = i % s.taps, oi = i / s.taps;     // oi = o * cin + ci
-    const size_t stride = static_cast<size_t>(s.taps) * s.cout * s.cin;
-    const size_t off = static_cast<size_t>(tap) * s.cout * s.cin + oi;
-    float acc = 0.f;
-    for (int c = 0; c < n_chunks; ++c) acc += partial[c * stride + off];
-    gw[i] = acc;
-}
+// grad_w (C_out, C_in, kt, 3, 3) index -> its place in a chunk's partial (tap, o, ci)
+struct CcWgradOffset {
+    CcShape s;
+    __device__ size_t operator()(int i) const {
+        const int tap = i % s.taps, oi = i / s.taps;     // oi = o * cin + ci
+        return static_cast<size_t>(tap) * s.cout * s.cin + oi;
+    }
+};
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // host
@@ -418,7 +400,7 @@ int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x
                              cudaStream_t stream) {
     const CcShape s = cc_shape(d);
     const long long tiles = cc_wgrad_tiles(s);
-    const int n_chunks = wgrad_chunks(tiles);
+    const int n_chunks = wgrad_chunks(tiles, WG_MAX_CHUNKS);
     float* partial = static_cast<float*>(workspace);
     if (n_chunks > 0) {
         FIERY_REQUIRE(tiles < (1ll << 31), "causal conv: too many pixel tiles");
@@ -443,10 +425,7 @@ int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x
         }
         FIERY_CUDA_CHECK(cudaGetLastError());
     }
-    const int n_red = s.cout * s.cin * s.taps;
-    causal_conv_wgrad_reduce_kernel<<<(n_red + 255) / 256, 256, 0, stream>>>(s, partial, n_chunks, gw);
-    FIERY_CUDA_CHECK(cudaGetLastError());
-    return FIERY_OK;
+    return launch_wgrad_reduce(partial, n_chunks, cc_partial_floats(s), s.cout * s.cin * s.taps, CcWgradOffset{s}, gw, stream);
 }
 
 }  // namespace fiery

@@ -123,6 +123,62 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// A ring of `stages` shared-memory stages that TMA fills and the consumers read in order: iteration `it` uses stage it % stages for
+// the (it / stages)-th time.  full[s] (count 1) completes when the producer has armed it and the stage's bytes have landed; empty[s]
+// completes when every consumer warp has released the stage.  The barriers lie in one array, full[stages] then empty[stages].  A
+// ring initialised with no consumer warps has no empty side: its kernels arm() a stage only after a CTA-wide barrier has shown every
+// consumer done with it.
+struct MbarRing {
+    uint64_t* full;
+    uint64_t* empty;
+    int stages;
+
+    __device__ __forceinline__ MbarRing(uint64_t* bars, int n) : full(bars), empty(bars + n), stages(n) {}
+
+    // one thread, before a CTA barrier
+    __device__ __forceinline__ void init(uint32_t consumer_warps) const {
+        for (int s = 0; s < stages; ++s) {
+            mbar_init(full + s, 1);
+            if (consumer_warps) mbar_init(empty + s, consumer_warps);
+        }
+        fence_mbar_init();
+    }
+    // announce the bytes that iteration it's loads bring into its stage; returns the stage
+    __device__ __forceinline__ int arm(int it, uint32_t bytes) const {
+        const int st = it % stages;
+        mbar_arrive_expect_tx(full + st, bytes);
+        return st;
+    }
+    // producer: wait until the consumers have released the stage's previous use, then arm it
+    __device__ __forceinline__ int produce(int it, uint32_t bytes) const {
+        const int st = it % stages, use = it / stages;
+        if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
+        mbar_arrive_expect_tx(full + st, bytes);
+        return st;
+    }
+    // consumer: wait until iteration it's stage has landed; returns the stage
+    __device__ __forceinline__ int consume(int it) const {
+        const int st = it % stages;
+        mbar_wait(full + st, (it / stages) & 1);
+        return st;
+    }
+    // consumer warp: every lane is done reading iteration it's stage
+    __device__ __forceinline__ void release(int it) const {
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(empty + it % stages);
+    }
+};
+
+// The dynamic shared memory, realigned to the 1024 bytes the 128-byte swizzle atoms need: the window itself is only guaranteed
+// 16-byte aligned, so launches reserve 1024 bytes of slack.
+__device__ __forceinline__ unsigned char* dynamic_smem_1024() {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    return reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+}
+
+// Named barrier `id` (1..15; 0 is __syncthreads) over n threads, for code paths that only some warps take
+__device__ __forceinline__ void named_barrier(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
 // L2 eviction-priority policies (createpolicy: a 64-bit descriptor covering the whole access) for the .L2::cache_hint forms:
 // evict_first for data used once (it streams past what should stay), evict_last for data that is used again soon,
 // evict_normal to hand lines back to the default priority.

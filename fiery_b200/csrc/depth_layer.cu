@@ -15,8 +15,8 @@
 //                channel, so a thread's float2 stores go to consecutive pixels of one plane of the head tensor.
 //   fp32 (TF32): wgmma has no MN-major TF32 operand, so the product is taken transposed, D (128 pixels x 128 output channels) =
 //                feat^T x W^T: the weight matrix is the K-major B operand as it lies, the feature tile is the A operand, read from
-//                shared memory into registers.  Warpgroup g owns pixel rows 64g .. 64g + 63, in the order dl_pixel() gives them
-//                (conflict-free fragment loads from the swizzled tile).
+//                shared memory into registers.  Warpgroup g owns pixel rows 64g .. 64g + 63, in the order tile_pixel() gives them
+//                (conflict-free fragment loads from the swizzled tile, wgmma.cuh).
 #include "wgmma.cuh"
 
 namespace fiery {
@@ -45,44 +45,24 @@ struct DlShape {
     static constexpr int SMEM = W_BYTES + STAGES * B_BYTES + 1024 + 256;
 };
 
-// fp32 path: accumulator row r (0..127) -> pixel of the tile.  The 8 rows one fragment load covers (r = 8t .. 8t + 7) are 4 pixels
-// from the first half of a 128-byte row of the swizzled tile and 4 from the second half, so with the 4 channels of the load they hit
-// 32 different banks.
-__device__ __forceinline__ int dl_pixel(int r) {
-    const int t = r >> 3, q = r & 7;
-    return (t >> 2) * 32 + (q >> 2) * 16 + (t & 3) * 4 + (q & 3);
-}
-
-// byte offset of (channel, pixel) in a feature tile of fp32 blocks (32 pixels x 128 channels, 128-byte swizzle)
-__device__ __forceinline__ uint32_t dl_feat_offset(int ch, int px) {
-    return (px >> 5) * DlShape<4>::B_BLK + ch * 128 + ((((px & 31) >> 2) ^ (ch & 7)) << 4) + (px & 3) * 4;
-}
-
 // ES: element size of the operands (2: fp16 / bf16; 4: fp32 read as TF32).  BF16 selects the 16-bit type.
 template <int ES, bool BF16>
 __global__ void __launch_bounds__(DL_THREADS, 1)
 depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __restrict__ bias, float* __restrict__ head, int n_out,
                    int pixels, int tiles_per_image, int n_tiles) {
     using S = DlShape<ES>;
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    unsigned char* s_w = smem;
+    unsigned char* s_w = dynamic_smem_1024();
     unsigned char* s_b = s_w + S::W_BYTES;
     uint64_t* w_full = reinterpret_cast<uint64_t*>(s_b + S::STAGES * S::B_BYTES);
-    uint64_t* b_full = w_full + 1;
-    uint64_t* b_empty = b_full + S::STAGES;
+    const MbarRing ring(w_full + 1, S::STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == DL_PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&maps.w);
         tma_prefetch_desc(&maps.feat);
-        mbar_init(w_full, 1);
-        for (int i = 0; i < S::STAGES; ++i) {
-            mbar_init(b_full + i, 1);
-            mbar_init(b_empty + i, 4 * DL_CONSUMERS);  // one arrival per consumer warp
-        }
-        fence_mbar_init();
+        mbar_init(w_full, 1);                          // published to the async proxy by the fence in ring.init
+        ring.init(4 * DL_CONSUMERS);
     }
     __syncthreads();
 
@@ -93,13 +73,11 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
             for (int a = 0; a < S::ATOMS; ++a) tma_load_2d(s_w + a * S::W_ATOM, &maps.w, w_full, a * S::EPR, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-                const int st = it % S::STAGES, use = it / S::STAGES;
-                if (use > 0) mbar_wait(b_empty + st, (use - 1) & 1);
+                const int st = ring.produce(it, S::B_BYTES);
                 const int img = t / tiles_per_image, p0 = (t % tiles_per_image) * DL_N;
                 unsigned char* dst = s_b + st * S::B_BYTES;
-                mbar_arrive_expect_tx(b_full + st, S::B_BYTES);
 #pragma unroll
-                for (int b = 0; b < S::NBLK; ++b) tma_load_3d(dst + b * S::B_BLK, &maps.feat, b_full + st, p0 + b * S::EPR, 0, img);   // pixels past the image: zeros
+                for (int b = 0; b < S::NBLK; ++b) tma_load_3d(dst + b * S::B_BLK, &maps.feat, ring.full + st, p0 + b * S::EPR, 0, img);   // pixels past the image: zeros
             }
         }
         return;
@@ -113,10 +91,8 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
     mbar_wait(w_full, 0);
     int it = 0;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-        const int st = it % S::STAGES, use = it / S::STAGES;
         const int img = t / tiles_per_image, p0 = (t % tiles_per_image) * DL_N;
-        const unsigned char* tile = s_b + st * S::B_BYTES;
-        mbar_wait(b_full + st, use & 1);
+        const unsigned char* tile = s_b + ring.consume(it) * S::B_BYTES;
         float acc[64];
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -134,16 +110,8 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
                 else wgmma_m64n128k16_f16_ss_tb(acc, da, db);
             }
         } else {
-            const int pa = dl_pixel(r0), pb = dl_pixel(r0 + 8);
             uint32_t a[DL_K / 8][4];
-#pragma unroll
-            for (int k = 0; k < DL_K / 8; ++k) {
-                const int ch = 8 * k + (lane & 3);
-                a[k][0] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch, pa));
-                a[k][1] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch, pb));
-                a[k][2] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch + 4, pa));
-                a[k][3] = *reinterpret_cast<const uint32_t*>(tile + dl_feat_offset(ch + 4, pb));
-            }
+            load_pixel_frags<DL_K / 8>(a, tile, DL_K, 0, tile_pixel(r0), tile_pixel(r0 + 8));
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < DL_K / 8; ++k) {
@@ -154,8 +122,7 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_empty + st);      // this warp's part of the tile has been read
+        ring.release(it);                              // this warp's part of the tile has been read
         if constexpr (ES == 2) {                       // rows = output channels r0, r0 + 8; columns = pixels
             float* out = head + (static_cast<size_t>(img) * n_out + r0) * pixels + p0;
             const float b0 = (bias && r0 < n_out) ? __ldg(bias + r0) : 0.f;
@@ -169,8 +136,8 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
                         *reinterpret_cast<float2*>(out + 8 * static_cast<size_t>(pixels) + p) = make_float2(acc[4 * j + 2] + b1, acc[4 * j + 3] + b1);
                 }
             }
-        } else {                                       // rows = pixels dl_pixel(r0), dl_pixel(r0 + 8); columns = output channels
-            const int pa = p0 + dl_pixel(r0), pb = p0 + dl_pixel(r0 + 8);
+        } else {                                       // rows = pixels tile_pixel(r0), tile_pixel(r0 + 8); columns = output channels
+            const int pa = p0 + tile_pixel(r0), pb = p0 + tile_pixel(r0 + 8);
             float* out = head + static_cast<size_t>(img) * n_out * pixels;
 #pragma unroll
             for (int j = 0; j < DL_M / 8; ++j) {
@@ -191,15 +158,7 @@ depth_layer_kernel(const __grid_constant__ DepthLayerMaps maps, const float* __r
 // dtype: 0 fp32 (TF32 math), 1 fp16, 2 bf16 -- of BOTH the feature map and the padded weight matrix
 int launch_depth_layer(int n_images, int pixels, int n_out, const void* feat, int dtype, const void* weight_padded, const float* bias,
                        float* head, cudaStream_t stream) {
-    FIERY_REQUIRE(n_images >= 0 && pixels >= 1 && n_out >= 1 && n_out <= DL_M, "depth layer: bad shape (%d images, %d pixels, %d outputs)",
-                  n_images, pixels, n_out);
-    FIERY_REQUIRE(dtype >= 0 && dtype <= 2, "depth layer: dtype %d not supported (0 fp32, 1 fp16, 2 bf16)", dtype);
-    if (n_images == 0) return FIERY_OK;
     const int es = dtype == 0 ? 4 : 2;
-    FIERY_REQUIRE((static_cast<long long>(pixels) * es) % 16 == 0 && pixels % 4 == 0,
-                  "depth layer: h*w = %d must give a 16-byte row pitch (and a multiple of 4)", pixels);
-    FIERY_REQUIRE((reinterpret_cast<uintptr_t>(feat) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight_padded) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(head) & 15) == 0, "depth layer: pointers must be 16-byte aligned");
     const CUtensorMapDataType dt = dtype == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     const cuuint32_t epr = 128 / es;
     DepthLayerMaps maps;

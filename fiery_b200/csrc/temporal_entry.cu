@@ -137,34 +137,13 @@ int launch_temporal_entry_pack(const fiery_temporal_entry_desc_t* d, const float
 // ------------------------------------------------------------------------------------------------------------------------------
 // shared device helpers
 // ------------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void te_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-
-// accumulator row r (0..127) -> pixel of the tile: rows 64g .. 64g + 63 map to pixels 64g .. 64g + 63, and the 8 rows one fragment
-// load covers hit 32 different banks of the swizzled tile (4 pixels from each half of a 128-byte row, 4 channels)
-__device__ __forceinline__ int te_pixel(int r) {
-    const int t = r >> 3, q = r & 7;
-    return (t >> 2) * 32 + (q >> 2) * 16 + (t & 3) * 4 + (q & 3);
-}
-// byte offset of (row, pixel) in a tile of 32-pixel blocks of `rows` 128-byte rows each, 128-byte swizzle
-__device__ __forceinline__ uint32_t te_offset(int rows, int row, int px) {
-    return (px >> 5) * rows * 128 + row * 128 + ((((px & 31) >> 2) ^ (row & 7)) << 4) + (px & 3) * 4;
-}
-
 // acc[c] (64 pixel rows x 64 columns of n-chunk c) += tile rows 32 kg .. 32 kg + 31 (as the register A operand, pixel rows pa / pb)
 // x the B atom at b_atom (NC*64 K-major rows of 32 fp32 k); 4 k-steps, drained before returning
 template <int NC>
 __device__ __forceinline__ void te_mma_group(float (&acc)[NC][32], const unsigned char* tile, int rows, int kg, int pa, int pb,
                                              uint32_t b_atom) {
-    const int lane = threadIdx.x & 31;
     uint32_t a[4][4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int ch = 32 * kg + 8 * k + (lane & 3);
-        a[k][0] = *reinterpret_cast<const uint32_t*>(tile + te_offset(rows, ch, pa));
-        a[k][1] = *reinterpret_cast<const uint32_t*>(tile + te_offset(rows, ch, pb));
-        a[k][2] = *reinterpret_cast<const uint32_t*>(tile + te_offset(rows, ch + 4, pa));
-        a[k][3] = *reinterpret_cast<const uint32_t*>(tile + te_offset(rows, ch + 4, pb));
-    }
+    load_pixel_frags<4>(a, tile, rows, 32 * kg, pa, pb);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k)
@@ -181,7 +160,7 @@ template <typename RowFn>
 __device__ __forceinline__ void te_store_cols(const float (&acc)[32], int h, float* stg, int bar_id, int n_valid_px, RowFn row_ptr) {
     const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int r0 = 16 * wq + (lane >> 2);
-    const int pa = te_pixel(r0), pb = te_pixel(r0 + 8);
+    const int pa = tile_pixel(r0), pb = tile_pixel(r0 + 8);
     const int cq = 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < 4; ++j)
@@ -191,7 +170,7 @@ __device__ __forceinline__ void te_store_cols(const float (&acc)[32], int h, flo
             stg[col * TE_STG_PITCH + pa] = acc[4 * (4 * h + j) + e];
             stg[col * TE_STG_PITCH + pb] = acc[4 * (4 * h + j) + 2 + e];
         }
-    te_bar(bar_id, 128);
+    named_barrier(bar_id, 128);
 #pragma unroll
     for (int col = 8 * wq; col < 8 * wq + 8; ++col) {
         float bias = 0.f;
@@ -201,7 +180,7 @@ __device__ __forceinline__ void te_store_cols(const float (&acc)[32], int h, flo
             *reinterpret_cast<float2*>(dst + 2 * lane) = make_float2(v.x + bias, v.y + bias);
         }
     }
-    te_bar(bar_id, 128);
+    named_barrier(bar_id, 128);
 }
 
 // the four segments' output-gradient tiles (round8(C_q) rows x 32 pixels per block, 2 blocks) of frame (b, t), pixels p0 ..
@@ -234,30 +213,23 @@ template <int NCH>
 __global__ void __launch_bounds__(TE_FWD_THREADS, 1)
 temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape s, const float* __restrict__ extra,
                           const float* __restrict__ w_extra, const TeOut out, int stages, int tiles_per_frame, int n_tiles) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     const int k32 = (s.Kpad + 31) & ~31;
     const int w_atom = NCH * 64 * 128;
     const int x_bytes = 4 * s.Kpad * 128;
-    unsigned char* s_w = smem;
+    unsigned char* s_w = dynamic_smem_1024();
     unsigned char* s_x = s_w + (k32 / 32) * w_atom;
     float* s_stg = reinterpret_cast<float*>(s_x + stages * x_bytes);
     float** s_rowptr = reinterpret_cast<float**>(s_stg + 2 * TE_STG_FLOATS);        // [2][256]
     float* s_rowbias = reinterpret_cast<float*>(s_rowptr + 2 * 256);                // [2][256]
     uint64_t* w_full = reinterpret_cast<uint64_t*>(s_rowbias + 2 * 256);
-    uint64_t* full = w_full + 1;
-    uint64_t* empty = full + stages;
+    const MbarRing ring(w_full + 1, stages);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&maps.w);
         tma_prefetch_desc(&maps.x);
-        mbar_init(w_full, 1);
-        for (int i = 0; i < stages; ++i) {
-            mbar_init(full + i, 1);
-            mbar_init(empty + i, 8);                   // one arrival per consumer warp
-        }
-        fence_mbar_init();
+        mbar_init(w_full, 1);                          // published to the async proxy by the fence in ring.init
+        ring.init(8);
     }
     __syncthreads();
 
@@ -267,14 +239,12 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
             for (int a = 0; a < k32 / 32; ++a) tma_load_3d(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-                const int st = it % stages, use = it / stages;
-                if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
+                const int st = ring.produce(it, x_bytes);
                 const int f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_FWD_PX;
                 unsigned char* dst = s_x + st * x_bytes;
-                mbar_arrive_expect_tx(full + st, x_bytes);
 #pragma unroll
                 for (int blk = 0; blk < TE_FWD_PX / 32; ++blk)
-                    tma_load_4d(dst + blk * s.Kpad * 128, &maps.x, full + st, p0 + 32 * blk, 0, f % s.frames, f / s.frames);
+                    tma_load_4d(dst + blk * s.Kpad * 128, &maps.x, ring.full + st, p0 + 32 * blk, 0, f % s.frames, f / s.frames);
             }
         }
         return;
@@ -283,17 +253,15 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
     // ===== consumers: warpgroup g owns pixel rows 64g .. 64g + 63 =====
     const int g = warp >> 2;
     const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
-    const int pa = te_pixel(r0), pb = te_pixel(r0 + 8);
+    const int pa = tile_pixel(r0), pb = tile_pixel(r0 + 8);
     const uint32_t w_addr = smem_addr(s_w);
     float* stg = s_stg + g * TE_STG_FLOATS;
     mbar_wait(w_full, 0);
     int it = 0;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-        const int st = it % stages, use = it / stages;
         const int f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_FWD_PX;
         const int b = f / s.frames, tt = f % s.frames;
-        const unsigned char* tile = s_x + st * x_bytes;
-        mbar_wait(full + st, use & 1);
+        const unsigned char* tile = s_x + ring.consume(it) * x_bytes;
         float acc[NCH][32];
 #pragma unroll
         for (int c = 0; c < NCH; ++c)
@@ -304,8 +272,7 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
             te_mma_group<NCH>(acc, tile, s.Kpad, kg, pa, pb, w_addr + kg * w_atom);
 #pragma unroll
         for (int c = 0; c < NCH; ++c) wgmma_fence_operands(acc[c]);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + st);        // this warp's part of the tile has been read
+        ring.release(it);                              // this warp's part of the tile has been read
 
         const int pbase = p0 + 64 * g;
         const int n_valid = s.pixels - pbase;
@@ -358,29 +325,22 @@ template <int NCHK>
 __global__ void __launch_bounds__(TE_DG_THREADS, 1)
 temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ gx, int stages,
                             int tiles_per_frame, int n_tiles) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     const int npad32 = (s.Npad + 31) & ~31;
     const int rows = (s.Npad + 63) & ~63;          // grad tile rows per 32-pixel block
     const int w_atom = NCHK * 64 * 128;
     const int g_bytes = 2 * rows * 128;
-    unsigned char* s_w = smem;
+    unsigned char* s_w = dynamic_smem_1024();
     unsigned char* s_g = s_w + (npad32 / 32) * w_atom;
     float* stg = reinterpret_cast<float*>(s_g + stages * g_bytes);
     uint64_t* w_full = reinterpret_cast<uint64_t*>(stg + TE_STG_FLOATS);
-    uint64_t* full = w_full + 1;
-    uint64_t* empty = full + stages;
+    const MbarRing ring(w_full + 1, stages);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 4 && lane == 0) {
         tma_prefetch_desc(&maps.w);
         for (int q = 0; q < s.n_seg; ++q) tma_prefetch_desc(&maps.g.gy[q]);
-        mbar_init(w_full, 1);
-        for (int i = 0; i < stages; ++i) {
-            mbar_init(full + i, 1);
-            mbar_init(empty + i, 4);
-        }
-        fence_mbar_init();
+        mbar_init(w_full, 1);                          // published to the async proxy by the fence in ring.init
+        ring.init(4);
     }
     __syncthreads();
 
@@ -390,27 +350,23 @@ temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeSh
             for (int a = 0; a < npad32 / 32; ++a) tma_load_3d(s_w + a * w_atom, &maps.w, w_full, 32 * a, 0, 0);
             int it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-                const int st = it % stages, use = it / stages;
-                if (use > 0) mbar_wait(empty + st, (use - 1) & 1);
+                const int st = ring.produce(it, 2 * s.Npad32 * 128);
                 const int f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_BWD_PX;
-                mbar_arrive_expect_tx(full + st, 2 * s.Npad32 * 128);
-                te_load_grad_tile(maps.g, s, s_g + st * g_bytes, rows, full + st, f / s.frames, f % s.frames, p0);
+                te_load_grad_tile(maps.g, s, s_g + st * g_bytes, rows, ring.full + st, f / s.frames, f % s.frames, p0);
             }
         }
         return;
     }
 
     const int r0 = 16 * warp + (lane >> 2);
-    const int pa = te_pixel(r0), pb = te_pixel(r0 + 8);
+    const int pa = tile_pixel(r0), pb = tile_pixel(r0 + 8);
     const uint32_t w_addr = smem_addr(s_w);
     mbar_wait(w_full, 0);
     int it = 0;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-        const int st = it % stages, use = it / stages;
         const int f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_BWD_PX;
         const int b = f / s.frames, tt = f % s.frames;
-        const unsigned char* tile = s_g + st * g_bytes;
-        mbar_wait(full + st, use & 1);
+        const unsigned char* tile = s_g + ring.consume(it) * g_bytes;
         float acc[NCHK][32];
 #pragma unroll
         for (int c = 0; c < NCHK; ++c)
@@ -421,8 +377,7 @@ temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeSh
             te_mma_group<NCHK>(acc, tile, rows, kg, pa, pb, w_addr + kg * w_atom);
 #pragma unroll
         for (int c = 0; c < NCHK; ++c) wgmma_fence_operands(acc[c]);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + st);
+        ring.release(it);
 
         float* base = gx + static_cast<size_t>(b) * s.sb + static_cast<size_t>(tt) * s.st + p0;
 #pragma unroll
@@ -449,7 +404,7 @@ struct TeWgradMaps {
 static long long te_bwd_tiles(int n_frames, int pixels) {
     return static_cast<long long>(n_frames) * ((pixels + TE_BWD_PX - 1) / TE_BWD_PX);
 }
-static int te_wgrad_chunks(int n_frames, int pixels) { return wgrad_chunks(te_bwd_tiles(n_frames, pixels)); }
+static int te_wgrad_chunks(int n_frames, int pixels) { return wgrad_chunks(te_bwd_tiles(n_frames, pixels), WG_MAX_CHUNKS); }
 // partial: (Nrows = round64(Npad)) x (Kx = round64(K + E)) floats per chunk
 static size_t te_partial_floats(const TeShape& s) {
     return static_cast<size_t>(round_up(s.Npad, 64)) * round_up(s.K + s.E, 64);
@@ -466,11 +421,10 @@ template <int NC>
 __global__ void __launch_bounds__(512, 1)
 temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeShape s, const float* __restrict__ extra,
                             float* __restrict__ partial, int stages, int tiles_per_frame, int n_tiles) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    unsigned char* smem = dynamic_smem_1024();
     const int rows = (s.Npad + 63) & ~63, xrows = 64 * NC;
     const int g_bytes = 2 * rows * 128, stage_bytes = g_bytes + 2 * xrows * 128;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
+    const MbarRing ring(reinterpret_cast<uint64_t*>(smem + stages * stage_bytes), stages);
     const int nthreads = blockDim.x;
     const int t0 = static_cast<int>(static_cast<long long>(blockIdx.x) * n_tiles / gridDim.x);
     const int t1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * n_tiles / gridDim.x);
@@ -479,19 +433,18 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
     auto load = [&](int i) {                       // tile t0 + i into stage i % stages
         const int t = t0 + i, f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_BWD_PX;
         const int b = f / s.frames, tt = f % s.frames;
-        unsigned char* dst = smem + (i % stages) * stage_bytes;
-        mbar_arrive_expect_tx(full + i % stages, tx_bytes);
-        te_load_grad_tile(maps.g, s, dst, rows, full + i % stages, b, tt, p0);
+        const int st = ring.arm(i, tx_bytes);
+        unsigned char* dst = smem + st * stage_bytes;
+        te_load_grad_tile(maps.g, s, dst, rows, ring.full + st, b, tt, p0);
 #pragma unroll
         for (int blk = 0; blk < TE_BWD_PX / 32; ++blk)
-            tma_load_4d(dst + g_bytes + blk * xrows * 128, &maps.x, full + i % stages, p0 + 32 * blk, 0, tt, b);
+            tma_load_4d(dst + g_bytes + blk * xrows * 128, &maps.x, ring.full + st, p0 + 32 * blk, 0, tt, b);
     };
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&maps.x);
         for (int q = 0; q < s.n_seg; ++q) tma_prefetch_desc(&maps.g.gy[q]);
-        for (int i = 0; i < stages; ++i) mbar_init(full + i, 1);
-        fence_mbar_init();
+        ring.init(0);
         for (int i = 0; i < stages - 1 && t0 + i < t1; ++i) load(i);
     }
     __syncthreads();
@@ -504,20 +457,18 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
         for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
 
     for (int i = 0; t0 + i < t1; ++i) {
-        te_bar(1, nthreads);                       // every warpgroup is done with tile i - 1: its stage may be refilled
+        named_barrier(1, nthreads);                // every warpgroup is done with tile i - 1: its stage may be refilled
         if (threadIdx.x == 0 && t0 + i + stages - 1 < t1) load(i + stages - 1);
-        const int st = i % stages;
-        mbar_wait(full + st, (i / stages) & 1);
-        unsigned char* tile = smem + st * stage_bytes;
+        unsigned char* tile = smem + ring.consume(i) * stage_bytes;
         if (s.E > 0) {                             // egopose rows K .. K + E - 1 of the input tile (zero past the frame's pixels)
             const int t = t0 + i, f = t / tiles_per_frame, p0 = (t % tiles_per_frame) * TE_BWD_PX;
             for (int idx = threadIdx.x; idx < s.E * TE_BWD_PX; idx += nthreads) {
                 const int j = idx / TE_BWD_PX, px = idx % TE_BWD_PX;
                 const float v = p0 + px < s.pixels ? __ldg(extra + static_cast<size_t>(f) * s.E + j) : 0.f;
-                *reinterpret_cast<uint32_t*>(tile + g_bytes + te_offset(xrows, s.K + j, px)) = to_tf32(v);
+                *reinterpret_cast<uint32_t*>(tile + g_bytes + tile_offset(xrows, s.K + j, px)) = to_tf32(v);
             }
             fence_proxy_async();
-            te_bar(2, nthreads);
+            named_barrier(2, nthreads);
         }
         const uint32_t g_addr = smem_addr(tile) + mb * 64 * 128, x_addr = smem_addr(tile + g_bytes);
         wgmma_fence();
@@ -550,21 +501,18 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
         }
 }
 
-// grad_w (N_out, K + E) = sum of the chunks' partials in ascending chunk order (zeros when there are none)
-__global__ void temporal_entry_wgrad_reduce_kernel(const TeShape s, const float* __restrict__ partial, int n_chunks, float* __restrict__ gw) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int ld = s.K + s.E;
-    if (i >= s.n_out * ld) return;
-    const int on = i / ld, k = i % ld;
-    int o = 0;
-    for (int q = 0; q < s.n_seg; ++q)
-        if (on >= s.nat_off[q] && on < s.nat_off[q + 1]) o = s.seg_off[q] + on - s.nat_off[q];
-    const int xrows = (ld + 63) & ~63;
-    const size_t stride = static_cast<size_t>((s.Npad + 63) & ~63) * xrows;
-    float acc = 0.f;
-    for (int c = 0; c < n_chunks; ++c) acc += partial[c * stride + static_cast<size_t>(o) * xrows + k];
-    gw[i] = acc;
-}
+// grad_w (N_out, K + E) index -> its place in a chunk's partial (padded row o, column k)
+struct TeWgradOffset {
+    TeShape s;
+    __device__ size_t operator()(int i) const {
+        const int ld = s.K + s.E;
+        const int on = i / ld, k = i % ld;
+        int o = 0;
+        for (int q = 0; q < s.n_seg; ++q)
+            if (on >= s.nat_off[q] && on < s.nat_off[q + 1]) o = s.seg_off[q] + on - s.nat_off[q];
+        return static_cast<size_t>(o) * ((ld + 63) & ~63) + k;
+    }
+};
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // host
@@ -673,7 +621,6 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
     const TeShape s = te_shape(d);
     const int n_frames = s.batch * s.frames;
     const int n_chunks = te_wgrad_chunks(n_frames, s.pixels);
-    const int n_red = s.n_out * (s.K + s.E);
     float* partial = static_cast<float*>(workspace);
     if (n_chunks > 0) {
         TeWgradMaps maps;
@@ -700,9 +647,7 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
         }
         FIERY_CUDA_CHECK(cudaGetLastError());
     }
-    temporal_entry_wgrad_reduce_kernel<<<(n_red + 255) / 256, 256, 0, stream>>>(s, partial, n_chunks, gw);
-    FIERY_CUDA_CHECK(cudaGetLastError());
-    return FIERY_OK;
+    return launch_wgrad_reduce(partial, n_chunks, te_partial_floats(s), s.n_out * (s.K + s.E), TeWgradOffset{s}, gw, stream);
 }
 
 }  // namespace fiery

@@ -17,6 +17,33 @@ __device__ __forceinline__ uint32_t to_tf32(float v) {
     return r;
 }
 
+// TF32 register A operand read from a pixel-major tile (depth_layer.cu's fp32 path, temporal_entry.cu): the tile is blocks of 32
+// pixels (128 bytes) x `rows` channel rows, 128-byte swizzle, as TMA writes it; the accumulator rows are the tile's pixels.
+// Accumulator row r (0..127) -> pixel of the tile: rows 64g .. 64g + 63 map to pixels 64g .. 64g + 63, and the 8 rows one fragment
+// load covers are 4 pixels from each half of a 128-byte row, so with the 4 channels of the load they hit 32 different banks.
+__device__ __forceinline__ int tile_pixel(int r) {
+    const int t = r >> 3, q = r & 7;
+    return (t >> 2) * 32 + (q >> 2) * 16 + (t & 3) * 4 + (q & 3);
+}
+// byte offset of (row, pixel) in such a tile
+__device__ __forceinline__ uint32_t tile_offset(int rows, int row, int px) {
+    return (px >> 5) * (rows * 128) + row * 128 + ((((px & 31) >> 2) ^ (row & 7)) << 4) + (px & 3) * 4;
+}
+// a[k] = the A fragment of the k-step over channel rows ch0 + 8k .. ch0 + 8k + 7, for this thread's pixel rows pa = tile_pixel(r0),
+// pb = tile_pixel(r0 + 8).  The fp32 bits go in as they are: the tensor core truncates them to TF32.
+template <int NK>
+__device__ __forceinline__ void load_pixel_frags(uint32_t (&a)[NK][4], const unsigned char* tile, int rows, int ch0, int pa, int pb) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int k = 0; k < NK; ++k) {
+        const int ch = ch0 + 8 * k + (lane & 3);
+        a[k][0] = *reinterpret_cast<const uint32_t*>(tile + tile_offset(rows, ch, pa));
+        a[k][1] = *reinterpret_cast<const uint32_t*>(tile + tile_offset(rows, ch, pb));
+        a[k][2] = *reinterpret_cast<const uint32_t*>(tile + tile_offset(rows, ch + 4, pa));
+        a[k][3] = *reinterpret_cast<const uint32_t*>(tile + tile_offset(rows, ch + 4, pb));
+    }
+}
+
 // Shared-memory matrix descriptor, 128-byte swizzle (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B).  K-major operand: rows
 // of 128 bytes along K, 8-row groups SBO = 1024 bytes apart, LBO unused.  MN-major operand (16-bit types only): 128-byte rows along
 // M/N, one k each; 8 consecutive k = one 1024-byte atom, SBO = stride between k-groups of 8, LBO = stride between 128-byte blocks
