@@ -48,6 +48,15 @@ class TemporalEntryDesc(ctypes.Structure):
     ]
 
 
+class SpatialSumsDesc(ctypes.Structure):
+    """Mirror of ``fiery_spatial_sums_desc_t``."""
+
+    _fields_ = [
+        ("batch", c_int32), ("channels", c_int32), ("frames", c_int32), ("pixels", c_int32),
+        ("stride_b", c_int64), ("stride_c", c_int64), ("stride_t", c_int64),
+    ]
+
+
 class CausalConv3dDesc(ctypes.Structure):
     """Mirror of ``fiery_causal_conv3d_desc_t``."""
 
@@ -103,6 +112,9 @@ SIGNATURES = {
     "fiery_temporal_entry_backward_weight_workspace_bytes": (c_size_t, [POINTER(TemporalEntryDesc)]),
     "fiery_temporal_entry_backward_weight": (c_int32, [POINTER(TemporalEntryDesc), c_void_p, c_void_p, POINTER(c_void_p), c_void_p,
                                                        c_void_p, c_void_p]),
+    "fiery_temporal_aggregation_forward": (c_int32, [POINTER(TemporalEntryDesc), POINTER(c_void_p), c_void_p, c_void_p, c_void_p,
+                                                     c_void_p]),
+    "fiery_spatial_sums": (c_int32, [POINTER(SpatialSumsDesc), c_void_p, c_void_p, c_void_p]),
     "fiery_causal_conv3d_packed_bytes": (c_size_t, [POINTER(CausalConv3dDesc)]),
     "fiery_causal_conv3d_pack_weights": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p]),
     "fiery_causal_conv3d_forward": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -171,10 +183,10 @@ def f32(t: torch.Tensor) -> torch.Tensor:
 # weights' memory alive, so no other tensor can take an address in the cache while its entry exists; a weight's version counter
 # (shared with its views, its aliases and the Parameter) changes with each in-place update, e.g. an optimizer step or a checkpoint
 # load.  One training step of a model with every layer swapped uses one pack per DepthLayer operand dtype, two for FirstConv (the
-# transposed one for the input gradient), three per TemporalBlock (its entry and two causal convolutions) and one per Bottleneck3D:
-# 15 for the four temporal blocks of a 5-frame receptive field.  The bound leaves room for in-between layers (up to four per block
-# there) without a step ever evicting a pack it uses again.
-_PACK_CACHE_SIZE = 32
+# transposed one for the input gradient), four per TemporalBlock (its entry, two causal convolutions and its aggregation) and one per
+# Bottleneck3D: 19 for the four temporal blocks of a 5-frame receptive field.  The bound leaves room for in-between layers (up to four
+# per block there) without a step ever evicting a pack it uses again.
+_PACK_CACHE_SIZE = 40
 _pack_cache: "collections.OrderedDict[tuple, tuple]" = collections.OrderedDict()
 
 

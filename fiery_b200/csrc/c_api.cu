@@ -116,8 +116,9 @@ size_t temporal_entry_packed_bytes(const fiery_temporal_entry_desc_t* d);
 int launch_temporal_entry_pack(const fiery_temporal_entry_desc_t* d, const float* w, float* packed, cudaStream_t stream);
 int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
                                   float* const* out, cudaStream_t stream);
-int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, float* gx,
-                                cudaStream_t stream);
+int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, const float* bias,
+                                float* gx, cudaStream_t stream);
+int launch_spatial_sums(const fiery_spatial_sums_desc_t* d, const float* x, float* sums, cudaStream_t stream);
 size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d);
 int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
                                 float* gw, void* workspace, cudaStream_t stream);
@@ -520,7 +521,34 @@ FIERY_API int fiery_temporal_entry_backward_data(const fiery_temporal_entry_desc
     FIERY_REQUIRE(aligned16(packed) && aligned16(grad_x), "temporal entry: pointers must be 16-byte aligned");
     for (int q = 0; q < desc->n_segments; ++q)
         FIERY_REQUIRE(grad_out[q] && aligned16(grad_out[q]), "temporal entry: grad_out[%d] is NULL or misaligned", q);
-    return launch_temporal_entry_dgrad(desc, grad_out, static_cast<const float*>(packed), grad_x, static_cast<cudaStream_t>(stream));
+    return launch_temporal_entry_dgrad(desc, grad_out, static_cast<const float*>(packed), nullptr, grad_x,
+                                       static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_temporal_aggregation_forward(const fiery_temporal_entry_desc_t* desc, const float* const* paths, const void* packed,
+                                                 const float* bias, float* out, void* stream) {
+    const int rc = check_temporal_entry_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(desc->extra_channels == 0, "temporal aggregation: extra_channels = %d must be 0", desc->extra_channels);
+    if (desc->batch == 0 || desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(paths && packed && out, "temporal aggregation: NULL pointer");
+    FIERY_REQUIRE(aligned16(packed) && aligned16(out), "temporal aggregation: pointers must be 16-byte aligned");
+    for (int q = 0; q < desc->n_segments; ++q)
+        FIERY_REQUIRE(paths[q] && aligned16(paths[q]), "temporal aggregation: paths[%d] is NULL or misaligned", q);
+    return launch_temporal_entry_dgrad(desc, paths, static_cast<const float*>(packed), bias, out, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_spatial_sums(const fiery_spatial_sums_desc_t* desc, const float* x, float* sums, void* stream) {
+    FIERY_REQUIRE(desc, "spatial sums: NULL desc");
+    FIERY_REQUIRE(desc->batch >= 0 && desc->channels >= 0 && desc->frames >= 0,
+                  "spatial sums: batch = %d, channels = %d, frames = %d must be >= 0", desc->batch, desc->channels, desc->frames);
+    FIERY_REQUIRE(desc->pixels >= 1, "spatial sums: pixels X*Y = %d must be >= 1", desc->pixels);
+    FIERY_REQUIRE(desc->stride_b >= 0 && desc->stride_c >= 0 && desc->stride_t >= 0,
+                  "spatial sums: strides (%lld, %lld, %lld) must be >= 0", (long long)desc->stride_b, (long long)desc->stride_c,
+                  (long long)desc->stride_t);
+    if (static_cast<long long>(desc->batch) * desc->channels * desc->frames == 0) return FIERY_OK;
+    FIERY_REQUIRE(x && sums, "spatial sums: NULL pointer");
+    return launch_spatial_sums(desc, x, sums, static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API size_t fiery_temporal_entry_backward_weight_workspace_bytes(const fiery_temporal_entry_desc_t* desc) {

@@ -321,10 +321,11 @@ struct TeDgradMaps {
     CUtensorMap w;                                 // T region: (Npad32, NCHK*64), box (32, NCHK*64), swizzle 128B
 };
 
-template <int NCHK>
-__global__ void __launch_bounds__(TE_DG_THREADS, 1)
-temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ gx, int stages,
-                            int tiles_per_frame, int n_tiles) {
+// BIAS: every output row k of frame f = (b, t) gets bias[f * K + k] added in the epilogue (the temporal aggregation's pooled-vector
+// term); the instantiation without it is the entry's input gradient.
+template <int NCHK, bool BIAS>
+__device__ __forceinline__ void te_dgrad_body(const TeDgradMaps& maps, const TeShape& s, float* __restrict__ gx,
+                                              const float* __restrict__ bias, int stages, int tiles_per_frame, int n_tiles) {
     const int npad32 = (s.Npad + 31) & ~31;
     const int rows = (s.Npad + 63) & ~63;          // grad tile rows per 32-pixel block
     const int w_atom = NCHK * 64 * 128;
@@ -385,12 +386,27 @@ temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeSh
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 if (64 * c + 32 * h >= s.K) continue;
-                te_store_cols(acc[c], h, stg, 1, s.pixels - p0, [&](int col, float&) -> float* {
+                te_store_cols(acc[c], h, stg, 1, s.pixels - p0, [&](int col, float& b_k) -> float* {
                     const int k = 64 * c + 32 * h + col;
+                    if (BIAS && k < s.K) b_k = __ldg(bias + static_cast<size_t>(f) * s.K + k);
                     return k < s.K ? base + static_cast<size_t>(k) * s.sc : nullptr;
                 });
             }
     }
+}
+
+template <int NCHK>
+__global__ void __launch_bounds__(TE_DG_THREADS, 1)
+temporal_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ gx, int stages,
+                            int tiles_per_frame, int n_tiles) {
+    te_dgrad_body<NCHK, false>(maps, s, gx, nullptr, stages, tiles_per_frame, n_tiles);
+}
+
+template <int NCHK>
+__global__ void __launch_bounds__(TE_DG_THREADS, 1)
+temporal_aggregation_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ out,
+                            const float* __restrict__ bias, int stages, int tiles_per_frame, int n_tiles) {
+    te_dgrad_body<NCHK, true>(maps, s, out, bias, stages, tiles_per_frame, n_tiles);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -588,8 +604,10 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
     return FIERY_OK;
 }
 
-int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, float* gx,
-                                cudaStream_t stream) {
+// bias: nullptr (the entry's input gradient) or (batch * frames, K) fp32 added to every pixel of its frame's row k (the temporal
+// aggregation's forward)
+int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, const float* bias,
+                                float* gx, cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const TePack p = te_pack_layout(s);
     TeDgradMaps maps;
@@ -605,12 +623,19 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
     FIERY_REQUIRE(n_tiles < (1ll << 31), "temporal entry: too many pixel tiles");
     unsigned grid = 0;
     if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
-    if (p.nchk == 1) {
+    const int nt = static_cast<int>(n_tiles);
+    if (p.nchk == 1 && bias == nullptr) {
         if ((rc = set_dynamic_smem(temporal_entry_dgrad_kernel<1>, smem)) != FIERY_OK) return rc;
-        temporal_entry_dgrad_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, static_cast<int>(n_tiles));
-    } else {
+        temporal_entry_dgrad_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, nt);
+    } else if (bias == nullptr) {
         if ((rc = set_dynamic_smem(temporal_entry_dgrad_kernel<2>, smem)) != FIERY_OK) return rc;
-        temporal_entry_dgrad_kernel<2><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, static_cast<int>(n_tiles));
+        temporal_entry_dgrad_kernel<2><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, nt);
+    } else if (p.nchk == 1) {
+        if ((rc = set_dynamic_smem(temporal_aggregation_kernel<1>, smem)) != FIERY_OK) return rc;
+        temporal_aggregation_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, bias, stages, tiles_per_frame, nt);
+    } else {
+        if ((rc = set_dynamic_smem(temporal_aggregation_kernel<2>, smem)) != FIERY_OK) return rc;
+        temporal_aggregation_kernel<2><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, bias, stages, tiles_per_frame, nt);
     }
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;

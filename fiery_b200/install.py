@@ -196,6 +196,35 @@ def use_tensor_core_causal_convs(model):
     return model
 
 
+def use_tensor_core_pyramid_pooling(model):
+    """Replace the ``pyramid_pooling`` (fiery/layers/temporal.py:167-215) of every ``TemporalBlock`` or ``TensorCoreTemporalBlock`` in
+    ``model.temporal_model.model`` of a ``Fiery`` instance by ``fiery_b200.temporal.TensorCorePyramidPooling``, which adopts its
+    ``features`` (``state_dict`` keys unchanged) and computes the pool from the input's spatial sums, with no average pool over the map
+    and no bilinear upsampling.  In a ``TensorCoreTemporalBlock`` whose aggregation conv the kernel covers, the aggregation then runs
+    as ``torch.ops.fiery_b200.temporal_aggregation``: no concat and no broadcast over the map.  Works before or after
+    ``use_tensor_core_temporal_model`` and ``use_tensor_core_causal_convs``.  Returns the model; a second call does nothing, and a
+    pooling that does not cover the whole map (several pool sizes, a kernel other than (2, X, Y)) is left alone with one warning."""
+    from .temporal import TensorCorePyramidPooling, pooling_reason
+    blocks = getattr(model.temporal_model, "model", None)
+    if blocks is None:
+        return model
+    skipped = []
+    for i, block in enumerate(blocks):
+        if type(block).__name__ not in ("TemporalBlock", "TensorCoreTemporalBlock") or not getattr(block, "use_pyramid_pooling", False):
+            continue
+        if isinstance(block.pyramid_pooling, TensorCorePyramidPooling):
+            continue
+        reason = pooling_reason(block.pyramid_pooling)
+        if reason is None:
+            block.pyramid_pooling = TensorCorePyramidPooling(block.pyramid_pooling)
+        else:
+            skipped.append(f"block {i}: {reason}")
+    if skipped:
+        _warn_once(("pyramid", tuple(skipped)), "fiery_b200: pyramid pooling(s) not covered by the spatial-sums kernel, left as is: "
+                   + "; ".join(skipped))
+    return model
+
+
 def uninstall():
     if not _saved:
         return

@@ -234,4 +234,87 @@ temporal_entry.register_autograd(_temporal_entry_backward, setup_context=_tempor
 torch.library.register_autocast("fiery_b200::temporal_entry", "cuda", torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# The temporal block's pyramid pooling and aggregation (fiery/layers/temporal.py:167-215, 268-276): ``spatial_sums`` (the pooling's
+# spatial means; csrc/spatial_sums.cu) and ``temporal_aggregation`` (the aggregation conv of the paths and the broadcast pooled vector,
+# without the concat or the broadcast; the entry's kernels in swapped roles).  Autocast: both run in fp32.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::spatial_sums", mutates_args=(), device_types="cuda")
+def spatial_sums(x: torch.Tensor) -> torch.Tensor:
+    """x (b, C, s, X, Y) -> (b, C, s) fp32 sums over each pixel plane; the order depends on X*Y only (bit-identical for a plane
+    whatever its strides or neighbours).  Its gradient is the broadcast of the output gradient over the map."""
+    from .temporal import spatial_sums as sums
+    return sums(x)
+
+
+@spatial_sums.register_fake
+def _(x):
+    return x.new_empty(tuple(x.shape[:3]), dtype=torch.float32)
+
+
+def _spatial_sums_setup_context(ctx, inputs, output):
+    (x,) = inputs
+    ctx.x_shape, ctx.x_dtype = tuple(x.shape), x.dtype
+
+
+def _spatial_sums_backward(ctx, grad):
+    return grad[..., None, None].to(ctx.x_dtype).expand(ctx.x_shape)
+
+
+spatial_sums.register_autograd(_spatial_sums_backward, setup_context=_spatial_sums_setup_context)
+torch.library.register_autocast("fiery_b200::spatial_sums", "cuda", torch.float32)
+
+
+@torch.library.custom_op("fiery_b200::temporal_aggregation", mutates_args=(), device_types="cuda")
+def temporal_aggregation(paths: List[torch.Tensor], weight: torch.Tensor, pooled: torch.Tensor) -> torch.Tensor:
+    """paths: 1..4 tensors (b, C_q, s, X, Y); weight (N, sum C_q + R, 1, 1, 1), the aggregation's bias-free 1x1x1 Conv3d; pooled
+    (b, R, s), constant over the map.  Returns the contiguous (b, N, s, X, Y) fp32 ``conv3d(cat([*paths, pooled broadcast], 1),
+    weight)`` without building the concat or the broadcast.  The weight's pack is made at most once per weight version."""
+    from .temporal import aggregation_forward
+    return aggregation_forward(paths, weight, pooled)
+
+
+@temporal_aggregation.register_fake
+def _(paths, weight, pooled):
+    b, _, s, h, w = paths[0].shape
+    return paths[0].new_empty((b, weight.shape[0], s, h, w), dtype=torch.float32)
+
+
+@torch.library.custom_op("fiery_b200::temporal_aggregation_backward", mutates_args=(), device_types="cuda")
+def temporal_aggregation_backward(grad: torch.Tensor, paths: List[torch.Tensor], weight: torch.Tensor, pooled: torch.Tensor,
+                                  need_paths: bool, need_weight: bool,
+                                  need_pooled: bool) -> Tuple[List[torch.Tensor], torch.Tensor, torch.Tensor]:
+    """(grad_paths, grad_weight, grad_pooled) of ``temporal_aggregation``, each in its input's shape and dtype (the paths' gradients
+    contiguous); a gradient that is not asked for is not computed and comes back empty.  The weight gradient is bit-reproducible."""
+    from .temporal import aggregation_backward
+    gp, gw, gv = aggregation_backward(grad, paths, weight, pooled, need_paths, need_weight, need_pooled)
+    return ([_cast_back(g, p) for g, p in zip(gp, paths)] if gp is not None else [p.new_empty((0,)) for p in paths],
+            _cast_back(gw, weight), _cast_back(gv, pooled))
+
+
+@temporal_aggregation_backward.register_fake
+def _(grad, paths, weight, pooled, need_paths, need_weight, need_pooled):
+    return ([p.new_empty(p.shape) if need_paths else p.new_empty((0,)) for p in paths],
+            weight.new_empty(weight.shape) if need_weight else weight.new_empty((0,)),
+            pooled.new_empty(pooled.shape) if need_pooled else pooled.new_empty((0,)))
+
+
+def _temporal_aggregation_setup_context(ctx, inputs, output):
+    paths, weight, pooled = inputs
+    ctx.save_for_backward(weight, pooled, *paths)
+
+
+def _temporal_aggregation_backward(ctx, grad):
+    weight, pooled, *paths = ctx.saved_tensors
+    need_p, need_w, need_v = any(bool(n) for n in ctx.needs_input_grad[0]), bool(ctx.needs_input_grad[1]), bool(ctx.needs_input_grad[2])
+    if not (need_p or need_w or need_v):
+        return [None] * len(paths), None, None
+    gp, gw, gv = torch.ops.fiery_b200.temporal_aggregation_backward(grad, paths, weight, pooled, need_p, need_w, need_v)
+    return ([g if n else None for g, n in zip(gp, ctx.needs_input_grad[0])], gw if need_w else None, gv if need_v else None)
+
+
+temporal_aggregation.register_autograd(_temporal_aggregation_backward, setup_context=_temporal_aggregation_setup_context)
+torch.library.register_autocast("fiery_b200::temporal_aggregation", "cuda", torch.float32)
+
+
 from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

@@ -15,6 +15,11 @@ unchanged) and replaces only those four convolutions; ``install.use_tensor_core_
 are constant over the map, so instead of concatenating them to the BEV (a 70-channel copy) the first block's GEMM takes the 64-channel
 BEV and the egopose enters as a per-(frame, output channel) bias; its pyramid pooling is computed from the BEV's spatial means and the
 egopose itself.  No CPU path.
+
+``TensorCorePyramidPooling`` (swapped in by ``install.use_tensor_core_pyramid_pooling``) computes the block's pyramid pooling from the
+input's spatial sums (``torch.ops.fiery_b200.spatial_sums``, csrc/spatial_sums.cu).  With it, a ``TensorCoreTemporalBlock`` runs its
+aggregation conv as ``torch.ops.fiery_b200.temporal_aggregation``: the entry's input-gradient GEMM in swapped roles with the pooled
+vector as a per-(frame, output channel) bias, so neither the concat nor the broadcast over the map is built.
 """
 from __future__ import annotations
 
@@ -31,6 +36,7 @@ from ._lib import _require_cuda, f32
 
 MAX_IN_CHANNELS, MAX_OUT_CHANNELS, MAX_EXTRA_CHANNELS = 128, 256, 8
 _warned_pixels = set()
+_warned = set()
 
 
 def _round8(n: int) -> int:
@@ -182,6 +188,109 @@ def entry_backward_weight(grads: Sequence[torch.Tensor], x: torch.Tensor, weight
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
+# spatial sums and the temporal aggregation (csrc/spatial_sums.cu; csrc/temporal_entry.cu in swapped roles)
+# ------------------------------------------------------------------------------------------------------------------------------
+def spatial_sums(x: torch.Tensor) -> torch.Tensor:
+    """x (b, C, s, X, Y) any float dtype -> (b, C, s) fp32 sums over each pixel plane, in a summation order that depends on X*Y only.
+    Read as it lies when x is fp32 with contiguous pixel planes (any b / C / s strides), else from a contiguous fp32 copy."""
+    _require_cuda(x, "x")
+    b, c, s, h, w = x.shape
+    planes_contiguous = (x.stride(4) == 1 or w == 1) and (x.stride(3) == w or h == 1)
+    xs = x if x.dtype == torch.float32 and planes_contiguous else f32(x)
+    out = torch.empty((b, c, s), dtype=torch.float32, device=x.device)
+    d = _lib.SpatialSumsDesc()
+    d.batch, d.channels, d.frames, d.pixels = b, c, s, h * w
+    d.stride_b, d.stride_c, d.stride_t = xs.stride(0), xs.stride(1), xs.stride(2)
+    _lib.call("fiery_spatial_sums", x.device, d, xs.data_ptr(), out.data_ptr())
+    return out
+
+
+def aggregation_reason(n_out: int, path_channels: Sequence[int], pixels: Optional[int] = None) -> Optional[str]:
+    """None if the aggregation kernel takes these shapes, else the reason: the entry's input gradient in swapped roles, so N (the
+    aggregation's output channels) has the entry's input limit and the paths its output limits."""
+    if not 1 <= n_out <= MAX_IN_CHANNELS:
+        return f"{n_out} aggregation output channels (the kernel takes 1..{MAX_IN_CHANNELS})"
+    return unsupported_reason(n_out, path_channels, 0, pixels)
+
+
+def _aggregation_desc(shape, path_channels: Sequence[int]) -> _lib.TemporalEntryDesc:
+    """the entry descriptor in swapped roles: K = N, segments = the paths, strides of the contiguous (b, N, s, X, Y) output (or input)"""
+    b, n, s, h, w = shape
+    return _desc(torch.empty((b, n, s, h, w), device="meta"), path_channels, 0)
+
+
+def pack_aggregation(weight: torch.Tensor, path_channels: Tuple[int, ...]) -> torch.Tensor:
+    """(N, sum C_q + R, 1, 1, 1) aggregation weight -> the entry pack of its path columns, transposed: (sum C_q, N)."""
+    _require_cuda(weight, "weight")
+    n = int(weight.shape[0])
+    wt = weight.detach().float().reshape(n, -1)[:, :sum(path_channels)].t().contiguous()
+    return pack_weights([t[..., None, None, None] for t in wt.split(list(path_channels), 0)], n)
+
+
+def _pooled_columns(weight: torch.Tensor, n_paths: int) -> torch.Tensor:
+    n = int(weight.shape[0])
+    return weight.detach().float().reshape(n, -1)[:, n_paths:]
+
+
+def aggregation_forward(paths: Sequence[torch.Tensor], weight: torch.Tensor, pooled: torch.Tensor) -> torch.Tensor:
+    """The aggregation conv of ``cat([*paths, pooled broadcast over the map], 1)`` without the concat: paths (b, C_q, s, X, Y), weight
+    (N, sum C_q + R, 1, 1, 1), pooled (b, R, s).  Returns the contiguous (b, N, s, X, Y) fp32 output; the pooled columns enter as the
+    per-(frame, output channel) bias W_P pooled, computed in fp32."""
+    _require_cuda(paths[0], "paths")
+    ps = [f32(p) for p in paths]
+    seg = tuple(int(p.shape[1]) for p in ps)
+    b, _, s, h, w = ps[0].shape
+    n = int(weight.shape[0])
+    if int(weight.shape[1]) != sum(seg) + pooled.shape[1] or tuple(pooled.shape) != (b, int(weight.shape[1]) - sum(seg), s):
+        raise ValueError(f"temporal aggregation: paths {[tuple(p.shape) for p in ps]}, pooled {tuple(pooled.shape)} and weight "
+                         f"{tuple(weight.shape)} do not match")
+    reason = aggregation_reason(n, seg, h * w)
+    if reason is not None:
+        raise _lib.FieryError(f"temporal aggregation: {reason}")
+    # bias[b, t, o] = sum_r W_P[o, r] pooled[b, r, t]: elementwise products and a sum, fp32 whatever the matmul precision setting
+    wp = _pooled_columns(weight, sum(seg))
+    bias = (f32(pooled).permute(0, 2, 1)[:, :, None, :] * wp).sum(-1).contiguous() if wp.shape[1] else None
+    out = torch.empty((b, n, s, h, w), dtype=torch.float32, device=ps[0].device)
+    packed = _lib.packed(pack_aggregation, weight, seg)
+    _lib.call("fiery_temporal_aggregation_forward", out.device, _aggregation_desc(out.shape, seg), _ptrs(ps), packed.data_ptr(),
+              bias.data_ptr() if bias is not None else 0, out.data_ptr())
+    return out
+
+
+def aggregation_backward(grad: torch.Tensor, paths: Sequence[torch.Tensor], weight: torch.Tensor, pooled: torch.Tensor,
+                         need_paths: bool, need_weight: bool, need_pooled: bool):
+    """(grad_paths, grad_weight, grad_pooled) of ``aggregation_forward``, fp32, None where not asked for.  grad_paths = A_q^T grad
+    (the entry's forward with x = grad), the path columns of grad_weight = sum grad paths^T (the entry's weight gradient,
+    bit-reproducible), and the pooled terms from G = the spatial sums of grad: grad_W_P = sum_{b,t} G pooled^T, grad_pooled = W_P^T G."""
+    lib = _lib.load()
+    g = f32(grad)
+    seg = tuple(int(p.shape[1]) for p in paths)
+    n, c = int(weight.shape[0]), sum(seg)
+    d = _aggregation_desc(g.shape, seg)
+    grad_paths = grad_weight = grad_pooled = None
+    if need_paths:
+        b, _, s, h, w = g.shape
+        grad_paths = [torch.empty((b, cq, s, h, w), dtype=torch.float32, device=g.device) for cq in seg]
+        packed = _lib.packed(pack_aggregation, weight, seg)
+        _lib.call("fiery_temporal_entry_forward", g.device, d, g.data_ptr(), 0, packed.data_ptr(), _ptrs(grad_paths))
+    if need_weight or need_pooled:
+        sums = spatial_sums(g)                                      # (b, N, s)
+        wp = _pooled_columns(weight, c)
+        v = f32(pooled)
+        if need_pooled:
+            grad_pooled = (wp[None, :, :, None] * sums[:, :, None, :]).sum(1)
+        if need_weight:
+            ps = [f32(p) for p in paths]
+            ws = torch.empty(max(int(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d)), 16), dtype=torch.uint8,
+                             device=g.device)
+            gw = torch.empty((c, n), dtype=torch.float32, device=g.device)
+            _lib.call("fiery_temporal_entry_backward_weight", g.device, d, g.data_ptr(), 0, _ptrs(ps), gw.data_ptr(), ws.data_ptr())
+            grad_wp = (sums[:, :, None, :] * v[:, None, :, :]).sum((0, 3))
+            grad_weight = torch.cat([gw.t(), grad_wp], 1).reshape(weight.shape)
+    return grad_paths, grad_weight, grad_pooled
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
 # module
 # ------------------------------------------------------------------------------------------------------------------------------
 def _is_1x1x1(conv) -> bool:
@@ -243,21 +352,41 @@ class TensorCoreTemporalBlock(nn.Module):
         convs = [p[0][0].conv, p[1][0].conv, p[2].conv]
         return convs + [self.projection[0]] if self.projection is not None else convs
 
-    def _tail(self, x: torch.Tensor, ys: Sequence[torch.Tensor], pooled: Optional[torch.Tensor]) -> torch.Tensor:
+    def _tail(self, x: torch.Tensor, ys: Sequence[torch.Tensor], pooled: Optional[torch.Tensor],
+              vector: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything after the four convolutions (temporal.py:268-281); ``x`` is the block input the skip adds when there is no
-        projection."""
+        projection.  ``pooled``: the pyramid pooling's broadcast, concatenated to the paths; ``vector``: instead, its (b, R, s) pooled
+        vector, which ``temporal_aggregation`` takes without a concat."""
         p = self.convolution_paths
         paths = []
         for i in range(3):
             entry = p[i][0] if i < 2 else p[i]
             y = entry.activation(entry.norm(ys[i]))
             paths.append(p[i][1](y) if i < 2 else y)
-        x_residual = torch.cat(paths, dim=1)
-        if pooled is not None:
-            x_residual = torch.cat([x_residual, pooled], dim=1)
-        x_residual = self.aggregation(x_residual)
+        if vector is not None:
+            agg = self.aggregation[0]
+            x_residual = agg.activation(agg.norm(torch.ops.fiery_b200.temporal_aggregation(paths, agg.conv.weight, vector)))
+        else:
+            x_residual = torch.cat(paths, dim=1)
+            if pooled is not None:
+                x_residual = torch.cat([x_residual, pooled], dim=1)
+            x_residual = self.aggregation(x_residual)
         skip = self.projection[1](ys[3]) if self.projection is not None else x
         return skip + x_residual
+
+    def _folds_pooling(self, h: int, w: int) -> bool:
+        """The pyramid pooling is the swapped module, its kernel covers this map and the aggregation kernel takes it: the block runs
+        the pooled vector through ``temporal_aggregation``.  A covered aggregation on an X*Y the kernel does not take warns once."""
+        pp = getattr(self, "pyramid_pooling", None)
+        if not (self.use_pyramid_pooling and isinstance(pp, TensorCorePyramidPooling) and pp.covers(h, w)):
+            return False
+        if aggregation_block_reason(self) is not None:
+            return False
+        if (h * w) % 4:
+            _warn_once(("aggregation", h * w), f"fiery_b200: TemporalBlock aggregation on X*Y = {h * w} pixels is not covered by the "
+                       "tensor-core kernel (it needs a multiple of 4); it runs as the reference's concat and Conv3d")
+            return False
+        return True
 
     def forward(self, *inputs):
         (x,) = inputs
@@ -273,6 +402,8 @@ class TensorCoreTemporalBlock(nn.Module):
             ys = [c(x) for c in convs]
         else:
             ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in convs], None)
+        if self._folds_pooling(x.shape[3], x.shape[4]):
+            return self._tail(x, ys, None, self.pyramid_pooling.vector(spatial_means(x)))
         pooled = self.pyramid_pooling(x) if self.use_pyramid_pooling else None
         return self._tail(x, ys, pooled)
 
@@ -283,7 +414,13 @@ class TensorCoreTemporalBlock(nn.Module):
             raise ValueError("the folded form needs a block with a projection: the skip would add the concatenated input")
         ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in self._entry_convs()], extra)
         pooled = None
-        if self.use_pyramid_pooling:
+        h, w = x.shape[3], x.shape[4]
+        if self.use_pyramid_pooling and isinstance(self.pyramid_pooling, TensorCorePyramidPooling) and self.pyramid_pooling.covers(h, w):
+            vector = self.pyramid_pooling.vector(torch.cat([spatial_means(x), extra.float().permute(0, 2, 1)], dim=1))
+            if self._folds_pooling(h, w):
+                return self._tail(x, ys, None, vector)
+            pooled = vector[..., None, None].expand(*vector.shape, h, w)
+        elif self.use_pyramid_pooling:
             means = torch.cat([x.float().mean(dim=(3, 4)), extra.float().permute(0, 2, 1)], dim=1)
             pooled = _pyramid_from_means(self.pyramid_pooling, means, x.shape[3], x.shape[4])
         return self._tail(x, ys, pooled)
@@ -303,6 +440,101 @@ def _pyramid_from_means(pp, means: torch.Tensor, h: int, w: int) -> torch.Tensor
         y = f.conv_bn_relu(pooled)[:, :, :-1]
         out.append(y.expand(b, y.shape[1], s, h, w))
     return torch.cat(out, 1)
+
+
+def _warn_once(key, msg: str) -> None:
+    if key not in _warned:
+        _warned.add(key)
+        warnings.warn(msg, RuntimeWarning, stacklevel=3)
+
+
+def spatial_means(x: torch.Tensor) -> torch.Tensor:
+    """(b, C, s, X, Y) -> (b, C, s) fp32 means over each pixel plane (``torch.ops.fiery_b200.spatial_sums`` / X*Y)."""
+    return torch.ops.fiery_b200.spatial_sums(x) / (x.shape[3] * x.shape[4])
+
+
+def pooling_reason(pp) -> Optional[str]:
+    """None if ``pp`` (a reference PyramidSpatioTemporalPooling) is one pool of the reference's (2, X, Y) window -- 2 frames, one
+    frame of padding in front that is not counted, stride (1, X, Y) -- that ``TensorCorePyramidPooling`` computes from spatial means,
+    else the reason.  Whether X x Y covers the map is checked at call time."""
+    feats = getattr(pp, "features", None)
+    if feats is None:
+        return f"{type(pp).__name__} does not have the PyramidSpatioTemporalPooling structure"
+    if len(feats) != 1:
+        return f"{len(feats)} pool sizes (the swap covers one pool over the whole map)"
+    ap = getattr(feats[0], "avgpool", None)
+    if not isinstance(ap, nn.AvgPool3d) or not hasattr(feats[0], "conv_bn_relu"):
+        return f"{feats[0]} is not an AvgPool3d followed by conv_bn_relu"
+    k = tuple(ap.kernel_size) if isinstance(ap.kernel_size, (tuple, list)) else (ap.kernel_size,) * 3
+    stride = tuple(ap.stride) if isinstance(ap.stride, (tuple, list)) else (ap.stride,) * 3
+    padding = tuple(ap.padding) if isinstance(ap.padding, (tuple, list)) else (ap.padding,) * 3
+    if (k[0] != 2 or stride != (1, k[1], k[2]) or padding != (1, 0, 0) or ap.count_include_pad or ap.ceil_mode
+            or ap.divisor_override is not None):
+        return f"pool {ap} is not the (2, X, Y) window with stride (1, X, Y) and one uncounted frame of padding"
+    return None
+
+
+def aggregation_block_reason(block) -> Optional[str]:
+    """None if ``block``'s aggregation conv (bias-free 1x1x1 over the three paths and the pooled channels) is covered by the
+    aggregation kernel, else the reason.  X*Y is checked at call time."""
+    try:
+        agg = block.aggregation[0]
+        conv, _, _ = agg.conv, agg.norm, agg.activation
+        seg = [int(block.half_channels)] * len(block.convolution_paths)
+    except (AttributeError, IndexError, TypeError):
+        return f"{type(block).__name__} does not have the TemporalBlock aggregation structure"
+    if not _is_1x1x1(conv):
+        return f"aggregation {conv} is not a bias-free 1x1x1 Conv3d"
+    if conv.in_channels <= sum(seg):
+        return f"aggregation takes {conv.in_channels} channels: no pooled channels after the paths' {sum(seg)}"
+    return aggregation_reason(conv.out_channels, seg)
+
+
+class TensorCorePyramidPooling(nn.Module):
+    """Drop-in for a reference ``PyramidSpatioTemporalPooling`` with one pool over the whole map (the one ``TemporalModel`` builds,
+    fiery/models/temporal_model.py:23).  It holds the reference module's ``features`` (``state_dict`` keys unchanged) and computes the
+    pool from the input's spatial means (``torch.ops.fiery_b200.spatial_sums``): the 2-frame window over the means, then the
+    reference's own ``conv_bn_relu`` on (b, C, s + 1, 1, 1), the padded last frame dropped after BN.  ``forward`` returns the
+    broadcast over the map as an expanded (stride-0) view; the bilinear upsampling of a 1x1 map it replaces is that broadcast, and
+    its adjoint a spatial sum.  Inside a ``TensorCoreTemporalBlock`` the block takes ``vector`` instead and never builds the broadcast.
+    A map its pool does not cover runs the reference's computation, with one warning."""
+
+    def __init__(self, pp):
+        super().__init__()
+        self.features = pp.features
+
+    @classmethod
+    def from_module(cls, pp) -> "TensorCorePyramidPooling":
+        reason = pooling_reason(pp)
+        if reason is not None:
+            raise ValueError(f"PyramidSpatioTemporalPooling not covered by the spatial-sums pooling: {reason}")
+        return cls(pp)
+
+    def covers(self, h: int, w: int) -> bool:
+        k = self.features[0].avgpool.kernel_size
+        return tuple(k)[1:] == (h, w) if isinstance(k, (tuple, list)) else (k, k) == (h, w)
+
+    def vector(self, means: torch.Tensor) -> torch.Tensor:
+        """(b, C, s) spatial means -> the (b, R, s) pooled vector.  The window averages frames t - 1 and t, and frame 0 alone (the pad
+        is not counted); the reference's extra last step (frame s - 1 alone) goes through BN with the others and is then dropped."""
+        window = torch.cat([means[..., :1], (means[..., :-1] + means[..., 1:]) / 2, means[..., -1:]], dim=2)
+        return self.features[0].conv_bn_relu(window[..., None, None])[:, :, :-1, 0, 0]
+
+    def forward(self, *inputs):
+        (x,) = inputs
+        b, _, s, h, w = x.shape
+        if not self.covers(h, w):
+            _warn_once(("pooling", h, w), f"fiery_b200: pyramid pooling {tuple(self.features[0].avgpool.kernel_size)} does not cover "
+                       f"the {h}x{w} map; it runs as the reference's average pool and bilinear upsampling")
+            out = []
+            for f in self.features:
+                y = f(x)[:, :, :-1].contiguous()
+                c = y.shape[1]
+                y = F.interpolate(y.reshape(b * s, c, *y.shape[-2:]), (h, w), mode="bilinear", align_corners=False)
+                out.append(y.reshape(b, c, s, h, w))
+            return torch.cat(out, 1)
+        v = self.vector(spatial_means(x))
+        return v[..., None, None].expand(*v.shape, h, w)
 
 
 def temporal_model_forward(temporal_model, bev: torch.Tensor, future_egomotion: torch.Tensor) -> torch.Tensor:

@@ -352,6 +352,44 @@ FIERY_API int fiery_temporal_entry_backward_weight(const fiery_temporal_entry_de
                                                    const float* const* grad_out, float* grad_w, void* workspace, void* stream);
 
 /*
+ * The temporal block's aggregation (TemporalBlock, fiery/layers/temporal.py:268-276) without the concat: a 1x1x1 convolution of
+ * cat([path_0, .., path_{n-1}, pooled broadcast over the map], channel) is sum_q A_q path_q plus, per frame, the pooled columns' product
+ * W_P v, a per-(frame, output channel) bias.  The sum is the entry's backward_data GEMM with the roles swapped:
+ *   desc.in_channels = N, the aggregation's output channels; desc.seg_channels[q] = C_q, path q's channels; desc.extra_channels = 0;
+ *   desc.in_stride_b / _t / _c: the strides of out (out[b * in_stride_b + t * in_stride_t + n * in_stride_c + p]);
+ *   packed: fiery_temporal_entry_pack_weights of the stacked (sum C_q, N) matrix [A_0^T; ..; A_{n-1}^T].
+ * paths[q]: (batch, C_q, frames, X, Y) fp32, contiguous; bias: NULL or (batch * frames, N) fp32, contiguous, row b * frames + t.
+ *   out[b, n, t, p] = sum_q sum_c A_q[n, c] * paths[q][b, c, t, p] + bias[b * frames + t, n], fully overwritten.
+ * wgmma, TF32 operands (the pack rounded to nearest, the paths truncated by the tensor core), fp32 accumulation; the bias is added in
+ * fp32.  Limits: those of fiery_temporal_entry_desc_t (N <= 128, sum of round8(C_q) <= 256, at most 4 paths, pixels % 4 == 0, strides
+ * multiples of 4 elements, pointers 16-byte aligned), and extra_channels == 0.  No workspace; batch * frames == 0 is a no-op.
+ * Its backward is the entry's forward (path gradients: x = grad_out with K = N, the same pack) and backward_weight (x = grad_out,
+ * grad_out[q] = paths[q]: the (sum C_q, N) transposed weight gradient), plus fiery_spatial_sums of grad_out for the bias.
+ */
+FIERY_API int fiery_temporal_aggregation_forward(const fiery_temporal_entry_desc_t* desc, const float* const* paths, const void* packed,
+                                                 const float* bias, float* out, void* stream);
+
+/*
+ * Per-plane spatial sums: sums[(b * channels + c) * frames + t] = sum over p < pixels of x[b * stride_b + c * stride_c + t * stride_t + p]
+ * for a fp32 tensor (batch, channels, frames, X, Y) whose pixel planes are contiguous (pixels = X*Y) and whose other strides are
+ * arbitrary (the permuted (b, s, C, X, Y) concat, a contiguous NCDHW tensor, a channel slice).  sums: batch * channels * frames fp32,
+ * fully overwritten.  Offsets in 64 bits.  Limits: batch, channels, frames >= 0 (a zero is a no-op); pixels >= 1; strides >= 0.  No
+ * workspace, no alignment requirement.  Summation order: the plane is cut into 4-pixel chunks; thread i of 256 adds chunks i, i + 256,
+ * ... in ascending order into one accumulator per chunk lane, its total is (lane 0 + lane 1) + (lane 2 + lane 3), the 32 threads of a
+ * warp reduce by an xor butterfly (16, 8, 4, 2, 1) and the 8 warp sums are added in ascending order.  The order depends on pixels only:
+ * a plane's sum is bit-identical whatever its strides or its neighbours; no atomics, graph-capturable.
+ */
+typedef struct {
+    int32_t batch;
+    int32_t channels;
+    int32_t frames;
+    int32_t pixels;               /* X*Y */
+    int64_t stride_b, stride_c, stride_t;   /* elements */
+} fiery_spatial_sums_desc_t;
+
+FIERY_API int fiery_spatial_sums(const fiery_spatial_sums_desc_t* desc, const float* x, float* sums, void* stream);
+
+/*
  * The temporal model's causal convolution (CausalConv3d, fiery/layers/temporal.py:65-85) without its BatchNorm and ReLU: a zero pad of
  * kt - 1 frames in front and one pixel around the map, then a bias-free Conv3d with kernel (kt, 3, 3), stride 1, dilation 1:
  *   y[b, o, t, p] = sum_{i, tau, dy, dx} W[o, i, tau, dy, dx] * x[b, i, t + tau - (kt - 1), p + (dy - 1, dx - 1)]
