@@ -1,10 +1,12 @@
-"""Cases and references shared by tests/test_temporal_cases_cpu.py and tests/test_temporal_envelope_gpu.py: the shapes that walk the
-causal convolution's (csrc/causal_conv.cu) and the temporal entry's (csrc/temporal_entry.cu) accepted range, the host rules those
-shapes are chosen by (kernel instantiation, tile and chunk counts, workspace size), guarded and poisoned buffers, TF32 rounding on bit
-patterns, and weights / inputs with a single 1.0 per channel whose expected results are made by indexing alone.  Importable without
-a GPU: tensors are created on the device the caller names."""
+"""Cases and references shared by tests/test_temporal_cases_cpu.py, tests/test_temporal_envelope_gpu.py and
+tests/test_temporal_tail_envelope_gpu.py: the shapes that walk the causal convolution's (csrc/causal_conv.cu), the temporal entry's and
+the temporal aggregation's (csrc/temporal_entry.cu) accepted range, the host rules those shapes are chosen by (kernel instantiation,
+ring depth, tile and chunk counts, workspace size), the spatial sums' summation order (csrc/spatial_sums.cu), guarded and poisoned
+buffers, TF32 rounding on bit patterns, and weights / inputs with a single 1.0 per channel whose expected results are made by indexing
+alone.  Importable without a GPU: tensors are created on the device the caller names."""
 import math
 
+import numpy as np
 import torch
 
 SENTINEL = -1.0e30
@@ -115,6 +117,110 @@ def entry_wgrad_tiles(b, s, pixels):
 def entry_workspace_bytes(b, s, pixels, K, segs, E):
     r64 = lambda v: (v + 63) // 64 * 64
     return wgrad_chunks(entry_wgrad_tiles(b, s, pixels)) * r64(sum(round8(c) for c in segs)) * r64(K + E) * 4
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# temporal aggregation: launch rules and case list.  A case is (N, path channels, R, (X, Y), batch, frames): N output channels, the
+# paths' channel counts, R pooled channels
+# ------------------------------------------------------------------------------------------------------------------------------
+TE_SMEM_MAX = 232448                               # sm_90 opt-in shared memory per block
+TE_SMEM_SLACK = 1024 + 256                         # alignment + barriers
+TE_STG_BYTES = 32 * 66 * 4                         # one staging tile: 32 channels x 64 pixels at a 66-float pitch
+TE_ROW_TABLE_BYTES = 2 * 256 * (8 + 4)             # the forward's per-warpgroup row table
+
+
+def _round_up(v, m):
+    return (v + m - 1) // m * m
+
+
+def te_stages(fixed_bytes, stage_bytes):
+    """ring depth: as many stages as fit next to the fixed shared memory, at most 4"""
+    return min((TE_SMEM_MAX - TE_SMEM_SLACK - fixed_bytes) // stage_bytes, 4)
+
+
+def aggregation_launches(n, paths, r):
+    """The kernels one aggregation case launches, by csrc/temporal_entry.cu's host rules with the roles swapped (K = N, the paths as
+    the segments, Npad = sum of round8(C_q)):
+      forward      ("aggregation", NCHK, stages): temporal_aggregation_kernel<NCHK>, NCHK = ceil(round32(N) / 64); with R = 0 there
+                   is no bias and it is ("dgrad", NCHK, stages), the entry's temporal_entry_dgrad_kernel<NCHK>;
+      grad_paths   ("forward", NCH, stages): temporal_entry_fwd_kernel<NCH>, NCH = round64(Npad) / 64;
+      grad_weight  ("wgrad", nc, threads, stages): temporal_entry_wgrad_kernel<nc>, nc = round64(N) / 64, one warpgroup per 64 rows.
+    stages: what te_stages leaves room for next to each kernel's fixed shared memory (the resident weight pack, staging)."""
+    kpad, npad = _round_up(n, 32), sum(round8(c) for c in paths)
+    npad32, rows = _round_up(npad, 32), _round_up(npad, 64)
+    nchk, nch, nc = (kpad + 63) // 64, rows // 64, _round_up(n, 64) // 64
+    dgrad = ("aggregation" if r else "dgrad", nchk, te_stages(nchk * 64 * npad32 * 4 + TE_STG_BYTES, 2 * rows * 128))
+    fwd = ("forward", nch, te_stages(nch * 64 * kpad * 4 + 2 * TE_STG_BYTES + TE_ROW_TABLE_BYTES, 4 * kpad * 128))
+    wgrad = ("wgrad", nc, 2 * rows, te_stages(64, 2 * (rows + 64 * nc) * 128))
+    return dgrad, fwd, wgrad
+
+
+def aggregation_launch_set(cases):
+    return {k for n, paths, r, *_ in cases for k in aggregation_launches(n, paths, r)}
+
+
+# every launch the rules produce over the accepted range: N = 1 .. 128, Npad = 8 .. 256 (any multiple of 8 is one path's round8),
+# with and without pooled channels
+ALL_AGG_LAUNCHES = aggregation_launch_set([(n, (npad,), r) for n in range(1, 129) for npad in range(8, 257, 8) for r in (0, 1)])
+
+# the maps: X*Y a multiple of 4; one partial tile (4, 60 pixels), exactly one 64- / 128-pixel tile, 4 pixels over, 4 under, and 40000
+AGG_GRIDS = {4: (2, 2), 60: (6, 10), 64: (8, 8), 128: (8, 16), 68: (4, 17), 132: (12, 11), 124: (4, 31), 188: (4, 47),
+             40000: (200, 200)}
+_AGG = [  # (N, paths, R, pixels, batch, frames), with each path set's Npad
+    (1, (1,), 1, 4, 1, 1),                         # Npad 8
+    (7, (8,), 0, 60, 2, 3),                        # 8
+    (8, (1, 8, 8), 23, 64, 3, 2),                  # 24
+    (9, (35, 35, 35), 0, 68, 2, 2),                # 120
+    (31, (65, 63), 1, 132, 2, 1),                  # 136
+    (32, (48, 48, 48), 0, 124, 1, 2),              # 144
+    (33, (57, 64, 3, 100), 23, 188, 1, 2),         # 240
+    (63, (100, 100), 0, 128, 1, 3),                # 208 (Npad32 224)
+    (64, (33, 31), 200, 40000, 1, 2),              # 72
+    (64, (1, 2, 3, 4), 23, 60, 2, 2),              # 32
+    (65, (8,), 23, 68, 2, 3),                      # 8
+    (96, (35, 35, 35), 0, 132, 2, 2),              # 120
+    (80, (65, 63), 23, 124, 1, 3),                 # 136
+    (96, (96, 96), 0, 64, 3, 1),                   # 192
+    (65, (64, 64, 64, 64), 1, 188, 1, 2),          # 256
+    (96, (256,), 0, 40000, 1, 1),                  # 256
+    (127, (1, 8, 8), 0, 4, 3, 2),                  # 24
+    (128, (33, 31), 23, 128, 2, 2),                # 72
+    (127, (48, 48, 48), 200, 40000, 1, 1),         # 144
+    (128, (100, 100), 1, 60, 2, 2),                # 208 (Npad32 224): one stage
+    (112, (57, 64, 3, 100), 0, 68, 1, 3),          # 240
+]
+AGG_CASES = [(n, paths, r, AGG_GRIDS[p], b, s) for n, paths, r, p, b, s in _AGG]
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# spatial sums: the kernel's summation order
+# ------------------------------------------------------------------------------------------------------------------------------
+SS_THREADS = 256
+
+
+def spatial_sums_model(planes, pixels):
+    """spatial_sums_kernel's sum of each plane, in its order, in fp32: planes (..., pixels) -> (...) np.float32.  The plane is cut into
+    4-pixel chunks (the last one zero-filled); thread i adds chunks i, i + 256, i + 512, ... lane by lane into four accumulators,
+    ascending; its total is (a0 + a1) + (a2 + a3); each warp's 32 totals are added by an xor butterfly (offsets 16, 8, 4, 2, 1), and the
+    eight warp sums in ascending order.  Threads past the last chunk add nothing: their zero pads here leave every sum as it is."""
+    x = np.asarray(planes, dtype=np.float32)
+    lead = x.shape[:-1]
+    x = x.reshape(-1, pixels)
+    rounds = -(-pixels // (4 * SS_THREADS))
+    chunks = np.zeros((x.shape[0], rounds * SS_THREADS * 4), np.float32)
+    chunks[:, :pixels] = x
+    chunks = chunks.reshape(-1, rounds, SS_THREADS, 4)
+    acc = np.zeros((x.shape[0], SS_THREADS, 4), np.float32)
+    for k in range(rounds):
+        acc = acc + chunks[:, k]
+    v = ((acc[..., 0] + acc[..., 1]) + (acc[..., 2] + acc[..., 3])).reshape(-1, SS_THREADS // 32, 32)
+    lane = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        v = v + v[..., lane ^ o]
+    total = v[:, 0, 0]
+    for w in range(1, SS_THREADS // 32):
+        total = total + v[:, w, 0]
+    return total.reshape(lead)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

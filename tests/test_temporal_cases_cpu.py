@@ -1,9 +1,12 @@
-"""CPU: the case lists and references of tests/_temporal_cases.py, rehearsed before tests/test_temporal_envelope_gpu.py spends GPU time on
-them -- which causal-convolution kernels the lists reach (and which tests/test_causal_conv_gpu.py's own list does not), the grid
-classes and tile counts they were chosen for against the C ABI's workspace sizes, TF32 rounding on hand-picked bit patterns, and the
-by-indexing expectations against fp64 F.conv3d and its gradients."""
+"""CPU: the case lists and references of tests/_temporal_cases.py, rehearsed before tests/test_temporal_envelope_gpu.py and
+tests/test_temporal_tail_envelope_gpu.py spend GPU time on them -- which causal-convolution and aggregation kernels, instantiations
+and ring depths the lists reach (and which the older lists do not), the grid classes and tile counts they were chosen for against the
+C ABI's workspace sizes, the spatial sums' order model against fp64 and on values whose sum shows the order, TF32 rounding on
+hand-picked bit patterns, and the by-indexing expectations against fp64 F.conv3d and its gradients."""
+import math
 import struct
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -37,6 +40,86 @@ def test_grid_list_covers_every_tile_class():
     assert all(sum(1 for g in TC.B_GRIDS if g[1] == y) == 2 for y in ys)
     assert all(sum(1 for g in TC.B_GRIDS if g[0] == x) >= 2 for x in xs)
     assert {(x % 8, y % 16) for x, y in TC.B_GRIDS} == {(a, c) for a in {x % 8 for x in xs} for c in (0, 4, 8, 12)}
+
+
+def test_aggregation_cases_reach_every_launch_and_the_old_list_does_not():
+    from tests.test_temporal_tail_gpu import AGG as OLD
+    got = TC.aggregation_launch_set(TC.AGG_CASES)
+    assert got == TC.ALL_AGG_LAUNCHES
+    kernels = {k[:2] for k in got}
+    assert {("aggregation", 1), ("aggregation", 2), ("dgrad", 1), ("dgrad", 2)} <= kernels
+    assert {("forward", nch) for nch in (1, 2, 3, 4)} | {("wgrad", 1), ("wgrad", 2)} <= kernels
+    assert {k[2] for k in got if k[0] == "wgrad"} == {128, 256, 384, 512}
+    # the ring depths: NCHK = 1 runs 4 / 3 / 2 stages, NCHK = 2 runs 4 / 2 / 1; one stage only for N > 64 with Npad32 >= 224
+    for kind in ("aggregation", "dgrad"):
+        assert {k[2] for k in got if k[:2] == (kind, 1)} == {4, 3, 2}
+        assert {k[2] for k in got if k[:2] == (kind, 2)} == {4, 2, 1}
+    for n in range(1, 129):
+        for npad in range(8, 257, 8):
+            one_stage = TC.aggregation_launches(n, (npad,), 1)[0][2] == 1
+            assert one_stage == (n > 64 and (npad + 31) // 32 * 32 >= 224), (n, npad)
+    ns = {n for n, *_ in TC.AGG_CASES}
+    assert {1, 7, 8, 9, 31, 32, 33, 63, 64, 65, 96, 127, 128} <= ns
+    assert {len(p) for _, p, *_ in TC.AGG_CASES} == {1, 2, 3, 4}
+    assert any(c % 8 for _, p, *_ in TC.AGG_CASES for c in p) and any(c % 8 == 0 for _, p, *_ in TC.AGG_CASES for c in p)
+    npads = {sum(TC.round8(c) for c in p) for _, p, *_ in TC.AGG_CASES}
+    assert {(v - 1) // 64 for v in npads} == {0, 1, 2, 3} and 256 in npads
+    assert {r for _, _, r, *_ in TC.AGG_CASES} >= {0, 1, 23} and max(r for _, _, r, *_ in TC.AGG_CASES) >= 128
+    assert {b for *_, b, _ in TC.AGG_CASES} == {1, 2, 3} == {s for *_, s in TC.AGG_CASES}
+    old = TC.aggregation_launch_set([(n, p, r) for p, r, n in OLD.values()])
+    assert {k[:2] for k in old if k[0] in ("aggregation", "dgrad")} == {("aggregation", 1)}
+
+
+def test_aggregation_maps_cover_every_tile_class():
+    pixels = {X * Y for _, _, _, (X, Y), _, _ in TC.AGG_CASES}
+    assert pixels == set(TC.AGG_GRIDS) and all(p % 4 == 0 for p in pixels)
+    assert all(X * Y == p for p, (X, Y) in TC.AGG_GRIDS.items())
+    for tile in (64, 128):                                      # the backward / aggregation tile and the forward's
+        assert {p % tile for p in pixels} >= {0, 4, tile - 4}, tile
+        assert tile in pixels and tile + 4 in pixels and tile - 4 in pixels
+    assert {4, 60} <= pixels and max(pixels) == 40000
+
+
+@pytest.mark.parametrize("n,paths,r,grid,b,s", TC.AGG_CASES[::4], ids=lambda v: str(v).replace(" ", ""))
+def test_aggregation_workspace_is_the_swapped_entry_rule(n, paths, r, grid, b, s):
+    from fiery_b200.temporal import backward_weight_workspace_bytes
+    X, Y = grid
+    assert backward_weight_workspace_bytes((b, n, s, X, Y), paths, 0) == TC.entry_workspace_bytes(b, s, X * Y, n, paths, 0)
+
+
+SUM_PIXELS = [1, 3, 4, 5, 255, 1023, 1024, 1025, 4095, 4096, 4097, 8193, 40000]
+
+
+@pytest.mark.parametrize("pixels", SUM_PIXELS)
+def test_spatial_sums_model_against_fp64(pixels):
+    gen = np.random.default_rng(pixels)
+    x = (gen.standard_normal((64, pixels)) * np.exp2(gen.integers(-4, 5, (64, pixels)))).astype(np.float32)
+    got = TC.spatial_sums_model(x, pixels)
+    assert got.dtype == np.float32 and got.shape == (64,)
+    ref = x.astype(np.float64).sum(1)
+    bound = 4 * math.sqrt(pixels) * np.spacing(np.abs(x).max(1).astype(np.float32)).astype(np.float64)
+    assert np.all(np.abs(got.astype(np.float64) - ref) <= bound), float(np.max(np.abs(got - ref) / bound))
+    ints = gen.integers(-3, 4, (2, 3, pixels)).astype(np.float32)
+    assert np.array_equal(TC.spatial_sums_model(ints, pixels), ints.astype(np.float64).sum(-1))
+
+
+def _with(pixels, values):
+    x = np.zeros(pixels, np.float32)
+    for i, v in values.items():
+        x[i] = v
+    return float(TC.spatial_sums_model(x, pixels))
+
+
+def test_spatial_sums_model_order_on_chosen_values():
+    """2^24 and two 1.0s: 2^24 + 1 rounds back to 2^24 (ties to even) but 2^24 + 2 is exact, so where the two 1.0s meet each other
+    before meeting 2^24 shows the order."""
+    big, pixels = 2.0 ** 24, 4 * 512 + 8               # thread 0 takes chunks 0, 256 and 512, thread 1 chunks 1, 257 and 513, ...
+    assert _with(pixels, {0: big, 1024: 1.0, 2048: 1.0}) == big          # one lane accumulator, in chunk order
+    assert _with(pixels, {0: big, 2: 1.0, 3: 1.0}) == big + 2            # lanes 2 and 3 are added before lanes 0 and 1
+    assert _with(pixels, {0: big, 1: 1.0, 2: 1.0}) == big                # lanes 0 and 1 first
+    assert _with(pixels, {0: big, 4: 1.0, 68: 1.0}) == big + 2           # threads 1 and 17 meet at butterfly offset 16
+    assert _with(pixels, {0: big, 4: 1.0, 8: 1.0}) == big                # threads 1 and 2 meet thread 0 first
+    assert _with(pixels, {0: big, 128: 1.0, 256: 1.0}) == big            # warps 0, 1, 2: added one after the other
 
 
 def _cc_desc(b, s, X, Y, cin, cout, kt):

@@ -45,7 +45,9 @@ def _tf32(t):
 # ------------------------------------------------------------------------------------------------------------------------------
 # spatial sums
 # ------------------------------------------------------------------------------------------------------------------------------
-SUM_GRIDS = [(1, 1), (1, 3), (3, 5), (8, 8), (52, 49), (200, 200), (400, 200)]
+# pixel counts around the kernel's loop edges too: 1024 pixels are one pass of 256 threads over 4-pixel chunks, 4096 one unrolled pass
+SUM_GRIDS = [(1, 1), (1, 3), (3, 5), (8, 8), (52, 49), (200, 200), (400, 200),
+             (3, 341), (32, 32), (5, 205), (3, 1365), (64, 64), (17, 241), (3, 2731)]
 
 
 def _sums_guarded(x):
@@ -231,9 +233,9 @@ def test_frozen_weight_and_input_launch_only_what_is_asked(monkeypatch):
 GRID = (52, 48)
 
 
-def _model(rf, inbetween, seed=0):
+def _model(rf, inbetween, seed=0, grid=GRID, start_out_channels=64, **kw):
     torch.manual_seed(seed)
-    m = temporal_model(70, rf, GRID, start_out_channels=64, inbetween_layers=inbetween)
+    m = temporal_model(70, rf, grid, start_out_channels=start_out_channels, inbetween_layers=inbetween, **kw)
     for mod in m.modules():
         if isinstance(mod, torch.nn.BatchNorm3d):
             mod.weight.data.uniform_(0.5, 1.5)
