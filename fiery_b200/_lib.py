@@ -9,7 +9,7 @@ from __future__ import annotations
 import collections
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
 
 import torch
 
@@ -63,6 +63,16 @@ class CausalConv3dDesc(ctypes.Structure):
     _fields_ = [
         ("batch", c_int32), ("frames", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("in_channels", c_int32),
         ("out_channels", c_int32), ("kt", c_int32),
+    ]
+
+
+class BatchNormDesc(ctypes.Structure):
+    """Mirror of ``fiery_batch_norm_desc_t``."""
+
+    _fields_ = [
+        ("batch", c_int32), ("channels", c_int32), ("frames", c_int32), ("pixels", c_int32),
+        ("stride_b", c_int64), ("stride_c", c_int64), ("stride_t", c_int64),
+        ("training", c_int32), ("relu", c_int32), ("eps", c_double),
     ]
 
 
@@ -121,6 +131,11 @@ SIGNATURES = {
     "fiery_causal_conv3d_backward_data": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_causal_conv3d_backward_weight_workspace_bytes": (c_size_t, [POINTER(CausalConv3dDesc)]),
     "fiery_causal_conv3d_backward_weight": (c_int32, [POINTER(CausalConv3dDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_batch_norm_workspace_bytes": (c_size_t, [POINTER(BatchNormDesc)]),
+    "fiery_batch_norm_forward": (c_int32, [POINTER(BatchNormDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_batch_norm_backward": (c_int32, [POINTER(BatchNormDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

@@ -6,8 +6,9 @@ kernels in csrc/causal_conv.cu) computes the pad and the convolution in one pass
 padded copy; both gradients run on the tensor cores too, and the weight gradient is bit-reproducible.
 
 ``TensorCoreCausalConv3d.from_module(m)`` adopts the reference module's children under the same names (``state_dict`` keys are
-unchanged) and replaces only the pad and the convolution; BatchNorm and ReLU stay the reference's own modules, so batch statistics
-train as before.  ``install.use_tensor_core_causal_convs`` swaps it into a model.  No CPU path.
+unchanged) and replaces only the pad and the convolution; BatchNorm and ReLU stay the module's own, called through
+``batch_norm.norm_act`` (one fused apply once ``install.use_fused_batch_norm`` has swapped the norm).
+``install.use_tensor_core_causal_convs`` swaps it into a model.  No CPU path.
 """
 from __future__ import annotations
 
@@ -19,6 +20,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import _require_cuda, f32
+from .batch_norm import norm_act
 from .ops import _register_conv
 
 MAX_CHANNELS = 64
@@ -182,4 +184,4 @@ class TensorCoreCausalConv3d(nn.Module):
             y = self.conv(self.pad(x))
         else:
             y = torch.ops.fiery_b200.causal_conv3d(x, self.conv.weight)
-        return self.activation(self.norm(y))
+        return norm_act(self.norm, self.activation, y)

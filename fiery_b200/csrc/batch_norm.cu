@@ -1,0 +1,366 @@
+// BatchNorm3d over a (b, C, s, X, Y) fp32 tensor with an optional fused ReLU and residual add, forward and backward, train and eval
+// (include/fiery_b200.h, fiery_batch_norm_*).  Every pass is bandwidth-bound; none uses atomics, and every summation order depends on
+// the shape only, so results are bit-reproducible and do not depend on where a plane lies in memory.
+//
+// Each (b, c, t) pixel plane is cut into pieces of BN_PIECE pixels (the last one shorter), so the partial pass has enough CTAs to
+// fill the GPU even when the planes are few and large.  One CTA takes one piece: thread i holds chunks i, i + 256, i + 512, i + 768
+// (4 pixels each) in registers.
+//   forward partial:  the piece's mean (block sum / count) and M2 = sum (x - piece mean)^2, both from the registers (two passes
+//                     over values read once);
+//   backward partial: sum g' and sum g' (x - mu), g' = dy masked by the forward's ReLU when it is fused.
+// A thread adds its chunks in ascending order, each chunk as (p0 + p1) + (p2 + p3); the warps reduce by an xor butterfly and the 8
+// warp sums are added in ascending order.  The per-channel finalize (one thread per channel) merges the channel's pieces in
+// ascending (b, t, piece) order in fp64: Chan's formula for (count, mean, M2), plain sums for the backward.  The apply passes use
+// the same pieces.
+#include "common.cuh"
+#include "plane_chunks.cuh"
+
+namespace fiery {
+
+constexpr int BN_THREADS = 256;
+constexpr int BN_CHUNKS = 4;                                   // chunks per thread: the whole piece sits in registers
+constexpr int BN_PIECE = BN_THREADS * BN_CHUNKS * 4;           // 4096 pixels
+constexpr long long BN_MAX_GRID = 1ll << 30;
+constexpr int BN_MIN_CTAS = 4;                                 // resident CTAs per SM the register budget allows
+
+struct BnShape {
+    long long pieces;                                          // batch * channels * frames * per_plane
+    long long per_channel;                                     // pieces of one channel: batch * frames * per_plane
+    long long sb, sc, st;                                      // x's strides, elements
+    int channels, frames, pixels, per_plane;
+};
+
+// Per-channel coefficients the finalize writes for the apply passes.  Forward: y = fmaf(scale, x, shift).  Backward:
+// dx = fmaf(scale, g', fmaf(k1, x - mean, k0)) in training, scale * g' in eval.
+struct BnCoef {
+    float scale, shift, mean, k1, k0;
+};
+
+struct BnPiece {
+    long long x_off, out_off, part;                            // x offset, offset in the contiguous tensors, partial index
+    int c, n;                                                  // channel, pixels in the piece
+};
+
+__device__ __forceinline__ BnPiece bn_piece(const BnShape& s, long long g) {
+    const long long plane = g / s.per_plane;
+    const int j = static_cast<int>(g - plane * s.per_plane);
+    const long long t = plane % s.frames, c = (plane / s.frames) % s.channels, b = plane / (static_cast<long long>(s.frames) * s.channels);
+    BnPiece p;
+    p.c = static_cast<int>(c);
+    p.n = min(BN_PIECE, s.pixels - j * BN_PIECE);
+    p.x_off = b * s.sb + c * s.sc + t * s.st + static_cast<long long>(j) * BN_PIECE;
+    p.out_off = plane * s.pixels + static_cast<long long>(j) * BN_PIECE;
+    p.part = c * s.per_channel + (b * s.frames + t) * s.per_plane + j;
+    return p;
+}
+
+// scale = gamma / sqrt(var + eps), shift = beta - mean * scale, in fp64 from the fp32 statistics and rounded once.  The forward's
+// finalize and both backward passes call it, so the backward's ReLU mask sees exactly the forward's scale and shift.
+__device__ __forceinline__ void bn_scale_shift(const float* __restrict__ w, const float* __restrict__ bias, float mean, float var,
+                                               double eps, int c, float& scale, float& shift) {
+    const double s = (w ? static_cast<double>(w[c]) : 1.0) / sqrt(static_cast<double>(var) + eps);
+    scale = static_cast<float>(s);
+    shift = static_cast<float>((bias ? static_cast<double>(bias[c]) : 0.0) - static_cast<double>(mean) * s);
+}
+
+// sum over the CTA in the order above; every thread gets the total.  sh: BN_THREADS / 32 floats.
+__device__ __forceinline__ float bn_block_sum(float v, float* sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float total = sh[0];
+#pragma unroll
+    for (int w = 1; w < BN_THREADS / 32; ++w) total += sh[w];
+    __syncthreads();                                           // sh is rewritten by the next call
+    return total;
+}
+
+__device__ __forceinline__ float bn_chunk_sum(float4 v) { return (v.x + v.y) + (v.z + v.w); }
+
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_stats_kernel(const BnShape s, const float* __restrict__ x, float2* __restrict__ part) {
+    __shared__ float sh[BN_THREADS / 32];
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const float* xp = x + p.x_off;
+        const bool vec = aligned16_ptr(xp);
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            v[u] = q < n_chunks ? load_chunk4(xp, q, p.n, vec) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        float a = 0.f;
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) a += bn_chunk_sum(v[u]);
+        const float mean = bn_block_sum(a, sh) / static_cast<float>(p.n);
+        float m2 = 0.f;
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int i = 4 * (threadIdx.x + u * BN_THREADS);
+            const float d0 = i < p.n ? v[u].x - mean : 0.f, d1 = i + 1 < p.n ? v[u].y - mean : 0.f;
+            const float d2 = i + 2 < p.n ? v[u].z - mean : 0.f, d3 = i + 3 < p.n ? v[u].w - mean : 0.f;
+            m2 += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+        }
+        m2 = bn_block_sum(m2, sh);
+        if (threadIdx.x == 0) part[p.part] = make_float2(mean, m2);
+    }
+}
+
+// One thread per channel.  training: Chan's merge of the pieces' (count, mean, M2) in fp64 -> mean and biased variance; eval: the
+// running statistics.  Writes the fp32 statistics and the forward's coefficients.
+__global__ void bn_finalize_forward_kernel(const BnShape s, const float2* __restrict__ part, const float* __restrict__ w,
+                                           const float* __restrict__ bias, const float* __restrict__ running_mean,
+                                           const float* __restrict__ running_var, int training, double eps, float* __restrict__ mean_out,
+                                           float* __restrict__ var_out, BnCoef* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= s.channels) return;
+    float mean, var;
+    if (training) {
+        double n = 0.0, m = 0.0, m2 = 0.0;
+        const float2* pc = part + c * s.per_channel;
+        for (long long k = 0; k < s.per_channel; ++k) {
+            const int j = static_cast<int>(k % s.per_plane);
+            const double nb = static_cast<double>(min(BN_PIECE, s.pixels - j * BN_PIECE));
+            const float2 pk = pc[k];
+            const double delta = static_cast<double>(pk.x) - m, nn = n + nb;
+            m += delta * (nb / nn);
+            m2 += static_cast<double>(pk.y) + delta * delta * (n * nb / nn);
+            n = nn;
+        }
+        mean = static_cast<float>(m);
+        var = static_cast<float>(m2 / n);
+    } else {
+        mean = running_mean[c];
+        var = running_var[c];
+    }
+    mean_out[c] = mean;
+    var_out[c] = var;
+    BnCoef k;
+    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
+    k.mean = mean;
+    k.k1 = k.k0 = 0.f;
+    coef[c] = k;
+}
+
+template <bool RELU, bool RESIDUAL>
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_apply_kernel(const BnShape s, const float* __restrict__ x, const BnCoef* __restrict__ coef,
+                                                              const float* __restrict__ residual, float* __restrict__ y) {
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const float* xp = x + p.x_off;
+        float* yp = y + p.out_off;
+        const float* rp = RESIDUAL ? residual + p.out_off : nullptr;
+        const bool vx = aligned16_ptr(xp), vy = aligned16_ptr(yp), vr = RESIDUAL && aligned16_ptr(rp);
+        const float scale = coef[p.c].scale, shift = coef[p.c].shift;
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS], r[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q < n_chunks) {
+                v[u] = load_chunk4(xp, q, p.n, vx);
+                if (RESIDUAL) r[u] = load_chunk4(rp, q, p.n, vr);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q >= n_chunks) continue;
+            float o[4] = {fmaf(scale, v[u].x, shift), fmaf(scale, v[u].y, shift), fmaf(scale, v[u].z, shift), fmaf(scale, v[u].w, shift)};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                if (RELU) o[e] = o[e] < 0.f ? 0.f : o[e];      // a NaN passes, as torch's ReLU lets it
+            }
+            if (RESIDUAL) {
+                o[0] += r[u].x;
+                o[1] += r[u].y;
+                o[2] += r[u].z;
+                o[3] += r[u].w;
+            }
+            store_chunk4(yp, q, p.n, vy, make_float4(o[0], o[1], o[2], o[3]));
+        }
+    }
+}
+
+// g' = dy where the forward's fmaf(scale, x, shift) was > 0 (ReLU fused), dy otherwise
+template <bool RELU>
+__device__ __forceinline__ float bn_masked(float dy, float x, float scale, float shift) {
+    return RELU ? (fmaf(scale, x, shift) > 0.f ? dy : 0.f) : dy;
+}
+
+template <bool RELU>
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_grad_sums_kernel(const BnShape s, const float* __restrict__ x, const float* __restrict__ dy,
+                                                                  const float* __restrict__ w, const float* __restrict__ bias,
+                                                                  const float* __restrict__ mean, const float* __restrict__ var,
+                                                                  double eps, float2* __restrict__ part) {
+    __shared__ float sh[BN_THREADS / 32];
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const float* xp = x + p.x_off;
+        const float* gp = dy + p.out_off;
+        const bool vx = aligned16_ptr(xp), vg = aligned16_ptr(gp);
+        const float mu = mean[p.c];
+        float scale = 0.f, shift = 0.f;
+        if (RELU) bn_scale_shift(w, bias, mu, var[p.c], eps, p.c, scale, shift);
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS], d[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            const bool in = q < n_chunks;                       // pixels past the piece read as x = 0, dy = 0: they add zero
+            v[u] = in ? load_chunk4(xp, q, p.n, vx) : make_float4(0.f, 0.f, 0.f, 0.f);
+            d[u] = in ? load_chunk4(gp, q, p.n, vg) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const float4 gm = make_float4(bn_masked<RELU>(d[u].x, v[u].x, scale, shift), bn_masked<RELU>(d[u].y, v[u].y, scale, shift),
+                                          bn_masked<RELU>(d[u].z, v[u].z, scale, shift), bn_masked<RELU>(d[u].w, v[u].w, scale, shift));
+            s1 += bn_chunk_sum(gm);
+            s2 += bn_chunk_sum(make_float4(gm.x * (v[u].x - mu), gm.y * (v[u].y - mu), gm.z * (v[u].z - mu), gm.w * (v[u].w - mu)));
+        }
+        s1 = bn_block_sum(s1, sh);
+        s2 = bn_block_sum(s2, sh);
+        if (threadIdx.x == 0) part[p.part] = make_float2(s1, s2);
+    }
+}
+
+// One thread per channel: the fp64 sums of the pieces' (sum g', sum g' (x - mu)) in ascending order (when reduced), the weight and
+// bias gradients, and the coefficients of dx.
+__global__ void bn_finalize_backward_kernel(const BnShape s, const float2* __restrict__ part, int reduced, const float* __restrict__ w,
+                                            const float* __restrict__ bias, const float* __restrict__ mean, const float* __restrict__ var,
+                                            int training, double eps, float* __restrict__ grad_w, float* __restrict__ grad_b,
+                                            BnCoef* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= s.channels) return;
+    double s1 = 0.0, s2 = 0.0;
+    if (reduced) {
+        const float2* pc = part + c * s.per_channel;
+        for (long long k = 0; k < s.per_channel; ++k) {
+            const float2 pk = pc[k];
+            s1 += static_cast<double>(pk.x);
+            s2 += static_cast<double>(pk.y);
+        }
+    }
+    BnCoef k;
+    k.mean = mean[c];
+    const float v = var[c];
+    bn_scale_shift(w, bias, k.mean, v, eps, c, k.scale, k.shift);
+    const double ve = static_cast<double>(v) + eps;
+    if (grad_w) grad_w[c] = static_cast<float>(s2 / sqrt(ve));
+    if (grad_b) grad_b[c] = static_cast<float>(s1);
+    const double n = static_cast<double>(s.per_channel / s.per_plane) * s.pixels;
+    k.k1 = training ? static_cast<float>(-static_cast<double>(k.scale) * s2 / (n * ve)) : 0.f;
+    k.k0 = training ? static_cast<float>(-static_cast<double>(k.scale) * s1 / n) : 0.f;
+    coef[c] = k;
+}
+
+template <bool RELU, bool TRAINING>
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_grad_apply_kernel(const BnShape s, const float* __restrict__ x, const float* __restrict__ dy,
+                                                                   const BnCoef* __restrict__ coef, float* __restrict__ dx) {
+    constexpr bool READ_X = RELU || TRAINING;
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const float* xp = x + p.x_off;
+        const float* gp = dy + p.out_off;
+        float* op = dx + p.out_off;
+        const bool vx = aligned16_ptr(xp), vg = aligned16_ptr(gp), vo = aligned16_ptr(op);
+        const BnCoef k = coef[p.c];
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS], d[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q < n_chunks) {
+                d[u] = load_chunk4(gp, q, p.n, vg);
+                if (READ_X) v[u] = load_chunk4(xp, q, p.n, vx);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q >= n_chunks) continue;
+            const float xs[4] = {READ_X ? v[u].x : 0.f, READ_X ? v[u].y : 0.f, READ_X ? v[u].z : 0.f, READ_X ? v[u].w : 0.f};
+            const float ds[4] = {d[u].x, d[u].y, d[u].z, d[u].w};
+            float o[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float gm = bn_masked<RELU>(ds[e], xs[e], k.scale, k.shift);
+                o[e] = TRAINING ? fmaf(k.scale, gm, fmaf(k.k1, xs[e] - k.mean, k.k0)) : k.scale * gm;
+            }
+            store_chunk4(op, q, p.n, vo, make_float4(o[0], o[1], o[2], o[3]));
+        }
+    }
+}
+
+static BnShape bn_shape(const fiery_batch_norm_desc_t* d) {
+    BnShape s;
+    s.channels = d->channels;
+    s.frames = d->frames;
+    s.pixels = d->pixels;
+    s.per_plane = (d->pixels + BN_PIECE - 1) / BN_PIECE;
+    s.per_channel = static_cast<long long>(d->batch) * d->frames * s.per_plane;
+    s.pieces = s.per_channel * d->channels;
+    s.sb = d->stride_b;
+    s.sc = d->stride_c;
+    s.st = d->stride_t;
+    return s;
+}
+
+static size_t bn_coef_bytes(int channels) { return (static_cast<size_t>(channels) * sizeof(BnCoef) + 255) / 256 * 256; }
+
+size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d) {
+    const BnShape s = bn_shape(d);
+    return bn_coef_bytes(d->channels) + static_cast<size_t>(s.pieces) * sizeof(float2);
+}
+
+static unsigned bn_grid(const BnShape& s) { return static_cast<unsigned>(s.pieces < BN_MAX_GRID ? s.pieces : BN_MAX_GRID); }
+
+int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
+                              const float* running_var, const float* residual, float* y, float* mean_out, float* var_out,
+                              void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
+    if (d->training) bn_stats_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, part);
+    bn_finalize_forward_kernel<<<fin, 128, 0, stream>>>(s, part, w, bias, running_mean, running_var, d->training, d->eps, mean_out, var_out,
+                                                         coef);
+    if (d->relu) {
+        if (residual) bn_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+        else bn_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+    } else {
+        if (residual) bn_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+        else bn_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
+                               const float* mean, const float* var, float* dx, float* grad_w, float* grad_b, void* workspace,
+                               cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
+    // the sums are needed for the weight and bias gradients, and for dx in training
+    const bool reduce = grad_w || grad_b || (dx && d->training);
+    if (reduce) {
+        if (d->relu) bn_grad_sums_kernel<true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+        else bn_grad_sums_kernel<false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+    }
+    bn_finalize_backward_kernel<<<fin, 128, 0, stream>>>(s, part, reduce, w, bias, mean, var, d->training, d->eps, grad_w, grad_b, coef);
+    if (dx) {
+        if (d->relu && d->training) bn_grad_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+        else if (d->relu) bn_grad_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+        else if (d->training) bn_grad_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+        else bn_grad_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+}  // namespace fiery

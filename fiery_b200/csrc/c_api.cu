@@ -123,6 +123,13 @@ size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d
 int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
                                 float* gw, void* workspace, cudaStream_t stream);
 size_t causal_conv_packed_bytes(const fiery_causal_conv3d_desc_t* d);
+size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d);
+int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
+                              const float* running_var, const float* residual, float* y, float* mean_out, float* var_out,
+                              void* workspace, cudaStream_t stream);
+int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
+                               const float* mean, const float* var, float* dx, float* grad_w, float* grad_b, void* workspace,
+                               cudaStream_t stream);
 int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w, float* packed, cudaStream_t stream);
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
 int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
@@ -631,6 +638,52 @@ FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc
         FIERY_REQUIRE(aligned16(x) && aligned16(grad_y) && aligned16(workspace), "causal conv: pointers must be 16-byte aligned");
     }
     return launch_causal_conv_wgrad(desc, x, grad_y, grad_w, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// The batch norm's shape limits, one place for every entry point.  The messages name the field.
+static int check_batch_norm_desc(const fiery_batch_norm_desc_t* d) {
+    FIERY_REQUIRE(d, "batch norm: NULL desc");
+    FIERY_REQUIRE(d->channels >= 1, "batch norm: channels = %d must be >= 1", d->channels);
+    FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0 && static_cast<long long>(d->batch) * d->frames >= 1,
+                  "batch norm: batch = %d, frames = %d must be >= 0 with batch * frames >= 1", d->batch, d->frames);
+    FIERY_REQUIRE(d->pixels >= 1, "batch norm: pixels X*Y = %d must be >= 1", d->pixels);
+    FIERY_REQUIRE(d->stride_b >= 0 && d->stride_c >= 0 && d->stride_t >= 0, "batch norm: strides (%lld, %lld, %lld) must be >= 0",
+                  (long long)d->stride_b, (long long)d->stride_c, (long long)d->stride_t);
+    FIERY_REQUIRE(d->training == 0 || d->training == 1, "batch norm: training = %d must be 0 or 1", d->training);
+    FIERY_REQUIRE(d->relu == 0 || d->relu == 1, "batch norm: relu = %d must be 0 or 1", d->relu);
+    FIERY_REQUIRE(d->eps >= 0.0, "batch norm: eps = %g must be >= 0", d->eps);
+    FIERY_REQUIRE(!d->training || static_cast<long long>(d->batch) * d->frames * d->pixels >= 2,
+                  "batch norm: n = batch * frames * pixels = %lld values per channel must be >= 2 in training",
+                  static_cast<long long>(d->batch) * d->frames * d->pixels);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* desc) {
+    if (check_batch_norm_desc(desc) != FIERY_OK) return 0;
+    return batch_norm_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_batch_norm_forward(const fiery_batch_norm_desc_t* desc, const float* x, const float* weight, const float* bias,
+                                       const float* running_mean, const float* running_var, const float* residual, float* y,
+                                       float* mean_out, float* var_out, void* workspace, void* stream) {
+    const int rc = check_batch_norm_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(x && y && mean_out && var_out && workspace, "batch norm: NULL x / y / mean_out / var_out / workspace");
+    FIERY_REQUIRE(desc->training || (running_mean && running_var), "batch norm: eval mode needs running_mean and running_var");
+    FIERY_REQUIRE(aligned16(workspace), "batch norm: workspace must be 16-byte aligned");
+    return launch_batch_norm_forward(desc, x, weight, bias, desc->training ? nullptr : running_mean, desc->training ? nullptr : running_var,
+                                     residual, y, mean_out, var_out, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, const float* x, const float* grad_y, const float* weight,
+                                        const float* bias, const float* mean, const float* var, float* grad_x, float* grad_weight,
+                                        float* grad_bias, void* workspace, void* stream) {
+    const int rc = check_batch_norm_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(x && grad_y && mean && var && workspace, "batch norm: NULL x / grad_y / mean / var / workspace");
+    FIERY_REQUIRE(aligned16(workspace), "batch norm: workspace must be 16-byte aligned");
+    return launch_batch_norm_backward(desc, x, grad_y, weight, bias, mean, var, grad_x, grad_weight, grad_bias, workspace,
+                                      static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

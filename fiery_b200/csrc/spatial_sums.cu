@@ -8,6 +8,7 @@
 // is read as one float4 (plane base 16-byte aligned) or as four floats changes the load only, so a plane's sum is bit-identical
 // whatever its strides, its neighbours or its place in the tensor.  No atomics.
 #include "common.cuh"
+#include "plane_chunks.cuh"
 
 namespace fiery {
 
@@ -20,17 +21,6 @@ struct SsShape {
     long long sb, sc, st;                          // elements
     int pixels;
 };
-
-__device__ __forceinline__ float4 ss_chunk(const float* __restrict__ p, int q, int pixels, bool vec) {
-    const int i = 4 * q;
-    if (vec && i + 3 < pixels) return __ldg(reinterpret_cast<const float4*>(p) + q);
-    float4 v;
-    v.x = __ldg(p + i);
-    v.y = i + 1 < pixels ? __ldg(p + i + 1) : 0.f;
-    v.z = i + 2 < pixels ? __ldg(p + i + 2) : 0.f;
-    v.w = i + 3 < pixels ? __ldg(p + i + 3) : 0.f;
-    return v;
-}
 
 __global__ void __launch_bounds__(SS_THREADS) spatial_sums_kernel(const SsShape s, const float* __restrict__ x, float* __restrict__ sums) {
     __shared__ float warp_sums[SS_THREADS / 32];
@@ -45,7 +35,7 @@ __global__ void __launch_bounds__(SS_THREADS) spatial_sums_kernel(const SsShape 
 #pragma unroll
             for (int u = 0; u < SS_UNROLL; ++u) {
                 const int q = q0 + u * SS_THREADS;
-                if (q < n_chunks) v[u] = ss_chunk(p, q, s.pixels, vec);
+                if (q < n_chunks) v[u] = load_chunk4(p, q, s.pixels, vec);
             }
 #pragma unroll
             for (int u = 0; u < SS_UNROLL; ++u) {

@@ -225,6 +225,34 @@ def use_tensor_core_pyramid_pooling(model):
     return model
 
 
+def use_fused_batch_norm(model):
+    """Replace every module whose type is exactly ``nn.BatchNorm3d`` under ``model.temporal_model.model`` of a ``Fiery`` instance -- in
+    reference blocks, swapped blocks and ``Bottleneck3D`` alike -- by ``fiery_b200.batch_norm.FusedBatchNorm3d``, which adopts its
+    Parameters and buffers (``state_dict`` keys unchanged) and runs on the batch-norm kernels.  In a ``TensorCoreTemporalBlock`` and a
+    ``TensorCoreCausalConv3d`` the ReLU after each norm, and the block's skip add, then run in the norm's apply pass.  The pyramid
+    pooling's ``conv_bn_relu`` (a (b, R, s + 1, 1, 1) tensor) keeps its ``nn.BatchNorm3d``.  A ``SyncBatchNorm`` is left as it is, with
+    one warning: cross-rank statistics are not covered.  Works before or after the other temporal swaps; a second call does nothing.
+    Returns the model."""
+    from .batch_norm import FusedBatchNorm3d
+    blocks = getattr(model.temporal_model, "model", None)
+    if blocks is None:
+        return model
+    slots = [(parent, key, child, f"{name}.{key}" if name else key)
+             for name, parent in blocks.named_modules() for key, child in parent.named_children()]
+    synced, fused = [], {}                           # fused: id of a replaced norm -> its FusedBatchNorm3d (one per module)
+    for parent, key, child, where in slots:
+        if "pyramid_pooling" in where.split("."):
+            continue
+        if type(child) is torch.nn.BatchNorm3d:
+            setattr(parent, key, fused.setdefault(id(child), FusedBatchNorm3d(child)))
+        elif isinstance(child, torch.nn.SyncBatchNorm):
+            synced.append(where)
+    if synced:
+        _warn_once(("batch_norm", tuple(synced)), "fiery_b200: SyncBatchNorm module(s) left as they are (the fused batch norm computes "
+                   "per-rank statistics only): " + ", ".join(synced))
+    return model
+
+
 def uninstall():
     if not _saved:
         return

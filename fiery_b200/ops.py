@@ -317,4 +317,72 @@ temporal_aggregation.register_autograd(_temporal_aggregation_backward, setup_con
 torch.library.register_autocast("fiery_b200::temporal_aggregation", "cuda", torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# The temporal model's BatchNorm3d with its ReLU and the block's residual add (fiery/layers/temporal.py:107-117, 65-85, 256-281):
+# ``batch_norm_act`` / ``batch_norm_act_backward`` (fiery_b200/batch_norm.py; kernels in csrc/batch_norm.cu).  The statistics
+# outputs are not differentiable and the operator updates no running buffer (FusedBatchNorm3d does, from them).  Autocast: fp32,
+# like the other temporal operators; a 16-bit input is widened and the output is fp32.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::batch_norm_act", mutates_args=(), device_types="cuda")
+def batch_norm_act(x: torch.Tensor, weight: Optional[torch.Tensor], bias: Optional[torch.Tensor], running_mean: Optional[torch.Tensor],
+                   running_var: Optional[torch.Tensor], residual: Optional[torch.Tensor], training: bool, eps: float,
+                   relu: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """x (b, C, s, X, Y), pixel planes read as they lie -> (y, mean, var): y the contiguous fp32 ``relu(batch_norm(x)) + residual``
+    (the ReLU when ``relu``, the add when ``residual`` is given), mean and the biased var the (C,) fp32 statistics used: the batch's
+    when ``training``, else copies of ``running_mean`` / ``running_var``.  Bit-reproducible: the order depends on the shape only."""
+    from .batch_norm import forward
+    return forward(x, weight, bias, running_mean, running_var, residual, training, eps, relu)
+
+
+@batch_norm_act.register_fake
+def _(x, weight, bias, running_mean, running_var, residual, training, eps, relu):
+    c = x.shape[1]
+    return (x.new_empty(tuple(x.shape), dtype=torch.float32), x.new_empty((c,), dtype=torch.float32),
+            x.new_empty((c,), dtype=torch.float32))
+
+
+@torch.library.custom_op("fiery_b200::batch_norm_act_backward", mutates_args=(), device_types="cuda")
+def batch_norm_act_backward(grad_y: torch.Tensor, x: torch.Tensor, weight: Optional[torch.Tensor], bias: Optional[torch.Tensor],
+                            mean: torch.Tensor, var: torch.Tensor, training: bool, eps: float, relu: bool, need_input: bool,
+                            need_weight: bool, need_bias: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(grad_x, grad_weight, grad_bias) of ``batch_norm_act``, each in its input's dtype (grad_x contiguous); a gradient that is not
+    asked for is not computed and comes back empty.  Needs only x and the forward's (mean, var): the output is not kept."""
+    from .batch_norm import backward
+    dx, dw, db = backward(grad_y, x, weight, bias, mean, var, training, eps, relu, need_input, need_weight, need_bias)
+    return _cast_back(dx, x), _cast_back(dw, weight if weight is not None else x), _cast_back(db, bias if bias is not None else x)
+
+
+@batch_norm_act_backward.register_fake
+def _(grad_y, x, weight, bias, mean, var, training, eps, relu, need_input, need_weight, need_bias):
+    c = x.shape[1]
+    return (x.new_empty(tuple(x.shape)) if need_input else x.new_empty((0,)),
+            weight.new_empty((c,)) if need_weight else x.new_empty((0,)),
+            bias.new_empty((c,)) if need_bias else x.new_empty((0,)))
+
+
+def _batch_norm_act_setup_context(ctx, inputs, output):
+    x, weight, bias, _rm, _rv, residual, training, eps, relu = inputs
+    _y, mean, var = output
+    ctx.mark_non_differentiable(mean, var)
+    ctx.training, ctx.eps, ctx.relu = training, eps, relu
+    ctx.residual_dtype = residual.dtype if residual is not None else None
+    ctx.save_for_backward(x, weight, bias, mean, var)
+
+
+def _batch_norm_act_backward(ctx, grad_y, _grad_mean, _grad_var):
+    x, weight, bias, mean, var = ctx.saved_tensors
+    need = ctx.needs_input_grad
+    need_x, need_w, need_b, need_r = bool(need[0]), bool(need[1]), bool(need[2]), bool(need[5])
+    dx = dw = db = None
+    if need_x or need_w or need_b:
+        dx, dw, db = torch.ops.fiery_b200.batch_norm_act_backward(grad_y, x, weight, bias, mean, var, ctx.training, ctx.eps, ctx.relu,
+                                                                  need_x, need_w, need_b)
+    grad_r = grad_y.to(ctx.residual_dtype) if need_r else None        # the residual is added as it is: its gradient is grad_y
+    return (dx if need_x else None, dw if need_w else None, db if need_b else None, None, None, grad_r, None, None, None)
+
+
+batch_norm_act.register_autograd(_batch_norm_act_backward, setup_context=_batch_norm_act_setup_context)
+torch.library.register_autocast("fiery_b200::batch_norm_act", "cuda", torch.float32)
+
+
 from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

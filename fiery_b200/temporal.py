@@ -33,6 +33,7 @@ import torch.nn.functional as F
 from . import _lib
 from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.temporal_entry)
 from ._lib import _require_cuda, f32
+from .batch_norm import norm_act
 
 MAX_IN_CHANNELS, MAX_OUT_CHANNELS, MAX_EXTRA_CHANNELS = 128, 256, 8
 _warned_pixels = set()
@@ -328,7 +329,8 @@ class TensorCoreTemporalBlock(nn.Module):
     """Drop-in for a reference ``TemporalBlock`` whose four 1x1x1 input convolutions run as one tensor-core GEMM
     (``torch.ops.fiery_b200.temporal_entry``).  It holds the reference block's children under the same names (``state_dict`` keys
     are unchanged) and looks them up at call time, so ``SyncBatchNorm.convert_sync_batchnorm`` works before or after the swap.  The
-    norms, activations, causal convolutions, pyramid pooling, aggregation and projection BN are the block's own modules."""
+    norms, activations, causal convolutions, pyramid pooling, aggregation and projection BN are the block's own modules; each norm
+    and its ReLU, and the last one with the skip add, go through ``batch_norm.norm_act``."""
 
     def __init__(self, block):
         super().__init__()
@@ -361,18 +363,19 @@ class TensorCoreTemporalBlock(nn.Module):
         paths = []
         for i in range(3):
             entry = p[i][0] if i < 2 else p[i]
-            y = entry.activation(entry.norm(ys[i]))
+            y = norm_act(entry.norm, entry.activation, ys[i])
             paths.append(p[i][1](y) if i < 2 else y)
-        if vector is not None:
-            agg = self.aggregation[0]
-            x_residual = agg.activation(agg.norm(torch.ops.fiery_b200.temporal_aggregation(paths, agg.conv.weight, vector)))
-        else:
-            x_residual = torch.cat(paths, dim=1)
-            if pooled is not None:
-                x_residual = torch.cat([x_residual, pooled], dim=1)
-            x_residual = self.aggregation(x_residual)
         skip = self.projection[1](ys[3]) if self.projection is not None else x
-        return skip + x_residual
+        agg = self.aggregation[0]
+        if vector is not None:
+            z = torch.ops.fiery_b200.temporal_aggregation(paths, agg.conv.weight, vector)
+        else:
+            z = torch.cat(paths, dim=1)
+            if pooled is not None:
+                z = torch.cat([z, pooled], dim=1)
+            z = agg.conv(z)
+        # skip + relu(bn(z)): with a FusedBatchNorm3d, one apply that adds the skip
+        return norm_act(agg.norm, agg.activation, z, residual=skip)
 
     def _folds_pooling(self, h: int, w: int) -> bool:
         """The pyramid pooling is the swapped module, its kernel covers this map and the aggregation kernel takes it: the block runs

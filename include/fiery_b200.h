@@ -434,6 +434,55 @@ FIERY_API size_t fiery_causal_conv3d_backward_weight_workspace_bytes(const fiery
 FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc_t* desc, const float* x, const float* grad_y,
                                                   float* grad_w, void* workspace, void* stream);
 
+/*
+ * BatchNorm3d (the temporal model's norms, fiery/layers/temporal.py) over x (batch, channels, frames, X, Y) fp32 whose pixel planes
+ * are contiguous (pixels = X*Y) and whose other strides are arbitrary, with an optional fused ReLU and an optional fused residual add.
+ * Per channel c, over n = batch * frames * pixels values:
+ *   training: mean and biased var of the batch;  eval: mean = running_mean[c], var = running_var[c];
+ *   scale = weight[c] / sqrt(var + eps), shift = bias[c] - mean * scale, in fp64 from the fp32 mean and var, rounded once
+ *   (weight NULL: 1; bias NULL: 0);
+ *   y = fmaf(scale, x, shift), then max(y, 0) when relu (a NaN stays NaN), then + residual when residual is not NULL.
+ * The backward, with g' = grad_y where the forward's fmaf(scale, x, shift) > 0 (relu) or g' = grad_y (no relu), and
+ * S1 = sum g', S2 = sum g' (x - mean):
+ *   grad_bias = S1, grad_weight = S2 / sqrt(var + eps);
+ *   training: grad_x = scale * (g' - S1 / n - (x - mean) * S2 / (n * (var + eps)));  eval: grad_x = scale * g'.
+ * mean and var are what the forward wrote to mean_out / var_out, and the backward takes the forward's weight and bias, so its ReLU
+ * mask is exactly where the forward's ReLU output was zero.  The residual's gradient is grad_y itself.
+ *
+ * y, residual, grad_y, grad_x: (batch, channels, frames, X, Y) fp32, contiguous.  weight, bias, running_mean, running_var, mean_out,
+ * var_out, mean, var, grad_weight, grad_bias: (channels,) fp32.  Any pointer may have 4-byte alignment (16-byte aligned pixel runs
+ * move as float4).  workspace: fiery_batch_norm_workspace_bytes(desc) bytes, 16-byte aligned, contents irrelevant (0 for a rejected
+ * descriptor).  The backward computes what is asked for: grad_x, grad_weight and grad_bias may each be NULL.  Offsets in 64 bits.
+ * Limits (FIERY_E_INVALID, the message names the field): channels >= 1; batch, frames >= 0 with batch * frames >= 1; pixels >= 1;
+ * strides >= 0; training and relu 0 or 1; eps >= 0; in training n >= 2; in eval running_mean and running_var are given.
+ *
+ * Summation order (no atomics; the order depends on the shape only, so results are bit-reproducible whatever the strides or the
+ * addresses, and graph-capturable): each pixel plane is cut into pieces of 4096 pixels, the last one shorter.  Within a piece, thread
+ * i of 256 holds 4-pixel chunks i, i + 256, i + 512, i + 768, adds them in ascending order, each chunk as (p0 + p1) + (p2 + p3), the 32
+ * threads of a warp reduce by an xor butterfly (16, 8, 4, 2, 1) and the 8 warp sums are added in ascending order, in fp32.  The
+ * forward reduces a piece to its mean (the sum over its count) and M2 = sum (x - piece mean)^2, the backward to S1 and S2.  Per
+ * channel, the pieces are merged in ascending (b, t, piece) order in fp64: Chan's formula for (count, mean, M2) in the forward, plain
+ * sums in the backward.  Kernels: csrc/batch_norm.cu.
+ */
+typedef struct {
+    int32_t batch;
+    int32_t channels;
+    int32_t frames;
+    int32_t pixels;               /* X*Y */
+    int64_t stride_b, stride_c, stride_t;   /* x's strides, elements */
+    int32_t training;             /* 1: batch statistics; 0: running statistics */
+    int32_t relu;                 /* 1: ReLU after the affine map */
+    double eps;
+} fiery_batch_norm_desc_t;
+
+FIERY_API size_t fiery_batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* desc);
+FIERY_API int fiery_batch_norm_forward(const fiery_batch_norm_desc_t* desc, const float* x, const float* weight, const float* bias,
+                                       const float* running_mean, const float* running_var, const float* residual, float* y,
+                                       float* mean_out, float* var_out, void* workspace, void* stream);
+FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, const float* x, const float* grad_y, const float* weight,
+                                        const float* bias, const float* mean, const float* var, float* grad_x, float* grad_weight,
+                                        float* grad_bias, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
