@@ -1,5 +1,6 @@
-"""ctypes binding of libfiery_b200.so (C ABI: include/fiery_b200.h), the one helper every launch goes through (``call``) and the
-cache of the tensor-core layers' weight packs (``packed``).
+"""ctypes binding of libfiery_b200.so (C ABI: include/fiery_b200.h), the one helper every launch goes through (``call``), the
+cache of the tensor-core layers' weight packs (``packed``), and the host rules the operators share: input layouts, workspaces and
+the once-only warnings of every swap and fallback (``warn_once``).
 
 There is no fallback: if the shared library is missing or a call fails this module raises.  Build it in-tree with
 ``python -m fiery_b200.build`` (the built ``.so`` travels with the repo snapshot to the GPU box).
@@ -9,6 +10,7 @@ from __future__ import annotations
 import collections
 import ctypes
 import os
+import warnings
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
 
 import torch
@@ -192,6 +194,30 @@ def call(entry: str, device: torch.device, *args) -> None:
 def f32(t: torch.Tensor) -> torch.Tensor:
     """A contiguous fp32 tensor: the layout the kernels read."""
     return t.float().contiguous() if t.dtype != torch.float32 else t.contiguous()
+
+
+def f32_planes(x: torch.Tensor) -> torch.Tensor:
+    """A (b, C, s, X, Y) tensor as the pixel-plane kernels read it: x itself when it is fp32 with contiguous pixel planes (any
+    b / C / s strides), else a contiguous fp32 copy."""
+    _, _, _, h, w = x.shape
+    planes_contiguous = (x.stride(4) == 1 or w == 1) and (x.stride(3) == w or h == 1)
+    return x if x.dtype == torch.float32 and planes_contiguous else f32(x)
+
+
+def workspace(nbytes: int, device: torch.device) -> torch.Tensor:
+    """A uint8 device workspace of ``nbytes`` bytes, never empty, so the kernels get a valid pointer even when they need none."""
+    return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+
+
+_warned = set()
+
+
+def warn_once(key, msg: str, stacklevel: int = 2) -> None:
+    """``warnings.warn(msg, RuntimeWarning)`` the first time ``key`` is seen, until ``install.uninstall()`` forgets them all;
+    ``stacklevel`` counts from the caller, as ``warnings.warn``'s does."""
+    if key not in _warned:
+        _warned.add(key)
+        warnings.warn(msg, RuntimeWarning, stacklevel=stacklevel + 1)
 
 
 # (pack function, args, device, the weights' data_ptrs) -> (the weights' versions, aliases of the weights, pack).  The aliases keep the

@@ -18,14 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import _require_cuda, f32
-
-
-def _input(x: torch.Tensor) -> torch.Tensor:
-    """x as the kernels read it: fp32 with contiguous pixel planes (any b / C / s strides), else a contiguous fp32 copy."""
-    _, _, _, h, w = x.shape
-    planes_contiguous = (x.stride(4) == 1 or w == 1) and (x.stride(3) == w or h == 1)
-    return x if x.dtype == torch.float32 and planes_contiguous else f32(x)
+from ._lib import _require_cuda, f32, f32_planes
 
 
 def _desc(x: torch.Tensor, training: bool, relu: bool, eps: float) -> _lib.BatchNormDesc:
@@ -46,8 +39,7 @@ def _per_channel(t: Optional[torch.Tensor], c: int, name: str) -> Optional[torch
 
 
 def _workspace(d: _lib.BatchNormDesc, device: torch.device) -> torch.Tensor:
-    n = int(_lib.load().fiery_batch_norm_workspace_bytes(d))
-    return torch.empty(max(n, 16), dtype=torch.uint8, device=device)
+    return _lib.workspace(_lib.load().fiery_batch_norm_workspace_bytes(d), device)
 
 
 def _check_count(x_shape, training: bool) -> None:
@@ -66,7 +58,7 @@ def forward(x: torch.Tensor, weight: Optional[torch.Tensor], bias: Optional[torc
     if x.dim() != 5:
         raise ValueError(f"batch norm: expected a 5-D (b, C, s, X, Y) input, got {tuple(x.shape)}")
     _check_count(x.shape, training)
-    xs = _input(x)
+    xs = f32_planes(x)
     c = int(xs.shape[1])
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
     rm, rv = _per_channel(running_mean, c, "running_mean"), _per_channel(running_var, c, "running_var")
@@ -89,7 +81,7 @@ def backward(grad_y: torch.Tensor, x: torch.Tensor, weight: Optional[torch.Tenso
              var: torch.Tensor, training: bool, eps: float, relu: bool, need_input: bool, need_weight: bool, need_bias: bool):
     """(grad_x, grad_weight, grad_bias) of ``forward`` in fp32 (grad_x contiguous), None where not asked for; ``mean`` / ``var`` are
     the forward's outputs, and the weight and bias the forward's, so the ReLU mask is the forward's."""
-    xs = _input(x)
+    xs = f32_planes(x)
     c = int(xs.shape[1])
     g = f32(grad_y)
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")

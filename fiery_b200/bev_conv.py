@@ -104,7 +104,7 @@ def first_conv_backward_weight(x: torch.Tensor, grad_y: torch.Tensor, workspace:
     xs, g = _channels_last_f32(x), _channels_last_f32(grad_y)
     need = backward_weight_workspace_bytes(B, H, W)
     if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+        workspace = _lib.workspace(need, x.device)
     out = torch.empty((64, 64, 7, 7), dtype=torch.float32, device=x.device)
     _lib.call("fiery_bev_first_conv_backward_weight", x.device, B, H, W, xs.data_ptr(), g.data_ptr(), out.data_ptr(),
               workspace.data_ptr())

@@ -12,7 +12,6 @@ unchanged) and replaces only the pad and the convolution; BatchNorm and ReLU sta
 """
 from __future__ import annotations
 
-import warnings
 from typing import Optional
 
 import torch
@@ -24,7 +23,6 @@ from .batch_norm import norm_act
 from .ops import _register_conv
 
 MAX_CHANNELS = 64
-_warned_widths = set()
 
 
 def unsupported_reason(in_channels: int, out_channels: int, kt: int, grid_y: Optional[int] = None) -> Optional[str]:
@@ -114,8 +112,7 @@ def conv_backward_weight(grad_y: torch.Tensor, x: torch.Tensor, weight: torch.Te
     kt = _check(x.shape, weight)
     xs, g = f32(x), f32(grad_y)
     d = _desc(xs.shape, int(weight.shape[0]), kt)
-    need = int(lib.fiery_causal_conv3d_backward_weight_workspace_bytes(d))
-    ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+    ws = _lib.workspace(lib.fiery_causal_conv3d_backward_weight_workspace_bytes(d), x.device)
     gw = torch.empty(tuple(weight.shape), dtype=torch.float32, device=x.device)
     _lib.call("fiery_causal_conv3d_backward_weight", x.device, d, xs.data_ptr(), g.data_ptr(), gw.data_ptr(), ws.data_ptr())
     return gw
@@ -177,10 +174,8 @@ class TensorCoreCausalConv3d(nn.Module):
         (x,) = inputs
         width = x.shape[4]
         if width % 4:
-            if width not in _warned_widths:
-                _warned_widths.add(width)
-                warnings.warn(f"fiery_b200: CausalConv3d input of Y = {width} map columns is not covered by the tensor-core kernels "
-                              "(they need a multiple of 4); it runs as the reference's pad and Conv3d", RuntimeWarning, stacklevel=2)
+            _lib.warn_once(("causal_width", width), f"fiery_b200: CausalConv3d input of Y = {width} map columns is not covered by the "
+                           "tensor-core kernels (they need a multiple of 4); it runs as the reference's pad and Conv3d")
             y = self.conv(self.pad(x))
         else:
             y = torch.ops.fiery_b200.causal_conv3d(x, self.conv.weight)

@@ -14,16 +14,15 @@ from __future__ import annotations
 
 import functools
 import importlib
-import warnings
 
 import torch
 
+from ._lib import _warned, warn_once
 from .geometry import VoxelsSumming
 from .lift import calculate_birds_eye_view_features
 from .warp import cumulative_warp_features, warp_features
 
 _saved = {}
-_warned = set()
 
 
 def unsupported_reason(model, x):
@@ -42,20 +41,14 @@ def unsupported_reason(model, x):
     return None
 
 
-def _warn_once(key, msg):
-    if key not in _warned:
-        _warned.add(key)
-        warnings.warn(msg, RuntimeWarning, stacklevel=3)
-
-
 def _bev_features(self, x, intrinsics, extrinsics):
     """Installed as ``Fiery.calculate_birds_eye_view_features``: the fused lift where the kernels cover the configuration,
     the reference's own method (unpatched behaviour, its own device) where they do not."""
     reason = unsupported_reason(self, x)
     if reason is None:
         return calculate_birds_eye_view_features(self, x, intrinsics, extrinsics)
-    _warn_once(("bev", reason), f"fiery_b200: lift configuration not covered by the CUDA kernels ({reason}); "
-                                "running the reference's own calculate_birds_eye_view_features")
+    warn_once(("bev", reason), f"fiery_b200: lift configuration not covered by the CUDA kernels ({reason}); "
+                               "running the reference's own calculate_birds_eye_view_features")
     return _saved["bev"](self, x, intrinsics, extrinsics)
 
 
@@ -103,8 +96,8 @@ def use_tensor_core_depth_layer(model):
     if isinstance(conv, DepthLayer):
         return model
     if conv.in_channels != 128 or conv.out_channels > 128 or conv.kernel_size != (1, 1):
-        _warn_once(("depth_layer", conv.in_channels, conv.out_channels),
-                   f"fiery_b200: depth_layer {conv.in_channels}->{conv.out_channels} not covered by the tensor-core kernel; left as is")
+        warn_once(("depth_layer", conv.in_channels, conv.out_channels),
+                  f"fiery_b200: depth_layer {conv.in_channels}->{conv.out_channels} not covered by the tensor-core kernel; left as is")
         return model
     model.encoder.depth_layer = DepthLayer.from_conv(conv)
     return model
@@ -127,10 +120,44 @@ def use_tensor_core_first_conv(model):
     if not covered:
         desc = (f"{conv.in_channels}->{conv.out_channels} k{conv.kernel_size} s{conv.stride}" if isinstance(conv, torch.nn.Conv2d)
                 else type(conv).__name__)
-        _warn_once(("first_conv", desc), f"fiery_b200: first_conv {desc} not covered by the tensor-core kernels (they are built for "
-                                         "Conv2d(64, 64, 7, stride=2, padding=3, bias=False)); left as is")
+        warn_once(("first_conv", desc), f"fiery_b200: first_conv {desc} not covered by the tensor-core kernels (they are built for "
+                                        "Conv2d(64, 64, 7, stride=2, padding=3, bias=False)); left as is")
         return model
     model.decoder.first_conv = FirstConv.from_conv(conv)
+    return model
+
+
+_TEMPORAL_BLOCKS = ("TemporalBlock", "TensorCoreTemporalBlock")
+
+
+def _blocks(blocks, *kinds):
+    """(index, name, block) of each block in ``blocks`` whose class is named one of ``kinds``."""
+    for i, (name, block) in enumerate(blocks._modules.items()):
+        if type(block).__name__ in kinds:
+            yield i, name, block
+
+
+def _swap(model, slots, swapped, reason, make, warning: str, entry: str = "{where}: {reason}", sep: str = "; "):
+    """Replace each module that ``slots(model.temporal_model.model)`` yields as ``(parent, name, module, where)`` by
+    ``setattr(parent, name, make(module))``, unless it already is a ``swapped`` or ``reason(module)`` gives a reason to leave it.  A
+    module reached under several names gets one replacement, set in each.  The modules left are listed, each as ``entry`` and
+    ``sep``-separated, in one warning after ``warning``, given once per list.  Returns the model."""
+    blocks = getattr(model.temporal_model, "model", None)
+    if blocks is None:
+        return model
+    made, skipped = {}, []                      # made: id of a replaced module -> its replacement
+    for parent, name, module, where in list(slots(blocks)):
+        if isinstance(module, swapped):
+            continue
+        why = reason(module)
+        if why is not None:
+            skipped.append(entry.format(where=where, reason=why))
+            continue
+        if id(module) not in made:
+            made[id(module)] = make(module)
+        setattr(parent, name, made[id(module)])
+    if skipped:
+        warn_once((warning, tuple(skipped)), warning + sep.join(skipped), stacklevel=3)
     return model
 
 
@@ -141,22 +168,12 @@ def use_tensor_core_temporal_model(model):
     nothing.  A ``TemporalModelIdentity`` (the static configs) is left alone, and so are blocks the kernels do not cover (wrong
     kernel size or bias, shapes outside the limits, an X*Y the TMA cannot take), with one warning."""
     from .temporal import TensorCoreTemporalBlock, block_reason
-    blocks = getattr(model.temporal_model, "model", None)
-    if blocks is None:
-        return model
-    skipped = []
-    for i, block in enumerate(blocks):
-        if isinstance(block, TensorCoreTemporalBlock) or type(block).__name__ != "TemporalBlock":
-            continue
-        reason = block_reason(block)
-        if reason is None:
-            blocks[i] = TensorCoreTemporalBlock(block)
-        else:
-            skipped.append(f"block {i}: {reason}")
-    if skipped:
-        _warn_once(("temporal", tuple(skipped)), "fiery_b200: TemporalBlock(s) not covered by the tensor-core kernels, left as is: "
-                   + "; ".join(skipped))
-    return model
+
+    def slots(blocks):
+        for i, name, block in _blocks(blocks, "TemporalBlock"):
+            yield blocks, name, block, f"block {i}"
+    return _swap(model, slots, TensorCoreTemporalBlock, block_reason, TensorCoreTemporalBlock,
+                 "fiery_b200: TemporalBlock(s) not covered by the tensor-core kernels, left as is: ")
 
 
 def use_tensor_core_causal_convs(model):
@@ -167,33 +184,16 @@ def use_tensor_core_causal_convs(model):
     or after ``use_tensor_core_temporal_model``.  Returns the model; a second call does nothing, and modules the kernels do not cover
     (more than 64 channels, another kernel size, a bias) are left alone with one warning."""
     from .causal_conv import TensorCoreCausalConv3d, module_reason
-    blocks = getattr(model.temporal_model, "model", None)
-    if blocks is None:
-        return model
-    skipped = []
-    for i, block in enumerate(blocks):
-        kind = type(block).__name__
-        if kind in ("TemporalBlock", "TensorCoreTemporalBlock"):
-            slots = [(block.convolution_paths[p], 1, f"block {i} path {p}") for p in (0, 1)]
-        elif kind == "Bottleneck3D":
-            slots = [(block.layers, "conv", f"block {i} bottleneck")]
-        else:
-            continue
-        for parent, key, where in slots:
-            m = parent[key] if isinstance(key, int) else getattr(parent, key)
-            if isinstance(m, TensorCoreCausalConv3d):
-                continue
-            reason = module_reason(m)
-            if reason is not None:
-                skipped.append(f"{where}: {reason}")
-            elif isinstance(key, int):
-                parent[key] = TensorCoreCausalConv3d(m)
+
+    def slots(blocks):
+        for i, _, block in _blocks(blocks, *_TEMPORAL_BLOCKS, "Bottleneck3D"):
+            if type(block).__name__ == "Bottleneck3D":
+                yield block.layers, "conv", block.layers.conv, f"block {i} bottleneck"
             else:
-                setattr(parent, key, TensorCoreCausalConv3d(m))
-    if skipped:
-        _warn_once(("causal", tuple(skipped)), "fiery_b200: CausalConv3d module(s) not covered by the tensor-core kernels, left as is: "
-                   + "; ".join(skipped))
-    return model
+                for p in (0, 1):
+                    yield block.convolution_paths[p], "1", block.convolution_paths[p][1], f"block {i} path {p}"
+    return _swap(model, slots, TensorCoreCausalConv3d, module_reason, TensorCoreCausalConv3d,
+                 "fiery_b200: CausalConv3d module(s) not covered by the tensor-core kernels, left as is: ")
 
 
 def use_tensor_core_pyramid_pooling(model):
@@ -205,24 +205,13 @@ def use_tensor_core_pyramid_pooling(model):
     ``use_tensor_core_temporal_model`` and ``use_tensor_core_causal_convs``.  Returns the model; a second call does nothing, and a
     pooling that does not cover the whole map (several pool sizes, a kernel other than (2, X, Y)) is left alone with one warning."""
     from .temporal import TensorCorePyramidPooling, pooling_reason
-    blocks = getattr(model.temporal_model, "model", None)
-    if blocks is None:
-        return model
-    skipped = []
-    for i, block in enumerate(blocks):
-        if type(block).__name__ not in ("TemporalBlock", "TensorCoreTemporalBlock") or not getattr(block, "use_pyramid_pooling", False):
-            continue
-        if isinstance(block.pyramid_pooling, TensorCorePyramidPooling):
-            continue
-        reason = pooling_reason(block.pyramid_pooling)
-        if reason is None:
-            block.pyramid_pooling = TensorCorePyramidPooling(block.pyramid_pooling)
-        else:
-            skipped.append(f"block {i}: {reason}")
-    if skipped:
-        _warn_once(("pyramid", tuple(skipped)), "fiery_b200: pyramid pooling(s) not covered by the spatial-sums kernel, left as is: "
-                   + "; ".join(skipped))
-    return model
+
+    def slots(blocks):
+        for i, _, block in _blocks(blocks, *_TEMPORAL_BLOCKS):
+            if getattr(block, "use_pyramid_pooling", False):
+                yield block, "pyramid_pooling", block.pyramid_pooling, f"block {i}"
+    return _swap(model, slots, TensorCorePyramidPooling, pooling_reason, TensorCorePyramidPooling,
+                 "fiery_b200: pyramid pooling(s) not covered by the spatial-sums kernel, left as is: ")
 
 
 def use_fused_batch_norm(model):
@@ -234,23 +223,20 @@ def use_fused_batch_norm(model):
     one warning: cross-rank statistics are not covered.  Works before or after the other temporal swaps; a second call does nothing.
     Returns the model."""
     from .batch_norm import FusedBatchNorm3d
-    blocks = getattr(model.temporal_model, "model", None)
-    if blocks is None:
-        return model
-    slots = [(parent, key, child, f"{name}.{key}" if name else key)
-             for name, parent in blocks.named_modules() for key, child in parent.named_children()]
-    synced, fused = [], {}                           # fused: id of a replaced norm -> its FusedBatchNorm3d (one per module)
-    for parent, key, child, where in slots:
-        if "pyramid_pooling" in where.split("."):
-            continue
-        if type(child) is torch.nn.BatchNorm3d:
-            setattr(parent, key, fused.setdefault(id(child), FusedBatchNorm3d(child)))
-        elif isinstance(child, torch.nn.SyncBatchNorm):
-            synced.append(where)
-    if synced:
-        _warn_once(("batch_norm", tuple(synced)), "fiery_b200: SyncBatchNorm module(s) left as they are (the fused batch norm computes "
-                   "per-rank statistics only): " + ", ".join(synced))
-    return model
+
+    def slots(blocks):
+        for name, parent in blocks.named_modules():
+            for key, child in parent.named_children():
+                where = f"{name}.{key}" if name else key
+                if "pyramid_pooling" not in where.split(".") and (type(child) is torch.nn.BatchNorm3d
+                                                                  or isinstance(child, torch.nn.SyncBatchNorm)):
+                    yield parent, key, child, where
+
+    def reason(norm):
+        return "per-rank statistics" if isinstance(norm, torch.nn.SyncBatchNorm) else None
+    # the warning's text gives the one reason, so it lists the skipped norms by name only
+    return _swap(model, slots, FusedBatchNorm3d, reason, FusedBatchNorm3d, "fiery_b200: SyncBatchNorm module(s) left as they are (the "
+                 "fused batch norm computes per-rank statistics only): ", entry="{where}", sep=", ")
 
 
 def uninstall():

@@ -23,7 +23,6 @@ vector as a per-(frame, output channel) bias, so neither the concat nor the broa
 """
 from __future__ import annotations
 
-import warnings
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -32,12 +31,10 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import ops as _ops  # noqa: F401  (registers torch.ops.fiery_b200.temporal_entry)
-from ._lib import _require_cuda, f32
+from ._lib import _require_cuda, f32, f32_planes, warn_once
 from .batch_norm import norm_act
 
 MAX_IN_CHANNELS, MAX_OUT_CHANNELS, MAX_EXTRA_CHANNELS = 128, 256, 8
-_warned_pixels = set()
-_warned = set()
 
 
 def _round8(n: int) -> int:
@@ -180,8 +177,7 @@ def entry_backward_weight(grads: Sequence[torch.Tensor], x: torch.Tensor, weight
     gs = [f32(g) for g in grads]
     e = f32(extra.detach()) if E and extra is not None else None
     d = _desc(xs, seg, E)
-    need = int(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d))
-    ws = torch.empty(max(need, 16), dtype=torch.uint8, device=x.device)
+    ws = _lib.workspace(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d), x.device)
     gw = torch.empty((sum(seg), K + E), dtype=torch.float32, device=x.device)
     _lib.call("fiery_temporal_entry_backward_weight", x.device, d, xs.data_ptr(), e.data_ptr() if e is not None else 0, _ptrs(gs),
               gw.data_ptr(), ws.data_ptr())
@@ -196,8 +192,7 @@ def spatial_sums(x: torch.Tensor) -> torch.Tensor:
     Read as it lies when x is fp32 with contiguous pixel planes (any b / C / s strides), else from a contiguous fp32 copy."""
     _require_cuda(x, "x")
     b, c, s, h, w = x.shape
-    planes_contiguous = (x.stride(4) == 1 or w == 1) and (x.stride(3) == w or h == 1)
-    xs = x if x.dtype == torch.float32 and planes_contiguous else f32(x)
+    xs = f32_planes(x)
     out = torch.empty((b, c, s), dtype=torch.float32, device=x.device)
     d = _lib.SpatialSumsDesc()
     d.batch, d.channels, d.frames, d.pixels = b, c, s, h * w
@@ -282,8 +277,7 @@ def aggregation_backward(grad: torch.Tensor, paths: Sequence[torch.Tensor], weig
             grad_pooled = (wp[None, :, :, None] * sums[:, :, None, :]).sum(1)
         if need_weight:
             ps = [f32(p) for p in paths]
-            ws = torch.empty(max(int(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d)), 16), dtype=torch.uint8,
-                             device=g.device)
+            ws = _lib.workspace(lib.fiery_temporal_entry_backward_weight_workspace_bytes(d), g.device)
             gw = torch.empty((c, n), dtype=torch.float32, device=g.device)
             _lib.call("fiery_temporal_entry_backward_weight", g.device, d, g.data_ptr(), 0, _ptrs(ps), gw.data_ptr(), ws.data_ptr())
             grad_wp = (sums[:, :, None, :] * v[:, None, :, :]).sum((0, 3))
@@ -304,7 +298,7 @@ def block_pixels(block) -> Optional[int]:
     pp = getattr(block, "pyramid_pooling", None) if getattr(block, "use_pyramid_pooling", False) else None
     if pp is None:
         return None
-    k = pp.features[0].avgpool.kernel_size
+    k = _triple(pp.features[0].avgpool.kernel_size)
     return int(k[1]) * int(k[2])
 
 
@@ -386,8 +380,8 @@ class TensorCoreTemporalBlock(nn.Module):
         if aggregation_block_reason(self) is not None:
             return False
         if (h * w) % 4:
-            _warn_once(("aggregation", h * w), f"fiery_b200: TemporalBlock aggregation on X*Y = {h * w} pixels is not covered by the "
-                       "tensor-core kernel (it needs a multiple of 4); it runs as the reference's concat and Conv3d")
+            warn_once(("aggregation", h * w), f"fiery_b200: TemporalBlock aggregation on X*Y = {h * w} pixels is not covered by the "
+                      "tensor-core kernel (it needs a multiple of 4); it runs as the reference's concat and Conv3d")
             return False
         return True
 
@@ -397,11 +391,8 @@ class TensorCoreTemporalBlock(nn.Module):
         pixels = x.shape[3] * x.shape[4]
         if pixels % 4:
             # only a block without pyramid pooling reaches this: install() checks the map size through its pooling kernel
-            if pixels not in _warned_pixels:
-                _warned_pixels.add(pixels)
-                warnings.warn(f"fiery_b200: TemporalBlock input of X*Y = {pixels} pixels is not covered by the tensor-core kernels "
-                              "(they need a multiple of 4); its 1x1x1 convolutions run as the reference's Conv3d", RuntimeWarning,
-                              stacklevel=2)
+            warn_once(("entry_pixels", pixels), f"fiery_b200: TemporalBlock input of X*Y = {pixels} pixels is not covered by the "
+                      "tensor-core kernels (they need a multiple of 4); its 1x1x1 convolutions run as the reference's Conv3d")
             ys = [c(x) for c in convs]
         else:
             ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in convs], None)
@@ -416,44 +407,45 @@ class TensorCoreTemporalBlock(nn.Module):
         if self.projection is None:
             raise ValueError("the folded form needs a block with a projection: the skip would add the concatenated input")
         ys = torch.ops.fiery_b200.temporal_entry(x, [c.weight for c in self._entry_convs()], extra)
-        pooled = None
+        if not self.use_pyramid_pooling:
+            return self._tail(x, ys, None)
         h, w = x.shape[3], x.shape[4]
-        if self.use_pyramid_pooling and isinstance(self.pyramid_pooling, TensorCorePyramidPooling) and self.pyramid_pooling.covers(h, w):
-            vector = self.pyramid_pooling.vector(torch.cat([spatial_means(x), extra.float().permute(0, 2, 1)], dim=1))
-            if self._folds_pooling(h, w):
-                return self._tail(x, ys, None, vector)
-            pooled = vector[..., None, None].expand(*vector.shape, h, w)
-        elif self.use_pyramid_pooling:
-            means = torch.cat([x.float().mean(dim=(3, 4)), extra.float().permute(0, 2, 1)], dim=1)
-            pooled = _pyramid_from_means(self.pyramid_pooling, means, x.shape[3], x.shape[4])
-        return self._tail(x, ys, pooled)
-
-
-def _pyramid_from_means(pp, means: torch.Tensor, h: int, w: int) -> torch.Tensor:
-    """PyramidSpatioTemporalPooling (temporal.py:152-178) for pool sizes that cover the whole (h, w) map, from the input's per-frame
-    spatial means (b, C, s): the spatial average is the mean itself, the temporal window (2, padding 1, not counting the pad) and
-    the 1x1x1 conv / bn / relu run on (b, C, s + 1, 1, 1), and the bilinear upsampling of a 1x1 map is a broadcast."""
-    b, _, s = means.shape
-    out = []
-    for f in pp.features:
-        k = tuple(f.avgpool.kernel_size)
-        if k[1:] != (h, w):
+        pp = self.pyramid_pooling
+        k = _uncovered_kernel(pp.features, h, w)
+        if k is not None:
             raise ValueError(f"pyramid pooling kernel {k} does not cover the {h}x{w} map; the folded form needs one that does")
-        pooled = F.avg_pool3d(means[..., None, None], (2, 1, 1), stride=1, padding=(1, 0, 0), count_include_pad=False)
-        y = f.conv_bn_relu(pooled)[:, :, :-1]
-        out.append(y.expand(b, y.shape[1], s, h, w))
-    return torch.cat(out, 1)
-
-
-def _warn_once(key, msg: str) -> None:
-    if key not in _warned:
-        _warned.add(key)
-        warnings.warn(msg, RuntimeWarning, stacklevel=3)
+        # the swapped pooling's means come from the spatial-sums kernel, as in its unfolded forward; the reference pooling's from torch
+        swapped = isinstance(pp, TensorCorePyramidPooling)
+        means = spatial_means(x) if swapped else x.float().mean(dim=(3, 4))
+        vector = pyramid_vector(pp.features, torch.cat([means, extra.float().permute(0, 2, 1)], dim=1))
+        if swapped and self._folds_pooling(h, w):
+            return self._tail(x, ys, None, vector)
+        return self._tail(x, ys, vector[..., None, None].expand(*vector.shape, h, w))
 
 
 def spatial_means(x: torch.Tensor) -> torch.Tensor:
     """(b, C, s, X, Y) -> (b, C, s) fp32 means over each pixel plane (``torch.ops.fiery_b200.spatial_sums`` / X*Y)."""
     return torch.ops.fiery_b200.spatial_sums(x) / (x.shape[3] * x.shape[4])
+
+
+def _triple(v) -> Tuple[int, int, int]:
+    """An ``AvgPool3d`` size as given (an int or a sequence) -> its (t, X, Y) tuple."""
+    return tuple(v) if isinstance(v, (tuple, list)) else (v,) * 3
+
+
+def _uncovered_kernel(features, h: int, w: int) -> Optional[Tuple[int, int, int]]:
+    """The kernel of the first pool in ``features`` that does not span the whole h x w map, or None if every pool does."""
+    return next((k for k in (_triple(f.avgpool.kernel_size) for f in features) if k[1:] != (h, w)), None)
+
+
+def pyramid_vector(features, means: torch.Tensor) -> torch.Tensor:
+    """The pyramid pooling of pools that each span the whole map, as the (b, R, s) vector of its values per frame, from the input's
+    spatial means (b, C, s).  The 2-frame window averages frames t - 1 and t, and frame 0 alone (the pad is not counted); each pool's
+    own ``conv_bn_relu`` runs on the (b, C, s + 1, 1, 1) window, whose extra last step (frame s - 1 alone) goes through BN with the
+    others and is then dropped; the pools' outputs are concatenated over channels.  The bilinear upsampling of a 1x1 map that the
+    reference applies next is a broadcast of this vector."""
+    window = torch.cat([means[..., :1], (means[..., :-1] + means[..., 1:]) / 2, means[..., -1:]], dim=2)[..., None, None]
+    return torch.cat([f.conv_bn_relu(window)[:, :, :-1, 0, 0] for f in features], 1)
 
 
 def pooling_reason(pp) -> Optional[str]:
@@ -468,9 +460,7 @@ def pooling_reason(pp) -> Optional[str]:
     ap = getattr(feats[0], "avgpool", None)
     if not isinstance(ap, nn.AvgPool3d) or not hasattr(feats[0], "conv_bn_relu"):
         return f"{feats[0]} is not an AvgPool3d followed by conv_bn_relu"
-    k = tuple(ap.kernel_size) if isinstance(ap.kernel_size, (tuple, list)) else (ap.kernel_size,) * 3
-    stride = tuple(ap.stride) if isinstance(ap.stride, (tuple, list)) else (ap.stride,) * 3
-    padding = tuple(ap.padding) if isinstance(ap.padding, (tuple, list)) else (ap.padding,) * 3
+    k, stride, padding = _triple(ap.kernel_size), _triple(ap.stride), _triple(ap.padding)
     if (k[0] != 2 or stride != (1, k[1], k[2]) or padding != (1, 0, 0) or ap.count_include_pad or ap.ceil_mode
             or ap.divisor_override is not None):
         return f"pool {ap} is not the (2, X, Y) window with stride (1, X, Y) and one uncounted frame of padding"
@@ -514,21 +504,18 @@ class TensorCorePyramidPooling(nn.Module):
         return cls(pp)
 
     def covers(self, h: int, w: int) -> bool:
-        k = self.features[0].avgpool.kernel_size
-        return tuple(k)[1:] == (h, w) if isinstance(k, (tuple, list)) else (k, k) == (h, w)
+        return _uncovered_kernel(self.features, h, w) is None
 
     def vector(self, means: torch.Tensor) -> torch.Tensor:
-        """(b, C, s) spatial means -> the (b, R, s) pooled vector.  The window averages frames t - 1 and t, and frame 0 alone (the pad
-        is not counted); the reference's extra last step (frame s - 1 alone) goes through BN with the others and is then dropped."""
-        window = torch.cat([means[..., :1], (means[..., :-1] + means[..., 1:]) / 2, means[..., -1:]], dim=2)
-        return self.features[0].conv_bn_relu(window[..., None, None])[:, :, :-1, 0, 0]
+        """(b, C, s) spatial means -> the (b, R, s) pooled vector (``pyramid_vector``)."""
+        return pyramid_vector(self.features, means)
 
     def forward(self, *inputs):
         (x,) = inputs
         b, _, s, h, w = x.shape
         if not self.covers(h, w):
-            _warn_once(("pooling", h, w), f"fiery_b200: pyramid pooling {tuple(self.features[0].avgpool.kernel_size)} does not cover "
-                       f"the {h}x{w} map; it runs as the reference's average pool and bilinear upsampling")
+            warn_once(("pooling", h, w), f"fiery_b200: pyramid pooling {_triple(self.features[0].avgpool.kernel_size)} does not cover "
+                      f"the {h}x{w} map; it runs as the reference's average pool and bilinear upsampling")
             out = []
             for f in self.features:
                 y = f(x)[:, :, :-1].contiguous()

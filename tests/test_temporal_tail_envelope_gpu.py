@@ -306,8 +306,7 @@ def test_uncovered_pixel_count_runs_the_concat_aggregation_with_one_warning(monk
     """A model built for a 51 x 49 map: the pooling covers the map, but X*Y = 2499 is not a multiple of 4.  install leaves the blocks
     to the reference (the entry needs the same multiple), so a block adopted by the bare constructor is what reaches the
     aggregation's own check: it warns once and runs the concat and Conv3d, and the step still matches fp64."""
-    for mod, name in ((temporal, "_warned"), (temporal, "_warned_pixels"), (install, "_warned")):
-        monkeypatch.setattr(mod, name, set())
+    monkeypatch.setattr(_lib, "_warned", set())
     grid = (51, 49)
     ref = _model(3, 0, seed=5, grid=grid)
     sw = copy.deepcopy(ref)
@@ -418,7 +417,7 @@ WIDE_GRID = (50, 52)          # 2600 pixels: a partial last tile of 64 and of 12
 @pytest.mark.parametrize("route", ["concat", "folded"])
 @pytest.mark.parametrize("rf,start,extra,covered", WIDE, ids=_ids)
 def test_wide_models_match_oracle(rf, start, extra, covered, route, monkeypatch):
-    monkeypatch.setattr(install, "_warned", set())
+    monkeypatch.setattr(_lib, "_warned", set())
     ref = _model(rf, 0, seed=rf + start, grid=WIDE_GRID, start_out_channels=start, extra_in_channels=extra)
     sw = copy.deepcopy(ref)
     h = _holder(sw)
