@@ -184,10 +184,11 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_apply_kernel(const
     }
 }
 
-// g' = dy where the forward's fmaf(scale, x, shift) was > 0 (ReLU fused), dy otherwise
+// g' = dy where the forward's fmaf(scale, x, shift) was not <= 0 (ReLU fused; a NaN passes, as torch's threshold_backward lets it),
+// dy otherwise
 template <bool RELU>
 __device__ __forceinline__ float bn_masked(float dy, float x, float scale, float shift) {
-    return RELU ? (fmaf(scale, x, shift) > 0.f ? dy : 0.f) : dy;
+    return RELU ? (fmaf(scale, x, shift) <= 0.f ? 0.f : dy) : dy;
 }
 
 template <bool RELU>

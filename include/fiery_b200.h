@@ -442,7 +442,8 @@ FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc
  *   scale = weight[c] / sqrt(var + eps), shift = bias[c] - mean * scale, in fp64 from the fp32 mean and var, rounded once
  *   (weight NULL: 1; bias NULL: 0);
  *   y = fmaf(scale, x, shift), then max(y, 0) when relu (a NaN stays NaN), then + residual when residual is not NULL.
- * The backward, with g' = grad_y where the forward's fmaf(scale, x, shift) > 0 (relu) or g' = grad_y (no relu), and
+ * The backward, with g' = grad_y where the forward's fmaf(scale, x, shift) is not <= 0 (relu; a NaN passes, as torch's
+ * threshold_backward), 0 where it is, or g' = grad_y (no relu), and
  * S1 = sum g', S2 = sum g' (x - mean):
  *   grad_bias = S1, grad_weight = S2 / sqrt(var + eps);
  *   training: grad_x = scale * (g' - S1 / n - (x - mean) * S2 / (n * (var + eps)));  eval: grad_x = scale * g'.
