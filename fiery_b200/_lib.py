@@ -78,6 +78,23 @@ class BatchNormDesc(ctypes.Structure):
     ]
 
 
+class SpatialGruDesc(ctypes.Structure):
+    """Mirror of ``fiery_spatial_gru_desc_t``."""
+
+    _fields_ = [
+        ("batch", c_int32), ("frames", c_int32), ("x_frames", c_int32), ("grid_x", c_int32), ("grid_y", c_int32),
+        ("x_channels", c_int32), ("h_channels", c_int32),
+        ("x_stride_b", c_int64), ("x_stride_t", c_int64), ("x_stride_c", c_int64),
+        ("training", c_int32), ("eps", c_double), ("bias_init", c_float),
+    ]
+
+
+class Conv3x3Desc(ctypes.Structure):
+    """Mirror of ``fiery_conv3x3_desc_t``."""
+
+    _fields_ = [("maps", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("in_channels", c_int32 * 2), ("out_channels", c_int32 * 2)]
+
+
 # name -> (restype, argtypes); every symbol include/fiery_b200.h declares
 SIGNATURES = {
     "fiery_abi_version": (c_int32, []),
@@ -138,6 +155,19 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_batch_norm_backward": (c_int32, [POINTER(BatchNormDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_spatial_gru_packed_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),
+    "fiery_spatial_gru_pack_weights": (c_int32, [POINTER(SpatialGruDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_spatial_gru_saved_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),
+    "fiery_spatial_gru_forward_workspace_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),
+    "fiery_spatial_gru_forward": (c_int32, [POINTER(SpatialGruDesc)] + [c_void_p] * 14),
+    "fiery_spatial_gru_backward_workspace_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),
+    "fiery_spatial_gru_backward": (c_int32, [POINTER(SpatialGruDesc)] + [c_void_p] * 19),
+    "fiery_conv3x3_packed_bytes": (c_size_t, [POINTER(Conv3x3Desc)]),
+    "fiery_conv3x3_pack_weights": (c_int32, [POINTER(Conv3x3Desc), c_void_p, c_void_p, c_void_p]),
+    "fiery_conv3x3_forward": (c_int32, [POINTER(Conv3x3Desc)] + [c_void_p] * 6),
+    "fiery_conv3x3_backward_data": (c_int32, [POINTER(Conv3x3Desc)] + [c_void_p] * 6),
+    "fiery_conv3x3_backward_weight_workspace_bytes": (c_size_t, [POINTER(Conv3x3Desc)]),
+    "fiery_conv3x3_backward_weight": (c_int32, [POINTER(Conv3x3Desc)] + [c_void_p] * 6),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

@@ -133,22 +133,27 @@ class FusedBatchNorm3d(nn.BatchNorm3d):
         return y
 
     def update_running_stats(self, mean: torch.Tensor, var: torch.Tensor, n: int) -> None:
-        """``_BatchNorm.forward``'s bookkeeping for a batch of n values per channel with this mean and biased variance, as device
-        tensor operations: nothing in training without tracked statistics, else ``num_batches_tracked += 1`` and each running
-        statistic moved toward the batch's by the momentum (``1 / num_batches_tracked`` when the momentum is None), the variance
-        as the unbiased n / (n - 1) var."""
-        if not (self.training and self.track_running_stats):
+        """``update_running_stats(self, mean, var, n)``."""
+        update_running_stats(self, mean, var, n)
+
+
+def update_running_stats(bn: nn.Module, mean: torch.Tensor, var: torch.Tensor, n: int) -> None:
+    """``_BatchNorm.forward``'s bookkeeping on the norm ``bn`` for a batch of n values per channel with this mean and biased variance,
+    as device tensor operations: nothing in eval or without tracked statistics, else ``num_batches_tracked += 1`` and each running
+    statistic moved toward the batch's by the momentum (``1 / num_batches_tracked`` when the momentum is None), the variance as the
+    unbiased n / (n - 1) var.  ``FusedBatchNorm3d`` calls it once per forward, the spatial GRU once per step."""
+    if not (bn.training and bn.track_running_stats):
+        return
+    with torch.no_grad():
+        factor = 0.0 if bn.momentum is None else bn.momentum
+        if bn.num_batches_tracked is not None:
+            bn.num_batches_tracked.add_(1)
+            if bn.momentum is None and bn.running_mean is not None:
+                factor = bn.num_batches_tracked.to(bn.running_mean.dtype).reciprocal()
+        if bn.running_mean is None:
             return
-        with torch.no_grad():
-            factor = 0.0 if self.momentum is None else self.momentum
-            if self.num_batches_tracked is not None:
-                self.num_batches_tracked.add_(1)
-                if self.momentum is None and self.running_mean is not None:
-                    factor = self.num_batches_tracked.to(self.running_mean.dtype).reciprocal()
-            if self.running_mean is None:
-                return
-            self.running_mean.lerp_(mean.to(self.running_mean.dtype), factor)
-            self.running_var.lerp_(var.to(self.running_var.dtype) * (n / (n - 1)), factor)
+        bn.running_mean.lerp_(mean.to(bn.running_mean.dtype), factor)
+        bn.running_var.lerp_(var.to(bn.running_var.dtype) * (n / (n - 1)), factor)
 
 
 def norm_act(norm: nn.Module, activation: nn.Module, y: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:

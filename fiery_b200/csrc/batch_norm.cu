@@ -364,4 +364,125 @@ int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x,
     return FIERY_OK;
 }
 
+// ------------------------------------------------------------------------------------------------------------------------------
+// The spatial GRU's state update (spatial_gru.cu) on one step's s (batch, channels, 1, X, Y): the statistics and finalize above, then
+//   h' = (1 - u) h + u max(fmaf(scale, s, shift), 0)
+// written straight to the output frame; its backward from dh' = grad_out + carry gives
+//   da = u dh' (then the BN + ReLU backward above on (s, da)), dG_u = dh' (a - h) u (1 - u), carry = (1 - u) dh'.
+// u and carry lie like s; h and the output frame have contiguous planes X*Y apart and their own batch strides.
+// ------------------------------------------------------------------------------------------------------------------------------
+struct GruPieceAt {
+    long long b, pix;                                          // batch element, first pixel of the piece
+};
+__device__ __forceinline__ GruPieceAt gru_piece_at(const BnShape& s, long long g) {
+    const long long plane = g / s.per_plane;
+    GruPieceAt r;
+    r.b = plane / s.channels;
+    r.pix = (g - plane * s.per_plane) * BN_PIECE;
+    return r;
+}
+
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) gru_blend_kernel(const BnShape s, const float* __restrict__ x, const BnCoef* __restrict__ coef,
+                                                               const float* __restrict__ u, const float* __restrict__ h, long long hsb,
+                                                               float* __restrict__ out, long long osb) {
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const GruPieceAt at = gru_piece_at(s, g);
+        const long long hw = static_cast<long long>(p.c) * s.pixels + at.pix;
+        const float* xp = x + p.x_off;
+        const float* up = u + p.x_off;
+        const float* hp = h + at.b * hsb + hw;
+        float* op = out + at.b * osb + hw;
+        const bool vx = aligned16_ptr(xp), vu = aligned16_ptr(up), vh = aligned16_ptr(hp), vo = aligned16_ptr(op);
+        const float scale = coef[p.c].scale, shift = coef[p.c].shift;
+        const int n_chunks = (p.n + 3) / 4;
+#pragma unroll
+        for (int k = 0; k < BN_CHUNKS; ++k) {
+            const int q = threadIdx.x + k * BN_THREADS;
+            if (q >= n_chunks) continue;
+            const float4 v = load_chunk4(xp, q, p.n, vx), uu = load_chunk4(up, q, p.n, vu), hh = load_chunk4(hp, q, p.n, vh);
+            const float vs[4] = {v.x, v.y, v.z, v.w}, us[4] = {uu.x, uu.y, uu.z, uu.w}, hs[4] = {hh.x, hh.y, hh.z, hh.w};
+            float o[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float a = fmaf(scale, vs[e], shift);
+                a = a < 0.f ? 0.f : a;                         // a NaN passes, as torch's ReLU lets it
+                o[e] = (1.f - us[e]) * hs[e] + us[e] * a;
+            }
+            store_chunk4(op, q, p.n, vo, make_float4(o[0], o[1], o[2], o[3]));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) gru_blend_grad_kernel(const BnShape s, const float* __restrict__ x, const float* __restrict__ w,
+                                                                    const float* __restrict__ bias, const float* __restrict__ mean,
+                                                                    const float* __restrict__ var, double eps, const float* __restrict__ u,
+                                                                    const float* __restrict__ h, long long hsb, const float* __restrict__ go,
+                                                                    long long gsb, float* __restrict__ carry, float* __restrict__ da,
+                                                                    float* __restrict__ dgu, long long dsb) {
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const GruPieceAt at = gru_piece_at(s, g);
+        const long long hw = static_cast<long long>(p.c) * s.pixels + at.pix;
+        float scale, shift;
+        bn_scale_shift(w, bias, mean[p.c], var[p.c], eps, p.c, scale, shift);
+        const float* xp = x + p.x_off;
+        const float* up = u + p.x_off;
+        float* cp = carry + p.x_off;
+        float* ap = da + p.x_off;
+        const float* hp = h + at.b * hsb + hw;
+        const float* gp = go + at.b * gsb + hw;
+        float* dp = dgu + at.b * dsb + hw;
+        const bool vx = aligned16_ptr(xp), vu = aligned16_ptr(up), vc = aligned16_ptr(cp), va = aligned16_ptr(ap);
+        const bool vh = aligned16_ptr(hp), vg = aligned16_ptr(gp), vd = aligned16_ptr(dp);
+        const int n_chunks = (p.n + 3) / 4;
+#pragma unroll
+        for (int k = 0; k < BN_CHUNKS; ++k) {
+            const int q = threadIdx.x + k * BN_THREADS;
+            if (q >= n_chunks) continue;
+            const float4 v = load_chunk4(xp, q, p.n, vx), uu = load_chunk4(up, q, p.n, vu), hh = load_chunk4(hp, q, p.n, vh);
+            const float4 gg = load_chunk4(gp, q, p.n, vg), cc = load_chunk4(cp, q, p.n, vc);
+            const float vs[4] = {v.x, v.y, v.z, v.w}, us[4] = {uu.x, uu.y, uu.z, uu.w}, hs[4] = {hh.x, hh.y, hh.z, hh.w};
+            const float gs[4] = {gg.x, gg.y, gg.z, gg.w}, cs[4] = {cc.x, cc.y, cc.z, cc.w};
+            float oa[4], od[4], oc[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float a = fmaf(scale, vs[e], shift);
+                a = a < 0.f ? 0.f : a;
+                const float dh = gs[e] + cs[e];
+                oa[e] = us[e] * dh;
+                od[e] = dh * (a - hs[e]) * (us[e] * (1.f - us[e]));
+                oc[e] = (1.f - us[e]) * dh;
+            }
+            store_chunk4(ap, q, p.n, va, make_float4(oa[0], oa[1], oa[2], oa[3]));
+            store_chunk4(dp, q, p.n, vd, make_float4(od[0], od[1], od[2], od[3]));
+            store_chunk4(cp, q, p.n, vc, make_float4(oc[0], oc[1], oc[2], oc[3]));
+        }
+    }
+}
+
+int launch_gru_blend_forward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
+                             const float* running_var, const float* u, const float* h, long long hsb, float* out, long long osb,
+                             float* mean_out, float* var_out, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
+    if (d->training) bn_stats_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, part);
+    bn_finalize_forward_kernel<<<fin, 128, 0, stream>>>(s, part, w, bias, running_mean, running_var, d->training, d->eps, mean_out, var_out,
+                                                         coef);
+    gru_blend_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, coef, u, h, hsb, out, osb);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_gru_blend_backward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* mean,
+                              const float* var, const float* u, const float* h, long long hsb, const float* go, long long gsb, float* carry,
+                              float* da, float* dgu, long long dsb, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    gru_blend_grad_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, w, bias, mean, var, d->eps, u, h, hsb, go, gsb, carry, da, dgu, dsb);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
 }  // namespace fiery

@@ -123,6 +123,24 @@ size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d
 int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
                                 float* gw, void* workspace, cudaStream_t stream);
 size_t causal_conv_packed_bytes(const fiery_causal_conv3d_desc_t* d);
+size_t conv3x3_packed_bytes(const fiery_conv3x3_desc_t* d);
+int launch_conv3x3_pack(const fiery_conv3x3_desc_t* d, const float* w, float* packed, cudaStream_t stream);
+int launch_conv3x3(const fiery_conv3x3_desc_t* d, int dgrad, const float* in0, const float* in1, const float* packed, float* out0,
+                   float* out1, cudaStream_t stream);
+size_t conv3x3_wgrad_workspace_bytes(const fiery_conv3x3_desc_t* d);
+int launch_conv3x3_wgrad(const fiery_conv3x3_desc_t* d, const float* x0, const float* x1, const float* gy, float* gw, void* workspace,
+                         cudaStream_t stream);
+size_t spatial_gru_packed_bytes(const fiery_spatial_gru_desc_t* d);
+int launch_spatial_gru_pack(const fiery_spatial_gru_desc_t* d, const float* w_gates, const float* w_state, float* packed, cudaStream_t stream);
+size_t spatial_gru_forward_workspace_bytes(const fiery_spatial_gru_desc_t* d);
+int launch_spatial_gru_forward(const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* packed, const float* b_gates,
+                               const float* bn_w, const float* bn_b, const float* running_mean, const float* running_var, float* out,
+                               float* saved, float* means, float* vars, void* workspace, cudaStream_t stream);
+size_t spatial_gru_backward_workspace_bytes(const fiery_spatial_gru_desc_t* d);
+int launch_spatial_gru_backward(const fiery_spatial_gru_desc_t* d, const float* grad_out, const float* x, const float* h0, const float* out,
+                                const float* saved_c, const float* means, const float* vars, const float* packed, const float* bn_w,
+                                const float* bn_b, float* grad_x, float* grad_h0, float* grad_w_gates, float* grad_b_gates,
+                                float* grad_w_state, float* grad_bn_w, float* grad_bn_b, void* workspace, cudaStream_t stream);
 size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d);
 int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
                               const float* running_var, const float* residual, float* y, float* mean_out, float* var_out,
@@ -684,6 +702,157 @@ FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, con
     FIERY_REQUIRE(aligned16(workspace), "batch norm: workspace must be 16-byte aligned");
     return launch_batch_norm_backward(desc, x, grad_y, weight, bias, mean, var, grad_x, grad_weight, grad_bias, workspace,
                                       static_cast<cudaStream_t>(stream));
+}
+
+// The spatial GRU's shape limits, one place for every entry point.  The messages name the field.
+static int check_spatial_gru_desc(const fiery_spatial_gru_desc_t* d) {
+    FIERY_REQUIRE(d, "spatial GRU: NULL desc");
+    FIERY_REQUIRE(d->batch >= 1 && d->frames >= 1, "spatial GRU: batch = %d, frames = %d must be >= 1", d->batch, d->frames);
+    FIERY_REQUIRE(d->x_frames == 1 || d->x_frames == d->frames, "spatial GRU: x_frames = %d must be 1 or frames = %d", d->x_frames, d->frames);
+    FIERY_REQUIRE(d->x_channels >= 1 && d->x_channels <= 64, "spatial GRU: x_channels = %d must be in 1..64", d->x_channels);
+    FIERY_REQUIRE(d->h_channels >= 1 && d->h_channels <= 64, "spatial GRU: h_channels = %d must be in 1..64", d->h_channels);
+    FIERY_REQUIRE(d->grid_x >= 1, "spatial GRU: grid_x = %d must be >= 1", d->grid_x);
+    FIERY_REQUIRE(d->grid_y >= 1 && d->grid_y % 4 == 0, "spatial GRU: grid_y = %d must be a positive multiple of 4 (16-byte TMA row pitch)",
+                  d->grid_y);
+    FIERY_REQUIRE(d->x_stride_b >= 0 && d->x_stride_t >= 0 && d->x_stride_c >= 0 && d->x_stride_b % 4 == 0 && d->x_stride_t % 4 == 0 &&
+                      d->x_stride_c % 4 == 0,
+                  "spatial GRU: x strides (%lld, %lld, %lld) must be non-negative multiples of 4 elements", (long long)d->x_stride_b,
+                  (long long)d->x_stride_t, (long long)d->x_stride_c);
+    FIERY_REQUIRE(d->training == 0 || d->training == 1, "spatial GRU: training = %d must be 0 or 1", d->training);
+    FIERY_REQUIRE(d->eps >= 0.0, "spatial GRU: eps = %g must be >= 0", d->eps);
+    FIERY_REQUIRE(!d->training || static_cast<long long>(d->batch) * d->grid_x * d->grid_y >= 2,
+                  "spatial GRU: batch * X * Y must be >= 2 in training");
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_spatial_gru_packed_bytes(const fiery_spatial_gru_desc_t* desc) {
+    if (check_spatial_gru_desc(desc) != FIERY_OK) return 0;
+    return spatial_gru_packed_bytes(desc);
+}
+
+FIERY_API int fiery_spatial_gru_pack_weights(const fiery_spatial_gru_desc_t* desc, const float* w_gates, const float* w_state, void* packed,
+                                             void* stream) {
+    const int rc = check_spatial_gru_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(w_gates && w_state && packed, "spatial GRU: NULL weight pointer");
+    FIERY_REQUIRE(aligned16(packed), "spatial GRU: packed weights must be 16-byte aligned");
+    return launch_spatial_gru_pack(desc, w_gates, w_state, static_cast<float*>(packed), static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_spatial_gru_saved_bytes(const fiery_spatial_gru_desc_t* desc) {
+    if (check_spatial_gru_desc(desc) != FIERY_OK) return 0;
+    return 4 * sizeof(float) * static_cast<size_t>(desc->frames) * desc->batch * desc->h_channels * desc->grid_x * desc->grid_y;
+}
+
+FIERY_API size_t fiery_spatial_gru_forward_workspace_bytes(const fiery_spatial_gru_desc_t* desc) {
+    if (check_spatial_gru_desc(desc) != FIERY_OK) return 0;
+    return spatial_gru_forward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_spatial_gru_forward(const fiery_spatial_gru_desc_t* desc, const float* x, const float* h0, const void* packed,
+                                        const float* b_gates, const float* bn_weight, const float* bn_bias, const float* running_mean,
+                                        const float* running_var, float* out, void* saved, float* means, float* vars, void* workspace,
+                                        void* stream) {
+    const int rc = check_spatial_gru_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(x && h0 && packed && b_gates && out && saved && means && vars && workspace, "spatial GRU: NULL pointer");
+    FIERY_REQUIRE(desc->training || (running_mean && running_var), "spatial GRU: eval mode needs running_mean and running_var");
+    FIERY_REQUIRE(aligned16(x) && aligned16(h0) && aligned16(packed) && aligned16(out) && aligned16(saved) && aligned16(workspace),
+                  "spatial GRU: pointers must be 16-byte aligned");
+    return launch_spatial_gru_forward(desc, x, h0, static_cast<const float*>(packed), b_gates, bn_weight, bn_bias,
+                                      desc->training ? nullptr : running_mean, desc->training ? nullptr : running_var, out,
+                                      static_cast<float*>(saved), means, vars, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_spatial_gru_backward_workspace_bytes(const fiery_spatial_gru_desc_t* desc) {
+    if (check_spatial_gru_desc(desc) != FIERY_OK) return 0;
+    return spatial_gru_backward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_spatial_gru_backward(const fiery_spatial_gru_desc_t* desc, const float* grad_out, const float* x, const float* h0,
+                                         const float* out, const void* saved, const float* means, const float* vars, const void* packed,
+                                         const float* bn_weight, const float* bn_bias, float* grad_x, float* grad_h0, float* grad_w_gates,
+                                         float* grad_b_gates, float* grad_w_state, float* grad_bn_weight, float* grad_bn_bias,
+                                         void* workspace, void* stream) {
+    const int rc = check_spatial_gru_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_out && x && h0 && out && saved && means && vars && packed && workspace, "spatial GRU: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_out) && aligned16(x) && aligned16(h0) && aligned16(out) && aligned16(saved) && aligned16(packed) &&
+                      aligned16(workspace) && (!grad_x || aligned16(grad_x)) && (!grad_h0 || aligned16(grad_h0)),
+                  "spatial GRU: pointers must be 16-byte aligned");
+    return launch_spatial_gru_backward(desc, grad_out, x, h0, out, static_cast<const float*>(saved), means, vars,
+                                       static_cast<const float*>(packed), bn_weight, bn_bias, grad_x, grad_h0, grad_w_gates, grad_b_gates,
+                                       grad_w_state, grad_bn_weight, grad_bn_bias, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// The 3x3 convolution's limits, one place for every entry point.  The messages name the field.
+static int check_conv3x3_desc(const fiery_conv3x3_desc_t* d) {
+    FIERY_REQUIRE(d, "3x3 conv: NULL desc");
+    FIERY_REQUIRE(d->maps >= 1, "3x3 conv: maps = %d must be >= 1", d->maps);
+    FIERY_REQUIRE(d->in_channels[0] >= 1 && d->in_channels[0] <= 64, "3x3 conv: in_channels[0] = %d must be in 1..64", d->in_channels[0]);
+    FIERY_REQUIRE(d->in_channels[1] >= 0 && d->in_channels[1] <= 64, "3x3 conv: in_channels[1] = %d must be in 0..64", d->in_channels[1]);
+    FIERY_REQUIRE(d->out_channels[0] >= 1 && d->out_channels[0] <= 64, "3x3 conv: out_channels[0] = %d must be in 1..64",
+                  d->out_channels[0]);
+    FIERY_REQUIRE(d->out_channels[1] >= 0 && d->out_channels[1] <= 64, "3x3 conv: out_channels[1] = %d must be in 0..64",
+                  d->out_channels[1]);
+    FIERY_REQUIRE(d->grid_x >= 1, "3x3 conv: grid_x = %d must be >= 1", d->grid_x);
+    FIERY_REQUIRE(d->grid_y >= 1 && d->grid_y % 4 == 0, "3x3 conv: grid_y = %d must be a positive multiple of 4 (16-byte TMA row pitch)",
+                  d->grid_y);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_conv3x3_packed_bytes(const fiery_conv3x3_desc_t* desc) {
+    if (check_conv3x3_desc(desc) != FIERY_OK) return 0;
+    return conv3x3_packed_bytes(desc);
+}
+
+FIERY_API int fiery_conv3x3_pack_weights(const fiery_conv3x3_desc_t* desc, const float* weight, void* packed, void* stream) {
+    const int rc = check_conv3x3_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(weight && packed && aligned16(packed), "3x3 conv: NULL weight or misaligned pack");
+    return launch_conv3x3_pack(desc, weight, static_cast<float*>(packed), static_cast<cudaStream_t>(stream));
+}
+
+// a segment pair: the first always given, the second when it has channels
+static int check_conv3x3_pair(const int* channels, const float* a, const float* b, const char* what) {
+    FIERY_REQUIRE(a && aligned16(a), "3x3 conv: %s0 is NULL or misaligned", what);
+    FIERY_REQUIRE(!channels[1] || (b && aligned16(b)), "3x3 conv: %s1 is NULL or misaligned", what);
+    return FIERY_OK;
+}
+
+FIERY_API int fiery_conv3x3_forward(const fiery_conv3x3_desc_t* desc, const float* x0, const float* x1, const void* packed, float* y0,
+                                    float* y1, void* stream) {
+    int rc = check_conv3x3_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if ((rc = check_conv3x3_pair(desc->in_channels, x0, x1, "x")) != FIERY_OK) return rc;
+    if ((rc = check_conv3x3_pair(desc->out_channels, y0, y1, "y")) != FIERY_OK) return rc;
+    FIERY_REQUIRE(packed && aligned16(packed), "3x3 conv: NULL or misaligned pack");
+    return launch_conv3x3(desc, 0, x0, x1, static_cast<const float*>(packed), y0, y1, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_conv3x3_backward_data(const fiery_conv3x3_desc_t* desc, const float* grad_y0, const float* grad_y1, const void* packed,
+                                          float* grad_x0, float* grad_x1, void* stream) {
+    int rc = check_conv3x3_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if ((rc = check_conv3x3_pair(desc->out_channels, grad_y0, grad_y1, "grad_y")) != FIERY_OK) return rc;
+    if ((rc = check_conv3x3_pair(desc->in_channels, grad_x0, grad_x1, "grad_x")) != FIERY_OK) return rc;
+    FIERY_REQUIRE(packed && aligned16(packed), "3x3 conv: NULL or misaligned pack");
+    return launch_conv3x3(desc, 1, grad_y0, grad_y1, static_cast<const float*>(packed), grad_x0, grad_x1, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_conv3x3_backward_weight_workspace_bytes(const fiery_conv3x3_desc_t* desc) {
+    if (check_conv3x3_desc(desc) != FIERY_OK) return 0;
+    return conv3x3_wgrad_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_conv3x3_backward_weight(const fiery_conv3x3_desc_t* desc, const float* x0, const float* x1, const float* grad_y,
+                                            float* grad_w, void* workspace, void* stream) {
+    int rc = check_conv3x3_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    if ((rc = check_conv3x3_pair(desc->in_channels, x0, x1, "x")) != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_y && aligned16(grad_y) && grad_w && workspace && aligned16(workspace),
+                  "3x3 conv: NULL or misaligned grad_y / grad_w / workspace");
+    return launch_conv3x3_wgrad(desc, x0, x1, grad_y, grad_w, workspace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

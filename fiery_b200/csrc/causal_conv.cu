@@ -27,30 +27,20 @@
 // operand; the x run of the tap's frame and row is loaded once, 4 columns early and 44 wide, and read as the register A operand at
 // each dx's shift (im2col from shared memory; 44-float rows put a fragment's 8 channels x 4 pixels on 32 banks).  The summation order
 // is wgrad_chunks.cuh's: bit-reproducible, no atomics.
+//
+// Both kernels are written over halo tiles and segments (causal_conv.cuh), so the spatial GRU (spatial_gru.cu) runs its 3x3
+// convolutions on them too: its inputs [x_t, h] are two halo tiles from two tensors, its outputs up to two segments of the accumulator
+// with their own epilogues.  A causal convolution is one map read at kt frame offsets and one stored segment.
+#include "causal_conv.cuh"
 #include "wgmma.cuh"
 #include "wgrad_chunks.cuh"
 
 namespace fiery {
 
-constexpr int CC_TX = 8, CC_TY = 16;               // output tile: rows x columns of the map
-// Every TMA box starts on a 16-byte boundary of the contiguous map row: the column padding comes from a box that starts 4 columns
-// early (zero fill at column -4 .. -1), and the MMA operands are read from it at the tap's shift.
-constexpr int CC_HX = CC_TX + 2, CC_HY = 28;       // halo box: rows x0 - 1 .. x0 + 8, columns y0 - 4 .. y0 + 23 (y0 - 1 .. y0 + 16 used)
 constexpr int CC_HY_OFF = 3;                       // halo column of input column y0 + c + dx - 1 is c + dx + CC_HY_OFF
-constexpr int CC_PLANE = CC_HX * CC_HY;            // floats per channel of a halo tile: 280 = 24 banks apart
-constexpr int CC_WSTAGES = 4;                      // weight-slice ring
 constexpr int CC_FWD_THREADS = 2 * 128 + 32;
-constexpr int CC_WG_PX = 32;                       // weight gradient: pixels per tile
 constexpr int CC_WG_STAGES = 4;
-constexpr int CC_WG_XP = 44;                       // weight gradient x tile: columns 32 run - 4 .. 32 run + 39, 44 = 12 banks apart
 constexpr int CC_WG_X_BYTES = 64 * CC_WG_XP * 4;   // 64 input-channel rows (zero past C_in): 11 KB, a multiple of 1024
-constexpr int CC_SMEM_SLACK = 1024 + 256;
-
-__host__ __device__ __forceinline__ int cc_round8(int v) { return (v + 7) / 8 * 8; }
-
-struct CcShape {
-    int batch, frames, X, Y, cin, cout, kt, taps;
-};
 
 static CcShape cc_shape(const fiery_causal_conv3d_desc_t* d) {
     return CcShape{d->batch, d->frames, d->grid_x, d->grid_y, d->in_channels, d->out_channels, d->kt, 9 * d->kt};
@@ -107,24 +97,47 @@ int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w,
 // ------------------------------------------------------------------------------------------------------------------------------
 // forward and input gradient
 // ------------------------------------------------------------------------------------------------------------------------------
-struct CcFwdMaps {
-    CUtensorMap x;                                 // input (Y, X, s, C, b), box (28, 10, 1, kpad, 1) = CC_HY x CC_HX, no swizzle
-    CUtensorMap w;                                 // pack (32, n, taps * ka), box (32, n, 1), swizzle 128B
-};
-struct CcFwdLaunch {
-    int frames, X, Y, kpad, ka, n_out, kt, t_off, tiles_x, tiles_y;
-};
+// one accumulator value of output segment o, channel ch, at (b, t, pixel pix)
+__device__ __forceinline__ void cc_epilogue(const CcOutSeg& o, float bias_init, size_t plane, int b, int ch, int t, size_t pix, float v) {
+    const size_t cp = static_cast<size_t>(ch) * plane + pix;
+    float* dst = o.p + b * o.sb + ch * o.sc + t * o.st + pix;
+    switch (o.mode) {
+        case CC_STORE: *dst = v; break;
+        case CC_ADD: *dst += v; break;
+        case CC_GATE_U: *dst = 1.f / (1.f + expf(-(v + o.bias[ch] + bias_init))); break;
+        case CC_GATE_R: {
+            const float r = 1.f / (1.f + expf(-(v + o.bias[ch] + bias_init)));
+            o.r[b * o.rsb + cp] = r;
+            *dst = (1.f - r) * o.h[b * o.hsb + cp];
+            break;
+        }
+        case CC_RESET_GRAD: {
+            const float r = o.r[b * o.rsb + cp], h = o.h[b * o.hsb + cp];
+            o.aux[b * o.asb + cp] = -v * h * (r * (1.f - r));
+            *dst += (1.f - r) * v;
+            break;
+        }
+        default: break;
+    }
+}
 
-template <int N>
+// SEG = false: the causal convolution -- kt halo tiles of map 0 with one channel count, a CC_WSTAGES ring, one stored segment; every
+// per-halo quantity is the uniform one, so its instantiations compile to the single-input kernel.  SEG = true: the per-halo maps,
+// channel counts and ring depth of CcFwdLaunch, and the segment epilogues.
+template <int N, bool SEG>
 __global__ void __launch_bounds__(CC_FWD_THREADS, 1)
-causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch L, float* __restrict__ out) {
-    const int w_bytes = L.ka * N * 128;
-    const int x_floats = L.kpad * CC_PLANE;
-    const int taps = 9 * L.kt;
+causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_constant__ CcFwdLaunch L) {
+    const int taps = 9 * L.halos;
+    const int stages = SEG ? L.stages : CC_WSTAGES;
+    const int w_bytes = SEG ? L.stage_bytes : L.ka[0] * N * 128;
+    const int x_floats = L.kpad[0] * CC_PLANE;                    // SEG = false: every halo tile
+    auto kpad_of = [&](int h) { return SEG ? L.kpad[h] : L.kpad[0]; };
+    auto ka_of = [&](int h) { return SEG ? L.ka[h] : L.ka[0]; };
+    auto x_off_of = [&](int h) { return SEG ? L.x_off[h] : h * x_floats; };
     unsigned char* s_w = dynamic_smem_1024();
-    const float* s_x = reinterpret_cast<const float*>(s_w + CC_WSTAGES * w_bytes);
-    uint64_t* x_full = reinterpret_cast<uint64_t*>(const_cast<float*>(s_x) + L.kt * x_floats);
-    const MbarRing ring(x_full + 1, CC_WSTAGES);
+    const float* s_x = reinterpret_cast<const float*>(s_w + stages * w_bytes);
+    uint64_t* x_full = reinterpret_cast<uint64_t*>(const_cast<float*>(s_x) + x_off_of(L.halos - 1) + kpad_of(L.halos - 1) * CC_PLANE);
+    const MbarRing ring(x_full + 1, stages);
 
     int tile = blockIdx.x;
     const int ty = tile % L.tiles_y;
@@ -135,7 +148,8 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 8 && lane == 0) {
-        tma_prefetch_desc(&maps.x);
+        tma_prefetch_desc(&maps.x[0]);
+        if (SEG && L.halos > 1 && L.map[1] != 0) tma_prefetch_desc(&maps.x[1]);
         tma_prefetch_desc(&maps.w);
         mbar_init(x_full, 1);                          // published to the async proxy by the fence in ring.init
         ring.init(8);
@@ -144,12 +158,17 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
 
     if (warp == 8) {
         if (lane == 0) {                               // ===== TMA producer: the halo tiles, then the taps' weight slices =====
-            mbar_arrive_expect_tx(x_full, L.kt * x_floats * 4);
-            for (int jt = 0; jt < L.kt; ++jt)
-                tma_load_5d(const_cast<float*>(s_x) + jt * x_floats, &maps.x, x_full, y0 - 4, x0 - 1, t + jt + L.t_off, 0, b);
+            int x_bytes = 0;
+            for (int h = 0; h < L.halos; ++h) x_bytes += kpad_of(h) * CC_PLANE * 4;
+            mbar_arrive_expect_tx(x_full, x_bytes);
+            for (int h = 0; h < L.halos; ++h)
+                tma_load_5d(const_cast<float*>(s_x) + x_off_of(h), &maps.x[SEG ? L.map[h] : 0], x_full, y0 - 4, x0 - 1, t + L.t_off[h], 0,
+                            b);
             for (int j = 0; j < taps; ++j) {
-                const int st = ring.produce(j, w_bytes);
-                for (int a = 0; a < L.ka; ++a) tma_load_3d(s_w + st * w_bytes + a * N * 128, &maps.w, ring.full + st, 0, 0, j * L.ka + a);
+                const int h = j / 9, ka = ka_of(h);
+                const int st = ring.produce(j, ka * N * 128);
+                const int atom = SEG ? L.atom0[h] + (j % 9) * ka : j * ka;
+                for (int a = 0; a < ka; ++a) tma_load_3d(s_w + st * w_bytes + a * N * 128, &maps.w, ring.full + st, 0, 0, atom + a);
             }
         }
         return;
@@ -158,7 +177,6 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
     // ===== consumers: warp w of warpgroup g owns tile row 4g + w; accumulator rows 16w + lane/4 (+ 8) = columns lane/4 (+ 8) =====
     const int row = 4 * (warp >> 2) + (warp & 3);
     const int col = lane >> 2, kq = lane & 3;
-    const int nks = L.kpad / 8;
     float acc[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
@@ -166,10 +184,11 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
 #pragma unroll 1
     for (int j = 0; j < taps; ++j) {
         const int jt = j / 9, ay = j / 3 % 3, ax = j % 3;
-        const float* h = s_x + jt * x_floats + (row + ay) * CC_HY + col + ax + CC_HY_OFF + kq * CC_PLANE;
+        const int nks = kpad_of(jt) / 8, ka = ka_of(jt);
+        const float* h = s_x + x_off_of(jt) + (row + ay) * CC_HY + col + ax + CC_HY_OFF + kq * CC_PLANE;
         const uint32_t wb = smem_addr(s_w + ring.consume(j) * w_bytes);
 #pragma unroll 1
-        for (int a = 0; a < L.ka; ++a) {               // 32 channels (4 k-steps) at a time
+        for (int a = 0; a < ka; ++a) {                 // 32 channels (4 k-steps) at a time
             uint32_t fr[4][4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -194,27 +213,74 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const CcFwdLaunch
     const int gx = x0 + row;
     if (gx >= L.X) return;
     const size_t plane = static_cast<size_t>(L.X) * L.Y;
+    if constexpr (!SEG) {
+        const CcOutSeg& o = L.seg[0];
 #pragma unroll
-    for (int jn = 0; jn < N / 8; ++jn)
+        for (int jn = 0; jn < N / 8; ++jn)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const int c = 8 * jn + 2 * kq + e;
-            if (c >= L.n_out) continue;
-            float* dst = out + ((static_cast<size_t>(b) * L.n_out + c) * L.frames + t) * plane + static_cast<size_t>(gx) * L.Y + y0 + col;
-            if (y0 + col < L.Y) dst[0] = acc[4 * jn + e];
-            if (y0 + col + 8 < L.Y) dst[8] = acc[4 * jn + 2 + e];
-        }
+            for (int e = 0; e < 2; ++e) {
+                const int c = 8 * jn + 2 * kq + e;
+                if (c >= o.n) continue;
+                float* dst = o.p + b * o.sb + c * o.sc + t * o.st + static_cast<size_t>(gx) * L.Y + y0 + col;
+                if (y0 + col < L.Y) dst[0] = acc[4 * jn + e];
+                if (y0 + col + 8 < L.Y) dst[8] = acc[4 * jn + 2 + e];
+            }
+    } else {
+        const size_t pix = static_cast<size_t>(gx) * L.Y + y0 + col;
+#pragma unroll
+        for (int jn = 0; jn < N / 8; ++jn)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int c = 8 * jn + 2 * kq + e;
+                for (int sg = 0; sg < L.nseg; ++sg) {
+                    const CcOutSeg& o = L.seg[sg];
+                    const int ch = c - o.c0;
+                    if (ch < 0 || ch >= o.n) continue;
+                    if (y0 + col < L.Y) cc_epilogue(o, L.bias_init, plane, b, ch, t, pix, acc[4 * jn + e]);
+                    if (y0 + col + 8 < L.Y) cc_epilogue(o, L.bias_init, plane, b, ch, t, pix + 8, acc[4 * jn + 2 + e]);
+                }
+            }
+    }
+}
+
+int cc_launch_fwd(int N, bool segments, const CcFwdMaps& maps, const CcFwdLaunch& L, long long n_tiles, cudaStream_t stream) {
+    FIERY_REQUIRE(n_tiles < (1ll << 31), "3x3 conv: too many pixel tiles");
+    if (n_tiles == 0) return FIERY_OK;
+    const int smem = cc_fwd_smem(L);
+    FIERY_REQUIRE(smem <= CC_MAX_SMEM, "3x3 conv: %d bytes of shared memory", smem);
+    FIERY_REQUIRE(segments || (N <= 64 && L.stages == CC_WSTAGES), "3x3 conv: the single-input kernel takes N <= 64");
+    int rc;
+    switch (N) {
+#define CC_FWD_CASE(NN)                                                                                                            \
+    case NN:                                                                                                                       \
+        if (segments) {                                                                                                            \
+            if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<NN, true>, smem)) != FIERY_OK) return rc;                            \
+            causal_conv_fwd_kernel<NN, true><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L);           \
+        } else {                                                                                                                   \
+            if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<NN, false>, smem)) != FIERY_OK) return rc;                           \
+            causal_conv_fwd_kernel<NN, false><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L);          \
+        }                                                                                                                          \
+        break;
+        CC_FWD_CASE(8) CC_FWD_CASE(16) CC_FWD_CASE(24) CC_FWD_CASE(32) CC_FWD_CASE(40) CC_FWD_CASE(48) CC_FWD_CASE(56) CC_FWD_CASE(64)
+#undef CC_FWD_CASE
+        case 96:
+            if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<96, true>, smem)) != FIERY_OK) return rc;
+            causal_conv_fwd_kernel<96, true><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L);
+            break;
+        case 128:
+            if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<128, true>, smem)) != FIERY_OK) return rc;
+            causal_conv_fwd_kernel<128, true><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L);
+            break;
+        default: return set_error(FIERY_E_INVALID, "3x3 conv: %d accumulator columns", N);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // weight gradient
 // ------------------------------------------------------------------------------------------------------------------------------
-struct CcWgradMaps {
-    CUtensorMap gy;                                // (Y, X, s, C_out, b), box (32, 1, 1, NO, 1), swizzle 128B
-    CUtensorMap x;                                 // (Y, X, s, C_in, b), box (44, 1, 1, 64, 1), no swizzle
-};
-
-static long long cc_wgrad_tiles(const CcShape& s) {
+long long cc_wgrad_tiles(const CcShape& s) {
     return static_cast<long long>(s.batch) * s.frames * s.X * ((s.Y + CC_WG_PX - 1) / CC_WG_PX);
 }
 static size_t cc_partial_floats(const CcShape& s) { return static_cast<size_t>(s.taps) * s.cout * s.cin; }
@@ -225,13 +291,14 @@ size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d) {
 }
 
 // grid (chunks, 3 kt): CTA (chunk, tau * 3 + dy) accumulates the taps (tau, dy, 0..2) over its chunk's tiles as D (input channels x
-// NO output channels) = x_tap gy^T.  Per tile the stage holds the x row run of frame t + tau - (kt - 1), row x + dy - 1 (64 channel rows
-// of 44 columns, read as the register A operand at column offset dx + 3) and the gy run (NO K-major rows of 32 pixels, the B operand).
-// Thread 0 issues the loads: at iteration i, after the barrier that ends the MMAs on tile i - 1, tile i + stages - 1 into that tile's
-// stage.
+// NO output channels) = x_tap gy^T.  Per tile the stage holds the x row run of frame t * fmul + foff + tau - (kt - 1), row x + dy - 1
+// (64 channel rows of 44 columns, read as the register A operand at column offset dx + 3) and the gy run (NO K-major rows of 32 pixels
+// from channel o0, the B operand).  Thread 0 issues the loads: at iteration i, after the barrier that ends the MMAs on tile i - 1, tile
+// i + stages - 1 into that tile's stage.
 template <int NO>
 __global__ void __launch_bounds__(128, 1)
-causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, float* __restrict__ partial, int n_tiles) {
+causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, const CcWgradSeg seg, float* __restrict__ partial,
+                         int n_tiles) {
     unsigned char* smem = dynamic_smem_1024();
     constexpr int STAGE_BYTES = CC_WG_X_BYTES + NO * 128;
     const MbarRing ring(reinterpret_cast<uint64_t*>(smem + CC_WG_STAGES * STAGE_BYTES), CC_WG_STAGES);
@@ -248,8 +315,10 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
         const int st = ring.arm(i, STAGE_BYTES);
         unsigned char* dst = smem + st * STAGE_BYTES;
         uint64_t* bar = ring.full + st;
-        tma_load_5d(dst, &maps.x, bar, CC_WG_PX * run - 4, x + dy - 1, tt + tau - (s.kt - 1), 0, b);
-        tma_load_5d(dst + CC_WG_X_BYTES, &maps.gy, bar, CC_WG_PX * run, x, tt, 0, b);
+        const int fx = tt * seg.fmul + seg.foff + tau - (s.kt - 1);
+        if (seg.first && fx < 0) tma_load_5d(dst, &maps.x_first, bar, CC_WG_PX * run - 4, x + dy - 1, 0, 0, b);
+        else tma_load_5d(dst, &maps.x, bar, CC_WG_PX * run - 4, x + dy - 1, fx, 0, b);
+        tma_load_5d(dst + CC_WG_X_BYTES, &maps.gy, bar, CC_WG_PX * run, x, tt, seg.o0, b);
     };
 
     if (threadIdx.x == 0) {
@@ -299,7 +368,7 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
     }
 
     // this chunk's partial: accumulator (row = input channel ci, column = output channel o) of tap (tau, dy, dx) ->
-    // partial[chunk][tap][o][ci]
+    // partial[chunk][tap][o0 + o][ci0 + ci]
     const size_t n_oi = static_cast<size_t>(s.cout) * s.cin;
 #pragma unroll
     for (int dx = 0; dx < 3; ++dx) {
@@ -307,13 +376,13 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const int ci = ra + 8 * half;
-            if (ci >= s.cin) continue;
+            if (ci >= seg.cin) continue;
 #pragma unroll
             for (int jn = 0; jn < NO / 8; ++jn)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int o = 8 * jn + 2 * kq + e;
-                    if (o < s.cout) dst[static_cast<size_t>(o) * s.cin + ci] = acc[dx][4 * jn + 2 * half + e];
+                    if (o < seg.n_o) dst[static_cast<size_t>(seg.o0 + o) * s.cin + seg.ci0 + ci] = acc[dx][4 * jn + 2 * half + e];
                 }
         }
     }
@@ -328,18 +397,52 @@ struct CcWgradOffset {
     }
 };
 
+int cc_launch_wgrad(const CcWgradMaps& maps, const CcShape& s, const CcWgradSeg& seg, float* partial, int n_chunks, cudaStream_t stream) {
+    const long long tiles = cc_wgrad_tiles(s);
+    FIERY_REQUIRE(tiles < (1ll << 31), "3x3 conv: too many pixel tiles");
+    if (n_chunks == 0) return FIERY_OK;
+    const int no = cc_round8(seg.n_o);
+    const int smem = CC_WG_STAGES * (CC_WG_X_BYTES + no * 128) + CC_SMEM_SLACK;
+    const dim3 grid(static_cast<unsigned>(n_chunks), static_cast<unsigned>(3 * s.kt));
+    int rc;
+    switch (no) {
+#define CC_WG_CASE(N)                                                                                                              \
+    case N:                                                                                                                        \
+        if ((rc = set_dynamic_smem(causal_conv_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                     \
+        causal_conv_wgrad_kernel<N><<<grid, 128, smem, stream>>>(maps, s, seg, partial, static_cast<int>(tiles));                   \
+        break;
+        CC_WG_CASE(8) CC_WG_CASE(16) CC_WG_CASE(24) CC_WG_CASE(32) CC_WG_CASE(40) CC_WG_CASE(48) CC_WG_CASE(56) CC_WG_CASE(64)
+#undef CC_WG_CASE
+        default: return set_error(FIERY_E_INVALID, "3x3 conv: %d output channels in one weight-gradient block", seg.n_o);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int cc_wgrad_reduce(const CcShape& s, const float* partial, int n_chunks, float* gw, cudaStream_t stream) {
+    return launch_wgrad_reduce(partial, n_chunks, cc_partial_floats(s), s.cout * s.cin * s.taps, CcWgradOffset{s}, gw, stream);
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------------------------
+int cc_encode_map(CUtensorMap* map, const float* t, int Y, int X, int S, int C, int B, const long long (&strides)[4], cuuint32_t box_y,
+                  cuuint32_t box_x, cuuint32_t box_c, CUtensorMapSwizzle swizzle, const char* what) {
+    cuuint64_t dims[5] = {static_cast<cuuint64_t>(Y), static_cast<cuuint64_t>(X), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(C),
+                          static_cast<cuuint64_t>(B)};
+    cuuint64_t st[4];
+    for (int i = 0; i < 4; ++i) st[i] = static_cast<cuuint64_t>(strides[i]) * 4;
+    cuuint32_t box[5] = {box_y, box_x, 1, box_c, 1};
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, t, dims, st, box, nullptr, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                             what);
+}
+
 // a contiguous (b, C, s, X, Y) activation as the 5-D map (Y, X, s, C, b)
 static int cc_encode_activation(CUtensorMap* map, const CcShape& s, const float* t, int channels, cuuint32_t box_y, cuuint32_t box_x,
                                 cuuint32_t box_c, CUtensorMapSwizzle swizzle, const char* what) {
-    const cuuint64_t Y = s.Y, X = s.X, S = s.frames, C = channels;
-    cuuint64_t dims[5] = {Y, X, S, C, static_cast<cuuint64_t>(s.batch)};
-    cuuint64_t strides[4] = {Y * 4, X * Y * 4, S * X * Y * 4, C * S * X * Y * 4};
-    cuuint32_t box[5] = {box_y, box_x, 1, box_c, 1};
-    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, t, dims, strides, box, nullptr, swizzle,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
+    const long long XY = static_cast<long long>(s.X) * s.Y;
+    const long long strides[4] = {s.Y, XY, s.frames * XY, static_cast<long long>(channels) * s.frames * XY};
+    return cc_encode_map(map, t, s.Y, s.X, s.frames, channels, s.batch, strides, box_y, box_x, box_c, swizzle, what);
 }
 
 // forward (dgrad = 0): x (C_in channels) -> y (C_out) with pack F; input gradient (dgrad = 1): gy (C_out) -> gx (C_in) with pack T
@@ -349,7 +452,7 @@ static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const 
     const CcPackDir p = dgrad ? cc_pack_dir(s.cin, s.cout, s.taps) : f;
     const float* w = dgrad ? packed + f.floats : packed;
     CcFwdMaps maps;
-    int rc = cc_encode_activation(&maps.x, s, in, dgrad ? s.cout : s.cin, CC_HY, CC_HX, static_cast<cuuint32_t>(p.kpad),
+    int rc = cc_encode_activation(&maps.x[0], s, in, dgrad ? s.cout : s.cin, CC_HY, CC_HX, static_cast<cuuint32_t>(p.kpad),
                                   CU_TENSOR_MAP_SWIZZLE_NONE, dgrad ? "causal conv output gradient" : "causal conv input");
     if (rc != FIERY_OK) return rc;
     {
@@ -360,32 +463,37 @@ static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const 
                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "causal conv weights")) != FIERY_OK)
             return rc;
     }
-    CcFwdLaunch L;
+    CcFwdLaunch L{};
     L.frames = s.frames;
     L.X = s.X;
     L.Y = s.Y;
-    L.kpad = p.kpad;
-    L.ka = p.ka;
-    L.n_out = dgrad ? s.cin : s.cout;
-    L.kt = s.kt;
-    L.t_off = dgrad ? 0 : -(s.kt - 1);
     L.tiles_x = (s.X + CC_TX - 1) / CC_TX;
     L.tiles_y = (s.Y + CC_TY - 1) / CC_TY;
+    L.halos = s.kt;                                // halo jt: frame t + jt - (kt - 1) (forward) or t + jt (input gradient)
+    L.stages = CC_WSTAGES;
+    L.stage_bytes = p.ka * p.n * 128;
+    for (int jt = 0; jt < s.kt; ++jt) {
+        L.map[jt] = 0;
+        L.t_off[jt] = jt - (dgrad ? 0 : s.kt - 1);
+        L.kpad[jt] = p.kpad;
+        L.ka[jt] = p.ka;
+        L.x_off[jt] = jt * p.kpad * CC_PLANE;
+        L.atom0[jt] = jt * 9 * p.ka;
+    }
+    const int n_out = dgrad ? s.cin : s.cout;
+    const long long plane = static_cast<long long>(s.X) * s.Y;
+    L.nseg = 1;
+    L.seg[0].p = out;
+    L.seg[0].st = plane;
+    L.seg[0].sc = s.frames * plane;
+    L.seg[0].sb = n_out * L.seg[0].sc;
+    L.seg[0].c0 = 0;
+    L.seg[0].n = n_out;
+    L.seg[0].mode = CC_STORE;
     const long long n_tiles = static_cast<long long>(s.batch) * s.frames * L.tiles_x * L.tiles_y;
     FIERY_REQUIRE(n_tiles < (1ll << 31), "causal conv: too many pixel tiles");
-    const int smem = CC_WSTAGES * p.ka * p.n * 128 + s.kt * p.kpad * CC_PLANE * 4 + CC_SMEM_SLACK;
-    switch (p.n) {
-#define CC_FWD_CASE(N)                                                                                                             \
-    case N:                                                                                                                        \
-        if ((rc = set_dynamic_smem(causal_conv_fwd_kernel<N>, smem)) != FIERY_OK) return rc;                                       \
-        causal_conv_fwd_kernel<N><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L, out);                 \
-        break;
-        CC_FWD_CASE(8) CC_FWD_CASE(16) CC_FWD_CASE(24) CC_FWD_CASE(32) CC_FWD_CASE(40) CC_FWD_CASE(48) CC_FWD_CASE(56) CC_FWD_CASE(64)
-#undef CC_FWD_CASE
-        default: return set_error(FIERY_E_INVALID, "causal conv: %d channels padded to %d", L.n_out, p.n);
-    }
-    FIERY_CUDA_CHECK(cudaGetLastError());
-    return FIERY_OK;
+    if (p.n > 64) return set_error(FIERY_E_INVALID, "causal conv: %d channels padded to %d", n_out, p.n);
+    return cc_launch_fwd(p.n, false, maps, L, n_tiles, stream);
 }
 
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream) {
@@ -411,21 +519,11 @@ int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x
         if (rc == FIERY_OK)
             rc = cc_encode_activation(&maps.x, s, x, s.cin, CC_WG_XP, 1, 64, CU_TENSOR_MAP_SWIZZLE_NONE, "causal conv input");
         if (rc != FIERY_OK) return rc;
-        const int smem = CC_WG_STAGES * (CC_WG_X_BYTES + no * 128) + CC_SMEM_SLACK;
-        const dim3 grid(static_cast<unsigned>(n_chunks), static_cast<unsigned>(3 * s.kt));
-        switch (no) {
-#define CC_WG_CASE(N)                                                                                                              \
-    case N:                                                                                                                        \
-        if ((rc = set_dynamic_smem(causal_conv_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                     \
-        causal_conv_wgrad_kernel<N><<<grid, 128, smem, stream>>>(maps, s, partial, static_cast<int>(tiles));                        \
-        break;
-            CC_WG_CASE(8) CC_WG_CASE(16) CC_WG_CASE(24) CC_WG_CASE(32) CC_WG_CASE(40) CC_WG_CASE(48) CC_WG_CASE(56) CC_WG_CASE(64)
-#undef CC_WG_CASE
-            default: return set_error(FIERY_E_INVALID, "causal conv: out_channels padded to %d", no);
-        }
-        FIERY_CUDA_CHECK(cudaGetLastError());
+        maps.x_first = maps.x;
+        const CcWgradSeg seg{0, s.cin, 0, s.cout, 1, 0, 0};
+        if ((rc = cc_launch_wgrad(maps, s, seg, partial, n_chunks, stream)) != FIERY_OK) return rc;
     }
-    return launch_wgrad_reduce(partial, n_chunks, cc_partial_floats(s), s.cout * s.cin * s.taps, CcWgradOffset{s}, gw, stream);
+    return cc_wgrad_reduce(s, partial, n_chunks, gw, stream);
 }
 
 }  // namespace fiery

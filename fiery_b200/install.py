@@ -137,12 +137,17 @@ def _blocks(blocks, *kinds):
             yield i, name, block
 
 
-def _swap(model, slots, swapped, reason, make, warning: str, entry: str = "{where}: {reason}", sep: str = "; "):
-    """Replace each module that ``slots(model.temporal_model.model)`` yields as ``(parent, name, module, where)`` by
-    ``setattr(parent, name, make(module))``, unless it already is a ``swapped`` or ``reason(module)`` gives a reason to leave it.  A
-    module reached under several names gets one replacement, set in each.  The modules left are listed, each as ``entry`` and
-    ``sep``-separated, in one warning after ``warning``, given once per list.  Returns the model."""
-    blocks = getattr(model.temporal_model, "model", None)
+def _temporal_blocks(model):
+    return getattr(model.temporal_model, "model", None)
+
+
+def _swap(model, slots, swapped, reason, make, warning: str, entry: str = "{where}: {reason}", sep: str = "; ", root=_temporal_blocks):
+    """Replace each module that ``slots(root(model))`` (by default ``model.temporal_model.model``) yields as ``(parent, name, module,
+    where)`` by ``setattr(parent, name, make(module))``, unless it already is a ``swapped`` or ``reason(module)`` gives a reason to
+    leave it.  A module reached under several names gets one replacement, set in each.  The modules left are listed, each as
+    ``entry`` and ``sep``-separated, in one warning after ``warning``, given once per list.  Nothing happens when ``root`` finds
+    nothing.  Returns the model."""
+    blocks = root(model)
     if blocks is None:
         return model
     made, skipped = {}, []                      # made: id of a replaced module -> its replacement
@@ -237,6 +242,26 @@ def use_fused_batch_norm(model):
     # the warning's text gives the one reason, so it lists the skipped norms by name only
     return _swap(model, slots, FusedBatchNorm3d, reason, FusedBatchNorm3d, "fiery_b200: SyncBatchNorm module(s) left as they are (the "
                  "fused batch norm computes per-rank statistics only): ", entry="{where}", sep=", ")
+
+
+def use_tensor_core_future_prediction(model):
+    """Replace every covered ``SpatialGRU`` in ``model.future_prediction.spatial_grus`` (fiery/models/future_prediction.py) of a
+    ``Fiery`` instance by ``fiery_b200.future_prediction.TensorCoreSpatialGRU``, which adopts the module's convolutions and its
+    ``ConvBlock`` (``state_dict`` keys unchanged) and runs all its steps as ``torch.ops.fiery_b200.spatial_gru``, forward and backward.
+    Returns the model; a second call does nothing, a model without future prediction is returned untouched, and GRUs the kernels do
+    not cover (another kernel size, a norm other than BatchNorm2d -- a SyncBatchNorm stays torch's --, an activation other than ReLU,
+    more than 64 input or hidden channels) are left alone with one warning.  The ``Bottleneck``s stay as they are."""
+    from .future_prediction import TensorCoreSpatialGRU, module_reason
+
+    def slots(grus):
+        for i, (name, gru) in enumerate(grus._modules.items()):
+            yield grus, name, gru, f"spatial_grus[{i}]"
+
+    def root(m):
+        fp = getattr(m, "future_prediction", None)
+        return getattr(fp, "spatial_grus", None) if fp is not None else None
+    return _swap(model, slots, TensorCoreSpatialGRU, module_reason, TensorCoreSpatialGRU.from_module,
+                 "fiery_b200: SpatialGRU(s) not covered by the tensor-core kernels, left as is: ", root=root)
 
 
 def uninstall():

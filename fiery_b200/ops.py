@@ -385,4 +385,89 @@ batch_norm_act.register_autograd(_batch_norm_act_backward, setup_context=_batch_
 torch.library.register_autocast("fiery_b200::batch_norm_act", "cuda", torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# The future prediction's SpatialGRU (fiery/layers/temporal.py:10-62): ``spatial_gru`` / ``spatial_gru_backward``
+# (fiery_b200/future_prediction.py; kernels in csrc/spatial_gru.cu).  The statistics and the saved tensors are not differentiable and
+# the operator updates no running buffer (TensorCoreSpatialGRU does, from the statistics).  Autocast: fp32, like the temporal
+# operators; under AMP the reference runs these convolutions in fp16.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::spatial_gru", mutates_args=(), device_types="cuda")
+def spatial_gru(x: torch.Tensor, h0: torch.Tensor, w_update: torch.Tensor, b_update: torch.Tensor, w_reset: torch.Tensor,
+                b_reset: torch.Tensor, w_state: torch.Tensor, bn_weight: Optional[torch.Tensor], bn_bias: Optional[torch.Tensor],
+                running_mean: Optional[torch.Tensor], running_var: Optional[torch.Tensor], frames: int, training: bool, eps: float,
+                bias_init: float) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """x (b, Tx, C_x, H, W) with Tx 1 (the same frame at every step) or ``frames``; h0 (b, C_h, H, W); the gates' (C_h, C_x + C_h, 3, 3)
+    weights and (C_h,) biases, the state conv's bias-free weight, its BatchNorm2d's affine parameters (or None) and, in eval, its
+    running statistics.  Returns (out, means, vars, saved): the contiguous (b, frames, C_h, H, W) fp32 states, the (frames, C_h)
+    statistics each step normalized with, and a uint8 buffer the backward reads.  Bit-reproducible."""
+    from .future_prediction import forward
+    return forward(x, h0, w_update, b_update, w_reset, b_reset, w_state, bn_weight, bn_bias, running_mean, running_var, frames, training,
+                   eps, bias_init)
+
+
+@spatial_gru.register_fake
+def _(x, h0, w_update, b_update, w_reset, b_reset, w_state, bn_weight, bn_bias, running_mean, running_var, frames, training, eps,
+      bias_init):
+    b, _, _, h, w = x.shape
+    ch = w_update.shape[0]
+    return (x.new_empty((b, frames, ch, h, w), dtype=torch.float32), x.new_empty((frames, ch), dtype=torch.float32),
+            x.new_empty((frames, ch), dtype=torch.float32), x.new_empty((16 * frames * b * ch * h * w,), dtype=torch.uint8))
+
+
+@torch.library.custom_op("fiery_b200::spatial_gru_backward", mutates_args=(), device_types="cuda")
+def spatial_gru_backward(grad_out: torch.Tensor, x: torch.Tensor, h0: torch.Tensor, out: torch.Tensor, saved: torch.Tensor,
+                         means: torch.Tensor, var: torch.Tensor, w_update: torch.Tensor, w_reset: torch.Tensor, w_state: torch.Tensor,
+                         bn_weight: Optional[torch.Tensor], bn_bias: Optional[torch.Tensor], frames: int, training: bool, eps: float,
+                         bias_init: float, need_x: bool, need_h0: bool, need_gates: bool, need_state: bool,
+                         need_bn: bool) -> List[torch.Tensor]:
+    """[grad_x, grad_h0, grad_w_update, grad_b_update, grad_w_reset, grad_b_reset, grad_w_state, grad_bn_weight, grad_bn_bias] of
+    ``spatial_gru``, each in its input's shape and dtype; a gradient that is not asked for is not computed and comes back empty.  The
+    recurrence runs in reverse; the weight gradients are bit-reproducible."""
+    from .future_prediction import backward
+    g = backward(grad_out, x, h0, out, saved, means, var, w_update, w_reset, w_state, bn_weight, bn_bias, frames, training, eps,
+                 bias_init, need_x, need_h0, need_gates, need_state, need_bn)
+    likes = (x, h0, w_update, w_update, w_reset, w_reset, w_state, bn_weight if bn_weight is not None else x,
+             bn_bias if bn_bias is not None else x)
+    return [_cast_back(gi, like) for gi, like in zip(g, likes)]
+
+
+@spatial_gru_backward.register_fake
+def _(grad_out, x, h0, out, saved, means, var, w_update, w_reset, w_state, bn_weight, bn_bias, frames, training, eps, bias_init,
+      need_x, need_h0, need_gates, need_state, need_bn):
+    ch = w_update.shape[0]
+    e = x.new_empty((0,))
+    return [x.new_empty(x.shape) if need_x else e, h0.new_empty(h0.shape) if need_h0 else e,
+            w_update.new_empty(w_update.shape) if need_gates else e, w_update.new_empty((ch,)) if need_gates else e,
+            w_reset.new_empty(w_reset.shape) if need_gates else e, w_reset.new_empty((ch,)) if need_gates else e,
+            w_state.new_empty(w_state.shape) if need_state else e,
+            bn_weight.new_empty((ch,)) if need_bn and bn_weight is not None else e,
+            bn_bias.new_empty((ch,)) if need_bn and bn_bias is not None else e]
+
+
+def _spatial_gru_setup_context(ctx, inputs, output):
+    (x, h0, w_u, _b_u, w_r, _b_r, w_s, bn_w, bn_b, _rm, _rv, frames, training, eps, bias_init) = inputs
+    out, means, var, saved = output
+    ctx.mark_non_differentiable(means, var, saved)
+    ctx.args = (frames, training, eps, bias_init)
+    ctx.save_for_backward(x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b)
+
+
+def _spatial_gru_backward(ctx, grad_out, _gm, _gv, _gs):
+    x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b = ctx.saved_tensors
+    n = ctx.needs_input_grad
+    need_x, need_h0 = bool(n[0]), bool(n[1])
+    need_gates, need_state, need_bn = bool(n[2] or n[3] or n[4] or n[5]), bool(n[6]), bool(n[7] or n[8])
+    if not (need_x or need_h0 or need_gates or need_state or need_bn):
+        return (None,) * 15
+    if grad_out is None:
+        grad_out = torch.zeros_like(out)
+    g = torch.ops.fiery_b200.spatial_gru_backward(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b, *ctx.args,
+                                                  need_x, need_h0, need_gates, need_state, need_bn)
+    return tuple(gi if bool(ni) else None for gi, ni in zip(g, n[:9])) + (None,) * 6
+
+
+spatial_gru.register_autograd(_spatial_gru_backward, setup_context=_spatial_gru_setup_context)
+torch.library.register_autocast("fiery_b200::spatial_gru", "cuda", torch.float32)
+
+
 from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

@@ -484,6 +484,97 @@ FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, con
                                         const float* bias, const float* mean, const float* var, float* grad_x, float* grad_weight,
                                         float* grad_bias, void* workspace, void* stream);
 
+/*
+ * The future prediction's SpatialGRU (fiery/layers/temporal.py:10-62) over T steps, without flow warping.  For t = 0 .. T-1, with
+ * h = h0 at t = 0 and out[:, t-1] after:
+ *   u = sigmoid(conv3x3([x_t, h], W_gates[:C_h]) + b_gates[:C_h] + bias_init)
+ *   r = sigmoid(conv3x3([x_t, h], W_gates[C_h:]) + b_gates[C_h:] + bias_init)
+ *   q = (1 - r) h,  s = conv3x3([x_t, q], W_state)  (no bias)
+ *   a = max(fmaf(scale, s, shift), 0) with batch_norm's scale and shift (fiery_batch_norm_*: this step's batch statistics in
+ *       training, the running ones in eval),  out[:, t] = (1 - u) h + u a
+ * conv3x3 is a 3x3 convolution with zero padding 1, [.,.] a concatenation along channels (never built).  wgmma, TF32 operands
+ * (weights and activations rounded to nearest when read), fp32 accumulation; the gates' sigmoid is 1 / (1 + expf(-v)).
+ *
+ * x: (batch, x_frames, x_channels, grid_x, grid_y) fp32 with contiguous pixel planes and the strides given in the desc (elements,
+ * multiples of 4); x_frames 1 means one frame read for every step.  h0, grad_h0: (batch, h_channels, X, Y) contiguous.  out,
+ * grad_out: (batch, frames, h_channels, X, Y) contiguous.  W_gates / grad_w_gates (2 h_channels, x_channels + h_channels, 3, 3),
+ * b_gates / grad_b_gates (2 h_channels), W_state / grad_w_state (h_channels, x_channels + h_channels, 3, 3), bn_weight, bn_bias,
+ * running_mean, running_var, grad_bn_weight, grad_bn_bias (h_channels): contiguous fp32.  grad_x: (batch, x_frames, x_channels, X, Y)
+ * contiguous (with x_frames 1 the sum over the steps).  means / vars: (frames, h_channels), each step's mean and biased variance
+ * (copies of the running ones in eval).  saved: fiery_spatial_gru_saved_bytes, u, r, q and s of every step as (frames, batch,
+ * h_channels, X, Y) each; the backward reads what the forward wrote there.  Workspaces: the *_workspace_bytes, 256-byte aligned,
+ * contents irrelevant.  The backward computes what is asked for: grad_x, grad_h0 and each parameter gradient may be NULL.
+ * Limits (FIERY_E_INVALID, the message names the field): 1 <= x_channels, h_channels <= 64; batch, frames >= 1; x_frames 1 or
+ * frames; grid_x >= 1; grid_y a positive multiple of 4; training 0 or 1; eps >= 0; in training batch * X * Y >= 2; pointers
+ * 16-byte aligned.
+ *
+ * Summation orders (no atomics; bit-reproducible, graph-capturable): the batch statistics as fiery_batch_norm_forward on each step's
+ * s; the weight gradients as fiery_causal_conv3d_backward_weight's over (batch, frames) with kt = 1; the gates' bias gradient, per
+ * channel, 256 threads each adding elements i, i + 256, ... of the (frame, batch) planes in ascending order, then a halving tree;
+ * grad_bn_weight / grad_bn_bias the steps' fiery_batch_norm_backward results added in ascending step order.  Kernels:
+ * csrc/spatial_gru.cu, csrc/causal_conv.cu, csrc/batch_norm.cu.
+ */
+typedef struct {
+    int32_t batch;
+    int32_t frames;               /* T: steps */
+    int32_t x_frames;             /* 1 or frames */
+    int32_t grid_x;
+    int32_t grid_y;
+    int32_t x_channels;
+    int32_t h_channels;
+    int64_t x_stride_b, x_stride_t, x_stride_c;   /* elements */
+    int32_t training;
+    double eps;
+    float bias_init;
+} fiery_spatial_gru_desc_t;
+
+FIERY_API size_t fiery_spatial_gru_packed_bytes(const fiery_spatial_gru_desc_t* desc);
+FIERY_API int fiery_spatial_gru_pack_weights(const fiery_spatial_gru_desc_t* desc, const float* w_gates, const float* w_state, void* packed,
+                                             void* stream);
+FIERY_API size_t fiery_spatial_gru_saved_bytes(const fiery_spatial_gru_desc_t* desc);
+FIERY_API size_t fiery_spatial_gru_forward_workspace_bytes(const fiery_spatial_gru_desc_t* desc);
+FIERY_API int fiery_spatial_gru_forward(const fiery_spatial_gru_desc_t* desc, const float* x, const float* h0, const void* packed,
+                                        const float* b_gates, const float* bn_weight, const float* bn_bias, const float* running_mean,
+                                        const float* running_var, float* out, void* saved, float* means, float* vars, void* workspace,
+                                        void* stream);
+FIERY_API size_t fiery_spatial_gru_backward_workspace_bytes(const fiery_spatial_gru_desc_t* desc);
+FIERY_API int fiery_spatial_gru_backward(const fiery_spatial_gru_desc_t* desc, const float* grad_out, const float* x, const float* h0,
+                                         const float* out, const void* saved, const float* means, const float* vars, const void* packed,
+                                         const float* bn_weight, const float* bn_bias, float* grad_x, float* grad_h0, float* grad_w_gates,
+                                         float* grad_b_gates, float* grad_w_state, float* grad_bn_weight, float* grad_bn_bias,
+                                         void* workspace, void* stream);
+
+/*
+ * The spatial GRU's 3x3 convolution on its own: zero padding 1, stride 1, no bias, on `maps` independent (X, Y) maps, the input the
+ * channel concatenation of two segments x0 (in_channels[0]) and x1 (in_channels[1], 0 for none), the output split into y0
+ * (out_channels[0]) and y1 (out_channels[1], 0 for none), each segment its own contiguous (maps, C, X, Y) fp32 tensor:
+ *   [y0, y1][m, o, p] = sum_{i, dy, dx} W[o, i, dy, dx] * [x0, x1][m, i, p + (dy - 1, dx - 1)]
+ * with W (out0 + out1, in0 + in1, 3, 3).  The same kernels, packs and weight-gradient blocks fiery_spatial_gru_* runs, with plain
+ * stores: TF32 operands rounded to nearest (grad_y truncated by the tensor core in the weight gradient), fp32 accumulation.
+ * backward_data: [gx0, gx1] from [gy0, gy1], each overwritten.  backward_weight: grad_w from x0, x1 and grad_y, ONE contiguous
+ * (maps, out0 + out1, X, Y) tensor, overwritten, in fiery_causal_conv3d_backward_weight's order (tiles over (maps, x, run), 64 output
+ * channels per block).  workspace: fiery_conv3x3_backward_weight_workspace_bytes, contents irrelevant.
+ * Limits (FIERY_E_INVALID): maps >= 1; 1 <= in_channels[0], out_channels[0] <= 64; 0 <= in_channels[1], out_channels[1] <= 64;
+ * grid_x >= 1; grid_y a positive multiple of 4; pointers 16-byte aligned.
+ */
+typedef struct {
+    int32_t maps;
+    int32_t grid_x;
+    int32_t grid_y;
+    int32_t in_channels[2];
+    int32_t out_channels[2];
+} fiery_conv3x3_desc_t;
+
+FIERY_API size_t fiery_conv3x3_packed_bytes(const fiery_conv3x3_desc_t* desc);
+FIERY_API int fiery_conv3x3_pack_weights(const fiery_conv3x3_desc_t* desc, const float* weight, void* packed, void* stream);
+FIERY_API int fiery_conv3x3_forward(const fiery_conv3x3_desc_t* desc, const float* x0, const float* x1, const void* packed, float* y0,
+                                    float* y1, void* stream);
+FIERY_API int fiery_conv3x3_backward_data(const fiery_conv3x3_desc_t* desc, const float* grad_y0, const float* grad_y1, const void* packed,
+                                          float* grad_x0, float* grad_x1, void* stream);
+FIERY_API size_t fiery_conv3x3_backward_weight_workspace_bytes(const fiery_conv3x3_desc_t* desc);
+FIERY_API int fiery_conv3x3_backward_weight(const fiery_conv3x3_desc_t* desc, const float* x0, const float* x1, const float* grad_y,
+                                            float* grad_w, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
