@@ -83,7 +83,15 @@ def gru_input(x: torch.Tensor) -> torch.Tensor:
     _, tx, _, h, w = x.shape
     ok = (x.dtype == torch.float32 and x.data_ptr() % 16 == 0 and (x.stride(4) == 1 or w == 1) and (x.stride(3) == w or h == 1)
           and x.stride(0) % 4 == 0 and x.stride(2) % 4 == 0 and (tx == 1 or x.stride(1) % 4 == 0))
-    return x if ok else f32(x)
+    return x if ok else _aligned_f32(x)
+
+
+def _aligned_f32(t: torch.Tensor) -> torch.Tensor:
+    """t as a contiguous, 16-byte aligned fp32 tensor: t itself when it is one, else a copy (a contiguous fp32 view at an odd offset,
+    e.g. a slice of a flat buffer, is copied too)"""
+    if t.dtype == torch.float32 and t.is_contiguous() and t.data_ptr() % 16 == 0:
+        return t
+    return t.to(torch.float32, memory_format=torch.contiguous_format, copy=True)
 
 
 def _per_channel(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
@@ -110,7 +118,7 @@ def forward(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, running_mean, running_va
     if not training and (running_mean is None or running_var is None):
         raise ValueError("spatial GRU: eval mode needs running_mean and running_var")
     xs = gru_input(x)
-    hs = f32(h0)
+    hs = _aligned_f32(h0)
     d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), training, eps, bias_init)
     lib = _lib.load()
     out = torch.empty((b, frames, ch, h, w), dtype=torch.float32, device=x.device)
@@ -134,7 +142,7 @@ def backward(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b,
     """The gradients of ``forward`` in fp32: (grad_x (x's shape, contiguous), grad_h0, grad_w_u, grad_b_u, grad_w_r, grad_b_r,
     grad_w_s, grad_bn_w, grad_bn_b), None where not asked for."""
     b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
-    xs, hs = gru_input(x), f32(h0)
+    xs, hs = gru_input(x), _aligned_f32(h0)
     d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), training, eps, bias_init)
     lib = _lib.load()
     dev = x.device
@@ -147,7 +155,7 @@ def backward(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b,
     gbw = new(ch) if need_bn and bn_w is not None else None
     gbb = new(ch) if need_bn and bn_b is not None else None
     ptr = lambda t: t.data_ptr() if t is not None else 0           # noqa: E731
-    go, packed = f32(grad_out), _packed(w_u, w_r, w_s)
+    go, packed = _aligned_f32(grad_out), _packed(w_u, w_r, w_s)
     ws = _lib.workspace(lib.fiery_spatial_gru_backward_workspace_bytes(d), dev)
     _lib.call("fiery_spatial_gru_backward", dev, d, go.data_ptr(), xs.data_ptr(), hs.data_ptr(), out.data_ptr(),
               saved.data_ptr(), means.data_ptr(), var.data_ptr(), packed.data_ptr(), ptr(bn_w), ptr(bn_b), ptr(gx),

@@ -493,7 +493,9 @@ FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, con
  *   a = max(fmaf(scale, s, shift), 0) with batch_norm's scale and shift (fiery_batch_norm_*: this step's batch statistics in
  *       training, the running ones in eval),  out[:, t] = (1 - u) h + u a
  * conv3x3 is a 3x3 convolution with zero padding 1, [.,.] a concatenation along channels (never built).  wgmma, TF32 operands
- * (weights and activations rounded to nearest when read), fp32 accumulation; the gates' sigmoid is 1 / (1 + expf(-v)).
+ * (weights and activations rounded to nearest when read), fp32 accumulation; the gates' sigmoid is 1 / (1 + expf(-v)).  NaN and
+ * +-inf follow these formulas in IEEE arithmetic: a non-finite x or h pixel reaches every output channel of its 3x3 neighbourhood
+ * (0 * NaN is NaN, zero weights included), the ReLU passes NaN, and in training a non-finite s makes its channel's statistics NaN.
  *
  * x: (batch, x_frames, x_channels, grid_x, grid_y) fp32 with contiguous pixel planes and the strides given in the desc (elements,
  * multiples of 4); x_frames 1 means one frame read for every step.  h0, grad_h0: (batch, h_channels, X, Y) contiguous.  out,
