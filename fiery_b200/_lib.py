@@ -155,6 +155,16 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_batch_norm_backward": (c_int32, [POINTER(BatchNormDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fiery_batch_norm_sync_workspace_bytes": (c_size_t, [POINTER(BatchNormDesc)]),
+    "fiery_batch_norm_local_stats": (c_int32, [POINTER(BatchNormDesc)] + [c_void_p] * 4),
+    "fiery_batch_norm_forward_gathered": (c_int32, [POINTER(BatchNormDesc), c_int32] + [c_void_p] * 11),
+    "fiery_batch_norm_local_grad_sums": (c_int32, [POINTER(BatchNormDesc)] + [c_void_p] * 11),
+    "fiery_batch_norm_backward_gathered": (c_int32, [POINTER(BatchNormDesc), c_int32] + [c_void_p] * 10),
+    "fiery_spatial_gru_forward_step_begin": (c_int32, [POINTER(SpatialGruDesc), c_int32] + [c_void_p] * 9),
+    "fiery_spatial_gru_forward_step_end": (c_int32, [POINTER(SpatialGruDesc), c_int32, c_int32] + [c_void_p] * 11),
+    "fiery_spatial_gru_backward_step_begin": (c_int32, [POINTER(SpatialGruDesc), c_int32] + [c_void_p] * 13),
+    "fiery_spatial_gru_backward_step_end": (c_int32, [POINTER(SpatialGruDesc), c_int32, c_int32] + [c_void_p] * 13),
+    "fiery_spatial_gru_backward_weights": (c_int32, [POINTER(SpatialGruDesc)] + [c_void_p] * 12),
     "fiery_spatial_gru_packed_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),
     "fiery_spatial_gru_pack_weights": (c_int32, [POINTER(SpatialGruDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
     "fiery_spatial_gru_saved_bytes": (c_size_t, [POINTER(SpatialGruDesc)]),

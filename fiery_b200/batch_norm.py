@@ -12,6 +12,7 @@ modules call ``activation(norm(y))``.  No CPU path.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -137,11 +138,12 @@ class FusedBatchNorm3d(nn.BatchNorm3d):
         update_running_stats(self, mean, var, n)
 
 
-def update_running_stats(bn: nn.Module, mean: torch.Tensor, var: torch.Tensor, n: int) -> None:
+def update_running_stats(bn: nn.Module, mean: torch.Tensor, var: torch.Tensor, n) -> None:
     """``_BatchNorm.forward``'s bookkeeping on the norm ``bn`` for a batch of n values per channel with this mean and biased variance,
     as device tensor operations: nothing in eval or without tracked statistics, else ``num_batches_tracked += 1`` and each running
     statistic moved toward the batch's by the momentum (``1 / num_batches_tracked`` when the momentum is None), the variance as the
-    unbiased n / (n - 1) var.  ``FusedBatchNorm3d`` calls it once per forward, the spatial GRU once per step."""
+    unbiased n / (n - 1) var.  n is an int, or a one-element fp64 device tensor (a group's count, which the host never sees).
+    ``FusedBatchNorm3d`` calls it once per forward, the spatial GRU once per step."""
     if not (bn.training and bn.track_running_stats):
         return
     with torch.no_grad():
@@ -152,14 +154,178 @@ def update_running_stats(bn: nn.Module, mean: torch.Tensor, var: torch.Tensor, n
                 factor = bn.num_batches_tracked.to(bn.running_mean.dtype).reciprocal()
         if bn.running_mean is None:
             return
+        unbiased = (n / (n - 1)).to(bn.running_var.dtype) if isinstance(n, torch.Tensor) else n / (n - 1)
         bn.running_mean.lerp_(mean.to(bn.running_mean.dtype), factor)
-        bn.running_var.lerp_(var.to(bn.running_var.dtype) * (n / (n - 1)), factor)
+        bn.running_var.lerp_(var.to(bn.running_var.dtype) * unbiased, factor)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# statistics over a process group (torch.nn.SyncBatchNorm): each rank's (C, 3) fp64 triplets are gathered, never all-reduced, and
+# the kernels merge them in ascending rank order, so every rank gets bit-identical statistics
+# ------------------------------------------------------------------------------------------------------------------------------
+def gather(t: torch.Tensor, group) -> torch.Tensor:
+    """(world, *t.shape): every rank's ``t`` in rank order, as torch's SyncBatchNorm gathers (``all_gather`` on gloo, else
+    ``all_gather_into_tensor``)."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    if dist.get_backend(group) == "gloo":
+        parts = [torch.empty_like(t) for _ in range(world)]
+        dist.all_gather(parts, t, group)
+        return torch.stack(parts)
+    out = t.new_empty((world,) + tuple(t.shape))
+    dist.all_gather_into_tensor(out, t, group)
+    return out
+
+
+def local_stats(x: torch.Tensor) -> torch.Tensor:
+    """x (b, C, s, X, Y) fp32 with contiguous pixel planes (``f32_planes``), b may be 0 -> this rank's (C, 3) fp64 (n, mean, M2)."""
+    d = _desc(x, True, False, 0.0)
+    stats = torch.empty((x.shape[1], 3), dtype=torch.float64, device=x.device)
+    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
+    _lib.call("fiery_batch_norm_local_stats", x.device, d, x.data_ptr() if x.numel() else 0, stats.data_ptr(), ws.data_ptr())
+    return stats
+
+
+def forward_gathered(gathered: torch.Tensor, x: torch.Tensor, weight, bias, residual, eps: float, relu: bool):
+    """(y, mean, var, count) from the group's gathered (world, C, 3) triplets: y ``relu(batch_norm(x)) + residual`` with the group's
+    mean and biased var, count the group's n as a (1,) fp64 device tensor."""
+    c = int(x.shape[1])
+    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
+    if residual is not None and tuple(residual.shape) != tuple(x.shape):
+        raise ValueError(f"batch norm: residual {tuple(residual.shape)} does not match x {tuple(x.shape)}")
+    r = f32(residual) if residual is not None else None
+    y = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
+    mean = torch.empty(c, dtype=torch.float32, device=x.device)
+    var = torch.empty(c, dtype=torch.float32, device=x.device)
+    count = torch.empty(1, dtype=torch.float64, device=x.device)
+    d = _desc(x, True, relu, eps)
+    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
+    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
+    _lib.call("fiery_batch_norm_forward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), ptr(x), ptr(w), ptr(bs),
+              ptr(r), ptr(y), mean.data_ptr(), var.data_ptr(), count.data_ptr(), ws.data_ptr())
+    return y, mean, var, count
+
+
+def local_grad_sums(grad_y: torch.Tensor, x: torch.Tensor, weight, bias, mean, var, eps: float, relu: bool, need_weight: bool,
+                    need_bias: bool):
+    """(sums, grad_weight, grad_bias): this rank's (C, 3) fp64 (n, S1, S2) and its own weight and bias gradients (None where not
+    asked for)."""
+    c = int(x.shape[1])
+    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
+    dw = torch.empty(c, dtype=torch.float32, device=x.device) if need_weight else None
+    db = torch.empty(c, dtype=torch.float32, device=x.device) if need_bias else None
+    sums = torch.empty((c, 3), dtype=torch.float64, device=x.device)
+    d = _desc(x, True, relu, eps)
+    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
+    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
+    _lib.call("fiery_batch_norm_local_grad_sums", x.device, d, ptr(x), ptr(grad_y), ptr(w), ptr(bs), mean.data_ptr(), var.data_ptr(),
+              sums.data_ptr(), ptr(dw), ptr(db), ws.data_ptr())
+    return sums, dw, db
+
+
+def backward_gathered(gathered: torch.Tensor, grad_y: torch.Tensor, x: torch.Tensor, weight, bias, mean, var, eps: float,
+                      relu: bool) -> torch.Tensor:
+    """grad_x (contiguous fp32) from the group's gathered (world, C, 3) (n, S1, S2)."""
+    c = int(x.shape[1])
+    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
+    dx = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
+    d = _desc(x, True, relu, eps)
+    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
+    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
+    _lib.call("fiery_batch_norm_backward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), ptr(x), ptr(grad_y), ptr(w),
+              ptr(bs), mean.data_ptr(), var.data_ptr(), ptr(dx), ws.data_ptr())
+    return dx
+
+
+class SyncBatchNormAct(torch.autograd.Function):
+    """``relu(batch_norm(x)) + residual`` with a group's statistics: local stats, one ``gather``, apply; the backward local sums, one
+    ``gather`` (when x needs its gradient), grad apply.  ``gather`` maps a (C, 3) fp64 tensor to the (world, C, 3) of every rank's,
+    in rank order.  Returns (y, mean, var, count), the last three not differentiable."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, eps: float, relu: bool, gather):
+        xs = f32_planes(x)
+        gathered = gather(local_stats(xs))
+        y, mean, var, count = forward_gathered(gathered, xs, weight, bias, residual, eps, relu)
+        ctx.mark_non_differentiable(mean, var, count)
+        ctx.eps, ctx.relu, ctx.gather = eps, relu, gather
+        ctx.x_dtype = x.dtype
+        ctx.residual_dtype = residual.dtype if residual is not None else None
+        ctx.save_for_backward(xs, weight, bias, mean, var)
+        return y, mean, var, count
+
+    @staticmethod
+    def backward(ctx, grad_y, _gm, _gv, _gc):
+        xs, weight, bias, mean, var = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = f32(grad_y)
+        sums, dw, db = local_grad_sums(g, xs, weight, bias, mean, var, ctx.eps, ctx.relu, bool(need[1]), bool(need[2]))
+        dx = None
+        if need[0]:
+            dx = backward_gathered(ctx.gather(sums), g, xs, weight, bias, mean, var, ctx.eps, ctx.relu).to(ctx.x_dtype)
+        cast = lambda t, like: t.to(like.dtype) if t is not None else None           # noqa: E731
+        grad_r = grad_y.to(ctx.residual_dtype) if need[3] else None
+        return dx, cast(dw, weight), cast(db, bias), grad_r, None, None, None
+
+
+def sync_group(norm: nn.Module):
+    """The process group whose statistics ``norm`` (a SyncBatchNorm) uses in this call, or None when it uses its own batch's:
+    torch's rule -- training with batch statistics, torch.distributed initialized, and a group of more than one rank."""
+    import torch.distributed as dist
+    batch_stats = norm.training or (norm.running_mean is None and norm.running_var is None)
+    if not (batch_stats and norm.training and dist.is_available() and dist.is_initialized()):
+        return None
+    group = norm.process_group if norm.process_group is not None else dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+class FusedSyncBatchNorm(nn.SyncBatchNorm):
+    """Drop-in for an ``nn.SyncBatchNorm`` that runs on the batch-norm kernels.  It adopts the module's Parameters, buffers and
+    ``process_group`` (the same objects: ``state_dict`` keys are unchanged).  When ``SyncBatchNorm`` would synchronize (training, batch
+    statistics, torch.distributed initialized, a group of more than one rank) it runs ``SyncBatchNormAct``: every rank's (n, mean, M2)
+    gathered and merged in rank order on the device, one gather forward and one backward, the running statistics moved with the
+    group's count without a host synchronisation.  Otherwise it computes exactly what ``FusedBatchNorm3d`` does.  Inputs of any rank
+    >= 2 are read as (b, C, 1, 1, rest) unless they are 5-D.  ``forward_act(x, relu, residual)`` is the fused entry."""
+
+    def __init__(self, bn: nn.SyncBatchNorm):
+        nn.Module.__init__(self)
+        for name in ("num_features", "eps", "momentum", "affine", "track_running_stats", "process_group"):
+            setattr(self, name, getattr(bn, name))
+        for name, p in bn._parameters.items():
+            self.register_parameter(name, p)
+        for name, b in bn._buffers.items():
+            self.register_buffer(name, b, persistent=name not in bn._non_persistent_buffers_set)
+        self.train(bn.training)
+
+    def forward(self, input: torch.Tensor) -> torch.Tensor:
+        return self.forward_act(input, relu=False)
+
+    def forward_act(self, x: torch.Tensor, relu: bool, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+        self._check_input_dim(x)
+        shape = x.shape
+        if x.dim() != 5:                                  # the trailing dims' product, not -1: an empty rank's x has 0 elements
+            x = x.reshape(shape[0], shape[1], 1, 1, math.prod(shape[2:]))
+            residual = residual.reshape(x.shape) if residual is not None else None
+        group = sync_group(self)
+        if group is None:
+            y = FusedBatchNorm3d.forward_act(self, x, relu, residual)
+        else:
+            _require_cuda(x, "x")
+            y, mean, var, count = SyncBatchNormAct.apply(x, self.weight, self.bias, residual, self.eps, relu,
+                                                           lambda t: gather(t, group))
+            self.update_running_stats(mean, var, count)
+        return y.reshape(shape)
+
+    def update_running_stats(self, mean: torch.Tensor, var: torch.Tensor, n) -> None:
+        """``update_running_stats(self, mean, var, n)``."""
+        update_running_stats(self, mean, var, n)
 
 
 def norm_act(norm: nn.Module, activation: nn.Module, y: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``activation(norm(y))``, plus ``residual`` when given (``residual + activation(norm(y))``): one fused apply when the norm is a
-    ``FusedBatchNorm3d`` and the activation an ``nn.ReLU``, otherwise exactly those module calls and that add."""
-    if isinstance(norm, FusedBatchNorm3d) and isinstance(activation, nn.ReLU):
+    ``FusedBatchNorm3d`` or a ``FusedSyncBatchNorm`` and the activation an ``nn.ReLU``, otherwise exactly those module calls and that
+    add."""
+    if isinstance(norm, (FusedBatchNorm3d, FusedSyncBatchNorm)) and isinstance(activation, nn.ReLU):
         return norm.forward_act(y, relu=True, residual=residual)
     out = activation(norm(y))
     return out if residual is None else residual + out

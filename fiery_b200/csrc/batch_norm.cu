@@ -108,6 +108,21 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_stats_kernel(const
     }
 }
 
+// Chan's merge of channel c's pieces' (count, mean, M2) in ascending (b, t, piece) order, in fp64
+__device__ __forceinline__ void bn_merge_pieces(const BnShape& s, const float2* __restrict__ part, int c, double& n, double& m, double& m2) {
+    n = m = m2 = 0.0;
+    const float2* pc = part + c * s.per_channel;
+    for (long long k = 0; k < s.per_channel; ++k) {
+        const int j = static_cast<int>(k % s.per_plane);
+        const double nb = static_cast<double>(min(BN_PIECE, s.pixels - j * BN_PIECE));
+        const float2 pk = pc[k];
+        const double delta = static_cast<double>(pk.x) - m, nn = n + nb;
+        m += delta * (nb / nn);
+        m2 += static_cast<double>(pk.y) + delta * delta * (n * nb / nn);
+        n = nn;
+    }
+}
+
 // One thread per channel.  training: Chan's merge of the pieces' (count, mean, M2) in fp64 -> mean and biased variance; eval: the
 // running statistics.  Writes the fp32 statistics and the forward's coefficients.
 __global__ void bn_finalize_forward_kernel(const BnShape s, const float2* __restrict__ part, const float* __restrict__ w,
@@ -118,17 +133,8 @@ __global__ void bn_finalize_forward_kernel(const BnShape s, const float2* __rest
     if (c >= s.channels) return;
     float mean, var;
     if (training) {
-        double n = 0.0, m = 0.0, m2 = 0.0;
-        const float2* pc = part + c * s.per_channel;
-        for (long long k = 0; k < s.per_channel; ++k) {
-            const int j = static_cast<int>(k % s.per_plane);
-            const double nb = static_cast<double>(min(BN_PIECE, s.pixels - j * BN_PIECE));
-            const float2 pk = pc[k];
-            const double delta = static_cast<double>(pk.x) - m, nn = n + nb;
-            m += delta * (nb / nn);
-            m2 += static_cast<double>(pk.y) + delta * delta * (n * nb / nn);
-            n = nn;
-        }
+        double n, m, m2;
+        bn_merge_pieces(s, part, c, n, m, m2);
         mean = static_cast<float>(m);
         var = static_cast<float>(m2 / n);
     } else {
@@ -481,6 +487,162 @@ int launch_gru_blend_backward(const fiery_batch_norm_desc_t* d, const float* x, 
                               float* da, float* dgu, long long dsb, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
     gru_blend_grad_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, w, bias, mean, var, d->eps, u, h, hsb, go, gsb, carry, da, dgu, dsb);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// Statistics over several ranks (fiery_batch_norm_*_gathered, fiery_spatial_gru_*_step_*).  Each rank reduces its own pieces as
+// above into one fp64 triplet per channel -- (n, mean, M2) forward, (n, S1, S2) backward -- the caller gathers the ranks' triplets
+// into (world, channels, 3), and the gathered finalize merges them in ascending rank order with the same formulas, starting from
+// rank 0's triplet (so one rank gives exactly the single-rank finalize's numbers).  A rank with no values has n = 0 and adds nothing.
+// ------------------------------------------------------------------------------------------------------------------------------
+__global__ void bn_local_forward_kernel(const BnShape s, const float2* __restrict__ part, double* __restrict__ stats) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= s.channels) return;
+    double n, m, m2;
+    bn_merge_pieces(s, part, c, n, m, m2);
+    stats[3 * c] = n;
+    stats[3 * c + 1] = m;
+    stats[3 * c + 2] = m2;
+}
+
+__global__ void bn_gathered_forward_kernel(int world, int channels, const double* __restrict__ gathered, const float* __restrict__ w,
+                                           const float* __restrict__ bias, double eps, float* __restrict__ mean_out,
+                                           float* __restrict__ var_out, double* __restrict__ count_out, BnCoef* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= channels) return;
+    double n = gathered[3 * c], m = gathered[3 * c + 1], m2 = gathered[3 * c + 2];
+    for (int r = 1; r < world; ++r) {
+        const double* g = gathered + (static_cast<long long>(r) * channels + c) * 3;
+        const double nb = g[0];
+        if (nb == 0.0) continue;
+        const double delta = g[1] - m, nn = n + nb;
+        m += delta * (nb / nn);
+        m2 += g[2] + delta * delta * (n * nb / nn);
+        n = nn;
+    }
+    const float mean = static_cast<float>(m), var = static_cast<float>(m2 / n);
+    mean_out[c] = mean;
+    var_out[c] = var;
+    if (c == 0 && count_out) *count_out = n;
+    BnCoef k;
+    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
+    k.mean = mean;
+    k.k1 = k.k0 = 0.f;
+    coef[c] = k;
+}
+
+// the rank's (n, S1, S2) and its own weight and bias gradients (S2 / sqrt(var + eps), S1: the local sums, as torch's SyncBatchNorm)
+__global__ void bn_local_backward_kernel(const BnShape s, const float2* __restrict__ part, const float* __restrict__ var, double eps,
+                                         float* __restrict__ grad_w, float* __restrict__ grad_b, double* __restrict__ sums) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= s.channels) return;
+    double s1 = 0.0, s2 = 0.0;                                 // bn_finalize_backward_kernel's sums, in its order
+    const float2* pc = part + c * s.per_channel;
+    for (long long k = 0; k < s.per_channel; ++k) {
+        const float2 pk = pc[k];
+        s1 += static_cast<double>(pk.x);
+        s2 += static_cast<double>(pk.y);
+    }
+    const double ve = static_cast<double>(var[c]) + eps;
+    if (grad_w) grad_w[c] = static_cast<float>(s2 / sqrt(ve));
+    if (grad_b) grad_b[c] = static_cast<float>(s1);
+    sums[3 * c] = static_cast<double>(s.per_channel / s.per_plane) * s.pixels;
+    sums[3 * c + 1] = s1;
+    sums[3 * c + 2] = s2;
+}
+
+__global__ void bn_gathered_backward_kernel(int world, int channels, const double* __restrict__ gathered, const float* __restrict__ w,
+                                            const float* __restrict__ bias, const float* __restrict__ mean, const float* __restrict__ var,
+                                            double eps, BnCoef* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= channels) return;
+    double n = gathered[3 * c], s1 = gathered[3 * c + 1], s2 = gathered[3 * c + 2];
+    for (int r = 1; r < world; ++r) {
+        const double* g = gathered + (static_cast<long long>(r) * channels + c) * 3;
+        n += g[0];
+        s1 += g[1];
+        s2 += g[2];
+    }
+    BnCoef k;
+    k.mean = mean[c];
+    const float v = var[c];
+    bn_scale_shift(w, bias, k.mean, v, eps, c, k.scale, k.shift);
+    const double ve = static_cast<double>(v) + eps;
+    k.k1 = static_cast<float>(-static_cast<double>(k.scale) * s2 / (n * ve));
+    k.k0 = static_cast<float>(-static_cast<double>(k.scale) * s1 / n);
+    coef[c] = k;
+}
+
+int launch_batch_norm_local_stats(const fiery_batch_norm_desc_t* d, const float* x, double* stats, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    if (s.pieces) bn_stats_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, part);
+    bn_local_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, stats);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* w,
+                                       const float* bias, const float* residual, float* y, float* mean_out, float* var_out,
+                                       double* count_out, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    const unsigned grid = bn_grid(s);
+    bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
+                                                                              var_out, count_out, coef);
+    if (s.pieces) {
+        if (d->relu) {
+            if (residual) bn_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+            else bn_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+        } else {
+            if (residual) bn_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+            else bn_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+        }
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
+                                      const float* mean, const float* var, double* sums, float* grad_w, float* grad_b, void* workspace,
+                                      cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    const unsigned grid = bn_grid(s);
+    if (s.pieces) {
+        if (d->relu) bn_grad_sums_kernel<true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+        else bn_grad_sums_kernel<false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+    }
+    bn_local_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, var, d->eps, grad_w, grad_b, sums);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* dy,
+                                        const float* w, const float* bias, const float* mean, const float* var, float* dx, void* workspace,
+                                        cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    bn_gathered_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, mean, var, d->eps, coef);
+    if (s.pieces) {
+        if (d->relu) bn_grad_apply_kernel<true, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+        else bn_grad_apply_kernel<false, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+// the spatial GRU's step under gathered statistics: the finalize above, then the blend into the output frame
+int launch_gru_blend_forward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* w,
+                                      const float* bias, const float* u, const float* h, long long hsb, float* out, long long osb,
+                                      float* mean_out, float* var_out, double* count_out, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
+                                                                              var_out, count_out, coef);
+    gru_blend_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, u, h, hsb, out, osb);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

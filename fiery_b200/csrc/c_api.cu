@@ -1,5 +1,6 @@
 // extern "C" boundary of libfiery_b200.so (declared in include/fiery_b200.h).  Argument validation, TMA descriptor
 // creation and launch dispatch; no torch types, no host<->device copies except where the header says so.
+#include <initializer_list>
 #include <stdarg.h>
 #include <string.h>
 
@@ -148,6 +149,33 @@ int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, 
 int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
                                const float* mean, const float* var, float* dx, float* grad_w, float* grad_b, void* workspace,
                                cudaStream_t stream);
+int launch_batch_norm_local_stats(const fiery_batch_norm_desc_t* d, const float* x, double* stats, void* workspace, cudaStream_t stream);
+int launch_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* w,
+                                       const float* bias, const float* residual, float* y, float* mean_out, float* var_out,
+                                       double* count_out, void* workspace, cudaStream_t stream);
+int launch_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
+                                      const float* mean, const float* var, double* sums, float* grad_w, float* grad_b, void* workspace,
+                                      cudaStream_t stream);
+int launch_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* dy,
+                                        const float* w, const float* bias, const float* mean, const float* var, float* dx, void* workspace,
+                                        cudaStream_t stream);
+int launch_spatial_gru_forward_step_begin(const fiery_spatial_gru_desc_t* d, int t, const float* x, const float* h0, const float* packed,
+                                          const float* b_gates, const float* out, float* saved, double* stats, void* workspace,
+                                          cudaStream_t stream);
+int launch_spatial_gru_forward_step_end(const fiery_spatial_gru_desc_t* d, int t, int world, const double* gathered, const float* h0,
+                                        const float* bn_w, const float* bn_b, float* out, const float* saved_c, float* means, float* vars,
+                                        double* count_out, void* workspace, cudaStream_t stream);
+int launch_spatial_gru_backward_step_begin(const fiery_spatial_gru_desc_t* d, int t, const float* grad_out, const float* h0, const float* out,
+                                           const float* saved_c, const float* means, const float* vars, const float* packed,
+                                           const float* bn_w, const float* bn_b, float* grad_h0, double* sums, void* workspace,
+                                           cudaStream_t stream);
+int launch_spatial_gru_backward_step_end(const fiery_spatial_gru_desc_t* d, int t, int world, const double* gathered, const float* h0,
+                                         const float* out, const float* saved_c, const float* means, const float* vars, const float* packed,
+                                         const float* bn_w, const float* bn_b, float* grad_x, float* grad_h0, void* workspace,
+                                         cudaStream_t stream);
+int launch_spatial_gru_backward_weights(const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* out, const float* saved_c,
+                                        const float* packed, float* grad_w_gates, float* grad_b_gates, float* grad_w_state, float* grad_bn_w,
+                                        float* grad_bn_b, void* workspace, cudaStream_t stream);
 int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w, float* packed, cudaStream_t stream);
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
 int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
@@ -658,22 +686,87 @@ FIERY_API int fiery_causal_conv3d_backward_weight(const fiery_causal_conv3d_desc
     return launch_causal_conv_wgrad(desc, x, grad_y, grad_w, workspace, static_cast<cudaStream_t>(stream));
 }
 
-// The batch norm's shape limits, one place for every entry point.  The messages name the field.
-static int check_batch_norm_desc(const fiery_batch_norm_desc_t* d) {
+// The batch norm's shape limits, one place for every entry point.  The messages name the field.  sync: the entries of a rank in a
+// group (fiery_batch_norm_*_gathered and their local phases), which take training only and a rank with no or a single value.
+static int check_batch_norm_desc(const fiery_batch_norm_desc_t* d, bool sync = false) {
     FIERY_REQUIRE(d, "batch norm: NULL desc");
     FIERY_REQUIRE(d->channels >= 1, "batch norm: channels = %d must be >= 1", d->channels);
-    FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0 && static_cast<long long>(d->batch) * d->frames >= 1,
-                  "batch norm: batch = %d, frames = %d must be >= 0 with batch * frames >= 1", d->batch, d->frames);
+    if (sync)
+        FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0, "batch norm: batch = %d, frames = %d must be >= 0", d->batch, d->frames);
+    else
+        FIERY_REQUIRE(d->batch >= 0 && d->frames >= 0 && static_cast<long long>(d->batch) * d->frames >= 1,
+                      "batch norm: batch = %d, frames = %d must be >= 0 with batch * frames >= 1", d->batch, d->frames);
     FIERY_REQUIRE(d->pixels >= 1, "batch norm: pixels X*Y = %d must be >= 1", d->pixels);
     FIERY_REQUIRE(d->stride_b >= 0 && d->stride_c >= 0 && d->stride_t >= 0, "batch norm: strides (%lld, %lld, %lld) must be >= 0",
                   (long long)d->stride_b, (long long)d->stride_c, (long long)d->stride_t);
+    if (sync) FIERY_REQUIRE(d->training == 1, "batch norm: training = %d must be 1 for statistics over a group", d->training);
     FIERY_REQUIRE(d->training == 0 || d->training == 1, "batch norm: training = %d must be 0 or 1", d->training);
     FIERY_REQUIRE(d->relu == 0 || d->relu == 1, "batch norm: relu = %d must be 0 or 1", d->relu);
     FIERY_REQUIRE(d->eps >= 0.0, "batch norm: eps = %g must be >= 0", d->eps);
-    FIERY_REQUIRE(!d->training || static_cast<long long>(d->batch) * d->frames * d->pixels >= 2,
+    FIERY_REQUIRE(sync || !d->training || static_cast<long long>(d->batch) * d->frames * d->pixels >= 2,
                   "batch norm: n = batch * frames * pixels = %lld values per channel must be >= 2 in training",
                   static_cast<long long>(d->batch) * d->frames * d->pixels);
     return FIERY_OK;
+}
+
+static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+
+static int check_world(int world, const double* gathered, const char* what) {
+    FIERY_REQUIRE(world >= 1, "%s: world = %d must be >= 1", what, world);
+    FIERY_REQUIRE(gathered, "%s: NULL gathered", what);
+    FIERY_REQUIRE(aligned8(gathered), "%s: gathered must be 8-byte aligned", what);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_batch_norm_sync_workspace_bytes(const fiery_batch_norm_desc_t* desc) {
+    if (check_batch_norm_desc(desc, true) != FIERY_OK) return 0;
+    return batch_norm_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_batch_norm_local_stats(const fiery_batch_norm_desc_t* desc, const float* x, double* stats, void* workspace, void* stream) {
+    const int rc = check_batch_norm_desc(desc, true);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE((x || desc->batch == 0 || desc->frames == 0) && stats && workspace, "batch norm: NULL x / stats / workspace");
+    FIERY_REQUIRE(aligned8(stats) && aligned16(workspace), "batch norm: stats must be 8-byte and workspace 16-byte aligned");
+    return launch_batch_norm_local_stats(desc, x, stats, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* desc, int32_t world, const double* gathered, const float* x,
+                                                const float* weight, const float* bias, const float* residual, float* y, float* mean_out,
+                                                float* var_out, double* count_out, void* workspace, void* stream) {
+    int rc = check_batch_norm_desc(desc, true);
+    if (rc != FIERY_OK || (rc = check_world(world, gathered, "batch norm")) != FIERY_OK) return rc;
+    const bool empty = desc->batch == 0 || desc->frames == 0;
+    FIERY_REQUIRE(((x && y) || empty) && mean_out && var_out && workspace, "batch norm: NULL x / y / mean_out / var_out / workspace");
+    FIERY_REQUIRE(aligned16(workspace) && (!count_out || aligned8(count_out)),
+                  "batch norm: workspace must be 16-byte and count_out 8-byte aligned");
+    return launch_batch_norm_forward_gathered(desc, world, gathered, x, weight, bias, residual, y, mean_out, var_out, count_out, workspace,
+                                              static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* desc, const float* x, const float* grad_y, const float* weight,
+                                               const float* bias, const float* mean, const float* var, double* sums, float* grad_weight,
+                                               float* grad_bias, void* workspace, void* stream) {
+    const int rc = check_batch_norm_desc(desc, true);
+    if (rc != FIERY_OK) return rc;
+    const bool empty = desc->batch == 0 || desc->frames == 0;
+    FIERY_REQUIRE(((x && grad_y) || empty) && mean && var && sums && workspace, "batch norm: NULL x / grad_y / mean / var / sums / workspace");
+    FIERY_REQUIRE(aligned8(sums) && aligned16(workspace), "batch norm: sums must be 8-byte and workspace 16-byte aligned");
+    return launch_batch_norm_local_grad_sums(desc, x, grad_y, weight, bias, mean, var, sums, grad_weight, grad_bias, workspace,
+                                             static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* desc, int32_t world, const double* gathered, const float* x,
+                                                 const float* grad_y, const float* weight, const float* bias, const float* mean,
+                                                 const float* var, float* grad_x, void* workspace, void* stream) {
+    int rc = check_batch_norm_desc(desc, true);
+    if (rc != FIERY_OK || (rc = check_world(world, gathered, "batch norm")) != FIERY_OK) return rc;
+    const bool empty = desc->batch == 0 || desc->frames == 0;
+    FIERY_REQUIRE(((x && grad_y && grad_x) || empty) && mean && var && workspace,
+                  "batch norm: NULL x / grad_y / grad_x / mean / var / workspace");
+    FIERY_REQUIRE(aligned16(workspace), "batch norm: workspace must be 16-byte aligned");
+    return launch_batch_norm_backward_gathered(desc, world, gathered, x, grad_y, weight, bias, mean, var, grad_x, workspace,
+                                               static_cast<cudaStream_t>(stream));
 }
 
 FIERY_API size_t fiery_batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* desc) {
@@ -783,6 +876,77 @@ FIERY_API int fiery_spatial_gru_backward(const fiery_spatial_gru_desc_t* desc, c
     return launch_spatial_gru_backward(desc, grad_out, x, h0, out, static_cast<const float*>(saved), means, vars,
                                        static_cast<const float*>(packed), bn_weight, bn_bias, grad_x, grad_h0, grad_w_gates, grad_b_gates,
                                        grad_w_state, grad_bn_weight, grad_bn_bias, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// the per-step entries' common checks: the desc in training, the step, and the 16-byte aligned pointers (NULL where allowed)
+static int check_spatial_gru_step(const fiery_spatial_gru_desc_t* d, int t, std::initializer_list<const void*> required,
+                                  std::initializer_list<const void*> optional) {
+    const int rc = check_spatial_gru_desc(d);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(d->training == 1, "spatial GRU: training = %d must be 1 for statistics over a group", d->training);
+    FIERY_REQUIRE(t >= 0 && t < d->frames, "spatial GRU: t = %d must be in 0..frames - 1 = %d", t, d->frames - 1);
+    for (const void* p : required) FIERY_REQUIRE(p, "spatial GRU: NULL pointer");
+    for (const void* p : required) FIERY_REQUIRE(aligned16(p), "spatial GRU: pointers must be 16-byte aligned");
+    for (const void* p : optional) FIERY_REQUIRE(!p || aligned16(p), "spatial GRU: pointers must be 16-byte aligned");
+    return FIERY_OK;
+}
+
+FIERY_API int fiery_spatial_gru_forward_step_begin(const fiery_spatial_gru_desc_t* desc, int32_t t, const float* x, const float* h0,
+                                                   const void* packed, const float* b_gates, const float* out, void* saved, double* stats,
+                                                   void* workspace, void* stream) {
+    const int rc = check_spatial_gru_step(desc, t, {x, h0, packed, out, saved, workspace}, {});
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(b_gates && stats, "spatial GRU: NULL b_gates / stats");
+    FIERY_REQUIRE(aligned8(stats), "spatial GRU: stats must be 8-byte aligned");
+    return launch_spatial_gru_forward_step_begin(desc, t, x, h0, static_cast<const float*>(packed), b_gates, out, static_cast<float*>(saved),
+                                                 stats, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_spatial_gru_forward_step_end(const fiery_spatial_gru_desc_t* desc, int32_t t, int32_t world, const double* gathered,
+                                                 const float* h0, const float* bn_weight, const float* bn_bias, float* out, const void* saved,
+                                                 float* means, float* vars, double* count_out, void* workspace, void* stream) {
+    int rc = check_spatial_gru_step(desc, t, {h0, out, saved, workspace}, {});
+    if (rc != FIERY_OK || (rc = check_world(world, gathered, "spatial GRU")) != FIERY_OK) return rc;
+    FIERY_REQUIRE(means && vars, "spatial GRU: NULL means / vars");
+    FIERY_REQUIRE(!count_out || aligned8(count_out), "spatial GRU: count_out must be 8-byte aligned");
+    return launch_spatial_gru_forward_step_end(desc, t, world, gathered, h0, bn_weight, bn_bias, out, static_cast<const float*>(saved), means,
+                                               vars, count_out, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_spatial_gru_backward_step_begin(const fiery_spatial_gru_desc_t* desc, int32_t t, const float* grad_out, const float* h0,
+                                                    const float* out, const void* saved, const float* means, const float* vars,
+                                                    const void* packed, const float* bn_weight, const float* bn_bias, float* grad_h0,
+                                                    double* sums, void* workspace, void* stream) {
+    const int rc = check_spatial_gru_step(desc, t, {grad_out, h0, out, saved, packed, workspace}, {grad_h0});
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(means && vars && sums, "spatial GRU: NULL means / vars / sums");
+    FIERY_REQUIRE(aligned8(sums), "spatial GRU: sums must be 8-byte aligned");
+    return launch_spatial_gru_backward_step_begin(desc, t, grad_out, h0, out, static_cast<const float*>(saved), means, vars,
+                                                  static_cast<const float*>(packed), bn_weight, bn_bias, grad_h0, sums, workspace,
+                                                  static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_spatial_gru_backward_step_end(const fiery_spatial_gru_desc_t* desc, int32_t t, int32_t world, const double* gathered,
+                                                  const float* h0, const float* out, const void* saved, const float* means, const float* vars,
+                                                  const void* packed, const float* bn_weight, const float* bn_bias, float* grad_x,
+                                                  float* grad_h0, void* workspace, void* stream) {
+    int rc = check_spatial_gru_step(desc, t, {h0, out, saved, packed, workspace}, {grad_x, grad_h0});
+    if (rc != FIERY_OK || (rc = check_world(world, gathered, "spatial GRU")) != FIERY_OK) return rc;
+    FIERY_REQUIRE(means && vars, "spatial GRU: NULL means / vars");
+    return launch_spatial_gru_backward_step_end(desc, t, world, gathered, h0, out, static_cast<const float*>(saved), means, vars,
+                                                static_cast<const float*>(packed), bn_weight, bn_bias, grad_x, grad_h0, workspace,
+                                                static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_spatial_gru_backward_weights(const fiery_spatial_gru_desc_t* desc, const float* x, const float* h0, const float* out,
+                                                 const void* saved, const void* packed, float* grad_w_gates, float* grad_b_gates,
+                                                 float* grad_w_state, float* grad_bn_weight, float* grad_bn_bias, void* workspace,
+                                                 void* stream) {
+    const int rc = check_spatial_gru_step(desc, 0, {x, h0, out, saved, packed, workspace}, {});
+    if (rc != FIERY_OK) return rc;
+    return launch_spatial_gru_backward_weights(desc, x, h0, out, static_cast<const float*>(saved), static_cast<const float*>(packed),
+                                               grad_w_gates, grad_b_gates, grad_w_state, grad_bn_weight, grad_bn_bias, workspace,
+                                               static_cast<cudaStream_t>(stream));
 }
 
 // The 3x3 convolution's limits, one place for every entry point.  The messages name the field.

@@ -34,6 +34,16 @@ size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d);
 int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
                                const float* mean, const float* var, float* dx, float* grad_w, float* grad_b, void* workspace,
                                cudaStream_t stream);
+int launch_batch_norm_local_stats(const fiery_batch_norm_desc_t* d, const float* x, double* stats, void* workspace, cudaStream_t stream);
+int launch_gru_blend_forward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* w,
+                                      const float* bias, const float* u, const float* h, long long hsb, float* out, long long osb,
+                                      float* mean_out, float* var_out, double* count_out, void* workspace, cudaStream_t stream);
+int launch_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* d, const float* x, const float* dy, const float* w, const float* bias,
+                                      const float* mean, const float* var, double* sums, float* grad_w, float* grad_b, void* workspace,
+                                      cudaStream_t stream);
+int launch_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* dy,
+                                        const float* w, const float* bias, const float* mean, const float* var, float* dx, void* workspace,
+                                        cudaStream_t stream);
 
 // accumulator columns of an output width: the instantiated N
 static int gru_n(int n) { return n <= 64 ? cc_round8(n) : (n <= 96 ? 96 : 128); }
@@ -237,62 +247,127 @@ size_t spatial_gru_forward_workspace_bytes(const fiery_spatial_gru_desc_t* d) {
     return batch_norm_workspace_bytes(&bn);
 }
 
+// The forward's maps and launches, set up once per call; gru_fwd_convs then runs step t's two convolutions.
+struct GruFwd {
+    GruGeom g;
+    GruPacks P;
+    GruSaved S;
+    long long osb, ssb;
+    CUtensorMap m_h0, m_out;
+    CcFwdMaps gate, state;
+    CcFwdLaunch Lg, Ls;
+    long long n_tiles;
+    fiery_batch_norm_desc_t bn;
+};
+
+static int gru_fwd_setup(const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* packed, const float* out,
+                         float* saved, GruFwd& F) {
+    const GruGeom& g = F.g = gru_geom(d);
+    const GruPacks& P = F.P = gru_packs(d);
+    F.S = gru_saved(saved, g);
+    F.osb = static_cast<long long>(g.T) * g.ch * g.XY;
+    F.ssb = g.ch * g.XY;
+    const long long xst = g.Tx > 1 ? d->x_stride_t : 0;
+    int rc;
+    CUtensorMap m_x, m_q;
+    if ((rc = gru_halo_map(&m_x, x, g, g.Tx, g.cx, g.Tx > 1 ? xst : g.XY, d->x_stride_c, d->x_stride_b, P.gate_f.kpad[0], "spatial GRU x")) ||
+        (rc = gru_halo_map(&F.m_h0, h0, g, 1, g.ch, g.XY, g.XY, F.ssb, P.gate_f.kpad[1], "spatial GRU h0")) ||
+        (rc = gru_halo_map(&F.m_out, out, g, g.T, g.ch, F.ssb, g.XY, F.osb, P.gate_f.kpad[1], "spatial GRU output")) ||
+        (rc = gru_halo_map(&m_q, F.S.q, g, g.T, g.ch, g.map_ch, g.XY, F.ssb, P.state_f.kpad[1], "spatial GRU q")))
+        return rc;
+    if ((rc = gru_weight_map(&F.gate.w, packed + P.off[0], P.gate_f)) || (rc = gru_weight_map(&F.state.w, packed + P.off[2], P.state_f)))
+        return rc;
+    F.Lg = gru_launch(g, P.gate_f);
+    F.Ls = gru_launch(g, P.state_f);
+    F.Lg.nseg = 2;
+    F.Lg.bias_init = d->bias_init;
+    F.Ls.nseg = 1;
+    F.n_tiles = static_cast<long long>(g.b) * F.Lg.tiles_x * F.Lg.tiles_y;
+    F.bn = gru_bn_desc(d, g);
+    F.gate.x[0] = m_x;
+    F.state.x[0] = m_x;
+    F.state.x[1] = m_q;
+    return FIERY_OK;
+}
+
+// step t's input state: h0 at t = 0, else out[:, t - 1], and its batch stride
+static const float* gru_h(const GruGeom& g, int t, const float* h0, const float* out, long long& hsb) {
+    hsb = t == 0 ? g.ch * g.XY : static_cast<long long>(g.T) * g.ch * g.XY;
+    return t == 0 ? h0 : out + static_cast<size_t>(t - 1) * g.ch * g.XY;
+}
+
+// step t's gates ([x_t, h] -> u, and r with q = (1 - r) h) and state convolution ([x_t, q] -> s)
+static int gru_fwd_convs(GruFwd& F, int t, const float* h0, const float* out, const float* b_gates, cudaStream_t stream) {
+    const GruGeom& g = F.g;
+    const size_t so = static_cast<size_t>(t) * g.map_ch;
+    long long hsb;
+    const float* h = gru_h(g, t, h0, out, hsb);
+    const int tx = g.Tx > 1 ? t : 0;
+    int rc;
+    F.gate.x[1] = t == 0 ? F.m_h0 : F.m_out;
+    F.Lg.t_off[0] = tx;
+    F.Lg.t_off[1] = t == 0 ? 0 : t - 1;
+    F.Lg.seg[0] = gru_seg(F.S.u + so, F.ssb, g.XY, 0, g.ch, CC_GATE_U);
+    F.Lg.seg[0].bias = b_gates;
+    F.Lg.seg[1] = gru_seg(F.S.q + so, F.ssb, g.XY, cc_round8(g.ch), g.ch, CC_GATE_R);
+    F.Lg.seg[1].bias = b_gates + g.ch;
+    F.Lg.seg[1].h = h;
+    F.Lg.seg[1].hsb = hsb;
+    F.Lg.seg[1].r = F.S.r + so;
+    F.Lg.seg[1].rsb = F.ssb;
+    if ((rc = cc_launch_fwd(F.P.gate_f.n, true, F.gate, F.Lg, F.n_tiles, stream)) != FIERY_OK) return rc;
+    F.Ls.t_off[0] = tx;
+    F.Ls.t_off[1] = t;
+    F.Ls.seg[0] = gru_seg(F.S.s + so, F.ssb, g.XY, 0, g.ch, CC_STORE);
+    return cc_launch_fwd(F.P.state_f.n, true, F.state, F.Ls, F.n_tiles, stream);
+}
+
 int launch_spatial_gru_forward(const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* packed, const float* b_gates,
                                const float* bn_w, const float* bn_b, const float* running_mean, const float* running_var, float* out,
                                float* saved, float* means, float* vars, void* workspace, cudaStream_t stream) {
-    const GruGeom g = gru_geom(d);
-    const GruPacks P = gru_packs(d);
-    const GruSaved S = gru_saved(saved, g);
-    const long long osb = static_cast<long long>(g.T) * g.ch * g.XY, ssb = g.ch * g.XY;
-    const long long xst = g.Tx > 1 ? d->x_stride_t : 0;
+    GruFwd F;
     int rc;
-    CUtensorMap m_x, m_h0, m_out, m_q;
-    if ((rc = gru_halo_map(&m_x, x, g, g.Tx, g.cx, g.Tx > 1 ? xst : g.XY, d->x_stride_c, d->x_stride_b, P.gate_f.kpad[0], "spatial GRU x")) ||
-        (rc = gru_halo_map(&m_h0, h0, g, 1, g.ch, g.XY, g.XY, ssb, P.gate_f.kpad[1], "spatial GRU h0")) ||
-        (rc = gru_halo_map(&m_out, out, g, g.T, g.ch, ssb, g.XY, osb, P.gate_f.kpad[1], "spatial GRU output")) ||
-        (rc = gru_halo_map(&m_q, S.q, g, g.T, g.ch, g.map_ch, g.XY, ssb, P.state_f.kpad[1], "spatial GRU q")))
-        return rc;
-    CcFwdMaps gate, state;
-    if ((rc = gru_weight_map(&gate.w, packed + P.off[0], P.gate_f)) || (rc = gru_weight_map(&state.w, packed + P.off[2], P.state_f))) return rc;
-    CcFwdLaunch Lg = gru_launch(g, P.gate_f), Ls = gru_launch(g, P.state_f);
-    Lg.nseg = 2;
-    Lg.bias_init = d->bias_init;
-    Ls.nseg = 1;
-    const long long n_tiles = static_cast<long long>(g.b) * Lg.tiles_x * Lg.tiles_y;
-    const fiery_batch_norm_desc_t bn = gru_bn_desc(d, g);
-    gate.x[0] = m_x;
-    state.x[0] = m_x;
-    state.x[1] = m_q;
+    if ((rc = gru_fwd_setup(d, x, h0, packed, out, saved, F)) != FIERY_OK) return rc;
+    const GruGeom& g = F.g;
     for (int t = 0; t < g.T; ++t) {
         const size_t so = static_cast<size_t>(t) * g.map_ch;
-        const float* h = t == 0 ? h0 : out + static_cast<size_t>(t - 1) * g.ch * g.XY;
-        const long long hsb = t == 0 ? ssb : osb;
-        const int tx = g.Tx > 1 ? t : 0;
-        // gates: [x_t, h] -> u, and r with q = (1 - r) h
-        gate.x[1] = t == 0 ? m_h0 : m_out;
-        Lg.t_off[0] = tx;
-        Lg.t_off[1] = t == 0 ? 0 : t - 1;
-        Lg.seg[0] = gru_seg(S.u + so, ssb, g.XY, 0, g.ch, CC_GATE_U);
-        Lg.seg[0].bias = b_gates;
-        Lg.seg[1] = gru_seg(S.q + so, ssb, g.XY, cc_round8(g.ch), g.ch, CC_GATE_R);
-        Lg.seg[1].bias = b_gates + g.ch;
-        Lg.seg[1].h = h;
-        Lg.seg[1].hsb = hsb;
-        Lg.seg[1].r = S.r + so;
-        Lg.seg[1].rsb = ssb;
-        if ((rc = cc_launch_fwd(P.gate_f.n, true, gate, Lg, n_tiles, stream)) != FIERY_OK) return rc;
-        // state: [x_t, q] -> s
-        Ls.t_off[0] = tx;
-        Ls.t_off[1] = t;
-        Ls.seg[0] = gru_seg(S.s + so, ssb, g.XY, 0, g.ch, CC_STORE);
-        if ((rc = cc_launch_fwd(P.state_f.n, true, state, Ls, n_tiles, stream)) != FIERY_OK) return rc;
+        long long hsb;
+        const float* h = gru_h(g, t, h0, out, hsb);
+        if ((rc = gru_fwd_convs(F, t, h0, out, b_gates, stream)) != FIERY_OK) return rc;
         // norm, ReLU and the blend into out[:, t]
-        if ((rc = launch_gru_blend_forward(&bn, S.s + so, bn_w, bn_b, running_mean, running_var, S.u + so, h, hsb,
-                                           out + static_cast<size_t>(t) * g.ch * g.XY, osb, means + static_cast<size_t>(t) * g.ch,
+        if ((rc = launch_gru_blend_forward(&F.bn, F.S.s + so, bn_w, bn_b, running_mean, running_var, F.S.u + so, h, hsb,
+                                           out + static_cast<size_t>(t) * g.ch * g.XY, F.osb, means + static_cast<size_t>(t) * g.ch,
                                            vars + static_cast<size_t>(t) * g.ch, workspace, stream)) != FIERY_OK)
             return rc;
     }
     return FIERY_OK;
+}
+
+// The forward one step at a time, for statistics gathered over several ranks between the two calls: begin runs step t's
+// convolutions and writes the rank's (n, mean, M2) of s; end merges the gathered triplets and blends into out[:, t].
+int launch_spatial_gru_forward_step_begin(const fiery_spatial_gru_desc_t* d, int t, const float* x, const float* h0, const float* packed,
+                                          const float* b_gates, const float* out, float* saved, double* stats, void* workspace,
+                                          cudaStream_t stream) {
+    GruFwd F;
+    int rc;
+    if ((rc = gru_fwd_setup(d, x, h0, packed, out, saved, F)) != FIERY_OK) return rc;
+    if ((rc = gru_fwd_convs(F, t, h0, out, b_gates, stream)) != FIERY_OK) return rc;
+    return launch_batch_norm_local_stats(&F.bn, F.S.s + static_cast<size_t>(t) * F.g.map_ch, stats, workspace, stream);
+}
+
+int launch_spatial_gru_forward_step_end(const fiery_spatial_gru_desc_t* d, int t, int world, const double* gathered, const float* h0,
+                                        const float* bn_w, const float* bn_b, float* out, const float* saved_c, float* means, float* vars,
+                                        double* count_out, void* workspace, cudaStream_t stream) {
+    const GruGeom g = gru_geom(d);
+    const GruSaved S = gru_saved(const_cast<float*>(saved_c), g);
+    const fiery_batch_norm_desc_t bn = gru_bn_desc(d, g);
+    const size_t so = static_cast<size_t>(t) * g.map_ch;
+    long long hsb;
+    const float* h = gru_h(g, t, h0, out, hsb);
+    return launch_gru_blend_forward_gathered(&bn, world, gathered, S.s + so, bn_w, bn_b, S.u + so, h, hsb,
+                                             out + static_cast<size_t>(t) * g.ch * g.XY, static_cast<long long>(g.T) * g.ch * g.XY,
+                                             means + static_cast<size_t>(t) * g.ch, vars + static_cast<size_t>(t) * g.ch, count_out,
+                                             workspace, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -401,70 +476,171 @@ static int gru_wgrad(const GruGeom& g, const fiery_spatial_gru_desc_t* d, const 
     return cc_wgrad_reduce(s, partial, chunks, gw, stream);
 }
 
+// The backward's maps and launches, set up once per call over the workspace W; gru_bwd_blend and gru_bwd_dgrads then run step t's
+// parts, gru_bwd_weights the gradients over all steps.  The state gradient `carry` is grad_h0 when it is asked for, else W.carry.
+struct GruBwd {
+    GruGeom g;
+    GruPacks P;
+    GruSaved S;
+    GruBwdWs W;
+    long long osb, ssb, gsb, xsb;
+    CcFwdMaps gate, state;
+    CcFwdLaunch Lg, Ls;
+    long long n_tiles;
+    fiery_batch_norm_desc_t bn;
+};
+
+static int gru_bwd_setup(const fiery_spatial_gru_desc_t* d, const float* saved_c, const float* packed, void* workspace, GruBwd& B) {
+    const GruGeom& g = B.g = gru_geom(d);
+    const GruPacks& P = B.P = gru_packs(d);
+    B.S = gru_saved(const_cast<float*>(saved_c), g);
+    B.W = gru_bwd_ws(d, workspace);
+    B.osb = static_cast<long long>(g.T) * g.ch * g.XY;
+    B.ssb = g.ch * g.XY;
+    B.gsb = 2 * B.ssb;
+    B.xsb = static_cast<long long>(g.Tx) * g.cx * g.XY;     // grad_x: contiguous (b, Tx, cx, X, Y)
+    B.bn = gru_bn_desc(d, g);
+    int rc;
+    CUtensorMap m_ds, m_dgu, m_dgr;
+    if ((rc = gru_halo_map(&m_ds, B.W.ds, g, g.T, g.ch, g.map_ch, g.XY, B.ssb, P.state_t.kpad[0], "spatial GRU ds")) ||
+        (rc = gru_halo_map(&m_dgu, B.W.dg, g, g.T, g.ch, 2 * g.map_ch, g.XY, B.gsb, P.gate_t.kpad[0], "spatial GRU dG_u")) ||
+        (rc = gru_halo_map(&m_dgr, B.W.dg + g.ch * g.XY, g, g.T, g.ch, 2 * g.map_ch, g.XY, B.gsb, P.gate_t.kpad[1], "spatial GRU dG_r")))
+        return rc;
+    if ((rc = gru_weight_map(&B.gate.w, packed + P.off[1], P.gate_t)) || (rc = gru_weight_map(&B.state.w, packed + P.off[3], P.state_t)))
+        return rc;
+    B.gate.x[0] = m_dgu;
+    B.gate.x[1] = m_dgr;
+    B.state.x[0] = m_ds;
+    B.state.x[1] = m_ds;
+    B.Lg = gru_launch(g, P.gate_t);
+    B.Ls = gru_launch(g, P.state_t);
+    B.Lg.nseg = 2;
+    B.Ls.nseg = 2;
+    B.n_tiles = static_cast<long long>(g.b) * B.Lg.tiles_x * B.Lg.tiles_y;
+    return FIERY_OK;
+}
+
+// step t's dh' = grad_out[:, t] + carry -> W.da, dG_u and the new carry
+static int gru_bwd_blend(GruBwd& B, int t, const float* grad_out, const float* h0, const float* out, const float* means, const float* vars,
+                         const float* bn_w, const float* bn_b, float* carry, cudaStream_t stream) {
+    const GruGeom& g = B.g;
+    const size_t so = static_cast<size_t>(t) * g.map_ch;
+    long long hsb;
+    const float* h = gru_h(g, t, h0, out, hsb);
+    return launch_gru_blend_backward(&B.bn, B.S.s + so, bn_w, bn_b, means + static_cast<size_t>(t) * g.ch, vars + static_cast<size_t>(t) * g.ch,
+                                     B.S.u + so, h, hsb, grad_out + static_cast<size_t>(t) * g.ch * g.XY, B.osb, carry, B.W.da,
+                                     B.W.dg + 2 * so, B.gsb, stream);
+}
+
+// step t's input gradients from its ds: the state dgrad (ds -> [dx_t, dq]; dq -> dG_r, carry), then the gates' ([dG_u, dG_r] ->
+// [dx_t, dh], both added)
+static int gru_bwd_dgrads(GruBwd& B, int t, const float* h0, const float* out, float* grad_x, float* carry, cudaStream_t stream) {
+    const GruGeom& g = B.g;
+    const size_t so = static_cast<size_t>(t) * g.map_ch;
+    long long hsb;
+    const float* h = gru_h(g, t, h0, out, hsb);
+    float* dg_t = B.W.dg + 2 * so;
+    const int tx = g.Tx > 1 ? t : 0;
+    float* dx_t = grad_x ? grad_x + static_cast<size_t>(tx) * g.cx * g.XY : nullptr;
+    const bool first_dx = g.Tx > 1 || t == g.T - 1;       // the state dgrad is the first write of this dx frame
+    int rc;
+    B.Ls.t_off[0] = t;
+    B.Ls.seg[0] = gru_seg(dx_t, B.xsb, g.XY, 0, g.cx, grad_x ? (first_dx ? CC_STORE : CC_ADD) : CC_SKIP);
+    B.Ls.seg[1] = gru_seg(carry, B.ssb, g.XY, cc_round8(g.cx), g.ch, CC_RESET_GRAD);
+    B.Ls.seg[1].h = h;
+    B.Ls.seg[1].hsb = hsb;
+    B.Ls.seg[1].r = B.S.r + so;
+    B.Ls.seg[1].rsb = B.ssb;
+    B.Ls.seg[1].aux = dg_t + g.ch * g.XY;
+    B.Ls.seg[1].asb = B.gsb;
+    if ((rc = cc_launch_fwd(B.P.state_t.n, true, B.state, B.Ls, B.n_tiles, stream)) != FIERY_OK) return rc;
+    B.Lg.t_off[0] = t;
+    B.Lg.t_off[1] = t;
+    B.Lg.seg[0] = gru_seg(dx_t, B.xsb, g.XY, 0, g.cx, grad_x ? CC_ADD : CC_SKIP);
+    B.Lg.seg[1] = gru_seg(carry, B.ssb, g.XY, cc_round8(g.cx), g.ch, CC_ADD);
+    return cc_launch_fwd(B.P.gate_t.n, true, B.gate, B.Lg, B.n_tiles, stream);
+}
+
+static int gru_bwd_weights(GruBwd& B, const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* out,
+                           float* grad_w_gates, float* grad_b_gates, float* grad_w_state, float* grad_bn_w, float* grad_bn_b,
+                           cudaStream_t stream);
+
 int launch_spatial_gru_backward(const fiery_spatial_gru_desc_t* d, const float* grad_out, const float* x, const float* h0, const float* out,
                                 const float* saved_c, const float* means, const float* vars, const float* packed, const float* bn_w,
                                 const float* bn_b, float* grad_x, float* grad_h0, float* grad_w_gates, float* grad_b_gates,
                                 float* grad_w_state, float* grad_bn_w, float* grad_bn_b, void* workspace, cudaStream_t stream) {
-    const GruGeom g = gru_geom(d);
-    const GruPacks P = gru_packs(d);
-    const GruSaved S = gru_saved(const_cast<float*>(saved_c), g);
-    const GruBwdWs W = gru_bwd_ws(d, workspace);
-    const long long osb = static_cast<long long>(g.T) * g.ch * g.XY, ssb = g.ch * g.XY, gsb = 2 * ssb;
-    const long long xsb = static_cast<long long>(g.Tx) * g.cx * g.XY;     // grad_x: contiguous (b, Tx, cx, X, Y)
-    const fiery_batch_norm_desc_t bn = gru_bn_desc(d, g);
-    float* carry = grad_h0 ? grad_h0 : W.carry;
-    FIERY_CUDA_CHECK(cudaMemsetAsync(carry, 0, static_cast<size_t>(g.map_ch) * 4, stream));
+    GruBwd B;
     int rc;
-    CUtensorMap m_ds, m_dgu, m_dgr, m_out, m_h0, m_q;
-    if ((rc = gru_halo_map(&m_ds, W.ds, g, g.T, g.ch, g.map_ch, g.XY, ssb, P.state_t.kpad[0], "spatial GRU ds")) ||
-        (rc = gru_halo_map(&m_dgu, W.dg, g, g.T, g.ch, 2 * g.map_ch, g.XY, gsb, P.gate_t.kpad[0], "spatial GRU dG_u")) ||
-        (rc = gru_halo_map(&m_dgr, W.dg + g.ch * g.XY, g, g.T, g.ch, 2 * g.map_ch, g.XY, gsb, P.gate_t.kpad[1], "spatial GRU dG_r")))
-        return rc;
-    CcFwdMaps gate, state;
-    if ((rc = gru_weight_map(&gate.w, packed + P.off[1], P.gate_t)) || (rc = gru_weight_map(&state.w, packed + P.off[3], P.state_t))) return rc;
-    gate.x[0] = m_dgu;
-    gate.x[1] = m_dgr;
-    state.x[0] = m_ds;
-    state.x[1] = m_ds;
-    CcFwdLaunch Lg = gru_launch(g, P.gate_t), Ls = gru_launch(g, P.state_t);
-    Lg.nseg = 2;
-    Ls.nseg = 2;
-    const long long n_tiles = static_cast<long long>(g.b) * Lg.tiles_x * Lg.tiles_y;
+    if ((rc = gru_bwd_setup(d, saved_c, packed, workspace, B)) != FIERY_OK) return rc;
+    const GruGeom& g = B.g;
+    float* carry = grad_h0 ? grad_h0 : B.W.carry;
+    FIERY_CUDA_CHECK(cudaMemsetAsync(carry, 0, static_cast<size_t>(g.map_ch) * 4, stream));
     for (int t = g.T - 1; t >= 0; --t) {
         const size_t so = static_cast<size_t>(t) * g.map_ch;
-        const float* h = t == 0 ? h0 : out + static_cast<size_t>(t - 1) * g.ch * g.XY;
-        const long long hsb = t == 0 ? ssb : osb;
-        float* dg_t = W.dg + 2 * so;
         // dh' -> da, dG_u, carry; then the norm's backward -> ds
-        if ((rc = launch_gru_blend_backward(&bn, S.s + so, bn_w, bn_b, means + static_cast<size_t>(t) * g.ch, vars + static_cast<size_t>(t) * g.ch,
-                                            S.u + so, h, hsb, grad_out + static_cast<size_t>(t) * g.ch * g.XY, osb, carry, W.da, dg_t, gsb,
-                                            stream)) != FIERY_OK)
+        if ((rc = gru_bwd_blend(B, t, grad_out, h0, out, means, vars, bn_w, bn_b, carry, stream)) != FIERY_OK) return rc;
+        if ((rc = launch_batch_norm_backward(&B.bn, B.S.s + so, B.W.da, bn_w, bn_b, means + static_cast<size_t>(t) * g.ch,
+                                             vars + static_cast<size_t>(t) * g.ch, B.W.ds + so, B.W.dgam + static_cast<size_t>(t) * g.ch,
+                                             B.W.dbet + static_cast<size_t>(t) * g.ch, B.W.bn, stream)) != FIERY_OK)
             return rc;
-        if ((rc = launch_batch_norm_backward(&bn, S.s + so, W.da, bn_w, bn_b, means + static_cast<size_t>(t) * g.ch,
-                                             vars + static_cast<size_t>(t) * g.ch, W.ds + so, W.dgam + static_cast<size_t>(t) * g.ch,
-                                             W.dbet + static_cast<size_t>(t) * g.ch, W.bn, stream)) != FIERY_OK)
-            return rc;
-        const int tx = g.Tx > 1 ? t : 0;
-        float* dx_t = grad_x ? grad_x + static_cast<size_t>(tx) * g.cx * g.XY : nullptr;
-        const bool first_dx = g.Tx > 1 || t == g.T - 1;       // the state dgrad is the first write of this dx frame
-        // state dgrad: ds -> [dx_t, dq]; dq -> dG_r, carry
-        Ls.t_off[0] = t;
-        Ls.seg[0] = gru_seg(dx_t, xsb, g.XY, 0, g.cx, grad_x ? (first_dx ? CC_STORE : CC_ADD) : CC_SKIP);
-        Ls.seg[1] = gru_seg(carry, ssb, g.XY, cc_round8(g.cx), g.ch, CC_RESET_GRAD);
-        Ls.seg[1].h = h;
-        Ls.seg[1].hsb = hsb;
-        Ls.seg[1].r = S.r + so;
-        Ls.seg[1].rsb = ssb;
-        Ls.seg[1].aux = dg_t + g.ch * g.XY;
-        Ls.seg[1].asb = gsb;
-        if ((rc = cc_launch_fwd(P.state_t.n, true, state, Ls, n_tiles, stream)) != FIERY_OK) return rc;
-        // gate dgrad: [dG_u, dG_r] -> [dx_t, dh], both added
-        Lg.t_off[0] = t;
-        Lg.t_off[1] = t;
-        Lg.seg[0] = gru_seg(dx_t, xsb, g.XY, 0, g.cx, grad_x ? CC_ADD : CC_SKIP);
-        Lg.seg[1] = gru_seg(carry, ssb, g.XY, cc_round8(g.cx), g.ch, CC_ADD);
-        if ((rc = cc_launch_fwd(P.gate_t.n, true, gate, Lg, n_tiles, stream)) != FIERY_OK) return rc;
+        if ((rc = gru_bwd_dgrads(B, t, h0, out, grad_x, carry, stream)) != FIERY_OK) return rc;
     }
+    return gru_bwd_weights(B, d, x, h0, out, grad_w_gates, grad_b_gates, grad_w_state, grad_bn_w, grad_bn_b, stream);
+}
+
+// The backward one step at a time (t = T-1 .. 0), for statistics gathered over several ranks between the two calls: begin runs the
+// blend's gradient and writes the rank's (n, S1, S2) of the norm's backward (and the step's local dgamma, dbeta); end merges the
+// gathered triplets into ds and runs the step's input gradients.  The workspace and grad_h0 (or NULL) are the same in every call.
+int launch_spatial_gru_backward_step_begin(const fiery_spatial_gru_desc_t* d, int t, const float* grad_out, const float* h0, const float* out,
+                                           const float* saved_c, const float* means, const float* vars, const float* packed,
+                                           const float* bn_w, const float* bn_b, float* grad_h0, double* sums, void* workspace,
+                                           cudaStream_t stream) {
+    GruBwd B;
+    int rc;
+    if ((rc = gru_bwd_setup(d, saved_c, packed, workspace, B)) != FIERY_OK) return rc;
+    const GruGeom& g = B.g;
+    float* carry = grad_h0 ? grad_h0 : B.W.carry;
+    if (t == g.T - 1) FIERY_CUDA_CHECK(cudaMemsetAsync(carry, 0, static_cast<size_t>(g.map_ch) * 4, stream));
+    if ((rc = gru_bwd_blend(B, t, grad_out, h0, out, means, vars, bn_w, bn_b, carry, stream)) != FIERY_OK) return rc;
+    return launch_batch_norm_local_grad_sums(&B.bn, B.S.s + static_cast<size_t>(t) * g.map_ch, B.W.da, bn_w, bn_b,
+                                             means + static_cast<size_t>(t) * g.ch, vars + static_cast<size_t>(t) * g.ch, sums,
+                                             B.W.dgam + static_cast<size_t>(t) * g.ch, B.W.dbet + static_cast<size_t>(t) * g.ch, B.W.bn, stream);
+}
+
+int launch_spatial_gru_backward_step_end(const fiery_spatial_gru_desc_t* d, int t, int world, const double* gathered, const float* h0,
+                                         const float* out, const float* saved_c, const float* means, const float* vars, const float* packed,
+                                         const float* bn_w, const float* bn_b, float* grad_x, float* grad_h0, void* workspace,
+                                         cudaStream_t stream) {
+    GruBwd B;
+    int rc;
+    if ((rc = gru_bwd_setup(d, saved_c, packed, workspace, B)) != FIERY_OK) return rc;
+    const GruGeom& g = B.g;
+    const size_t so = static_cast<size_t>(t) * g.map_ch;
+    if ((rc = launch_batch_norm_backward_gathered(&B.bn, world, gathered, B.S.s + so, B.W.da, bn_w, bn_b, means + static_cast<size_t>(t) * g.ch,
+                                                  vars + static_cast<size_t>(t) * g.ch, B.W.ds + so, B.W.bn, stream)) != FIERY_OK)
+        return rc;
+    return gru_bwd_dgrads(B, t, h0, out, grad_x, grad_h0 ? grad_h0 : B.W.carry, stream);
+}
+
+int launch_spatial_gru_backward_weights(const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* out, const float* saved_c,
+                                        const float* packed, float* grad_w_gates, float* grad_b_gates, float* grad_w_state, float* grad_bn_w,
+                                        float* grad_bn_b, void* workspace, cudaStream_t stream) {
+    GruBwd B;
+    int rc;
+    if ((rc = gru_bwd_setup(d, saved_c, packed, workspace, B)) != FIERY_OK) return rc;
+    return gru_bwd_weights(B, d, x, h0, out, grad_w_gates, grad_b_gates, grad_w_state, grad_bn_w, grad_bn_b, stream);
+}
+
+// the weight gradients over all steps, the gates' bias gradient, and dgamma, dbeta summed over the steps in ascending order
+static int gru_bwd_weights(GruBwd& B, const fiery_spatial_gru_desc_t* d, const float* x, const float* h0, const float* out,
+                           float* grad_w_gates, float* grad_b_gates, float* grad_w_state, float* grad_bn_w, float* grad_bn_b,
+                           cudaStream_t stream) {
+    const GruGeom& g = B.g;
+    const GruBwdWs& W = B.W;
+    const long long osb = B.osb, ssb = B.ssb;
+    const GruSaved& S = B.S;
+    int rc;
+    CUtensorMap m_out, m_h0, m_q;
     if (grad_w_gates || grad_w_state) {
         const long long bst[4] = {g.Y, ssb, g.XY, osb};
         const long long hst[4] = {g.Y, ssb, g.XY, ssb};

@@ -20,7 +20,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import _require_cuda, f32
-from .batch_norm import update_running_stats
+from .batch_norm import FusedSyncBatchNorm, gather, sync_group, update_running_stats
 
 MAX_CHANNELS = 64
 
@@ -166,6 +166,129 @@ def backward(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b,
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
+# the GRU with each step's statistics over a process group (its norm a FusedSyncBatchNorm): one gather per step each way.  One rank's
+# passes are generators: each yields the step's (C, 3) fp64 triplet and is sent back the group's (world, C, 3), so autograd drives
+# one of them with a collective (``run_steps``) and a test can drive several in lockstep.
+# ------------------------------------------------------------------------------------------------------------------------------
+def run_steps(steps, gather):
+    """Run the generator ``steps`` to its end, answering each triplet it yields with ``gather(triplet)``; returns its result."""
+    try:
+        triplet = next(steps)
+        while True:
+            triplet = steps.send(gather(triplet))
+    except StopIteration as done:
+        return done.value
+
+
+def sync_forward_steps(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames: int, eps: float, bias_init: float):
+    """One rank's training forward over ``frames`` steps through the per-step entries (fiery_spatial_gru_forward_step_*): per step it
+    yields this rank's (n, mean, M2) of s and takes the group's gathered triplets.  Returns (out, means, vars, counts, saved), counts
+    (frames,) fp64 on the device, each step's group count.  A rank with batch 0 yields n = 0 and takes the group's statistics."""
+    _require_cuda(x, "x")
+    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dev = x.device
+    means = torch.empty((frames, ch), dtype=torch.float32, device=dev)
+    var = torch.empty((frames, ch), dtype=torch.float32, device=dev)
+    counts = torch.empty(frames, dtype=torch.float64, device=dev)
+    out = torch.empty((b, frames, ch, h, w), dtype=torch.float32, device=dev)
+    if b == 0:
+        from .batch_norm import forward_gathered
+        empty = torch.empty((0, ch, 1, h, w), dtype=torch.float32, device=dev)
+        for t in range(frames):
+            gathered = yield torch.zeros((ch, 3), dtype=torch.float64, device=dev)
+            _, means[t], var[t], counts[t:t + 1] = forward_gathered(gathered, empty, bn_w, bn_b, None, eps, True)
+        return out, means, var, counts, torch.empty(0, dtype=torch.uint8, device=dev)
+    xs, hs = gru_input(x), _aligned_f32(h0)
+    d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), True, eps, bias_init)
+    lib = _lib.load()
+    saved = torch.empty(int(lib.fiery_spatial_gru_saved_bytes(d)), dtype=torch.uint8, device=dev)
+    bias = torch.cat([b_u.detach(), b_r.detach()]).float()
+    bw, bb = _per_channel(bn_w), _per_channel(bn_b)
+    packed = _packed(w_u, w_r, w_s)
+    ws = _lib.workspace(lib.fiery_spatial_gru_forward_workspace_bytes(d), dev)           # kept across the steps
+    for t in range(frames):
+        stats = torch.empty((ch, 3), dtype=torch.float64, device=dev)
+        _lib.call("fiery_spatial_gru_forward_step_begin", dev, d, t, xs.data_ptr(), hs.data_ptr(), packed.data_ptr(), bias.data_ptr(),
+                  out.data_ptr(), saved.data_ptr(), stats.data_ptr(), ws.data_ptr())
+        gathered = yield stats
+        _lib.call("fiery_spatial_gru_forward_step_end", dev, d, t, int(gathered.shape[0]), gathered.data_ptr(), hs.data_ptr(), _ptr(bw),
+                  _ptr(bb), out.data_ptr(), saved.data_ptr(), means.data_ptr(), var.data_ptr(), counts[t:].data_ptr(), ws.data_ptr())
+    return out, means, var, counts, saved
+
+
+def sync_backward_steps(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b, frames: int, eps: float, bias_init: float,
+                        need):
+    """The gradients of ``sync_forward_steps`` (``need``: 9 flags for x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b): per step, t = T-1 ..
+    0, it yields this rank's (n, S1, S2) and takes the group's gathered triplets, then runs the weight gradients.  Returns (grad_x,
+    grad_h0, grad_w_u, grad_b_u, grad_w_r, grad_b_r, grad_w_s, grad_bn_w, grad_bn_b), None where not asked for; the parameter
+    gradients are this rank's own (the local sums, as torch's).  With grad_h0 not asked for, the carried gradient lives in the
+    workspace."""
+    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dev = x.device
+    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
+    gx = new(b, tx, cx, h, w) if need[0] else None
+    gh = new(b, ch, h, w) if need[1] else None
+    gwg, gbg = (new(2 * ch, cx + ch, 3, 3), new(2 * ch)) if any(need[2:6]) else (None, None)
+    gws = new(ch, cx + ch, 3, 3) if need[6] else None
+    bw, bb = _per_channel(bn_w), _per_channel(bn_b)
+    gbw = new(ch) if need[7] and bw is not None else None
+    gbb = new(ch) if need[8] and bb is not None else None
+    if b == 0:
+        for _ in range(frames):
+            yield torch.zeros((ch, 3), dtype=torch.float64, device=dev)
+        for g in (gx, gh, gwg, gbg, gws, gbw, gbb):
+            if g is not None:
+                g.zero_()
+    else:
+        xs, hs = gru_input(x), _aligned_f32(h0)
+        d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), True, eps, bias_init)
+        lib = _lib.load()
+        go = _aligned_f32(grad_out) if grad_out is not None else torch.zeros_like(out)
+        packed = _packed(w_u, w_r, w_s)
+        ws = _lib.workspace(lib.fiery_spatial_gru_backward_workspace_bytes(d), dev)      # kept across the steps and the weights call
+        for t in reversed(range(frames)):
+            sums = torch.empty((ch, 3), dtype=torch.float64, device=dev)
+            _lib.call("fiery_spatial_gru_backward_step_begin", dev, d, t, go.data_ptr(), hs.data_ptr(), out.data_ptr(), saved.data_ptr(),
+                      means.data_ptr(), var.data_ptr(), packed.data_ptr(), _ptr(bw), _ptr(bb), _ptr(gh), sums.data_ptr(), ws.data_ptr())
+            gathered = yield sums
+            _lib.call("fiery_spatial_gru_backward_step_end", dev, d, t, int(gathered.shape[0]), gathered.data_ptr(), hs.data_ptr(),
+                      out.data_ptr(), saved.data_ptr(), means.data_ptr(), var.data_ptr(), packed.data_ptr(), _ptr(bw), _ptr(bb), _ptr(gx),
+                      _ptr(gh), ws.data_ptr())
+        _lib.call("fiery_spatial_gru_backward_weights", dev, d, xs.data_ptr(), hs.data_ptr(), out.data_ptr(), saved.data_ptr(),
+                  packed.data_ptr(), _ptr(gwg), _ptr(gbg), _ptr(gws), _ptr(gbw), _ptr(gbb), ws.data_ptr())
+    cast = lambda g, like: g.to(like.dtype) if g is not None else None           # noqa: E731
+    split = lambda g: (cast(g[:ch], w_u), cast(g[ch:], w_u)) if g is not None else (None, None)  # noqa: E731
+    (gwu, gwr), (gbu, gbr) = split(gwg), split(gbg)
+    return cast(gx, x), cast(gh, h0), gwu, gbu, gwr, gbr, cast(gws, w_s), cast(gbw, bn_w), cast(gbb, bn_b)
+
+
+class SyncSpatialGRU(torch.autograd.Function):
+    """The SpatialGRU in training over ``frames`` steps with each step's batch statistics over a group: ``sync_forward_steps`` and
+    ``sync_backward_steps`` run with ``gather``, which maps a (C, 3) fp64 tensor to the (world, C, 3) of every rank's, in rank order.
+    Returns (out, means, vars, counts): counts (frames,) fp64, each step's group count, on the device."""
+
+    @staticmethod
+    def forward(ctx, x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames: int, eps: float, bias_init: float, gather):
+        out, means, var, counts, saved = run_steps(
+            sync_forward_steps(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames, eps, bias_init), gather)
+        ctx.mark_non_differentiable(means, var, counts)
+        ctx.args = (frames, eps, bias_init, gather)
+        ctx.save_for_backward(x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b)
+        return out, means, var, counts
+
+    @staticmethod
+    def backward(ctx, grad_out, _gm, _gv, _gc):
+        x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b = ctx.saved_tensors
+        frames, eps, bias_init, gather = ctx.args
+        need = tuple(bool(n) for n in ctx.needs_input_grad[:9])
+        if not any(need):
+            return (None,) * 13
+        grads = run_steps(sync_backward_steps(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b, frames, eps, bias_init,
+                                              need), gather)
+        return grads + (None,) * 4
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
 # the 3x3 convolution on its own (fiery_conv3x3_*): the GRU's kernels with plain stores, for tests and benchmarks
 # ------------------------------------------------------------------------------------------------------------------------------
 def conv3x3_desc(maps: int, h: int, w: int, in_channels, out_channels) -> _lib.Conv3x3Desc:
@@ -217,8 +340,9 @@ def module_reason(gru) -> Optional[str]:
         return f"{type(gru).__name__} does not have the SpatialGRU structure"
     if not (_is_conv3x3(cu, True) and _is_conv3x3(cr, True) and _is_conv3x3(st.conv, False)):
         return "the convolutions are not 3x3 with padding 1 and stride 1 (gates with a bias, the state without)"
-    if type(getattr(st, "norm", None)) is not nn.BatchNorm2d:
-        return f"norm {type(getattr(st, 'norm', None)).__name__} (the kernels take BatchNorm2d)"
+    norm = getattr(st, "norm", None)
+    if not (type(norm) is nn.BatchNorm2d or isinstance(norm, FusedSyncBatchNorm)):
+        return f"norm {type(norm).__name__} (the kernels take BatchNorm2d, or a SyncBatchNorm swapped by use_fused_sync_batch_norm)"
     if type(getattr(st, "activation", None)) is not nn.ReLU:
         return f"activation {type(getattr(st, 'activation', None)).__name__} (the kernels take ReLU)"
     cx, ch = int(gru.input_size), int(gru.hidden_size)
@@ -231,7 +355,8 @@ class TensorCoreSpatialGRU(nn.Module):
     """Drop-in for a reference ``SpatialGRU`` whose T steps run as ``torch.ops.fiery_b200.spatial_gru``.  It holds the reference
     module's ``conv_update``, ``conv_reset`` and ``conv_state_tilde`` under the same names (``state_dict`` keys unchanged, the
     Parameters shared) and looks them up at call time.  The norm's running statistics move once per step, in step order, as
-    ``nn.BatchNorm2d`` moves them.  ``state=None`` starts from zeros, as the reference does.  A map whose width is not a multiple of
+    ``nn.BatchNorm2d`` moves them.  A norm swapped to ``FusedSyncBatchNorm`` that synchronizes in this call runs ``SyncSpatialGRU``:
+    each step's statistics over its process group, one gather per step each way.  ``state=None`` starts from zeros, as the reference does.  A map whose width is not a multiple of
     4, a ``flow``, a CPU input, or a norm or activation changed after the swap (e.g. by ``SyncBatchNorm.convert_sync_batchnorm``) runs
     the reference's own forward, with one warning."""
 
@@ -276,6 +401,15 @@ class TensorCoreSpatialGRU(nn.Module):
         if x.stride(4) != 1 or x.stride(3) != w:
             x = x.contiguous()                        # a map broadcast over the pixels: materialized once, read by forward and backward
         bn = self.conv_state_tilde.norm
+        group = sync_group(bn) if isinstance(bn, FusedSyncBatchNorm) else None
+        if group is not None:
+            out, means, var, counts = SyncSpatialGRU.apply(
+                x, state, self.conv_update.weight, self.conv_update.bias, self.conv_reset.weight, self.conv_reset.bias,
+                self.conv_state_tilde.conv.weight, bn.weight, bn.bias, frames, bn.eps, float(self.gru_bias_init),
+                lambda t: gather(t, group))
+            for t in range(frames):
+                update_running_stats(bn, means[t], var[t], counts[t:t + 1])
+            return out
         batch_stats = bn.training or (bn.running_mean is None and bn.running_var is None)
         out, means, var, _saved = torch.ops.fiery_b200.spatial_gru(
             x, state, self.conv_update.weight, self.conv_update.bias, self.conv_reset.weight, self.conv_reset.bias,

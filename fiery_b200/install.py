@@ -225,23 +225,56 @@ def use_fused_batch_norm(model):
     Parameters and buffers (``state_dict`` keys unchanged) and runs on the batch-norm kernels.  In a ``TensorCoreTemporalBlock`` and a
     ``TensorCoreCausalConv3d`` the ReLU after each norm, and the block's skip add, then run in the norm's apply pass.  The pyramid
     pooling's ``conv_bn_relu`` (a (b, R, s + 1, 1, 1) tensor) keeps its ``nn.BatchNorm3d``.  A ``SyncBatchNorm`` is left as it is, with
-    one warning: cross-rank statistics are not covered.  Works before or after the other temporal swaps; a second call does nothing.
-    Returns the model."""
-    from .batch_norm import FusedBatchNorm3d
+    one warning (``use_fused_sync_batch_norm`` swaps those); a ``FusedSyncBatchNorm`` is left as it is, silently.  Works before or
+    after the other temporal swaps; a second call does nothing.  Returns the model."""
+    from .batch_norm import FusedBatchNorm3d, FusedSyncBatchNorm
 
+    def reason(norm):
+        return "per-rank statistics" if isinstance(norm, torch.nn.SyncBatchNorm) else None
+    # the warning's text gives the one reason, so it lists the skipped norms by name only; a FusedSyncBatchNorm is already swapped
+    return _swap(model, _temporal_norms(torch.nn.BatchNorm3d, any_sync=True), (FusedBatchNorm3d, FusedSyncBatchNorm), reason,
+                 FusedBatchNorm3d, "fiery_b200: SyncBatchNorm module(s) left as they are (use_fused_batch_norm computes per-rank "
+                 "statistics only; use_fused_sync_batch_norm swaps them): ", entry="{where}", sep=", ")
+
+
+def _temporal_norms(kind, any_sync: bool = False):
+    """``_swap``'s slots for every module of type exactly ``kind`` (and, with ``any_sync``, every ``nn.SyncBatchNorm``) under the
+    temporal model, but the pyramid pooling's."""
     def slots(blocks):
         for name, parent in blocks.named_modules():
             for key, child in parent.named_children():
                 where = f"{name}.{key}" if name else key
-                if "pyramid_pooling" not in where.split(".") and (type(child) is torch.nn.BatchNorm3d
-                                                                  or isinstance(child, torch.nn.SyncBatchNorm)):
+                if "pyramid_pooling" not in where.split(".") and (type(child) is kind
+                                                                  or (any_sync and isinstance(child, torch.nn.SyncBatchNorm))):
                     yield parent, key, child, where
+    return slots
 
-    def reason(norm):
-        return "per-rank statistics" if isinstance(norm, torch.nn.SyncBatchNorm) else None
-    # the warning's text gives the one reason, so it lists the skipped norms by name only
-    return _swap(model, slots, FusedBatchNorm3d, reason, FusedBatchNorm3d, "fiery_b200: SyncBatchNorm module(s) left as they are (the "
-                 "fused batch norm computes per-rank statistics only): ", entry="{where}", sep=", ")
+
+def use_fused_sync_batch_norm(model):
+    """Replace every module of type exactly ``nn.SyncBatchNorm`` under ``model.temporal_model.model`` that ``use_fused_batch_norm``
+    would swap were it a ``BatchNorm3d`` (the pyramid pooling's stays), and the ``conv_state_tilde.norm`` of every SpatialGRU in
+    ``model.future_prediction.spatial_grus`` (the reference's or a ``TensorCoreSpatialGRU``), by
+    ``fiery_b200.batch_norm.FusedSyncBatchNorm``.  It adopts the module's Parameters, buffers and ``process_group`` (``state_dict``
+    keys unchanged) and gathers every rank's statistics and merges them on the kernels, as ``SyncBatchNorm`` would synchronize them;
+    a swapped GRU then runs one gather per step each way.  Call it after ``SyncBatchNorm.convert_sync_batchnorm``; it works before or
+    after the other temporal swaps and ``use_tensor_core_future_prediction`` (which then accepts the GRUs), and a second call does
+    nothing.  Returns the model."""
+    from .batch_norm import FusedSyncBatchNorm
+    temporal = lambda m: _temporal_blocks(m) if hasattr(m, "temporal_model") else None      # noqa: E731  (a model may have none)
+    _swap(model, _temporal_norms(torch.nn.SyncBatchNorm), FusedSyncBatchNorm, lambda m: None, FusedSyncBatchNorm, "", root=temporal)
+
+    def gru_norms(grus):
+        for i, (_, gru) in enumerate(grus._modules.items()):
+            st = getattr(gru, "conv_state_tilde", None)
+            norm = getattr(st, "norm", None) if st is not None else None
+            if type(norm) is torch.nn.SyncBatchNorm:
+                yield st, "norm", norm, f"spatial_grus[{i}]"
+    return _swap(model, gru_norms, FusedSyncBatchNorm, lambda m: None, FusedSyncBatchNorm, "", root=_spatial_grus)
+
+
+def _spatial_grus(model):
+    fp = getattr(model, "future_prediction", None)
+    return getattr(fp, "spatial_grus", None) if fp is not None else None
 
 
 def use_tensor_core_future_prediction(model):
@@ -256,12 +289,8 @@ def use_tensor_core_future_prediction(model):
     def slots(grus):
         for i, (name, gru) in enumerate(grus._modules.items()):
             yield grus, name, gru, f"spatial_grus[{i}]"
-
-    def root(m):
-        fp = getattr(m, "future_prediction", None)
-        return getattr(fp, "spatial_grus", None) if fp is not None else None
     return _swap(model, slots, TensorCoreSpatialGRU, module_reason, TensorCoreSpatialGRU.from_module,
-                 "fiery_b200: SpatialGRU(s) not covered by the tensor-core kernels, left as is: ", root=root)
+                 "fiery_b200: SpatialGRU(s) not covered by the tensor-core kernels, left as is: ", root=_spatial_grus)
 
 
 def uninstall():

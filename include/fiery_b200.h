@@ -485,6 +485,36 @@ FIERY_API int fiery_batch_norm_backward(const fiery_batch_norm_desc_t* desc, con
                                         float* grad_bias, void* workspace, void* stream);
 
 /*
+ * The batch norm in training with batch statistics over a group of `world` ranks (torch.nn.SyncBatchNorm), in two phases each way;
+ * the caller gathers every rank's triplets between them (no collective runs in the library):
+ *   forward:  fiery_batch_norm_local_stats -> stats (channels, 3) fp64 (n, mean, M2) of this rank's x, its pieces merged as
+ *             fiery_batch_norm_forward merges them;  gather to gathered (world, channels, 3), rank r at [r];
+ *             fiery_batch_norm_forward_gathered -> the group's mean and biased var (mean_out, var_out), y as fiery_batch_norm_forward
+ *             computes it from them, and count_out[0] = the group's n (fp64, may be NULL; the running variance's unbiased factor).
+ *   backward: fiery_batch_norm_local_grad_sums -> sums (channels, 3) fp64 (n, S1, S2) of this rank, and this rank's grad_weight =
+ *             S2 / sqrt(var + eps), grad_bias = S1 (each may be NULL; the local sums, as torch's);  gather;
+ *             fiery_batch_norm_backward_gathered -> grad_x from the group's S1, S2 and n.
+ * The gathered finalize merges the ranks in ascending rank order in fp64, starting from rank 0's triplet: Chan's formula for
+ * (n, mean, M2), plain sums for (n, S1, S2); a rank with n = 0 adds nothing.  Every rank computes the same numbers, and with world 1
+ * they are bit for bit fiery_batch_norm_forward's / _backward's.  mean and var are the gathered forward's outputs.
+ * Limits as above, except: training must be 1; batch * frames may be 0 (a rank with no values still writes its triplet) and a rank
+ * may hold a single value; world >= 1.  stats, sums, gathered, count_out: 8-byte aligned.  workspace:
+ * fiery_batch_norm_sync_workspace_bytes(desc), 16-byte aligned, contents irrelevant.  A group n of 0 or 1 gives NaN / 0 statistics
+ * (the library cannot see the group's n on the host).
+ */
+FIERY_API size_t fiery_batch_norm_sync_workspace_bytes(const fiery_batch_norm_desc_t* desc);
+FIERY_API int fiery_batch_norm_local_stats(const fiery_batch_norm_desc_t* desc, const float* x, double* stats, void* workspace, void* stream);
+FIERY_API int fiery_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* desc, int32_t world, const double* gathered, const float* x,
+                                                const float* weight, const float* bias, const float* residual, float* y, float* mean_out,
+                                                float* var_out, double* count_out, void* workspace, void* stream);
+FIERY_API int fiery_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* desc, const float* x, const float* grad_y, const float* weight,
+                                               const float* bias, const float* mean, const float* var, double* sums, float* grad_weight,
+                                               float* grad_bias, void* workspace, void* stream);
+FIERY_API int fiery_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* desc, int32_t world, const double* gathered, const float* x,
+                                                 const float* grad_y, const float* weight, const float* bias, const float* mean,
+                                                 const float* var, float* grad_x, void* workspace, void* stream);
+
+/*
  * The future prediction's SpatialGRU (fiery/layers/temporal.py:10-62) over T steps, without flow warping.  For t = 0 .. T-1, with
  * h = h0 at t = 0 and out[:, t-1] after:
  *   u = sigmoid(conv3x3([x_t, h], W_gates[:C_h]) + b_gates[:C_h] + bias_init)
@@ -545,6 +575,43 @@ FIERY_API int fiery_spatial_gru_backward(const fiery_spatial_gru_desc_t* desc, c
                                          const float* bn_weight, const float* bn_bias, float* grad_x, float* grad_h0, float* grad_w_gates,
                                          float* grad_b_gates, float* grad_w_state, float* grad_bn_weight, float* grad_bn_bias,
                                          void* workspace, void* stream);
+
+/*
+ * The SpatialGRU in training with each step's batch statistics over a group of `world` ranks (its norm a SyncBatchNorm), one step
+ * at a time: the caller gathers every rank's (channels, 3) fp64 triplets into (world, channels, 3) between a step's two calls, as
+ * for fiery_batch_norm_local_stats / _forward_gathered and _local_grad_sums / _backward_gathered.
+ *   forward, t = 0 .. T-1:  step_begin (step t's gates and state convolution; stats = this rank's (n, mean, M2) of s), then
+ *                           step_end (the group's mean and var into means[t], vars[t], count_out[0] = the group's n (may be NULL),
+ *                           and the blend into out[:, t]);
+ *   backward, t = T-1 .. 0: step_begin (the blend's gradient; sums = this rank's (n, S1, S2) of the norm's backward), then
+ *                           step_end (the norm's input gradient from the group's sums, and step t's input gradients into grad_x
+ *                           and the carried state gradient);
+ *   then backward_weights:  the weight gradients, the gates' bias gradient, and grad_bn_weight / grad_bn_bias, each the sum over
+ *                           the steps, in ascending order, of this rank's S2 / sqrt(var + eps) and S1 (the local sums, as torch's).
+ * Arguments are fiery_spatial_gru_forward's / _backward's, the same in every call of a sequence; the forward calls share one
+ * fiery_spatial_gru_forward_workspace_bytes workspace and the backward calls one fiery_spatial_gru_backward_workspace_bytes workspace,
+ * kept from the first call of the sequence to the last (with grad_h0 NULL, the carried gradient lives there).  With world 1 every
+ * output is bit for bit fiery_spatial_gru_forward's / _backward's.  Limits as fiery_spatial_gru_*, and: training 1; 0 <= t < frames;
+ * world >= 1; stats, sums, gathered, count_out 8-byte aligned.
+ */
+FIERY_API int fiery_spatial_gru_forward_step_begin(const fiery_spatial_gru_desc_t* desc, int32_t t, const float* x, const float* h0,
+                                                   const void* packed, const float* b_gates, const float* out, void* saved, double* stats,
+                                                   void* workspace, void* stream);
+FIERY_API int fiery_spatial_gru_forward_step_end(const fiery_spatial_gru_desc_t* desc, int32_t t, int32_t world, const double* gathered,
+                                                 const float* h0, const float* bn_weight, const float* bn_bias, float* out, const void* saved,
+                                                 float* means, float* vars, double* count_out, void* workspace, void* stream);
+FIERY_API int fiery_spatial_gru_backward_step_begin(const fiery_spatial_gru_desc_t* desc, int32_t t, const float* grad_out, const float* h0,
+                                                    const float* out, const void* saved, const float* means, const float* vars,
+                                                    const void* packed, const float* bn_weight, const float* bn_bias, float* grad_h0,
+                                                    double* sums, void* workspace, void* stream);
+FIERY_API int fiery_spatial_gru_backward_step_end(const fiery_spatial_gru_desc_t* desc, int32_t t, int32_t world, const double* gathered,
+                                                  const float* h0, const float* out, const void* saved, const float* means, const float* vars,
+                                                  const void* packed, const float* bn_weight, const float* bn_bias, float* grad_x,
+                                                  float* grad_h0, void* workspace, void* stream);
+FIERY_API int fiery_spatial_gru_backward_weights(const fiery_spatial_gru_desc_t* desc, const float* x, const float* h0, const float* out,
+                                                 const void* saved, const void* packed, float* grad_w_gates, float* grad_b_gates,
+                                                 float* grad_w_state, float* grad_bn_weight, float* grad_bn_bias, void* workspace,
+                                                 void* stream);
 
 /*
  * The spatial GRU's 3x3 convolution on its own: zero padding 1, stride 1, no bias, on `maps` independent (X, Y) maps, the input the
