@@ -39,8 +39,34 @@ def _per_channel(t: Optional[torch.Tensor], c: int, name: str) -> Optional[torch
     return f32(t.detach())
 
 
-def _workspace(d: _lib.BatchNormDesc, device: torch.device) -> torch.Tensor:
-    return _lib.workspace(_lib.load().fiery_batch_norm_workspace_bytes(d), device)
+def _workspace(d: _lib.BatchNormDesc, device: torch.device, group: bool = False) -> torch.Tensor:
+    """The workspace of a call with ``d``; ``group``: of a rank in a group, whose batch may be 0."""
+    lib = _lib.load()
+    return _lib.workspace(lib.fiery_batch_norm_sync_workspace_bytes(d) if group else lib.fiery_batch_norm_workspace_bytes(d), device)
+
+
+def _ptr(t: Optional[torch.Tensor]) -> int:
+    """t's device address, 0 for None or an empty tensor (a rank with no values)."""
+    return t.data_ptr() if t is not None and t.numel() else 0
+
+
+def _forward_operands(x: torch.Tensor, weight, bias, residual):
+    """(weight, bias, residual, y, mean, var) of a forward over x: the operands as the kernels read them, and the outputs."""
+    c = int(x.shape[1])
+    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
+    if residual is not None and tuple(residual.shape) != tuple(x.shape):
+        raise ValueError(f"batch norm: residual {tuple(residual.shape)} does not match x {tuple(x.shape)}")
+    r = f32(residual) if residual is not None else None
+    y = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
+    mean = torch.empty(c, dtype=torch.float32, device=x.device)
+    var = torch.empty(c, dtype=torch.float32, device=x.device)
+    return w, bs, r, y, mean, var
+
+
+def _param_grads(c: int, device: torch.device, need_weight: bool, need_bias: bool):
+    """(grad_weight, grad_bias): (C,) fp32 outputs, None where not asked for."""
+    new = lambda: torch.empty(c, dtype=torch.float32, device=device)           # noqa: E731
+    return new() if need_weight else None, new() if need_bias else None
 
 
 def _check_count(x_shape, training: bool) -> None:
@@ -61,19 +87,12 @@ def forward(x: torch.Tensor, weight: Optional[torch.Tensor], bias: Optional[torc
     _check_count(x.shape, training)
     xs = f32_planes(x)
     c = int(xs.shape[1])
-    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
+    w, bs, r, y, mean, var = _forward_operands(xs, weight, bias, residual)
     rm, rv = _per_channel(running_mean, c, "running_mean"), _per_channel(running_var, c, "running_var")
     if not training and (rm is None or rv is None):
         raise ValueError("batch norm: eval mode needs running_mean and running_var")
-    if residual is not None and tuple(residual.shape) != tuple(xs.shape):
-        raise ValueError(f"batch norm: residual {tuple(residual.shape)} does not match x {tuple(xs.shape)}")
-    r = f32(residual) if residual is not None else None
-    y = torch.empty(tuple(xs.shape), dtype=torch.float32, device=x.device)
-    mean = torch.empty(c, dtype=torch.float32, device=x.device)
-    var = torch.empty(c, dtype=torch.float32, device=x.device)
     d = _desc(xs, training, relu, eps)
-    ptr = lambda t: t.data_ptr() if t is not None else 0           # noqa: E731
-    _lib.call("fiery_batch_norm_forward", x.device, d, xs.data_ptr(), ptr(w), ptr(bs), ptr(rm), ptr(rv), ptr(r), y.data_ptr(),
+    _lib.call("fiery_batch_norm_forward", x.device, d, xs.data_ptr(), _ptr(w), _ptr(bs), _ptr(rm), _ptr(rv), _ptr(r), y.data_ptr(),
               mean.data_ptr(), var.data_ptr(), _workspace(d, x.device).data_ptr())
     return y, mean, var
 
@@ -87,12 +106,10 @@ def backward(grad_y: torch.Tensor, x: torch.Tensor, weight: Optional[torch.Tenso
     g = f32(grad_y)
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
     dx = torch.empty(tuple(xs.shape), dtype=torch.float32, device=x.device) if need_input else None
-    dw = torch.empty(c, dtype=torch.float32, device=x.device) if need_weight else None
-    db = torch.empty(c, dtype=torch.float32, device=x.device) if need_bias else None
+    dw, db = _param_grads(c, x.device, need_weight, need_bias)
     d = _desc(xs, training, relu, eps)
-    ptr = lambda t: t.data_ptr() if t is not None else 0           # noqa: E731
-    _lib.call("fiery_batch_norm_backward", x.device, d, xs.data_ptr(), g.data_ptr(), ptr(w), ptr(bs), f32(mean).data_ptr(),
-              f32(var).data_ptr(), ptr(dx), ptr(dw), ptr(db), _workspace(d, x.device).data_ptr())
+    _lib.call("fiery_batch_norm_backward", x.device, d, xs.data_ptr(), g.data_ptr(), _ptr(w), _ptr(bs), f32(mean).data_ptr(),
+              f32(var).data_ptr(), _ptr(dx), _ptr(dw), _ptr(db), _workspace(d, x.device).data_ptr())
     return dx, dw, db
 
 
@@ -181,28 +198,18 @@ def local_stats(x: torch.Tensor) -> torch.Tensor:
     """x (b, C, s, X, Y) fp32 with contiguous pixel planes (``f32_planes``), b may be 0 -> this rank's (C, 3) fp64 (n, mean, M2)."""
     d = _desc(x, True, False, 0.0)
     stats = torch.empty((x.shape[1], 3), dtype=torch.float64, device=x.device)
-    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
-    _lib.call("fiery_batch_norm_local_stats", x.device, d, x.data_ptr() if x.numel() else 0, stats.data_ptr(), ws.data_ptr())
+    _lib.call("fiery_batch_norm_local_stats", x.device, d, _ptr(x), stats.data_ptr(), _workspace(d, x.device, group=True).data_ptr())
     return stats
 
 
 def forward_gathered(gathered: torch.Tensor, x: torch.Tensor, weight, bias, residual, eps: float, relu: bool):
     """(y, mean, var, count) from the group's gathered (world, C, 3) triplets: y ``relu(batch_norm(x)) + residual`` with the group's
     mean and biased var, count the group's n as a (1,) fp64 device tensor."""
-    c = int(x.shape[1])
-    w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
-    if residual is not None and tuple(residual.shape) != tuple(x.shape):
-        raise ValueError(f"batch norm: residual {tuple(residual.shape)} does not match x {tuple(x.shape)}")
-    r = f32(residual) if residual is not None else None
-    y = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
-    mean = torch.empty(c, dtype=torch.float32, device=x.device)
-    var = torch.empty(c, dtype=torch.float32, device=x.device)
+    w, bs, r, y, mean, var = _forward_operands(x, weight, bias, residual)
     count = torch.empty(1, dtype=torch.float64, device=x.device)
     d = _desc(x, True, relu, eps)
-    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
-    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
-    _lib.call("fiery_batch_norm_forward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), ptr(x), ptr(w), ptr(bs),
-              ptr(r), ptr(y), mean.data_ptr(), var.data_ptr(), count.data_ptr(), ws.data_ptr())
+    _lib.call("fiery_batch_norm_forward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), _ptr(x), _ptr(w), _ptr(bs),
+              _ptr(r), _ptr(y), mean.data_ptr(), var.data_ptr(), count.data_ptr(), _workspace(d, x.device, group=True).data_ptr())
     return y, mean, var, count
 
 
@@ -212,14 +219,11 @@ def local_grad_sums(grad_y: torch.Tensor, x: torch.Tensor, weight, bias, mean, v
     asked for)."""
     c = int(x.shape[1])
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
-    dw = torch.empty(c, dtype=torch.float32, device=x.device) if need_weight else None
-    db = torch.empty(c, dtype=torch.float32, device=x.device) if need_bias else None
+    dw, db = _param_grads(c, x.device, need_weight, need_bias)
     sums = torch.empty((c, 3), dtype=torch.float64, device=x.device)
     d = _desc(x, True, relu, eps)
-    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
-    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
-    _lib.call("fiery_batch_norm_local_grad_sums", x.device, d, ptr(x), ptr(grad_y), ptr(w), ptr(bs), mean.data_ptr(), var.data_ptr(),
-              sums.data_ptr(), ptr(dw), ptr(db), ws.data_ptr())
+    _lib.call("fiery_batch_norm_local_grad_sums", x.device, d, _ptr(x), _ptr(grad_y), _ptr(w), _ptr(bs), mean.data_ptr(), var.data_ptr(),
+              sums.data_ptr(), _ptr(dw), _ptr(db), _workspace(d, x.device, group=True).data_ptr())
     return sums, dw, db
 
 
@@ -230,10 +234,8 @@ def backward_gathered(gathered: torch.Tensor, grad_y: torch.Tensor, x: torch.Ten
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
     dx = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
     d = _desc(x, True, relu, eps)
-    ptr = lambda t: t.data_ptr() if t is not None and t.numel() else 0           # noqa: E731
-    ws = _lib.workspace(_lib.load().fiery_batch_norm_sync_workspace_bytes(d), x.device)
-    _lib.call("fiery_batch_norm_backward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), ptr(x), ptr(grad_y), ptr(w),
-              ptr(bs), mean.data_ptr(), var.data_ptr(), ptr(dx), ws.data_ptr())
+    _lib.call("fiery_batch_norm_backward_gathered", x.device, d, int(gathered.shape[0]), gathered.data_ptr(), _ptr(x), _ptr(grad_y), _ptr(w),
+              _ptr(bs), mean.data_ptr(), var.data_ptr(), _ptr(dx), _workspace(d, x.device, group=True).data_ptr())
     return dx
 
 
@@ -288,17 +290,11 @@ class FusedSyncBatchNorm(nn.SyncBatchNorm):
     >= 2 are read as (b, C, 1, 1, rest) unless they are 5-D.  ``forward_act(x, relu, residual)`` is the fused entry."""
 
     def __init__(self, bn: nn.SyncBatchNorm):
-        nn.Module.__init__(self)
-        for name in ("num_features", "eps", "momentum", "affine", "track_running_stats", "process_group"):
-            setattr(self, name, getattr(bn, name))
-        for name, p in bn._parameters.items():
-            self.register_parameter(name, p)
-        for name, b in bn._buffers.items():
-            self.register_buffer(name, b, persistent=name not in bn._non_persistent_buffers_set)
-        self.train(bn.training)
+        FusedBatchNorm3d.__init__(self, bn)
+        self.process_group = bn.process_group
 
-    def forward(self, input: torch.Tensor) -> torch.Tensor:
-        return self.forward_act(input, relu=False)
+    forward = FusedBatchNorm3d.forward
+    update_running_stats = FusedBatchNorm3d.update_running_stats
 
     def forward_act(self, x: torch.Tensor, relu: bool, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
         self._check_input_dim(x)
@@ -315,10 +311,6 @@ class FusedSyncBatchNorm(nn.SyncBatchNorm):
                                                            lambda t: gather(t, group))
             self.update_running_stats(mean, var, count)
         return y.reshape(shape)
-
-    def update_running_stats(self, mean: torch.Tensor, var: torch.Tensor, n) -> None:
-        """``update_running_stats(self, mean, var, n)``."""
-        update_running_stats(self, mean, var, n)
 
 
 def norm_act(norm: nn.Module, activation: nn.Module, y: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -108,6 +108,15 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_stats_kernel(const
     }
 }
 
+// Chan's formula in fp64: (n, m, m2) merged with a part of nb values, mean mb and M2 m2b (fp32 for a piece, fp64 for a rank)
+template <typename T>
+__device__ __forceinline__ void bn_chan_step(double& n, double& m, double& m2, double nb, T mb, T m2b) {
+    const double delta = static_cast<double>(mb) - m, nn = n + nb;
+    m += delta * (nb / nn);
+    m2 += static_cast<double>(m2b) + delta * delta * (n * nb / nn);
+    n = nn;
+}
+
 // Chan's merge of channel c's pieces' (count, mean, M2) in ascending (b, t, piece) order, in fp64
 __device__ __forceinline__ void bn_merge_pieces(const BnShape& s, const float2* __restrict__ part, int c, double& n, double& m, double& m2) {
     n = m = m2 = 0.0;
@@ -116,11 +125,21 @@ __device__ __forceinline__ void bn_merge_pieces(const BnShape& s, const float2* 
         const int j = static_cast<int>(k % s.per_plane);
         const double nb = static_cast<double>(min(BN_PIECE, s.pixels - j * BN_PIECE));
         const float2 pk = pc[k];
-        const double delta = static_cast<double>(pk.x) - m, nn = n + nb;
-        m += delta * (nb / nn);
-        m2 += static_cast<double>(pk.y) + delta * delta * (n * nb / nn);
-        n = nn;
+        bn_chan_step(n, m, m2, nb, pk.x, pk.y);
     }
+}
+
+// The forward finalizes' output for channel c: the statistics, the group's count n (by channel 0, if count_out) and the coefficients
+__device__ __forceinline__ void bn_forward_out(const float* w, const float* bias, float mean, float var, double n, double eps, int c,
+                                               float* mean_out, float* var_out, double* count_out, BnCoef* coef) {
+    mean_out[c] = mean;
+    var_out[c] = var;
+    if (c == 0 && count_out) *count_out = n;
+    BnCoef k;
+    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
+    k.mean = mean;
+    k.k1 = k.k0 = 0.f;
+    coef[c] = k;
 }
 
 // One thread per channel.  training: Chan's merge of the pieces' (count, mean, M2) in fp64 -> mean and biased variance; eval: the
@@ -141,13 +160,7 @@ __global__ void bn_finalize_forward_kernel(const BnShape s, const float2* __rest
         mean = running_mean[c];
         var = running_var[c];
     }
-    mean_out[c] = mean;
-    var_out[c] = var;
-    BnCoef k;
-    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
-    k.mean = mean;
-    k.k1 = k.k0 = 0.f;
-    coef[c] = k;
+    bn_forward_out(w, bias, mean, var, 0.0, eps, c, mean_out, var_out, nullptr, coef);
 }
 
 template <bool RELU, bool RESIDUAL>
@@ -234,33 +247,45 @@ __global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) bn_grad_sums_kernel(c
     }
 }
 
-// One thread per channel: the fp64 sums of the pieces' (sum g', sum g' (x - mu)) in ascending order (when reduced), the weight and
-// bias gradients, and the coefficients of dx.
+// The fp64 sums (S1, S2) of channel c's pieces' (sum g', sum g' (x - mu)) in ascending (b, t, piece) order, and from them the weight
+// and bias gradients S2 / sqrt(var + eps) and S1, each when asked for
+__device__ __forceinline__ void bn_sum_pieces(const BnShape& s, const float2* part, const float* var, double eps, int c, float* grad_w,
+                                              float* grad_b, double& s1, double& s2) {
+    s1 = s2 = 0.0;
+    const float2* pc = part + c * s.per_channel;
+    for (long long k = 0; k < s.per_channel; ++k) {
+        const float2 pk = pc[k];
+        s1 += static_cast<double>(pk.x);
+        s2 += static_cast<double>(pk.y);
+    }
+    const double ve = static_cast<double>(var[c]) + eps;
+    if (grad_w) grad_w[c] = static_cast<float>(s2 / sqrt(ve));
+    if (grad_b) grad_b[c] = static_cast<float>(s1);
+}
+
+// The training backward's coefficients of channel c from its n values' sums: the forward's scale and shift (so its ReLU mask), k1, k0
+__device__ __forceinline__ BnCoef bn_backward_coef(const float* w, const float* bias, float mean, float var, double eps, int c, double n,
+                                                   double s1, double s2) {
+    BnCoef k;
+    k.mean = mean;
+    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
+    const double ve = static_cast<double>(var) + eps;
+    k.k1 = static_cast<float>(-static_cast<double>(k.scale) * s2 / (n * ve));
+    k.k0 = static_cast<float>(-static_cast<double>(k.scale) * s1 / n);
+    return k;
+}
+
+// One thread per channel: the pieces' sums (when reduced), the weight and bias gradients, and the coefficients of dx.
 __global__ void bn_finalize_backward_kernel(const BnShape s, const float2* __restrict__ part, int reduced, const float* __restrict__ w,
                                             const float* __restrict__ bias, const float* __restrict__ mean, const float* __restrict__ var,
                                             int training, double eps, float* __restrict__ grad_w, float* __restrict__ grad_b,
                                             BnCoef* __restrict__ coef) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= s.channels) return;
-    double s1 = 0.0, s2 = 0.0;
-    if (reduced) {
-        const float2* pc = part + c * s.per_channel;
-        for (long long k = 0; k < s.per_channel; ++k) {
-            const float2 pk = pc[k];
-            s1 += static_cast<double>(pk.x);
-            s2 += static_cast<double>(pk.y);
-        }
-    }
-    BnCoef k;
-    k.mean = mean[c];
-    const float v = var[c];
-    bn_scale_shift(w, bias, k.mean, v, eps, c, k.scale, k.shift);
-    const double ve = static_cast<double>(v) + eps;
-    if (grad_w) grad_w[c] = static_cast<float>(s2 / sqrt(ve));
-    if (grad_b) grad_b[c] = static_cast<float>(s1);
-    const double n = static_cast<double>(s.per_channel / s.per_plane) * s.pixels;
-    k.k1 = training ? static_cast<float>(-static_cast<double>(k.scale) * s2 / (n * ve)) : 0.f;
-    k.k0 = training ? static_cast<float>(-static_cast<double>(k.scale) * s1 / n) : 0.f;
+    double s1 = 0.0, s2 = 0.0;                                 // the gradients asked for imply reduced
+    if (reduced) bn_sum_pieces(s, part, var, eps, c, grad_w, grad_b, s1, s2);
+    BnCoef k = bn_backward_coef(w, bias, mean[c], var[c], eps, c, static_cast<double>(s.per_channel / s.per_plane) * s.pixels, s1, s2);
+    if (!training) k.k1 = k.k0 = 0.f;
     coef[c] = k;
 }
 
@@ -325,23 +350,54 @@ size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d) {
 
 static unsigned bn_grid(const BnShape& s) { return static_cast<unsigned>(s.pieces < BN_MAX_GRID ? s.pieces : BN_MAX_GRID); }
 
+// The workspace: the per-channel coefficients, then one partial per piece
+struct BnWork { BnCoef* coef; float2* part; };
+static BnWork bn_work(const fiery_batch_norm_desc_t* d, void* workspace) {
+    return {static_cast<BnCoef*>(workspace), reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels))};
+}
+
+// The forward's statistics and coefficients: the batch's (the stats pass and the merge) in training, the running ones in eval
+static void bn_batch_coef(const fiery_batch_norm_desc_t* d, const BnShape& s, const float* x, const float* w, const float* bias,
+                          const float* running_mean, const float* running_var, float* mean_out, float* var_out, BnCoef* coef, float2* part,
+                          cudaStream_t stream) {
+    if (d->training) bn_stats_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, part);
+    bn_finalize_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, w, bias, running_mean, running_var, d->training, d->eps,
+                                                                              mean_out, var_out, coef);
+}
+
+// The passes over the pieces below launch nothing for a rank of a group with no values (no pieces).
+static void bn_apply(const fiery_batch_norm_desc_t* d, const BnShape& s, const float* x, const BnCoef* coef, const float* residual, float* y,
+                     cudaStream_t stream) {
+    if (!s.pieces) return;
+    if (d->relu && residual) bn_apply_kernel<true, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+    else if (d->relu) bn_apply_kernel<true, false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+    else if (residual) bn_apply_kernel<false, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
+    else bn_apply_kernel<false, false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
+}
+
+static void bn_grad_sums(const fiery_batch_norm_desc_t* d, const BnShape& s, const float* x, const float* dy, const float* w, const float* bias,
+                         const float* mean, const float* var, float2* part, cudaStream_t stream) {
+    if (!s.pieces) return;
+    if (d->relu) bn_grad_sums_kernel<true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+    else bn_grad_sums_kernel<false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
+}
+
+static void bn_grad_apply(const fiery_batch_norm_desc_t* d, const BnShape& s, const float* x, const float* dy, const BnCoef* coef, float* dx,
+                          cudaStream_t stream) {
+    if (!s.pieces) return;
+    if (d->relu && d->training) bn_grad_apply_kernel<true, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+    else if (d->relu) bn_grad_apply_kernel<true, false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+    else if (d->training) bn_grad_apply_kernel<false, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+    else bn_grad_apply_kernel<false, false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
+}
+
 int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
                               const float* running_var, const float* residual, float* y, float* mean_out, float* var_out,
                               void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
-    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
-    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
-    if (d->training) bn_stats_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, part);
-    bn_finalize_forward_kernel<<<fin, 128, 0, stream>>>(s, part, w, bias, running_mean, running_var, d->training, d->eps, mean_out, var_out,
-                                                         coef);
-    if (d->relu) {
-        if (residual) bn_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
-        else bn_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
-    } else {
-        if (residual) bn_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
-        else bn_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
-    }
+    const auto [coef, part] = bn_work(d, workspace);
+    bn_batch_coef(d, s, x, w, bias, running_mean, running_var, mean_out, var_out, coef, part, stream);
+    bn_apply(d, s, x, coef, residual, y, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -350,22 +406,13 @@ int launch_batch_norm_backward(const fiery_batch_norm_desc_t* d, const float* x,
                                const float* mean, const float* var, float* dx, float* grad_w, float* grad_b, void* workspace,
                                cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
-    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
-    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
+    const auto [coef, part] = bn_work(d, workspace);
     // the sums are needed for the weight and bias gradients, and for dx in training
     const bool reduce = grad_w || grad_b || (dx && d->training);
-    if (reduce) {
-        if (d->relu) bn_grad_sums_kernel<true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
-        else bn_grad_sums_kernel<false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
-    }
-    bn_finalize_backward_kernel<<<fin, 128, 0, stream>>>(s, part, reduce, w, bias, mean, var, d->training, d->eps, grad_w, grad_b, coef);
-    if (dx) {
-        if (d->relu && d->training) bn_grad_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-        else if (d->relu) bn_grad_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-        else if (d->training) bn_grad_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-        else bn_grad_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-    }
+    if (reduce) bn_grad_sums(d, s, x, dy, w, bias, mean, var, part, stream);
+    bn_finalize_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, reduce, w, bias, mean, var, d->training, d->eps,
+                                                                               grad_w, grad_b, coef);
+    if (dx) bn_grad_apply(d, s, x, dy, coef, dx, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -471,13 +518,9 @@ int launch_gru_blend_forward(const fiery_batch_norm_desc_t* d, const float* x, c
                              const float* running_var, const float* u, const float* h, long long hsb, float* out, long long osb,
                              float* mean_out, float* var_out, void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
-    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
-    const unsigned grid = bn_grid(s), fin = (d->channels + 127) / 128;
-    if (d->training) bn_stats_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, part);
-    bn_finalize_forward_kernel<<<fin, 128, 0, stream>>>(s, part, w, bias, running_mean, running_var, d->training, d->eps, mean_out, var_out,
-                                                         coef);
-    gru_blend_kernel<<<grid, BN_THREADS, 0, stream>>>(s, x, coef, u, h, hsb, out, osb);
+    const auto [coef, part] = bn_work(d, workspace);
+    bn_batch_coef(d, s, x, w, bias, running_mean, running_var, mean_out, var_out, coef, part, stream);
+    gru_blend_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, u, h, hsb, out, osb);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -515,39 +558,18 @@ __global__ void bn_gathered_forward_kernel(int world, int channels, const double
     double n = gathered[3 * c], m = gathered[3 * c + 1], m2 = gathered[3 * c + 2];
     for (int r = 1; r < world; ++r) {
         const double* g = gathered + (static_cast<long long>(r) * channels + c) * 3;
-        const double nb = g[0];
-        if (nb == 0.0) continue;
-        const double delta = g[1] - m, nn = n + nb;
-        m += delta * (nb / nn);
-        m2 += g[2] + delta * delta * (n * nb / nn);
-        n = nn;
+        if (g[0] != 0.0) bn_chan_step(n, m, m2, g[0], g[1], g[2]);           // a rank with no values adds nothing
     }
-    const float mean = static_cast<float>(m), var = static_cast<float>(m2 / n);
-    mean_out[c] = mean;
-    var_out[c] = var;
-    if (c == 0 && count_out) *count_out = n;
-    BnCoef k;
-    bn_scale_shift(w, bias, mean, var, eps, c, k.scale, k.shift);
-    k.mean = mean;
-    k.k1 = k.k0 = 0.f;
-    coef[c] = k;
+    bn_forward_out(w, bias, static_cast<float>(m), static_cast<float>(m2 / n), n, eps, c, mean_out, var_out, count_out, coef);
 }
 
-// the rank's (n, S1, S2) and its own weight and bias gradients (S2 / sqrt(var + eps), S1: the local sums, as torch's SyncBatchNorm)
+// the rank's (n, S1, S2) and its own weight and bias gradients (the local sums, as torch's SyncBatchNorm)
 __global__ void bn_local_backward_kernel(const BnShape s, const float2* __restrict__ part, const float* __restrict__ var, double eps,
                                          float* __restrict__ grad_w, float* __restrict__ grad_b, double* __restrict__ sums) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= s.channels) return;
-    double s1 = 0.0, s2 = 0.0;                                 // bn_finalize_backward_kernel's sums, in its order
-    const float2* pc = part + c * s.per_channel;
-    for (long long k = 0; k < s.per_channel; ++k) {
-        const float2 pk = pc[k];
-        s1 += static_cast<double>(pk.x);
-        s2 += static_cast<double>(pk.y);
-    }
-    const double ve = static_cast<double>(var[c]) + eps;
-    if (grad_w) grad_w[c] = static_cast<float>(s2 / sqrt(ve));
-    if (grad_b) grad_b[c] = static_cast<float>(s1);
+    double s1, s2;
+    bn_sum_pieces(s, part, var, eps, c, grad_w, grad_b, s1, s2);
     sums[3 * c] = static_cast<double>(s.per_channel / s.per_plane) * s.pixels;
     sums[3 * c + 1] = s1;
     sums[3 * c + 2] = s2;
@@ -565,19 +587,12 @@ __global__ void bn_gathered_backward_kernel(int world, int channels, const doubl
         s1 += g[1];
         s2 += g[2];
     }
-    BnCoef k;
-    k.mean = mean[c];
-    const float v = var[c];
-    bn_scale_shift(w, bias, k.mean, v, eps, c, k.scale, k.shift);
-    const double ve = static_cast<double>(v) + eps;
-    k.k1 = static_cast<float>(-static_cast<double>(k.scale) * s2 / (n * ve));
-    k.k0 = static_cast<float>(-static_cast<double>(k.scale) * s1 / n);
-    coef[c] = k;
+    coef[c] = bn_backward_coef(w, bias, mean[c], var[c], eps, c, n, s1, s2);
 }
 
 int launch_batch_norm_local_stats(const fiery_batch_norm_desc_t* d, const float* x, double* stats, void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
+    float2* part = bn_work(d, workspace).part;
     if (s.pieces) bn_stats_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, part);
     bn_local_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, stats);
     FIERY_CUDA_CHECK(cudaGetLastError());
@@ -588,19 +603,10 @@ int launch_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* d, int wor
                                        const float* bias, const float* residual, float* y, float* mean_out, float* var_out,
                                        double* count_out, void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
-    const unsigned grid = bn_grid(s);
+    BnCoef* coef = bn_work(d, workspace).coef;
     bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
                                                                               var_out, count_out, coef);
-    if (s.pieces) {
-        if (d->relu) {
-            if (residual) bn_apply_kernel<true, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
-            else bn_apply_kernel<true, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
-        } else {
-            if (residual) bn_apply_kernel<false, true><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, residual, y);
-            else bn_apply_kernel<false, false><<<grid, BN_THREADS, 0, stream>>>(s, x, coef, nullptr, y);
-        }
-    }
+    bn_apply(d, s, x, coef, residual, y, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -609,12 +615,8 @@ int launch_batch_norm_local_grad_sums(const fiery_batch_norm_desc_t* d, const fl
                                       const float* mean, const float* var, double* sums, float* grad_w, float* grad_b, void* workspace,
                                       cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    float2* part = reinterpret_cast<float2*>(static_cast<char*>(workspace) + bn_coef_bytes(d->channels));
-    const unsigned grid = bn_grid(s);
-    if (s.pieces) {
-        if (d->relu) bn_grad_sums_kernel<true><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
-        else bn_grad_sums_kernel<false><<<grid, BN_THREADS, 0, stream>>>(s, x, dy, w, bias, mean, var, d->eps, part);
-    }
+    float2* part = bn_work(d, workspace).part;
+    bn_grad_sums(d, s, x, dy, w, bias, mean, var, part, stream);
     bn_local_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, part, var, d->eps, grad_w, grad_b, sums);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
@@ -624,12 +626,9 @@ int launch_batch_norm_backward_gathered(const fiery_batch_norm_desc_t* d, int wo
                                         const float* w, const float* bias, const float* mean, const float* var, float* dx, void* workspace,
                                         cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    BnCoef* coef = bn_work(d, workspace).coef;
     bn_gathered_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, mean, var, d->eps, coef);
-    if (s.pieces) {
-        if (d->relu) bn_grad_apply_kernel<true, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-        else bn_grad_apply_kernel<false, true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, dy, coef, dx);
-    }
+    bn_grad_apply(d, s, x, dy, coef, dx, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }
@@ -639,7 +638,7 @@ int launch_gru_blend_forward_gathered(const fiery_batch_norm_desc_t* d, int worl
                                       const float* bias, const float* u, const float* h, long long hsb, float* out, long long osb,
                                       float* mean_out, float* var_out, double* count_out, void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = static_cast<BnCoef*>(workspace);
+    BnCoef* coef = bn_work(d, workspace).coef;
     bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
                                                                               var_out, count_out, coef);
     gru_blend_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, x, coef, u, h, hsb, out, osb);

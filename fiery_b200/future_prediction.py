@@ -109,31 +109,51 @@ def _check(x: torch.Tensor, h0: torch.Tensor, w_u: torch.Tensor, frames: int) ->
     return b, tx, cx, h, w, ch
 
 
+def _forward_operands(dims, x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames: int, training: bool, eps: float, bias_init: float):
+    """(d, x, h0, weight pack, gate biases, norm weight, norm bias, saved, workspace) as the kernels take them; hold them until the end."""
+    b, tx, cx, h, w, ch = dims
+    xs, hs = gru_input(x), _aligned_f32(h0)
+    d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), training, eps, bias_init)
+    lib = _lib.load()
+    saved = torch.empty(int(lib.fiery_spatial_gru_saved_bytes(d)), dtype=torch.uint8, device=x.device)
+    bias = torch.empty(2 * ch, dtype=torch.float32, device=x.device)            # the two gate biases, without a map op (cat)
+    bias[:ch], bias[ch:] = b_u.detach(), b_r.detach()
+    ws = _lib.workspace(lib.fiery_spatial_gru_forward_workspace_bytes(d), x.device)
+    return d, xs, hs, _packed(w_u, w_r, w_s), bias, _per_channel(bn_w), _per_channel(bn_b), saved, ws
+
+
+def _grads(dims, device, need, bn_w, bn_b):
+    """(grad_x, grad_h0, the gates' weight and bias (the update's C_h rows, then the reset's), grad_w_s, grad_bn_w, grad_bn_b) fp32, None
+    where ``need`` (9 flags: x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b) does not ask or the norm has no such parameter."""
+    b, tx, cx, h, w, ch = dims
+    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=device)  # noqa: E731
+    gwg, gbg = (new(2 * ch, cx + ch, 3, 3), new(2 * ch)) if any(need[2:6]) else (None, None)
+    return (new(b, tx, cx, h, w) if need[0] else None, new(b, ch, h, w) if need[1] else None, gwg, gbg,
+            new(ch, cx + ch, 3, 3) if need[6] else None, new(ch) if need[7] and bn_w is not None else None,
+            new(ch) if need[8] and bn_b is not None else None)
+
+
+def _split_gates(g: Optional[torch.Tensor], ch: int, take):
+    """The gates' (2 C_h, ...) gradient as (take(the update's rows), take(the reset's rows)); (None, None) for None."""
+    return (take(g[:ch]), take(g[ch:])) if g is not None else (None, None)
+
+
 def forward(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, running_mean, running_var, frames: int, training: bool, eps: float,
             bias_init: float):
     """(out (b, T, C_h, H, W), means (T, C_h), vars (T, C_h), saved): the SpatialGRU over ``frames`` steps; x (b, Tx, C_x, H, W) with
     Tx 1 (one frame read at every step) or T.  ``saved`` holds u, r, q and s of every step for the backward."""
     _require_cuda(x, "x")
-    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dims = b, _, _, h, w, ch = _check(x, h0, w_u, frames)
     if not training and (running_mean is None or running_var is None):
         raise ValueError("spatial GRU: eval mode needs running_mean and running_var")
-    xs = gru_input(x)
-    hs = _aligned_f32(h0)
-    d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), training, eps, bias_init)
-    lib = _lib.load()
+    d, xs, hs, packed, bias, bw, bb, saved, ws = _forward_operands(dims, x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames, training,
+                                                                    eps, bias_init)
+    rm, rv = _per_channel(running_mean), _per_channel(running_var)
     out = torch.empty((b, frames, ch, h, w), dtype=torch.float32, device=x.device)
     means = torch.empty((frames, ch), dtype=torch.float32, device=x.device)
     var = torch.empty((frames, ch), dtype=torch.float32, device=x.device)
-    saved = torch.empty(int(lib.fiery_spatial_gru_saved_bytes(d)), dtype=torch.uint8, device=x.device)
-    bias = torch.empty(2 * ch, dtype=torch.float32, device=x.device)
-    bias[:ch].copy_(b_u.detach())
-    bias[ch:].copy_(b_r.detach())
-    ptr = lambda t: t.data_ptr() if t is not None else 0           # noqa: E731
-    bn_w, bn_b, rm, rv = (_per_channel(t) for t in (bn_w, bn_b, running_mean, running_var))   # held until the call returns
-    packed = _packed(w_u, w_r, w_s)
-    ws = _lib.workspace(lib.fiery_spatial_gru_forward_workspace_bytes(d), x.device)
-    _lib.call("fiery_spatial_gru_forward", x.device, d, xs.data_ptr(), hs.data_ptr(), packed.data_ptr(), bias.data_ptr(), ptr(bn_w),
-              ptr(bn_b), ptr(rm), ptr(rv), out.data_ptr(), saved.data_ptr(), means.data_ptr(), var.data_ptr(), ws.data_ptr())
+    _lib.call("fiery_spatial_gru_forward", x.device, d, xs.data_ptr(), hs.data_ptr(), packed.data_ptr(), bias.data_ptr(), _ptr(bw),
+              _ptr(bb), _ptr(rm), _ptr(rv), out.data_ptr(), saved.data_ptr(), means.data_ptr(), var.data_ptr(), ws.data_ptr())
     return out, means, var, saved
 
 
@@ -141,27 +161,19 @@ def backward(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, bn_w, bn_b,
              bias_init: float, need_x: bool, need_h0: bool, need_gates: bool, need_state: bool, need_bn: bool):
     """The gradients of ``forward`` in fp32: (grad_x (x's shape, contiguous), grad_h0, grad_w_u, grad_b_u, grad_w_r, grad_b_r,
     grad_w_s, grad_bn_w, grad_bn_b), None where not asked for."""
-    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dims = b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
     xs, hs = gru_input(x), _aligned_f32(h0)
     d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), training, eps, bias_init)
     lib = _lib.load()
     dev = x.device
-    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
-    gx = new(b, tx, cx, h, w) if need_x else None
-    gh = new(b, ch, h, w) if need_h0 else None
-    gwg, gbg = (new(2 * ch, cx + ch, 3, 3), new(2 * ch)) if need_gates else (None, None)
-    gws = new(ch, cx + ch, 3, 3) if need_state else None
     bn_w, bn_b = _per_channel(bn_w), _per_channel(bn_b)
-    gbw = new(ch) if need_bn and bn_w is not None else None
-    gbb = new(ch) if need_bn and bn_b is not None else None
-    ptr = lambda t: t.data_ptr() if t is not None else 0           # noqa: E731
+    gx, gh, gwg, gbg, gws, gbw, gbb = _grads(dims, dev, (need_x, need_h0) + (need_gates,) * 4 + (need_state, need_bn, need_bn), bn_w, bn_b)
     go, packed = _aligned_f32(grad_out), _packed(w_u, w_r, w_s)
     ws = _lib.workspace(lib.fiery_spatial_gru_backward_workspace_bytes(d), dev)
     _lib.call("fiery_spatial_gru_backward", dev, d, go.data_ptr(), xs.data_ptr(), hs.data_ptr(), out.data_ptr(),
-              saved.data_ptr(), means.data_ptr(), var.data_ptr(), packed.data_ptr(), ptr(bn_w), ptr(bn_b), ptr(gx),
-              ptr(gh), ptr(gwg), ptr(gbg), ptr(gws), ptr(gbw), ptr(gbb), ws.data_ptr())
-    split = lambda g, n: (g[:n].clone(), g[n:].clone()) if g is not None else (None, None)  # noqa: E731
-    (gwu, gwr), (gbu, gbr) = split(gwg, ch), split(gbg, ch)
+              saved.data_ptr(), means.data_ptr(), var.data_ptr(), packed.data_ptr(), _ptr(bn_w), _ptr(bn_b), _ptr(gx),
+              _ptr(gh), _ptr(gwg), _ptr(gbg), _ptr(gws), _ptr(gbw), _ptr(gbb), ws.data_ptr())
+    (gwu, gwr), (gbu, gbr) = _split_gates(gwg, ch, torch.Tensor.clone), _split_gates(gbg, ch, torch.Tensor.clone)
     return gx, gh, gwu, gbu, gwr, gbr, gws, gbw, gbb
 
 
@@ -185,7 +197,7 @@ def sync_forward_steps(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames: int, 
     yields this rank's (n, mean, M2) of s and takes the group's gathered triplets.  Returns (out, means, vars, counts, saved), counts
     (frames,) fp64 on the device, each step's group count.  A rank with batch 0 yields n = 0 and takes the group's statistics."""
     _require_cuda(x, "x")
-    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dims = b, _, _, h, w, ch = _check(x, h0, w_u, frames)
     dev = x.device
     means = torch.empty((frames, ch), dtype=torch.float32, device=dev)
     var = torch.empty((frames, ch), dtype=torch.float32, device=dev)
@@ -198,14 +210,8 @@ def sync_forward_steps(x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames: int, 
             gathered = yield torch.zeros((ch, 3), dtype=torch.float64, device=dev)
             _, means[t], var[t], counts[t:t + 1] = forward_gathered(gathered, empty, bn_w, bn_b, None, eps, True)
         return out, means, var, counts, torch.empty(0, dtype=torch.uint8, device=dev)
-    xs, hs = gru_input(x), _aligned_f32(h0)
-    d = _desc(b, frames, tx, h, w, cx, ch, (xs.stride(0), xs.stride(1), xs.stride(2)), True, eps, bias_init)
-    lib = _lib.load()
-    saved = torch.empty(int(lib.fiery_spatial_gru_saved_bytes(d)), dtype=torch.uint8, device=dev)
-    bias = torch.cat([b_u.detach(), b_r.detach()]).float()
-    bw, bb = _per_channel(bn_w), _per_channel(bn_b)
-    packed = _packed(w_u, w_r, w_s)
-    ws = _lib.workspace(lib.fiery_spatial_gru_forward_workspace_bytes(d), dev)           # kept across the steps
+    d, xs, hs, packed, bias, bw, bb, saved, ws = _forward_operands(dims, x, h0, w_u, b_u, w_r, b_r, w_s, bn_w, bn_b, frames, True, eps,
+                                                                    bias_init)    # ws is kept across the steps
     for t in range(frames):
         stats = torch.empty((ch, 3), dtype=torch.float64, device=dev)
         _lib.call("fiery_spatial_gru_forward_step_begin", dev, d, t, xs.data_ptr(), hs.data_ptr(), packed.data_ptr(), bias.data_ptr(),
@@ -223,16 +229,10 @@ def sync_backward_steps(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, 
     grad_h0, grad_w_u, grad_b_u, grad_w_r, grad_b_r, grad_w_s, grad_bn_w, grad_bn_b), None where not asked for; the parameter
     gradients are this rank's own (the local sums, as torch's).  With grad_h0 not asked for, the carried gradient lives in the
     workspace."""
-    b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
+    dims = b, tx, cx, h, w, ch = _check(x, h0, w_u, frames)
     dev = x.device
-    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
-    gx = new(b, tx, cx, h, w) if need[0] else None
-    gh = new(b, ch, h, w) if need[1] else None
-    gwg, gbg = (new(2 * ch, cx + ch, 3, 3), new(2 * ch)) if any(need[2:6]) else (None, None)
-    gws = new(ch, cx + ch, 3, 3) if need[6] else None
     bw, bb = _per_channel(bn_w), _per_channel(bn_b)
-    gbw = new(ch) if need[7] and bw is not None else None
-    gbb = new(ch) if need[8] and bb is not None else None
+    gx, gh, gwg, gbg, gws, gbw, gbb = _grads(dims, dev, need, bw, bb)
     if b == 0:
         for _ in range(frames):
             yield torch.zeros((ch, 3), dtype=torch.float64, device=dev)
@@ -257,8 +257,7 @@ def sync_backward_steps(grad_out, x, h0, out, saved, means, var, w_u, w_r, w_s, 
         _lib.call("fiery_spatial_gru_backward_weights", dev, d, xs.data_ptr(), hs.data_ptr(), out.data_ptr(), saved.data_ptr(),
                   packed.data_ptr(), _ptr(gwg), _ptr(gbg), _ptr(gws), _ptr(gbw), _ptr(gbb), ws.data_ptr())
     cast = lambda g, like: g.to(like.dtype) if g is not None else None           # noqa: E731
-    split = lambda g: (cast(g[:ch], w_u), cast(g[ch:], w_u)) if g is not None else (None, None)  # noqa: E731
-    (gwu, gwr), (gbu, gbr) = split(gwg), split(gbg)
+    (gwu, gwr), (gbu, gbr) = (_split_gates(g, ch, lambda t: t.to(w_u.dtype)) for g in (gwg, gbg))
     return cast(gx, x), cast(gh, h0), gwu, gbu, gwr, gbr, cast(gws, w_s), cast(gbw, bn_w), cast(gbb, bn_b)
 
 
