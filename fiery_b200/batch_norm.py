@@ -202,9 +202,19 @@ def local_stats(x: torch.Tensor) -> torch.Tensor:
     return stats
 
 
+def _check_gathered(gathered: torch.Tensor, x: torch.Tensor) -> None:
+    """The kernels read ``gathered`` as contiguous (world, C, 3) fp64 on x's device; anything else would be read as other numbers."""
+    c = int(x.shape[1])
+    if (gathered.dtype != torch.float64 or gathered.dim() != 3 or gathered.shape[0] < 1 or tuple(gathered.shape[1:]) != (c, 3)
+            or not gathered.is_contiguous() or gathered.device != x.device):
+        raise ValueError(f"batch norm: gathered must be a contiguous (world, {c}, 3) fp64 tensor, got {tuple(gathered.shape)} "
+                         f"{gathered.dtype} with strides {gathered.stride()} on {gathered.device}")
+
+
 def forward_gathered(gathered: torch.Tensor, x: torch.Tensor, weight, bias, residual, eps: float, relu: bool):
     """(y, mean, var, count) from the group's gathered (world, C, 3) triplets: y ``relu(batch_norm(x)) + residual`` with the group's
     mean and biased var, count the group's n as a (1,) fp64 device tensor."""
+    _check_gathered(gathered, x)
     w, bs, r, y, mean, var = _forward_operands(x, weight, bias, residual)
     count = torch.empty(1, dtype=torch.float64, device=x.device)
     d = _desc(x, True, relu, eps)
@@ -231,6 +241,7 @@ def backward_gathered(gathered: torch.Tensor, grad_y: torch.Tensor, x: torch.Ten
                       relu: bool) -> torch.Tensor:
     """grad_x (contiguous fp32) from the group's gathered (world, C, 3) (n, S1, S2)."""
     c = int(x.shape[1])
+    _check_gathered(gathered, x)
     w, bs = _per_channel(weight, c, "weight"), _per_channel(bias, c, "bias")
     dx = torch.empty(tuple(x.shape), dtype=torch.float32, device=x.device)
     d = _desc(x, True, relu, eps)
@@ -287,7 +298,8 @@ class FusedSyncBatchNorm(nn.SyncBatchNorm):
     statistics, torch.distributed initialized, a group of more than one rank) it runs ``SyncBatchNormAct``: every rank's (n, mean, M2)
     gathered and merged in rank order on the device, one gather forward and one backward, the running statistics moved with the
     group's count without a host synchronisation.  Otherwise it computes exactly what ``FusedBatchNorm3d`` does.  Inputs of any rank
-    >= 2 are read as (b, C, 1, 1, rest) unless they are 5-D.  ``forward_act(x, relu, residual)`` is the fused entry."""
+    >= 2 are read as (b, C, 1, 1, rest) unless they are 5-D, and one with no elements as (0, C, 1, 1, 1): such a rank takes part in
+    the gathers with n = 0, as in torch's SyncBatchNorm.  ``forward_act(x, relu, residual)`` is the fused entry."""
 
     def __init__(self, bn: nn.SyncBatchNorm):
         FusedBatchNorm3d.__init__(self, bn)
@@ -299,7 +311,10 @@ class FusedSyncBatchNorm(nn.SyncBatchNorm):
     def forward_act(self, x: torch.Tensor, relu: bool, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
         self._check_input_dim(x)
         shape = x.shape
-        if x.dim() != 5:                                  # the trailing dims' product, not -1: an empty rank's x has 0 elements
+        if x.numel() == 0:                                # an empty rank, whichever dim is 0: batch 0 takes part with n = 0, where
+            x = x.reshape(0, shape[1], 1, 1, 1)           # a plane of 0 pixels is not a valid shape
+            residual = residual.reshape(x.shape) if residual is not None else None
+        elif x.dim() != 5:
             x = x.reshape(shape[0], shape[1], 1, 1, math.prod(shape[2:]))
             residual = residual.reshape(x.shape) if residual is not None else None
         group = sync_group(self)

@@ -116,24 +116,35 @@ def fma64(a, b, c):
 # ------------------------------------------------------------------------------------------------------------------------------
 # the finalize's fp64 steps
 # ------------------------------------------------------------------------------------------------------------------------------
-def chan_merge(means, m2s, counts, contracted):
-    """bn_finalize_forward_kernel's merge: means, m2s (C, K) fp32 piece partials and counts (K,) in merge order -> (mean, var) (C,)
-    fp32.  contracted: m += delta * (nb / nn) and m2 += M2 + delta^2 * (n nb / nn) as fp64 fmas (nvcc's default), else each product
-    rounded before its add."""
+def chan_step(n, m, m2, nb, mb, m2b, contracted):
+    """bn_chan_step: (n, m, m2) fp64 merged with a part of nb values, mean mb and M2 m2b.  contracted: m += delta * (nb / nn) and
+    m2 += M2 + delta^2 * (n nb / nn) as fp64 fmas (nvcc's default), else each product rounded before its add."""
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        delta = np.asarray(mb, np.float64) - m
+        nn = n + nb
+        if contracted:
+            m = fma64(delta, nb / nn, m)
+            m2 = m2 + fma64(delta * delta, n * nb / nn, np.asarray(m2b, np.float64))
+        else:
+            m = m + delta * (nb / nn)
+            m2 = m2 + (np.asarray(m2b, np.float64) + delta * delta * (n * nb / nn))
+    return nn, m, m2
+
+
+def chan_merge64(means, m2s, counts, contracted):
+    """bn_merge_pieces: means, m2s (C, K) fp32 piece partials and counts (K,) in merge order -> the fp64 (n, m, m2) (C,) before any
+    cast, from (0, 0, 0): a rank's local triplet (bn_local_forward_kernel), (0, 0, 0) for K = 0"""
     means, m2s = np.asarray(means, np.float32), np.asarray(m2s, np.float32)
     c = means.shape[0]
     n, m, m2 = np.zeros(c), np.zeros(c), np.zeros(c)
     for k in range(means.shape[1]):
-        nb = float(counts[k])
-        delta = means[:, k].astype(np.float64) - m
-        nn = n + nb
-        if contracted:
-            m = fma64(delta, nb / nn, m)
-            m2 = m2 + fma64(delta * delta, n * nb / nn, m2s[:, k].astype(np.float64))
-        else:
-            m = m + delta * (nb / nn)
-            m2 = m2 + (m2s[:, k].astype(np.float64) + delta * delta * (n * nb / nn))
-        n = nn
+        n, m, m2 = chan_step(n, m, m2, float(counts[k]), means[:, k].astype(np.float64), m2s[:, k], contracted)
+    return n, m, m2
+
+
+def chan_merge(means, m2s, counts, contracted):
+    """bn_finalize_forward_kernel's merge: ``chan_merge64`` -> (mean, var) (C,) fp32"""
+    n, m, m2 = chan_merge64(means, m2s, counts, contracted)
     return m.astype(np.float32), (m2 / n).astype(np.float32)
 
 
@@ -343,3 +354,175 @@ SHAPES = [
 SHAPE_LIST = [shape for shape, _ in SHAPES]
 PIXELS = [1, 2, 3, 5, 7, 4092, 4093, 4094, 4095, 4096, 4097, 4098, 4099, 4100, 8191, 8192, 8193, 12289, 40000, 80000]
 CHANNELS = [1, 127, 128, 129, 255, 256, 1000]
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# a process group (fiery_batch_norm_*_gathered): every rank's local triplet, gathered and merged in ascending rank order
+# ------------------------------------------------------------------------------------------------------------------------------
+def merge_ranks(triplets, contracted, descending=False, skip_empty=True):
+    """bn_gathered_forward_kernel's merge: triplets (world, C, 3) fp64 (n, mean, M2) -> (n, m, m2) (C,) fp64: rank 0's triplet, then
+    Chan's step with each later rank in ascending order, a rank with n = 0 skipped.  ``descending`` and ``skip_empty=False`` are the
+    two ways of getting it wrong that tests/test_sync_batch_norm_cases_cpu.py shows the splits can see."""
+    t = np.asarray(triplets, np.float64)[::-1] if descending else np.asarray(triplets, np.float64)
+    n, m, m2 = t[0, :, 0].copy(), t[0, :, 1].copy(), t[0, :, 2].copy()
+    for r in range(1, t.shape[0]):
+        nn, mm, mm2 = chan_step(n, m, m2, t[r, :, 0], t[r, :, 1], t[r, :, 2], contracted)
+        keep = t[r, :, 0] != 0 if skip_empty else np.ones_like(n, bool)
+        n, m, m2 = np.where(keep, nn, n), np.where(keep, mm, m), np.where(keep, mm2, m2)
+    return n, m, m2
+
+
+def sum_ranks(triplets):
+    """bn_gathered_backward_kernel's sum: (world, C, 3) (n, S1, S2) -> each summed over the ranks in ascending order, in fp64"""
+    return tuple(seq_sum64(np.moveaxis(np.asarray(triplets, np.float64)[..., k], 0, -1)) for k in range(3))
+
+
+def local_triplet(x, contracted):
+    """bn_local_forward_kernel: x (b, C, s, pixels) fp32, b or s may be 0 -> (C, 3) fp64 (n, mean, M2)"""
+    x = np.asarray(x, np.float32)
+    bsz, c, s, pixels = x.shape
+    if bsz * s == 0:
+        return np.zeros((c, 3))
+    sums = bn_piece_sums_model(x, pixels)
+    pm = sums / piece_counts(pixels)
+    d = x - np.repeat(pm, piece_sizes(pixels), axis=-1)
+    m2 = bn_piece_sums_model(d * d, pixels)
+    counts = np.tile(piece_counts(pixels), bsz * s)
+    return np.stack(chan_merge64(channel_pieces(pm, pixels), channel_pieces(m2, pixels), counts, contracted), axis=1)
+
+
+MUTATIONS = {
+    "descending": "the ranks merged in descending order",
+    "no_skip": "no n = 0 skip in the forward merge",
+    "rank_n": "the rank's own n instead of the group's in the backward coefficients",
+    "piece_count": "a rank's backward count written as per_channel * pixels (pieces times pixels)",
+    "group_s2": "dgamma from the group's S2 instead of the rank's own",
+}
+
+
+def restate_group(shards, w, b, rs, dys, relu, eps, contracted=False, mutation=None):
+    """The group path restated: shards, rs, dys lists of (b_r, C, s, pixels) fp32 per rank (b_r may be 0; rs / dys entries may be
+    None) -> dict of the group's mean, var (C,) fp32 and count (fp64), the gathered forward and backward triplets, and per rank lists
+    y, dx, dw, db (each rank's own dgamma / dbeta).  A group of one is ``restate``; ``mutation`` (a key of MUTATIONS) restates a
+    wrong kernel."""
+    shards = [np.asarray(x, np.float32) for x in shards]
+    c, s, pixels = shards[0].shape[1:]
+    fwd = np.stack([local_triplet(x, contracted) for x in shards])
+    n, m, m2 = merge_ranks(fwd, contracted, descending=mutation == "descending", skip_empty=mutation != "no_skip")
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mean, var = m.astype(np.float32), (m2 / n).astype(np.float32)
+    scale, shift_u, shift_c = scale_shift(w, b, mean, var, eps)
+    shift = shift_c if contracted else shift_u
+    out = dict(mean=mean, var=var, count=n, scale=scale, shift=shift, gathered_forward=fwd, y=[], dx=[], dw=[], db=[], s1=[], s2=[])
+    pres, gs, dmus, bwd = [], [], [], []
+    for x, r, dy in zip(shards, rs, dys):
+        pre = fmaf_exact(_bc(scale), x, _bc(shift))
+        y = np.where(pre < 0, np.float32(0), pre) if relu else pre
+        out["y"].append((y + np.asarray(r, np.float32)).astype(np.float32) if r is not None else y)
+        dy = np.asarray(dy, np.float32) if dy is not None else np.zeros_like(x)
+        with np.errstate(invalid="ignore"):
+            g = np.where(pre <= 0, np.float32(0), dy) if relu else dy
+            dmu = (x - _bc(mean)).astype(np.float32)
+        if x.shape[0] * s:
+            s1 = seq_sum64(channel_pieces(bn_piece_sums_model(g, pixels), pixels))
+            s2 = seq_sum64(channel_pieces(bn_piece_sums_model(g * dmu, pixels), pixels))
+        else:
+            s1 = s2 = np.zeros(c)
+        per = len(piece_sizes(pixels)) if mutation == "piece_count" else 1
+        bwd.append(np.stack([np.full(c, float(x.shape[0] * s * per * pixels)), s1, s2], axis=1))
+        pres.append(pre)
+        gs.append(g)
+        dmus.append(dmu)
+        out["s1"].append(s1)
+        out["s2"].append(s2)
+    bwd = np.stack(bwd)
+    out["gathered_backward"] = bwd
+    nb, s1g, s2g = sum_ranks(bwd)
+    for k, (g, dmu) in enumerate(zip(gs, dmus)):
+        dw, db, k1, k0 = backward_coefficients(scale, out["s1"][k], s2g if mutation == "group_s2" else out["s2"][k], var, eps, 1.0)
+        n_coef = bwd[k, 0, 0] if mutation == "rank_n" else nb[0]
+        _, _, k1, k0 = backward_coefficients(scale, s1g, s2g, var, eps, n_coef)
+        out["dw"].append(dw)
+        out["db"].append(db)
+        out["dx"].append(fmaf_exact(_bc(scale), g, fmaf_exact(_bc(k1), dmu, _bc(k0))))
+    return out
+
+
+def shards_of(t, sizes):
+    """t (B, ...) split along the batch into pieces of the given sizes (some 0)"""
+    cuts = np.cumsum([0] + list(sizes))
+    assert cuts[-1] == t.shape[0], (sizes, t.shape)
+    return [t[cuts[i]:cuts[i + 1]] for i in range(len(sizes))]
+
+
+def exact_group_case(shape, sizes, seed, eps=0.0, offsets=False):
+    """An ``exact_case`` for a group: inputs (b, C, s, X, Y) split along the batch into ``sizes``.  offsets=False: every piece has
+    mean mu_c, so Chan's delta is 0 across the ranks too.  offsets=True: the ranks' means are mu_c + a_r for integers a_r with the
+    non-empty ranks' counts in ratios 1 : 1 : 2 : 4 (sizes must be so), sum n_r a_r = 0 and in-rank variance 14 - eps, so the group's
+    var + eps is 16 with the cross-rank delta^2 term non-zero, and every nb / nn a power of two.  Returns the case dict of
+    ``exact_case`` (x, r, dy whole-batch (b, C, s, pixels)) with "sizes" added."""
+    if not offsets:
+        case = exact_case(shape, seed, eps=eps)
+        case["sizes"] = list(sizes)
+        return case
+    b, c, s, X, Y = shape
+    pixels = X * Y
+    full = [k for k in sizes if k]
+    assert len(full) == 4 and [k // full[0] for k in full] == [1, 1, 2, 4] and full[0] * 8 == sum(full) == b, (sizes, shape)
+    rng = np.random.default_rng(seed)
+    a = iter((3, -1, 1, -1))                                    # 3 - 1 + 2 - 4 = 0, and sum n_r a_r^2 / n = 2
+    v = 14 - eps
+    assert v == int(v) and v > 0, eps
+    mu = rng.integers(-8, 9, c)
+    parts = []
+    for k in sizes:
+        if k == 0:
+            parts.append(np.zeros((0, c, s, pixels)))
+            continue
+        d = exact_deviations(k, c, s, pixels, int(v), rng)
+        assert d is not None, f"no exact deviations for {k} of {shape}"
+        parts.append(mu.reshape(1, c, 1, 1) + next(a) + d)
+    x = np.concatenate(parts).astype(np.float32)
+    w = np.resize(GAMMAS, c).astype(np.float32)
+    t = np.array([(3, -2, 0, 1)[ch % 4] for ch in range(c)])
+    bias = (-(w / np.float32(4.0)) * t).astype(np.float32)
+    return dict(x=x, w=w, b=bias, rm=mu.astype(np.float32), rv=np.full(c, 16 - eps, np.float32),
+                r=rng.integers(-4, 5, x.shape).astype(np.float32), dy=rng.integers(-3, 4, x.shape).astype(np.float32),
+                eps=float(eps), mu=mu, var=16 - eps, sizes=list(sizes))
+
+
+def _spread(total, ranks, empty):
+    """``total`` batch elements over ``ranks`` ranks, none on the ranks in ``empty``, the others as even as can be (earlier ones more)"""
+    full = [r for r in range(ranks) if r not in empty]
+    out = [0] * ranks
+    for i in range(total):
+        out[full[i % len(full)]] += 1
+    return out
+
+
+# (name, sizes(B) -> per-rank batch sizes or None where the split does not apply, why it is there)
+SPLITS = [
+    ("all", lambda B: [B], "one rank: the single-rank finalize's numbers"),
+    ("0+all", lambda B: [0, B], "an empty rank 0: the merge starts from (0, 0, 0) and the first step must be exact"),
+    ("0+0+a+b", lambda B: [0, 0, B - B // 2, B // 2], "two leading empty ranks: only the n = 0 skip keeps nb / nn from 0 / 0"),
+    ("a+0+b+0", lambda B: [B - B // 2, 0, B // 2, 0], "empty ranks between and after the data"),
+    ("1+1", lambda B: [1, 1] if B == 2 else None, "two ranks of one batch element: single-value ranks on 1-pixel planes"),
+    ("1+rest", lambda B: [1, B - 1] if B >= 2 else None, "one element on rank 0, the rest on rank 1: unequal counts"),
+    ("0x5+all", lambda B: [0] * 5 + [B], "all data on the last of six ranks"),
+    ("8:3empty", lambda B: _spread(B, 8, (0, 3, 6)), "8 ranks, 3 of them (0, 3 and 6) empty, the others uneven"),
+    ("64", lambda B: [1 if (37 * r) % 64 < B else 0 for r in range(64)] if B <= 64 else None,
+     "64 ranks, each holding one batch element or none"),
+]
+SPLIT_NAMES = [name for name, _, _ in SPLITS]
+
+
+def split_sizes(name, B):
+    return dict((n, f) for n, f, _ in SPLITS)[name](B)
+
+
+def cancelling_case(c, seed):
+    """x (7, C, 1, 2) whose batch elements hold 2a, a, a, -a, -a, -a, -a (a full-mantissa value per channel): the group's mean is 0
+    exactly, so the fp32 mean is the fp64 merge's rounding residue, whose bits depend on the order of the ranks' merge"""
+    a = ((np.random.default_rng(seed).random(c) + 0.5) * 1000).astype(np.float32).reshape(1, c, 1, 1)
+    return np.concatenate([np.broadcast_to(2 * a, (1, c, 1, 2)), np.broadcast_to(a, (2, c, 1, 2)),
+                           np.broadcast_to(-a, (4, c, 1, 2))]).astype(np.float32)
