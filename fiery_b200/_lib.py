@@ -95,6 +95,13 @@ class Conv3x3Desc(ctypes.Structure):
     _fields_ = [("maps", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("in_channels", c_int32 * 2), ("out_channels", c_int32 * 2)]
 
 
+class BottleneckDesc(ctypes.Structure):
+    """Mirror of ``fiery_bottleneck_desc_t``."""
+
+    _fields_ = [("maps", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("channels", c_int32), ("training", c_int32),
+                ("eps", c_double)]
+
+
 # name -> (restype, argtypes); every symbol include/fiery_b200.h declares
 SIGNATURES = {
     "fiery_abi_version": (c_int32, []),
@@ -178,6 +185,13 @@ SIGNATURES = {
     "fiery_conv3x3_backward_data": (c_int32, [POINTER(Conv3x3Desc)] + [c_void_p] * 6),
     "fiery_conv3x3_backward_weight_workspace_bytes": (c_size_t, [POINTER(Conv3x3Desc)]),
     "fiery_conv3x3_backward_weight": (c_int32, [POINTER(Conv3x3Desc)] + [c_void_p] * 6),
+    "fiery_bottleneck_packed_bytes": (c_size_t, [POINTER(BottleneckDesc)]),
+    "fiery_bottleneck_pack_weights": (c_int32, [POINTER(BottleneckDesc)] + [c_void_p] * 5),
+    "fiery_bottleneck_forward_workspace_bytes": (c_size_t, [POINTER(BottleneckDesc)]),
+    "fiery_bottleneck_forward": (c_int32, [POINTER(BottleneckDesc), c_void_p, c_void_p, POINTER(c_void_p)] + [c_void_p] * 7),
+    "fiery_bottleneck_backward_workspace_bytes": (c_size_t, [POINTER(BottleneckDesc)]),
+    "fiery_bottleneck_backward": (c_int32, [POINTER(BottleneckDesc)] + [c_void_p] * 7 + [POINTER(c_void_p)] + [c_void_p] * 4
+                                  + [POINTER(c_void_p), c_void_p, c_void_p]),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),
@@ -265,9 +279,10 @@ def warn_once(key, msg: str, stacklevel: int = 2) -> None:
 # (shared with its views, its aliases and the Parameter) changes with each in-place update, e.g. an optimizer step or a checkpoint
 # load.  One training step of a model with every layer swapped uses one pack per DepthLayer operand dtype, two for FirstConv (the
 # transposed one for the input gradient), four per TemporalBlock (its entry, two causal convolutions and its aggregation) and one per
-# Bottleneck3D: 19 for the four temporal blocks of a 5-frame receptive field.  The bound leaves room for in-between layers (up to four
-# per block there) without a step ever evicting a pack it uses again.
-_PACK_CACHE_SIZE = 40
+# Bottleneck3D: 19 for the four temporal blocks of a 5-frame receptive field, and one per SpatialGRU and Bottleneck: 12 for a swapped
+# FuturePrediction.  The bound leaves room for in-between layers (up to four per block there) without a step ever evicting a pack it
+# uses again.
+_PACK_CACHE_SIZE = 48
 _pack_cache: "collections.OrderedDict[tuple, tuple]" = collections.OrderedDict()
 
 

@@ -12,7 +12,7 @@
 // warp sums are added in ascending order.  The per-channel finalize (one thread per channel) merges the channel's pieces in
 // ascending (b, t, piece) order in fp64: Chan's formula for (count, mean, M2), plain sums for the backward.  The apply passes use
 // the same pieces.
-#include "common.cuh"
+#include "bn_coef.cuh"
 #include "plane_chunks.cuh"
 
 namespace fiery {
@@ -28,12 +28,6 @@ struct BnShape {
     long long per_channel;                                     // pieces of one channel: batch * frames * per_plane
     long long sb, sc, st;                                      // x's strides, elements
     int channels, frames, pixels, per_plane;
-};
-
-// Per-channel coefficients the finalize writes for the apply passes.  Forward: y = fmaf(scale, x, shift).  Backward:
-// dx = fmaf(scale, g', fmaf(k1, x - mean, k0)) in training, scale * g' in eval.
-struct BnCoef {
-    float scale, shift, mean, k1, k0;
 };
 
 struct BnPiece {
@@ -398,6 +392,15 @@ int launch_batch_norm_forward(const fiery_batch_norm_desc_t* d, const float* x, 
     const auto [coef, part] = bn_work(d, workspace);
     bn_batch_coef(d, s, x, w, bias, running_mean, running_var, mean_out, var_out, coef, part, stream);
     bn_apply(d, s, x, coef, residual, y, stream);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+int launch_batch_norm_coef(const fiery_batch_norm_desc_t* d, const float* x, const float* w, const float* bias, const float* running_mean,
+                           const float* running_var, float* mean_out, float* var_out, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    const auto [coef, part] = bn_work(d, workspace);
+    bn_batch_coef(d, s, x, w, bias, running_mean, running_var, mean_out, var_out, coef, part, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

@@ -177,6 +177,17 @@ int launch_spatial_gru_backward_weights(const fiery_spatial_gru_desc_t* d, const
                                         const float* packed, float* grad_w_gates, float* grad_b_gates, float* grad_w_state, float* grad_bn_w,
                                         float* grad_bn_b, void* workspace, cudaStream_t stream);
 int launch_causal_conv_pack(const fiery_causal_conv3d_desc_t* d, const float* w, float* packed, cudaStream_t stream);
+size_t bottleneck_packed_bytes(const fiery_bottleneck_desc_t* d);
+int launch_bottleneck_pack(const fiery_bottleneck_desc_t* d, const float* w_down, const float* w_conv, const float* w_up, void* packed,
+                           cudaStream_t stream);
+size_t bottleneck_forward_workspace_bytes(const fiery_bottleneck_desc_t* d);
+int launch_bottleneck_forward(const fiery_bottleneck_desc_t* d, const float* x, const void* packed, const float* const* norms, float* y1,
+                              float* y2, float* y3, float* out, float* stats, void* workspace, cudaStream_t stream);
+size_t bottleneck_backward_workspace_bytes(const fiery_bottleneck_desc_t* d);
+int launch_bottleneck_backward(const fiery_bottleneck_desc_t* d, const float* grad_out, const float* x, const float* y1, const float* y2,
+                               const float* y3, const float* stats, const void* packed, const float* const* norms, float* grad_x,
+                               float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms, void* workspace,
+                               cudaStream_t stream);
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
 int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
 size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d);
@@ -1017,6 +1028,76 @@ FIERY_API int fiery_conv3x3_backward_weight(const fiery_conv3x3_desc_t* desc, co
     FIERY_REQUIRE(grad_y && aligned16(grad_y) && grad_w && workspace && aligned16(workspace),
                   "3x3 conv: NULL or misaligned grad_y / grad_w / workspace");
     return launch_conv3x3_wgrad(desc, x0, x1, grad_y, grad_w, workspace, static_cast<cudaStream_t>(stream));
+}
+
+
+// The Bottleneck's limits, one place for every entry point: those of the kernels it chains.  The messages name the field.
+static int check_bottleneck_desc(const fiery_bottleneck_desc_t* d) {
+    FIERY_REQUIRE(d, "bottleneck: NULL desc");
+    FIERY_REQUIRE(d->maps >= 1, "bottleneck: maps = %d must be >= 1", d->maps);
+    FIERY_REQUIRE(d->channels >= 2 && d->channels <= 128, "bottleneck: channels = %d must be in 2..128 (M = channels / 2 <= 64)",
+                  d->channels);
+    FIERY_REQUIRE(d->grid_x >= 1, "bottleneck: grid_x = %d must be >= 1", d->grid_x);
+    FIERY_REQUIRE(d->grid_y >= 1 && d->grid_y % 4 == 0, "bottleneck: grid_y = %d must be a positive multiple of 4 (16-byte TMA row pitch)",
+                  d->grid_y);
+    FIERY_REQUIRE(static_cast<long long>(d->grid_x) * d->grid_y < (1ll << 31), "bottleneck: grid_x * grid_y = %lld pixels must be < 2^31",
+                  static_cast<long long>(d->grid_x) * d->grid_y);
+    FIERY_REQUIRE(d->training == 0 || d->training == 1, "bottleneck: training = %d must be 0 or 1", d->training);
+    FIERY_REQUIRE(d->eps >= 0.0, "bottleneck: eps = %g must be >= 0", d->eps);
+    FIERY_REQUIRE(!d->training || static_cast<long long>(d->maps) * d->grid_x * d->grid_y >= 2,
+                  "bottleneck: maps * grid_x * grid_y = %lld values per channel must be >= 2 in training",
+                  static_cast<long long>(d->maps) * d->grid_x * d->grid_y);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_bottleneck_packed_bytes(const fiery_bottleneck_desc_t* desc) {
+    if (check_bottleneck_desc(desc) != FIERY_OK) return 0;
+    return bottleneck_packed_bytes(desc);
+}
+
+FIERY_API int fiery_bottleneck_pack_weights(const fiery_bottleneck_desc_t* desc, const float* w_down, const float* w_conv, const float* w_up,
+                                            void* packed, void* stream) {
+    const int rc = check_bottleneck_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(w_down && w_conv && w_up && packed, "bottleneck: NULL weight pointer");
+    FIERY_REQUIRE(aligned16(packed), "bottleneck: packed weights must be 16-byte aligned");
+    return launch_bottleneck_pack(desc, w_down, w_conv, w_up, packed, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_bottleneck_forward_workspace_bytes(const fiery_bottleneck_desc_t* desc) {
+    if (check_bottleneck_desc(desc) != FIERY_OK) return 0;
+    return bottleneck_forward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_bottleneck_forward(const fiery_bottleneck_desc_t* desc, const float* x, const void* packed, const float* const* norms,
+                                       float* y1, float* y2, float* y3, float* out, float* stats, void* workspace, void* stream) {
+    const int rc = check_bottleneck_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(x && packed && norms && y1 && y2 && y3 && out && stats && workspace, "bottleneck: NULL pointer");
+    for (int i = 0; i < 3 && !desc->training; ++i)
+        FIERY_REQUIRE(norms[4 * i + 2] && norms[4 * i + 3], "bottleneck: eval mode needs norm %d's running_mean and running_var", i);
+    FIERY_REQUIRE(aligned16(x) && aligned16(packed) && aligned16(y1) && aligned16(y2) && aligned16(y3) && aligned16(out) && aligned16(workspace),
+                  "bottleneck: pointers must be 16-byte aligned");
+    return launch_bottleneck_forward(desc, x, packed, norms, y1, y2, y3, out, stats, workspace, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_bottleneck_backward_workspace_bytes(const fiery_bottleneck_desc_t* desc) {
+    if (check_bottleneck_desc(desc) != FIERY_OK) return 0;
+    return bottleneck_backward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_bottleneck_backward(const fiery_bottleneck_desc_t* desc, const float* grad_out, const float* x, const float* y1,
+                                        const float* y2, const float* y3, const float* stats, const void* packed, const float* const* norms,
+                                        float* grad_x, float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
+                                        void* workspace, void* stream) {
+    const int rc = check_bottleneck_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_out && x && y1 && y2 && y3 && stats && packed && norms && grad_norms && workspace, "bottleneck: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_out) && aligned16(x) && aligned16(y1) && aligned16(y2) && aligned16(y3) && aligned16(packed) &&
+                      aligned16(workspace) && (!grad_x || aligned16(grad_x)),
+                  "bottleneck: pointers must be 16-byte aligned");
+    return launch_bottleneck_backward(desc, grad_out, x, y1, y2, y3, stats, packed, norms, grad_x, grad_w_down, grad_w_conv, grad_w_up,
+                                      grad_norms, workspace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

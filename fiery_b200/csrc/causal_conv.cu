@@ -31,6 +31,7 @@
 // Both kernels are written over halo tiles and segments (causal_conv.cuh), so the spatial GRU (spatial_gru.cu) runs its 3x3
 // convolutions on them too: its inputs [x_t, h] are two halo tiles from two tensors, its outputs up to two segments of the accumulator
 // with their own epilogues.  A causal convolution is one map read at kt frame offsets and one stored segment.
+#include "bn_coef.cuh"
 #include "causal_conv.cuh"
 #include "wgmma.cuh"
 #include "wgrad_chunks.cuh"
@@ -123,10 +124,11 @@ __device__ __forceinline__ void cc_epilogue(const CcOutSeg& o, float bias_init, 
 
 // SEG = false: the causal convolution -- kt halo tiles of map 0 with one channel count, a CC_WSTAGES ring, one stored segment; every
 // per-halo quantity is the uniform one, so its instantiations compile to the single-input kernel.  SEG = true: the per-halo maps,
-// channel counts and ring depth of CcFwdLaunch, and the segment epilogues.
-template <int N, bool SEG>
-__global__ void __launch_bounds__(CC_FWD_THREADS, 1)
-causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_constant__ CcFwdLaunch L) {
+// channel counts and ring depth of CcFwdLaunch, and the segment epilogues.  BN (with SEG = false, one halo): the Bottleneck's 3x3
+// convolution -- once the halo tile has landed, each of its values of channel c < cin at a map position becomes
+// bn_relu_apply(coef[c], v) in shared memory; the zero fill outside the map (the padding of the normalized map) stays 0.
+template <int N, bool SEG, bool BN>
+__device__ __forceinline__ void cc_fwd_body(const CcFwdMaps& maps, const CcFwdLaunch& L, const BnCoef* __restrict__ coef, int cin) {
     const int taps = 9 * L.halos;
     const int stages = SEG ? L.stages : CC_WSTAGES;
     const int w_bytes = SEG ? L.stage_bytes : L.ka[0] * N * 128;
@@ -181,6 +183,15 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_cons
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
     mbar_wait(x_full, 0);
+    if constexpr (BN) {                                // the halo tile is read by generic loads only: a barrier suffices
+        float* hx = const_cast<float*>(s_x);
+        for (int idx = threadIdx.x; idx < cin * CC_PLANE; idx += 256) {
+            const int c = idx / CC_PLANE, r = idx % CC_PLANE;
+            const int gx = x0 - 1 + r / CC_HY, gy = y0 - 4 + r % CC_HY;
+            if (gx >= 0 && gx < L.X && gy >= 0 && gy < L.Y) hx[idx] = bn_relu_apply(coef[c], hx[idx]);
+        }
+        named_barrier(1, 256);
+    }
 #pragma unroll 1
     for (int j = 0; j < taps; ++j) {
         const int jt = j / 9, ay = j / 3 % 3, ax = j % 3;
@@ -243,6 +254,19 @@ causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_cons
     }
 }
 
+template <int N, bool SEG>
+__global__ void __launch_bounds__(CC_FWD_THREADS, 1)
+causal_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_constant__ CcFwdLaunch L) {
+    cc_fwd_body<N, SEG, false>(maps, L, nullptr, 0);
+}
+
+template <int N>
+__global__ void __launch_bounds__(CC_FWD_THREADS, 1)
+bottleneck_conv_fwd_kernel(const __grid_constant__ CcFwdMaps maps, const __grid_constant__ CcFwdLaunch L, const BnCoef* __restrict__ coef,
+                           int cin) {
+    cc_fwd_body<N, false, true>(maps, L, coef, cin);
+}
+
 int cc_launch_fwd(int N, bool segments, const CcFwdMaps& maps, const CcFwdLaunch& L, long long n_tiles, cudaStream_t stream) {
     FIERY_REQUIRE(n_tiles < (1ll << 31), "3x3 conv: too many pixel tiles");
     if (n_tiles == 0) return FIERY_OK;
@@ -294,11 +318,12 @@ size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d) {
 // NO output channels) = x_tap gy^T.  Per tile the stage holds the x row run of frame t * fmul + foff + tau - (kt - 1), row x + dy - 1
 // (64 channel rows of 44 columns, read as the register A operand at column offset dx + 3) and the gy run (NO K-major rows of 32 pixels
 // from channel o0, the B operand).  Thread 0 issues the loads: at iteration i, after the barrier that ends the MMAs on tile i - 1, tile
-// i + stages - 1 into that tile's stage.
-template <int NO>
-__global__ void __launch_bounds__(128, 1)
-causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, const CcWgradSeg seg, float* __restrict__ partial,
-                         int n_tiles) {
+// i + stages - 1 into that tile's stage.  BN (kt = 1): the Bottleneck's 3x3 convolution -- once a tile's x run has landed, each of
+// its values of channel c < cin at a map position becomes bn_relu_apply(coef[c], v) in shared memory; the zero fill outside the map
+// (the padding of the normalized map) stays 0.
+template <int NO, bool BN>
+__device__ __forceinline__ void cc_wgrad_body(const CcWgradMaps& maps, const CcShape& s, const CcWgradSeg& seg, float* __restrict__ partial,
+                                              int n_tiles, const BnCoef* __restrict__ coef) {
     unsigned char* smem = dynamic_smem_1024();
     constexpr int STAGE_BYTES = CC_WG_X_BYTES + NO * 128;
     const MbarRing ring(reinterpret_cast<uint64_t*>(smem + CC_WG_STAGES * STAGE_BYTES), CC_WG_STAGES);
@@ -341,6 +366,18 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
         __syncthreads();                           // every warp is done with tile i - 1: its stage may be refilled
         if (threadIdx.x == 0 && t0 + i + CC_WG_STAGES - 1 < t1) load(i + CC_WG_STAGES - 1);
         const int st = ring.consume(i);
+        if constexpr (BN) {                        // generic writes the TMA later overwrites: fence, then barrier
+            float* xr = reinterpret_cast<float*>(smem + st * STAGE_BYTES);
+            const int t = t0 + i, run = t % runs, gx = (t / runs) % s.X + dy - 1;
+            if (gx >= 0 && gx < s.X) {
+                for (int idx = threadIdx.x; idx < seg.cin * CC_WG_XP; idx += 128) {
+                    const int c = idx / CC_WG_XP, gy = CC_WG_PX * run - 4 + idx % CC_WG_XP;
+                    if (gy >= 0 && gy < s.Y) xr[idx] = bn_relu_apply(coef[c], xr[idx]);
+                }
+            }
+            fence_proxy_async();
+            __syncthreads();
+        }
         const float* xs = reinterpret_cast<const float*>(smem + st * STAGE_BYTES) + ra * CC_WG_XP + kq + 3;
         const uint32_t g_addr = smem_addr(smem + st * STAGE_BYTES + CC_WG_X_BYTES);
         uint32_t a[CC_WG_PX / 8][3][4];
@@ -386,6 +423,20 @@ causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape
                 }
         }
     }
+}
+
+template <int NO>
+__global__ void __launch_bounds__(128, 1)
+causal_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, const CcWgradSeg seg, float* __restrict__ partial,
+                         int n_tiles) {
+    cc_wgrad_body<NO, false>(maps, s, seg, partial, n_tiles, nullptr);
+}
+
+template <int NO>
+__global__ void __launch_bounds__(128, 1)
+bottleneck_conv_wgrad_kernel(const __grid_constant__ CcWgradMaps maps, const CcShape s, const CcWgradSeg seg, float* __restrict__ partial,
+                             int n_tiles, const BnCoef* __restrict__ coef) {
+    cc_wgrad_body<NO, true>(maps, s, seg, partial, n_tiles, coef);
 }
 
 // grad_w (C_out, C_in, kt, 3, 3) index -> its place in a chunk's partial (tap, o, ci)
@@ -445,8 +496,32 @@ static int cc_encode_activation(CUtensorMap* map, const CcShape& s, const float*
     return cc_encode_map(map, t, s.Y, s.X, s.frames, channels, s.batch, strides, box_y, box_x, box_c, swizzle, what);
 }
 
-// forward (dgrad = 0): x (C_in channels) -> y (C_out) with pack F; input gradient (dgrad = 1): gy (C_out) -> gx (C_in) with pack T
-static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const float* in, const float* packed, float* out, cudaStream_t stream) {
+// The Bottleneck's forward: bottleneck_conv_fwd_kernel<N>, N = the output channels rounded up to 8 (8 .. 64)
+static int cc_launch_bn_fwd(int N, const CcFwdMaps& maps, const CcFwdLaunch& L, long long n_tiles, const BnCoef* coef, int cin,
+                            cudaStream_t stream) {
+    if (n_tiles == 0) return FIERY_OK;
+    const int smem = cc_fwd_smem(L);
+    FIERY_REQUIRE(smem <= CC_MAX_SMEM, "3x3 conv: %d bytes of shared memory", smem);
+    int rc;
+    switch (N) {
+#define CC_BN_FWD_CASE(NN)                                                                                                         \
+    case NN:                                                                                                                       \
+        if ((rc = set_dynamic_smem(bottleneck_conv_fwd_kernel<NN>, smem)) != FIERY_OK) return rc;                                 \
+        bottleneck_conv_fwd_kernel<NN><<<static_cast<unsigned>(n_tiles), CC_FWD_THREADS, smem, stream>>>(maps, L, coef, cin);      \
+        break;
+        CC_BN_FWD_CASE(8) CC_BN_FWD_CASE(16) CC_BN_FWD_CASE(24) CC_BN_FWD_CASE(32) CC_BN_FWD_CASE(40) CC_BN_FWD_CASE(48)
+        CC_BN_FWD_CASE(56) CC_BN_FWD_CASE(64)
+#undef CC_BN_FWD_CASE
+        default: return set_error(FIERY_E_INVALID, "bottleneck: %d accumulator columns in the 3x3 conv", N);
+    }
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+// forward (dgrad = 0): x (C_in channels) -> y (C_out) with pack F; input gradient (dgrad = 1): gy (C_out) -> gx (C_in) with pack T.
+// coef (forward, kt = 1 only): the Bottleneck's BN + ReLU prologue on x, or nullptr.
+static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const float* in, const float* packed, float* out,
+                          cudaStream_t stream, const BnCoef* coef = nullptr) {
     const CcShape s = cc_shape(d);
     const CcPackDir f = cc_pack_dir(s.cout, s.cin, s.taps);
     const CcPackDir p = dgrad ? cc_pack_dir(s.cin, s.cout, s.taps) : f;
@@ -493,6 +568,10 @@ static int cc_launch_conv(const fiery_causal_conv3d_desc_t* d, int dgrad, const 
     const long long n_tiles = static_cast<long long>(s.batch) * s.frames * L.tiles_x * L.tiles_y;
     FIERY_REQUIRE(n_tiles < (1ll << 31), "causal conv: too many pixel tiles");
     if (p.n > 64) return set_error(FIERY_E_INVALID, "causal conv: %d channels padded to %d", n_out, p.n);
+    if (coef) {
+        FIERY_REQUIRE(!dgrad && s.kt == 1, "bottleneck: the BN prologue runs in the forward of a (1, 3, 3) conv only");
+        return cc_launch_bn_fwd(p.n, maps, L, n_tiles, coef, s.cin, stream);
+    }
     return cc_launch_fwd(p.n, false, maps, L, n_tiles, stream);
 }
 
@@ -504,8 +583,14 @@ int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* g
     return cc_launch_conv(d, 1, gy, packed, gx, stream);
 }
 
-int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const float* gy, float* gw, void* workspace,
-                             cudaStream_t stream) {
+int launch_bottleneck_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, const BnCoef* coef, float* y,
+                                   cudaStream_t stream) {
+    return cc_launch_conv(d, 0, x, packed, y, stream, coef);
+}
+
+// coef: nullptr (the causal convolution's weight gradient) or the Bottleneck's BN + ReLU prologue on x (kt = 1)
+static int cc_launch_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const float* gy, const BnCoef* coef, float* gw,
+                                void* workspace, cudaStream_t stream) {
     const CcShape s = cc_shape(d);
     const long long tiles = cc_wgrad_tiles(s);
     const int n_chunks = wgrad_chunks(tiles, WG_MAX_CHUNKS);
@@ -521,9 +606,37 @@ int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x
         if (rc != FIERY_OK) return rc;
         maps.x_first = maps.x;
         const CcWgradSeg seg{0, s.cin, 0, s.cout, 1, 0, 0};
-        if ((rc = cc_launch_wgrad(maps, s, seg, partial, n_chunks, stream)) != FIERY_OK) return rc;
+        if (coef) {
+            FIERY_REQUIRE(s.kt == 1, "bottleneck: the BN prologue runs in the weight gradient of a (1, 3, 3) conv only");
+            const int smem = CC_WG_STAGES * (CC_WG_X_BYTES + no * 128) + CC_SMEM_SLACK;
+            const dim3 grid(static_cast<unsigned>(n_chunks), 3u);
+            switch (no) {
+#define CC_BN_WG_CASE(N)                                                                                                           \
+    case N:                                                                                                                        \
+        if ((rc = set_dynamic_smem(bottleneck_conv_wgrad_kernel<N>, smem)) != FIERY_OK) return rc;                                 \
+        bottleneck_conv_wgrad_kernel<N><<<grid, 128, smem, stream>>>(maps, s, seg, partial, static_cast<int>(tiles), coef);         \
+        break;
+                CC_BN_WG_CASE(8) CC_BN_WG_CASE(16) CC_BN_WG_CASE(24) CC_BN_WG_CASE(32) CC_BN_WG_CASE(40) CC_BN_WG_CASE(48)
+                CC_BN_WG_CASE(56) CC_BN_WG_CASE(64)
+#undef CC_BN_WG_CASE
+                default: return set_error(FIERY_E_INVALID, "bottleneck: %d output channels in the 3x3 weight gradient", s.cout);
+            }
+            FIERY_CUDA_CHECK(cudaGetLastError());
+        } else if ((rc = cc_launch_wgrad(maps, s, seg, partial, n_chunks, stream)) != FIERY_OK) {
+            return rc;
+        }
     }
     return cc_wgrad_reduce(s, partial, n_chunks, gw, stream);
+}
+
+int launch_causal_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const float* gy, float* gw, void* workspace,
+                             cudaStream_t stream) {
+    return cc_launch_conv_wgrad(d, x, gy, nullptr, gw, workspace, stream);
+}
+
+int launch_bottleneck_conv_wgrad(const fiery_causal_conv3d_desc_t* d, const float* x, const BnCoef* coef, const float* gy, float* gw,
+                                 void* workspace, cudaStream_t stream) {
+    return cc_launch_conv_wgrad(d, x, gy, coef, gw, workspace, stream);
 }
 
 }  // namespace fiery

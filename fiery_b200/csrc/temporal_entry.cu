@@ -25,6 +25,7 @@
 // operands.  With E > 0 the egopose is written into the input tile's rows K .. K + E - 1 (TF32-rounded) so its columns come out of the
 // same MMAs.  The 64-pixel tiles are cut into chunks whose boundaries depend on (frames, X*Y) only; each chunk stores its partial and a
 // reduce kernel adds the partials in ascending chunk order: bit-reproducible, no atomics.
+#include "bn_coef.cuh"
 #include "wgmma.cuh"
 #include "wgrad_chunks.cuh"
 
@@ -138,12 +139,25 @@ int launch_temporal_entry_pack(const fiery_temporal_entry_desc_t* d, const float
 // shared device helpers
 // ------------------------------------------------------------------------------------------------------------------------------
 // acc[c] (64 pixel rows x 64 columns of n-chunk c) += tile rows 32 kg .. 32 kg + 31 (as the register A operand, pixel rows pa / pb)
-// x the B atom at b_atom (NC*64 K-major rows of 32 fp32 k); 4 k-steps, drained before returning
-template <int NC>
+// x the B atom at b_atom (NC*64 K-major rows of 32 fp32 k); 4 k-steps, drained before returning.  BN: each fragment value v of
+// channel row ch becomes bn_relu_apply(coef[ch], v) (coef: one entry per tile row, zero past the input's channels) before the
+// tensor core truncates it, as it truncates the plain input.
+template <int NC, bool BN = false>
 __device__ __forceinline__ void te_mma_group(float (&acc)[NC][32], const unsigned char* tile, int rows, int kg, int pa, int pb,
-                                             uint32_t b_atom) {
+                                             uint32_t b_atom, const BnCoef* coef = nullptr) {
     uint32_t a[4][4];
     load_pixel_frags<4>(a, tile, rows, 32 * kg, pa, pb);
+    if constexpr (BN) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int ch = 32 * kg + 8 * k + (threadIdx.x & 3);
+            const BnCoef lo = coef[ch], hi = coef[ch + 4];
+            a[k][0] = __float_as_uint(bn_relu_apply(lo, __uint_as_float(a[k][0])));
+            a[k][1] = __float_as_uint(bn_relu_apply(lo, __uint_as_float(a[k][1])));
+            a[k][2] = __float_as_uint(bn_relu_apply(hi, __uint_as_float(a[k][2])));
+            a[k][3] = __float_as_uint(bn_relu_apply(hi, __uint_as_float(a[k][3])));
+        }
+    }
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k)
@@ -155,8 +169,9 @@ __device__ __forceinline__ void te_mma_group(float (&acc)[NC][32], const unsigne
 
 // One warpgroup's epilogue for 32 accumulator columns (n-chunk c, half h) of its 64 pixel rows: fragments -> staging (channel rows
 // of 64 pixels) -> one 256-byte row store per channel.  row_ptr(col) gives the destination of column col's 64 pixels (nullptr: skip)
-// and its bias.  bar_id: the warpgroup's named barrier.
-template <typename RowFn>
+// and its bias; with RES also the row of 64 pixels added after the bias (row_ptr(col, bias, res)).  bar_id: the warpgroup's named
+// barrier.
+template <bool RES = false, typename RowFn>
 __device__ __forceinline__ void te_store_cols(const float (&acc)[32], int h, float* stg, int bar_id, int n_valid_px, RowFn row_ptr) {
     const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int r0 = 16 * wq + (lane >> 2);
@@ -174,10 +189,20 @@ __device__ __forceinline__ void te_store_cols(const float (&acc)[32], int h, flo
 #pragma unroll
     for (int col = 8 * wq; col < 8 * wq + 8; ++col) {
         float bias = 0.f;
-        float* dst = row_ptr(col, bias);
-        if (dst != nullptr && 2 * lane < n_valid_px) {
-            const float2 v = *reinterpret_cast<const float2*>(stg + col * TE_STG_PITCH + 2 * lane);
-            *reinterpret_cast<float2*>(dst + 2 * lane) = make_float2(v.x + bias, v.y + bias);
+        if constexpr (RES) {
+            const float* res = nullptr;
+            float* dst = row_ptr(col, bias, res);
+            if (dst != nullptr && 2 * lane < n_valid_px) {
+                const float2 v = *reinterpret_cast<const float2*>(stg + col * TE_STG_PITCH + 2 * lane);
+                const float2 r = *reinterpret_cast<const float2*>(res + 2 * lane);
+                *reinterpret_cast<float2*>(dst + 2 * lane) = make_float2((v.x + bias) + r.x, (v.y + bias) + r.y);
+            }
+        } else {
+            float* dst = row_ptr(col, bias);
+            if (dst != nullptr && 2 * lane < n_valid_px) {
+                const float2 v = *reinterpret_cast<const float2*>(stg + col * TE_STG_PITCH + 2 * lane);
+                *reinterpret_cast<float2*>(dst + 2 * lane) = make_float2(v.x + bias, v.y + bias);
+            }
         }
     }
     named_barrier(bar_id, 128);
@@ -209,10 +234,12 @@ struct TeOut {
 
 constexpr int TE_FWD_THREADS = 2 * 128 + 32;
 
-template <int NCH>
-__global__ void __launch_bounds__(TE_FWD_THREADS, 1)
-temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape s, const float* __restrict__ extra,
-                          const float* __restrict__ w_extra, const TeOut out, int stages, int tiles_per_frame, int n_tiles) {
+// BN: the Bottleneck's up projection -- every input value goes through bn_relu_apply with its channel's coefficients (coef, K
+// entries, copied to s_coef with zeros up to Kpad) as the consumers read it; the instantiation without it is the entry's forward.
+template <int NCH, bool BN>
+__device__ __forceinline__ void te_fwd_body(const TeFwdMaps& maps, const TeShape& s, const float* __restrict__ extra,
+                                            const float* __restrict__ w_extra, const TeOut& out, int stages, int tiles_per_frame, int n_tiles,
+                                            const BnCoef* __restrict__ coef, BnCoef* s_coef) {
     const int k32 = (s.Kpad + 31) & ~31;
     const int w_atom = NCH * 64 * 128;
     const int x_bytes = 4 * s.Kpad * 128;
@@ -231,6 +258,8 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
         mbar_init(w_full, 1);                          // published to the async proxy by the fence in ring.init
         ring.init(8);
     }
+    if constexpr (BN)
+        for (int c = threadIdx.x; c < s.Kpad; c += blockDim.x) s_coef[c] = c < s.K ? coef[c] : BnCoef{};
     __syncthreads();
 
     if (warp == 8) {
@@ -269,7 +298,7 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
             for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
 #pragma unroll 1
         for (int kg = 0; kg < k32 / 32; ++kg)          // 32 channels (4 k-steps, 16 fragment registers) at a time
-            te_mma_group<NCH>(acc, tile, s.Kpad, kg, pa, pb, w_addr + kg * w_atom);
+            te_mma_group<NCH, BN>(acc, tile, s.Kpad, kg, pa, pb, w_addr + kg * w_atom, s_coef);
 #pragma unroll
         for (int c = 0; c < NCH; ++c) wgmma_fence_operands(acc[c]);
         ring.release(it);                              // this warp's part of the tile has been read
@@ -311,6 +340,21 @@ temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape 
     }
 }
 
+template <int NCH>
+__global__ void __launch_bounds__(TE_FWD_THREADS, 1)
+temporal_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape s, const float* __restrict__ extra,
+                          const float* __restrict__ w_extra, const TeOut out, int stages, int tiles_per_frame, int n_tiles) {
+    te_fwd_body<NCH, false>(maps, s, extra, w_extra, out, stages, tiles_per_frame, n_tiles, nullptr, nullptr);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(TE_FWD_THREADS, 1)
+bottleneck_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape s, const TeOut out, int stages, int tiles_per_frame,
+                            int n_tiles, const BnCoef* __restrict__ coef) {
+    __shared__ BnCoef s_coef[128];
+    te_fwd_body<NCH, true>(maps, s, nullptr, nullptr, out, stages, tiles_per_frame, n_tiles, coef, s_coef);
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------
 // input gradient
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -322,10 +366,12 @@ struct TeDgradMaps {
 };
 
 // BIAS: every output row k of frame f = (b, t) gets bias[f * K + k] added in the epilogue (the temporal aggregation's pooled-vector
-// term); the instantiation without it is the entry's input gradient.
-template <int NCHK, bool BIAS>
+// term); RES: every output value gets the value of res at its place (res has gx's strides) added after that (the Bottleneck's skip
+// connection); the instantiation with neither is the entry's input gradient.
+template <int NCHK, bool BIAS, bool RES = false>
 __device__ __forceinline__ void te_dgrad_body(const TeDgradMaps& maps, const TeShape& s, float* __restrict__ gx,
-                                              const float* __restrict__ bias, int stages, int tiles_per_frame, int n_tiles) {
+                                              const float* __restrict__ bias, int stages, int tiles_per_frame, int n_tiles,
+                                              const float* __restrict__ res = nullptr) {
     const int npad32 = (s.Npad + 31) & ~31;
     const int rows = (s.Npad + 63) & ~63;          // grad tile rows per 32-pixel block
     const int w_atom = NCHK * 64 * 128;
@@ -380,17 +426,26 @@ __device__ __forceinline__ void te_dgrad_body(const TeDgradMaps& maps, const TeS
         for (int c = 0; c < NCHK; ++c) wgmma_fence_operands(acc[c]);
         ring.release(it);
 
-        float* base = gx + static_cast<size_t>(b) * s.sb + static_cast<size_t>(tt) * s.st + p0;
+        const size_t off = static_cast<size_t>(b) * s.sb + static_cast<size_t>(tt) * s.st + p0;
+        float* base = gx + off;
 #pragma unroll
         for (int c = 0; c < NCHK; ++c)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 if (64 * c + 32 * h >= s.K) continue;
-                te_store_cols(acc[c], h, stg, 1, s.pixels - p0, [&](int col, float& b_k) -> float* {
-                    const int k = 64 * c + 32 * h + col;
-                    if (BIAS && k < s.K) b_k = __ldg(bias + static_cast<size_t>(f) * s.K + k);
-                    return k < s.K ? base + static_cast<size_t>(k) * s.sc : nullptr;
-                });
+                if constexpr (RES) {
+                    te_store_cols<true>(acc[c], h, stg, 1, s.pixels - p0, [&](int col, float&, const float*& r) -> float* {
+                        const int k = 64 * c + 32 * h + col;
+                        r = res + off + static_cast<size_t>(k) * s.sc;
+                        return k < s.K ? base + static_cast<size_t>(k) * s.sc : nullptr;
+                    });
+                } else {
+                    te_store_cols(acc[c], h, stg, 1, s.pixels - p0, [&](int col, float& b_k) -> float* {
+                        const int k = 64 * c + 32 * h + col;
+                        if (BIAS && k < s.K) b_k = __ldg(bias + static_cast<size_t>(f) * s.K + k);
+                        return k < s.K ? base + static_cast<size_t>(k) * s.sc : nullptr;
+                    });
+                }
             }
     }
 }
@@ -407,6 +462,13 @@ __global__ void __launch_bounds__(TE_DG_THREADS, 1)
 temporal_aggregation_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ out,
                             const float* __restrict__ bias, int stages, int tiles_per_frame, int n_tiles) {
     te_dgrad_body<NCHK, true>(maps, s, out, bias, stages, tiles_per_frame, n_tiles);
+}
+
+template <int NCHK>
+__global__ void __launch_bounds__(TE_DG_THREADS, 1)
+bottleneck_entry_dgrad_kernel(const __grid_constant__ TeDgradMaps maps, const TeShape s, float* __restrict__ gx,
+                              const float* __restrict__ res, int stages, int tiles_per_frame, int n_tiles) {
+    te_dgrad_body<NCHK, false, true>(maps, s, gx, nullptr, stages, tiles_per_frame, n_tiles, res);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -433,10 +495,13 @@ size_t temporal_entry_wgrad_workspace_bytes(const fiery_temporal_entry_desc_t* d
 
 // grid: one CTA per chunk; warpgroup mb (of Nrows / 64) accumulates output rows 64 mb .. 64 mb + 63 against all NC column chunks.
 // Thread 0 issues the loads: at iteration it, after the barrier that ends every warpgroup's MMAs on tile it - 1, tile it + stages - 1.
-template <int NC>
-__global__ void __launch_bounds__(512, 1)
-temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeShape s, const float* __restrict__ extra,
-                            float* __restrict__ partial, int stages, int tiles_per_frame, int n_tiles) {
+// BN: the Bottleneck's up projection -- before the MMAs read a landed input tile, its values of channels k < K at pixels inside the
+// frame become bn_relu_apply(s_coef[k], v) in shared memory (the zero fill past the frame's pixels stays 0); the tensor core then
+// truncates them as it truncates the plain input.  The instantiation without it is the entry's weight gradient.
+template <int NC, bool BN>
+__device__ __forceinline__ void te_wgrad_body(const TeWgradMaps& maps, const TeShape& s, const float* __restrict__ extra,
+                                              float* __restrict__ partial, int stages, int tiles_per_frame, int n_tiles,
+                                              const BnCoef* __restrict__ coef, BnCoef* s_coef) {
     unsigned char* smem = dynamic_smem_1024();
     const int rows = (s.Npad + 63) & ~63, xrows = 64 * NC;
     const int g_bytes = 2 * rows * 128, stage_bytes = g_bytes + 2 * xrows * 128;
@@ -463,6 +528,8 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
         ring.init(0);
         for (int i = 0; i < stages - 1 && t0 + i < t1; ++i) load(i);
     }
+    if constexpr (BN)
+        for (int c = threadIdx.x; c < s.K; c += nthreads) s_coef[c] = coef[c];
     __syncthreads();
 
     const int mb = threadIdx.x >> 7;
@@ -482,6 +549,18 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
                 const int j = idx / TE_BWD_PX, px = idx % TE_BWD_PX;
                 const float v = p0 + px < s.pixels ? __ldg(extra + static_cast<size_t>(f) * s.E + j) : 0.f;
                 *reinterpret_cast<uint32_t*>(tile + g_bytes + tile_offset(xrows, s.K + j, px)) = to_tf32(v);
+            }
+            fence_proxy_async();
+            named_barrier(2, nthreads);
+        }
+        if constexpr (BN) {                        // generic writes, then the async proxy's MMAs read them: fence, then barrier
+            const int t = t0 + i, n_px = min(TE_BWD_PX, s.pixels - (t % tiles_per_frame) * TE_BWD_PX);
+            for (int idx = threadIdx.x; idx < s.K * TE_BWD_PX; idx += nthreads) {
+                const int k = idx / TE_BWD_PX, px = idx % TE_BWD_PX;
+                if (px < n_px) {
+                    float* v = reinterpret_cast<float*>(tile + g_bytes + tile_offset(xrows, k, px));
+                    *v = bn_relu_apply(s_coef[k], *v);
+                }
             }
             fence_proxy_async();
             named_barrier(2, nthreads);
@@ -515,6 +594,21 @@ temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeSh
                 *reinterpret_cast<float2*>(dst + static_cast<size_t>(o) * xrows + 64 * c + 8 * j + cq) =
                     make_float2(acc[c][4 * j + 2 * half], acc[c][4 * j + 2 * half + 1]);
         }
+}
+
+template <int NC>
+__global__ void __launch_bounds__(512, 1)
+temporal_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeShape s, const float* __restrict__ extra,
+                            float* __restrict__ partial, int stages, int tiles_per_frame, int n_tiles) {
+    te_wgrad_body<NC, false>(maps, s, extra, partial, stages, tiles_per_frame, n_tiles, nullptr, nullptr);
+}
+
+template <int NC>
+__global__ void __launch_bounds__(512, 1)
+bottleneck_entry_wgrad_kernel(const __grid_constant__ TeWgradMaps maps, const TeShape s, float* __restrict__ partial, int stages,
+                              int tiles_per_frame, int n_tiles, const BnCoef* __restrict__ coef) {
+    __shared__ BnCoef s_coef[128];
+    te_wgrad_body<NC, true>(maps, s, nullptr, partial, stages, tiles_per_frame, n_tiles, coef, s_coef);
 }
 
 // grad_w (N_out, K + E) index -> its place in a chunk's partial (padded row o, column k)
@@ -570,8 +664,11 @@ static int te_stages(int fixed_bytes, int stage_bytes) {
     return n < 4 ? n : 4;
 }
 
-int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
-                                  float* const* out, cudaStream_t stream) {
+constexpr int TE_COEF_BYTES = 128 * sizeof(BnCoef);  // the BN instantiations' static shared memory
+
+// coef: nullptr (the entry's forward) or the Bottleneck's BN + ReLU prologue coefficients (K entries)
+static int te_launch_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
+                             float* const* out, const BnCoef* coef, cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const TePack p = te_pack_layout(s);
     TeFwdMaps maps;
@@ -581,7 +678,7 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
     TeOut o{};
     for (int q = 0; q < s.n_seg; ++q) o.p[q] = out[q];
     const int fixed = static_cast<int>(p.f_floats * 4) + 2 * TE_STG_FLOATS * 4 + TE_ROW_TABLE_BYTES;
-    const int stages = te_stages(fixed, 4 * s.Kpad * 128);
+    const int stages = te_stages(fixed + (coef ? TE_COEF_BYTES : 0), 4 * s.Kpad * 128);
     const int smem = fixed + stages * 4 * s.Kpad * 128 + TE_SMEM_SLACK;
     const int tiles_per_frame = (s.pixels + TE_FWD_PX - 1) / TE_FWD_PX;
     const long long n_tiles = static_cast<long long>(s.batch) * s.frames * tiles_per_frame;
@@ -589,6 +686,22 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
     unsigned grid = 0;
     if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     const float* we = packed + p.f_floats + p.t_floats;
+    if (coef) {
+        FIERY_REQUIRE(s.E == 0 && s.Kpad <= 128, "bottleneck: the up projection takes no extra channels and K <= 128");
+        switch (p.nch) {
+#define TE_BN_FWD_CASE(N)                                                                                                           \
+    case N:                                                                                                                         \
+        if ((rc = set_dynamic_smem(bottleneck_entry_fwd_kernel<N>, smem)) != FIERY_OK) return rc;                                   \
+        bottleneck_entry_fwd_kernel<N><<<grid, TE_FWD_THREADS, smem, stream>>>(maps, s, o, stages, tiles_per_frame,                 \
+                                                                               static_cast<int>(n_tiles), coef);                    \
+        break;
+            TE_BN_FWD_CASE(1) TE_BN_FWD_CASE(2)
+#undef TE_BN_FWD_CASE
+            default: return set_error(FIERY_E_INVALID, "bottleneck: up projection N_out padded to %d rows", s.Npad);
+        }
+        FIERY_CUDA_CHECK(cudaGetLastError());
+        return FIERY_OK;
+    }
     switch (p.nch) {
 #define TE_FWD_CASE(N)                                                                                                              \
     case N:                                                                                                                         \
@@ -604,10 +717,20 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
     return FIERY_OK;
 }
 
+int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
+                                  float* const* out, cudaStream_t stream) {
+    return te_launch_forward(d, x, extra, packed, out, nullptr, stream);
+}
+
+int launch_bottleneck_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* packed, const BnCoef* coef, float* out,
+                                    cudaStream_t stream) {
+    return te_launch_forward(d, x, nullptr, packed, &out, coef, stream);
+}
+
 // bias: nullptr (the entry's input gradient) or (batch * frames, K) fp32 added to every pixel of its frame's row k (the temporal
-// aggregation's forward)
-int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, const float* bias,
-                                float* gx, cudaStream_t stream) {
+// aggregation's forward); res: nullptr or a tensor laid out as gx, added to it (the Bottleneck's input gradient plus its skip)
+static int te_launch_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, const float* bias,
+                           const float* res, float* gx, cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const TePack p = te_pack_layout(s);
     TeDgradMaps maps;
@@ -624,7 +747,15 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
     unsigned grid = 0;
     if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     const int nt = static_cast<int>(n_tiles);
-    if (p.nchk == 1 && bias == nullptr) {
+    if (res != nullptr) {
+        if (p.nchk == 1) {
+            if ((rc = set_dynamic_smem(bottleneck_entry_dgrad_kernel<1>, smem)) != FIERY_OK) return rc;
+            bottleneck_entry_dgrad_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, res, stages, tiles_per_frame, nt);
+        } else {
+            if ((rc = set_dynamic_smem(bottleneck_entry_dgrad_kernel<2>, smem)) != FIERY_OK) return rc;
+            bottleneck_entry_dgrad_kernel<2><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, res, stages, tiles_per_frame, nt);
+        }
+    } else if (p.nchk == 1 && bias == nullptr) {
         if ((rc = set_dynamic_smem(temporal_entry_dgrad_kernel<1>, smem)) != FIERY_OK) return rc;
         temporal_entry_dgrad_kernel<1><<<grid, TE_DG_THREADS, smem, stream>>>(maps, s, gx, stages, tiles_per_frame, nt);
     } else if (bias == nullptr) {
@@ -641,8 +772,19 @@ int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const floa
     return FIERY_OK;
 }
 
-int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
-                                float* gw, void* workspace, cudaStream_t stream) {
+int launch_temporal_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* const* gy, const float* packed, const float* bias,
+                                float* gx, cudaStream_t stream) {
+    return te_launch_dgrad(d, gy, packed, bias, nullptr, gx, stream);
+}
+
+int launch_bottleneck_entry_dgrad(const fiery_temporal_entry_desc_t* d, const float* gy, const float* packed, const float* res, float* gx,
+                                  cudaStream_t stream) {
+    return te_launch_dgrad(d, &gy, packed, nullptr, res, gx, stream);
+}
+
+// coef: nullptr (the entry's weight gradient) or the Bottleneck's BN + ReLU prologue coefficients of x (K entries)
+static int te_launch_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
+                           const BnCoef* coef, float* gw, void* workspace, cudaStream_t stream) {
     const TeShape s = te_shape(d);
     const int n_frames = s.batch * s.frames;
     const int n_chunks = te_wgrad_chunks(n_frames, s.pixels);
@@ -654,12 +796,19 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
         if (rc != FIERY_OK) return rc;
         const int rows = round_up(s.Npad, 64), nc = round_up(s.K + s.E, 64) / 64;
         const int stage_bytes = 2 * (rows + 64 * nc) * 128;
-        const int stages = te_stages(64, stage_bytes);
+        const int stages = te_stages(64 + (coef ? TE_COEF_BYTES : 0), stage_bytes);
         const int smem = stages * stage_bytes + TE_SMEM_SLACK;
         const int tiles_per_frame = (s.pixels + TE_BWD_PX - 1) / TE_BWD_PX;
         FIERY_REQUIRE(te_bwd_tiles(n_frames, s.pixels) < (1ll << 31), "temporal entry: too many pixel tiles");
         const int n_tiles = static_cast<int>(te_bwd_tiles(n_frames, s.pixels));
         const unsigned threads = static_cast<unsigned>(2 * rows);          // one warpgroup per 64 output rows
+        if (coef) {
+            FIERY_REQUIRE(nc == 1 && s.E == 0, "bottleneck: the up projection's weight gradient takes K <= 64 and no extra channels");
+            if ((rc = set_dynamic_smem(bottleneck_entry_wgrad_kernel<1>, smem)) != FIERY_OK) return rc;
+            bottleneck_entry_wgrad_kernel<1><<<n_chunks, threads, smem, stream>>>(maps, s, partial, stages, tiles_per_frame, n_tiles, coef);
+            FIERY_CUDA_CHECK(cudaGetLastError());
+            return launch_wgrad_reduce(partial, n_chunks, te_partial_floats(s), s.n_out * (s.K + s.E), TeWgradOffset{s}, gw, stream);
+        }
         switch (nc) {
 #define TE_WG_CASE(N)                                                                                                              \
     case N:                                                                                                                        \
@@ -673,6 +822,16 @@ int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const floa
         FIERY_CUDA_CHECK(cudaGetLastError());
     }
     return launch_wgrad_reduce(partial, n_chunks, te_partial_floats(s), s.n_out * (s.K + s.E), TeWgradOffset{s}, gw, stream);
+}
+
+int launch_temporal_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* const* gy,
+                                float* gw, void* workspace, cudaStream_t stream) {
+    return te_launch_wgrad(d, x, extra, gy, nullptr, gw, workspace, stream);
+}
+
+int launch_bottleneck_entry_wgrad(const fiery_temporal_entry_desc_t* d, const float* x, const BnCoef* coef, const float* gy, float* gw,
+                                  void* workspace, cudaStream_t stream) {
+    return te_launch_wgrad(d, x, nullptr, &gy, coef, gw, workspace, stream);
 }
 
 }  // namespace fiery

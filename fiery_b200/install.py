@@ -293,6 +293,29 @@ def use_tensor_core_future_prediction(model):
                  "fiery_b200: SpatialGRU(s) not covered by the tensor-core kernels, left as is: ", root=_spatial_grus)
 
 
+def _res_blocks(model):
+    fp = getattr(model, "future_prediction", None)
+    return getattr(fp, "res_blocks", None) if fp is not None else None
+
+
+def use_tensor_core_bottlenecks(model):
+    """Replace every covered ``Bottleneck`` in ``model.future_prediction.res_blocks`` (fiery/models/future_prediction.py) of a
+    ``Fiery`` instance by ``fiery_b200.bottleneck.TensorCoreBottleneck``, which adopts the module's ``layers`` (``state_dict`` keys
+    unchanged) and runs it as ``torch.ops.fiery_b200.bottleneck``: each inner BatchNorm2d and ReLU is applied as the next convolution
+    reads its input, forward and backward.  Works before or after ``use_tensor_core_future_prediction``.  Returns the model; a second
+    call does nothing, a model without future prediction is returned untouched, and Bottlenecks the kernels do not cover (a skip
+    projection, another kernel size, dropout > 0, a norm other than BatchNorm2d -- a SyncBatchNorm stays torch's --, more than 128
+    channels) are left alone with one warning."""
+    from .bottleneck import TensorCoreBottleneck, module_reason
+
+    def slots(res_blocks):
+        for i, (_, stack) in enumerate(res_blocks._modules.items()):
+            for name, block in stack._modules.items():
+                yield stack, name, block, f"res_blocks[{i}][{name}]"
+    return _swap(model, slots, TensorCoreBottleneck, module_reason, TensorCoreBottleneck.from_module,
+                 "fiery_b200: Bottleneck(s) not covered by the tensor-core kernels, left as is: ", root=_res_blocks)
+
+
 def uninstall():
     if not _saved:
         return

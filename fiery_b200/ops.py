@@ -470,4 +470,84 @@ spatial_gru.register_autograd(_spatial_gru_backward, setup_context=_spatial_gru_
 torch.library.register_autocast("fiery_b200::spatial_gru", "cuda", torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# The future prediction's Bottleneck (fiery/layers/convolutions.py:64-168, the plain variant): ``bottleneck`` / ``bottleneck_backward``
+# (fiery_b200/bottleneck.py; csrc/bottleneck.cu).  Besides the output it returns the pre-norm maps y1, y2, y3 and the norms'
+# statistics, which the backward reads; they are not differentiable, and the operator updates no running buffer
+# (TensorCoreBottleneck does, from the statistics).  Autocast: fp32, like the other future-prediction operators.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::bottleneck", mutates_args=(), device_types="cuda")
+def bottleneck(x: torch.Tensor, w_down: torch.Tensor, w_conv: torch.Tensor, w_up: torch.Tensor, bn1_weight: Optional[torch.Tensor],
+               bn1_bias: Optional[torch.Tensor], bn1_mean: Optional[torch.Tensor], bn1_var: Optional[torch.Tensor],
+               bn2_weight: Optional[torch.Tensor], bn2_bias: Optional[torch.Tensor], bn2_mean: Optional[torch.Tensor],
+               bn2_var: Optional[torch.Tensor], bn3_weight: Optional[torch.Tensor], bn3_bias: Optional[torch.Tensor],
+               bn3_mean: Optional[torch.Tensor], bn3_var: Optional[torch.Tensor], training: bool,
+               eps: float) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """x (N, C, H, W) -> (out, y1, y2, y3, stats): out = relu(bn3(W_up relu(bn2(conv3x3(relu(bn1(W_down x))))))) + x, contiguous
+    fp32; y1, y2 (N, C / 2, H, W) and y3 (N, C, H, W) the pre-norm maps; stats the (2 (2 (C / 2) + C),) fp32 means and biased
+    variances each norm used (the batch's when ``training``, else copies of the running ones: bnI_mean / bnI_var).  Bit-reproducible."""
+    from .bottleneck import forward
+    return forward(x, w_down, w_conv, w_up, [bn1_weight, bn1_bias, bn1_mean, bn1_var, bn2_weight, bn2_bias, bn2_mean, bn2_var,
+                                             bn3_weight, bn3_bias, bn3_mean, bn3_var], training, eps)
+
+
+@bottleneck.register_fake
+def _(x, w_down, w_conv, w_up, bn1_weight, bn1_bias, bn1_mean, bn1_var, bn2_weight, bn2_bias, bn2_mean, bn2_var, bn3_weight, bn3_bias,
+      bn3_mean, bn3_var, training, eps):
+    n, c, h, w = x.shape
+    m = c // 2
+    new = lambda *shape: x.new_empty(shape, dtype=torch.float32)  # noqa: E731
+    return new(n, c, h, w), new(n, m, h, w), new(n, m, h, w), new(n, c, h, w), new(4 * m + 2 * c)
+
+
+@torch.library.custom_op("fiery_b200::bottleneck_backward", mutates_args=(), device_types="cuda")
+def bottleneck_backward(grad_out: torch.Tensor, x: torch.Tensor, y1: torch.Tensor, y2: torch.Tensor, y3: torch.Tensor,
+                        stats: torch.Tensor, w_down: torch.Tensor, w_conv: torch.Tensor, w_up: torch.Tensor,
+                        bn1_weight: Optional[torch.Tensor], bn1_bias: Optional[torch.Tensor], bn2_weight: Optional[torch.Tensor],
+                        bn2_bias: Optional[torch.Tensor], bn3_weight: Optional[torch.Tensor], bn3_bias: Optional[torch.Tensor],
+                        training: bool, eps: float, need: List[bool]) -> List[torch.Tensor]:
+    """[grad_x, grad_w_down, grad_w_conv, grad_w_up, then each norm's grad weight and grad bias] of ``bottleneck``, each in its
+    input's shape and dtype; ``need`` (10 flags in that order) says which are computed, the others come back empty."""
+    from .bottleneck import backward
+    norms = [bn1_weight, bn1_bias, None, None, bn2_weight, bn2_bias, None, None, bn3_weight, bn3_bias, None, None]
+    g = backward(grad_out, x, y1, y2, y3, stats, w_down, w_conv, w_up, norms, training, eps, need)
+    likes = [x, w_down, w_conv, w_up, bn1_weight, bn1_bias, bn2_weight, bn2_bias, bn3_weight, bn3_bias]
+    return [_cast_back(gi, like if like is not None else x) for gi, like in zip(g, likes)]
+
+
+@bottleneck_backward.register_fake
+def _(grad_out, x, y1, y2, y3, stats, w_down, w_conv, w_up, bn1_weight, bn1_bias, bn2_weight, bn2_bias, bn3_weight, bn3_bias, training,
+      eps, need):
+    likes = [x, w_down, w_conv, w_up, bn1_weight, bn1_bias, bn2_weight, bn2_bias, bn3_weight, bn3_bias]
+    return [like.new_empty(like.shape) if nd and like is not None else x.new_empty((0,)) for like, nd in zip(likes, need)]
+
+
+def _bottleneck_setup_context(ctx, inputs, output):
+    x, w_d, w_c, w_u, n1w, n1b, _m1, _v1, n2w, n2b, _m2, _v2, n3w, n3b, _m3, _v3, training, eps = inputs
+    _out, y1, y2, y3, stats = output
+    ctx.mark_non_differentiable(y1, y2, y3, stats)
+    ctx.args = (training, eps)
+    ctx.save_for_backward(x, y1, y2, y3, stats, w_d, w_c, w_u, n1w, n1b, n2w, n2b, n3w, n3b)
+
+
+_BOTTLENECK_GRAD_SLOTS = (0, 1, 2, 3, 4, 5, 8, 9, 12, 13)          # the inputs bottleneck_backward's gradients belong to
+
+
+def _bottleneck_backward(ctx, grad_out, _g1, _g2, _g3, _gs):
+    x, y1, y2, y3, stats, w_d, w_c, w_u, n1w, n1b, n2w, n2b, n3w, n3b = ctx.saved_tensors
+    need = [bool(ctx.needs_input_grad[i]) for i in _BOTTLENECK_GRAD_SLOTS]
+    grads = [None] * 18
+    if not any(need) or grad_out is None:
+        return tuple(grads)
+    g = torch.ops.fiery_b200.bottleneck_backward(grad_out, x, y1, y2, y3, stats, w_d, w_c, w_u, n1w, n1b, n2w, n2b, n3w, n3b, *ctx.args,
+                                                 need)
+    for slot, gi, nd in zip(_BOTTLENECK_GRAD_SLOTS, g, need):
+        grads[slot] = gi if nd else None
+    return tuple(grads)
+
+
+bottleneck.register_autograd(_bottleneck_backward, setup_context=_bottleneck_setup_context)
+torch.library.register_autocast("fiery_b200::bottleneck", "cuda", torch.float32)
+
+
 from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

@@ -644,6 +644,66 @@ FIERY_API size_t fiery_conv3x3_backward_weight_workspace_bytes(const fiery_conv3
 FIERY_API int fiery_conv3x3_backward_weight(const fiery_conv3x3_desc_t* desc, const float* x0, const float* x1, const float* grad_y,
                                             float* grad_w, void* workspace, void* stream);
 
+/*
+ * The future prediction's Bottleneck (fiery/layers/convolutions.py:64-168, the plain variant: out_channels = in_channels = C, a 3x3
+ * convolution with padding 1 and stride 1, no projection, dropout 0) on `maps` independent (X, Y) maps, with M = C / 2 (integer
+ * division, the reference's int(in_channels / 2)):
+ *   y1 = W_down x                       (1x1, C -> M)
+ *   y2 = conv3x3(relu(bn1(y1)))         (M -> M; the zero padding is relu(bn1(y1))'s)
+ *   y3 = W_up relu(bn2(y2))             (1x1, M -> C)
+ *   out = relu(bn3(y3)) + x
+ * Each bn_i is fiery_batch_norm_forward's (training: this call's batch statistics; eval: the running ones), so relu(bn_i(y)) is
+ * max(fmaf(scale, y, shift), 0) with its fp64-derived scale and shift.  relu(bn1(y1)) and relu(bn2(y2)) are never stored: each value
+ * is computed as the next convolution reads it, exactly the fp32 value fiery_batch_norm_forward (relu 1) would write, and then
+ * treated as that convolution treats its input (the 3x3 rounds it to TF32 nearest, the 1x1 lets the tensor core truncate it).  So y1
+ * is fiery_temporal_entry_forward's (batch = maps, frames = 1), y2 fiery_causal_conv3d_forward's (kt = 1) on fiery_batch_norm_forward's
+ * output of y1, y3 the entry's on bn2's output, out fiery_batch_norm_forward's (relu 1, residual x) of y3, bit for bit.
+ *
+ * The backward, from g = grad_out: dy3 = bn3's backward (relu) of (y3, g); grad_w_up from the entry weight gradient of relu(bn2(y2))
+ * (computed as its tile is read) and dy3; da2 = W_up^T dy3; dy2 = bn2's backward of (y2, da2); grad_w_conv from the 3x3 weight gradient
+ * of relu(bn1(y1)) (computed as its run is read) and dy2; da1 = the 3x3 input gradient of dy2; dy1 = bn1's backward of (y1, da1);
+ * grad_w_down = the entry weight gradient of (x, dy1); grad_x = W_down^T dy1 + g, the add in the input gradient's epilogue (one fp32 add
+ * of the same two values).  Each is bit for bit that composition of fiery_temporal_entry_*, fiery_causal_conv3d_* and
+ * fiery_batch_norm_backward.  The backward computes what is asked for: grad_x, each weight gradient and each grad_norms entry may be
+ * NULL (a NULL weight gradient launches nothing for it, and the stages below the last gradient asked for do not run).
+ *
+ * x, out, y3, grad_out, grad_x: (maps, C, X, Y) fp32, contiguous; y1, y2: (maps, M, X, Y).  W_down / grad_w_down (M, C), W_conv /
+ * grad_w_conv (M, M, 3, 3), W_up / grad_w_up (C, M): fp32, contiguous (a 1x1 conv weight's trailing (1, 1) dropped).  norms: 12
+ * pointers, norm i = 0, 1, 2 (M, M, C channels) at [4i .. 4i + 3]: weight, bias, running_mean, running_var; weight / bias may be NULL
+ * (1 / 0); running_* are read in eval only.  grad_norms: 6 pointers, [2i] = grad weight and [2i + 1] = grad bias of norm i, each may
+ * be NULL.  stats: 2 (2M + C) fp32, written by the forward and read by the backward: mean1, var1, mean2, var2 (M each), mean3, var3 (C
+ * each), the biased variances (copies of the running statistics in eval).  Workspaces: the *_workspace_bytes, 16-byte aligned,
+ * contents irrelevant (0 bytes for a rejected descriptor).
+ * Limits (FIERY_E_INVALID, the message names the field): 2 <= channels <= 128 (M <= 64 for the 3x3 kernels, K <= 128 for the entry);
+ * maps >= 1; grid_x >= 1; grid_y a positive multiple of 4 (so pixels X*Y % 4 == 0); training 0 or 1; eps >= 0; in training
+ * maps * X * Y >= 2; pointers 16-byte aligned.
+ *
+ * Summation orders: the reused kernels' (no atomics, no host synchronisation; bit-reproducible and graph-capturable): the statistics
+ * and norm gradients as fiery_batch_norm_*, the 1x1 weight gradients as fiery_temporal_entry_backward_weight's over (maps, 1 frame),
+ * the 3x3's as fiery_causal_conv3d_backward_weight's with kt = 1.  Kernels: csrc/bottleneck.cu on csrc/temporal_entry.cu,
+ * csrc/causal_conv.cu and csrc/batch_norm.cu.
+ */
+typedef struct {
+    int32_t maps;                 /* N: independent maps (batch * frames) */
+    int32_t grid_x;
+    int32_t grid_y;
+    int32_t channels;             /* C: in_channels = out_channels */
+    int32_t training;             /* 1: batch statistics; 0: running statistics */
+    double eps;
+} fiery_bottleneck_desc_t;
+
+FIERY_API size_t fiery_bottleneck_packed_bytes(const fiery_bottleneck_desc_t* desc);
+FIERY_API int fiery_bottleneck_pack_weights(const fiery_bottleneck_desc_t* desc, const float* w_down, const float* w_conv, const float* w_up,
+                                            void* packed, void* stream);
+FIERY_API size_t fiery_bottleneck_forward_workspace_bytes(const fiery_bottleneck_desc_t* desc);
+FIERY_API int fiery_bottleneck_forward(const fiery_bottleneck_desc_t* desc, const float* x, const void* packed, const float* const* norms,
+                                       float* y1, float* y2, float* y3, float* out, float* stats, void* workspace, void* stream);
+FIERY_API size_t fiery_bottleneck_backward_workspace_bytes(const fiery_bottleneck_desc_t* desc);
+FIERY_API int fiery_bottleneck_backward(const fiery_bottleneck_desc_t* desc, const float* grad_out, const float* x, const float* y1,
+                                        const float* y2, const float* y3, const float* stats, const void* packed, const float* const* norms,
+                                        float* grad_x, float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
+                                        void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
