@@ -192,6 +192,10 @@ SIGNATURES = {
     "fiery_bottleneck_backward_workspace_bytes": (c_size_t, [POINTER(BottleneckDesc)]),
     "fiery_bottleneck_backward": (c_int32, [POINTER(BottleneckDesc)] + [c_void_p] * 7 + [POINTER(c_void_p)] + [c_void_p] * 4
                                   + [POINTER(c_void_p), c_void_p, c_void_p]),
+    "fiery_bottleneck_sync_forward_stage": (c_int32, [POINTER(BottleneckDesc), c_int32, c_int32] + [c_void_p] * 3 + [POINTER(c_void_p)]
+                                            + [c_void_p] * 9),
+    "fiery_bottleneck_sync_backward_stage": (c_int32, [POINTER(BottleneckDesc), c_int32, c_int32] + [c_void_p] * 8 + [POINTER(c_void_p)]
+                                             + [c_void_p] * 4 + [POINTER(c_void_p)] + [c_void_p] * 3),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),

@@ -602,14 +602,20 @@ int launch_batch_norm_local_stats(const fiery_batch_norm_desc_t* d, const float*
     return FIERY_OK;
 }
 
+int launch_batch_norm_coef_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* w, const float* bias,
+                                    float* mean_out, float* var_out, double* count_out, void* workspace, cudaStream_t stream) {
+    bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
+                                                                              var_out, count_out, bn_work(d, workspace).coef);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
 int launch_batch_norm_forward_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* x, const float* w,
                                        const float* bias, const float* residual, float* y, float* mean_out, float* var_out,
                                        double* count_out, void* workspace, cudaStream_t stream) {
     const BnShape s = bn_shape(d);
-    BnCoef* coef = bn_work(d, workspace).coef;
-    bn_gathered_forward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(world, d->channels, gathered, w, bias, d->eps, mean_out,
-                                                                              var_out, count_out, coef);
-    bn_apply(d, s, x, coef, residual, y, stream);
+    launch_batch_norm_coef_gathered(d, world, gathered, w, bias, mean_out, var_out, count_out, workspace, stream);
+    bn_apply(d, s, x, bn_work(d, workspace).coef, residual, y, stream);
     FIERY_CUDA_CHECK(cudaGetLastError());
     return FIERY_OK;
 }

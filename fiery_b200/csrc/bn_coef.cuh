@@ -24,4 +24,9 @@ int launch_batch_norm_coef(const fiery_batch_norm_desc_t* d, const float* x, con
                            const float* running_var, float* mean_out, float* var_out, void* workspace, cudaStream_t stream);
 size_t batch_norm_workspace_bytes(const fiery_batch_norm_desc_t* d);
 
+// The same from a group's gathered (world, channels, 3) (n, mean, M2) triplets (fiery_batch_norm_forward_gathered without the apply
+// pass): the group's statistics, count_out[0] = the group's n (may be NULL) and the coefficients at the start of the workspace.
+int launch_batch_norm_coef_gathered(const fiery_batch_norm_desc_t* d, int world, const double* gathered, const float* w, const float* bias,
+                                    float* mean_out, float* var_out, double* count_out, void* workspace, cudaStream_t stream);
+
 }  // namespace fiery

@@ -188,6 +188,14 @@ int launch_bottleneck_backward(const fiery_bottleneck_desc_t* d, const float* gr
                                const float* y3, const float* stats, const void* packed, const float* const* norms, float* grad_x,
                                float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms, void* workspace,
                                cudaStream_t stream);
+int launch_bottleneck_sync_forward_stage(const fiery_bottleneck_desc_t* d, int stage, int world, const double* gathered, const float* x,
+                                         const void* packed, const float* const* norms, float* y1, float* y2, float* y3, float* out,
+                                         float* stats, double* counts, double* local, void* workspace, cudaStream_t stream);
+int launch_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t* d, int stage, int world, const double* gathered,
+                                          const float* grad_out, const float* x, const float* y1, const float* y2, const float* y3,
+                                          const float* stats, const void* packed, const float* const* norms, float* grad_x,
+                                          float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms, double* local,
+                                          void* workspace, cudaStream_t stream);
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
 int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
 size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d);
@@ -1098,6 +1106,51 @@ FIERY_API int fiery_bottleneck_backward(const fiery_bottleneck_desc_t* desc, con
                   "bottleneck: pointers must be 16-byte aligned");
     return launch_bottleneck_backward(desc, grad_out, x, y1, y2, y3, stats, packed, norms, grad_x, grad_w_down, grad_w_conv, grad_w_up,
                                       grad_norms, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// the group stages' common checks: the desc in training, the stage, and the gathered triplets of stages 1..3
+static int check_bottleneck_stage(const fiery_bottleneck_desc_t* d, int stage, int world, const double* gathered) {
+    int rc = check_bottleneck_desc(d);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(d->training == 1, "bottleneck: training = %d must be 1 for statistics over a group", d->training);
+    FIERY_REQUIRE(stage >= 0 && stage <= 3, "bottleneck: stage = %d must be in 0..3", stage);
+    if (stage > 0 && (rc = check_world(world, gathered, "bottleneck")) != FIERY_OK) return rc;
+    return FIERY_OK;
+}
+
+FIERY_API int fiery_bottleneck_sync_forward_stage(const fiery_bottleneck_desc_t* desc, int32_t stage, int32_t world, const double* gathered,
+                                                  const float* x, const void* packed, const float* const* norms, float* y1, float* y2,
+                                                  float* y3, float* out, float* stats, double* counts, double* local, void* workspace,
+                                                  void* stream) {
+    const int rc = check_bottleneck_stage(desc, stage, world, gathered);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(x && packed && norms && y1 && y2 && y3 && out && stats && workspace, "bottleneck: NULL pointer");
+    FIERY_REQUIRE(aligned16(x) && aligned16(packed) && aligned16(y1) && aligned16(y2) && aligned16(y3) && aligned16(out) && aligned16(workspace),
+                  "bottleneck: pointers must be 16-byte aligned");
+    if (stage < 3) FIERY_REQUIRE(local, "bottleneck: NULL local");
+    if (stage < 3) FIERY_REQUIRE(aligned8(local), "bottleneck: local must be 8-byte aligned");
+    if (stage > 0) FIERY_REQUIRE(counts, "bottleneck: NULL counts");
+    if (stage > 0) FIERY_REQUIRE(aligned8(counts), "bottleneck: counts must be 8-byte aligned");
+    return launch_bottleneck_sync_forward_stage(desc, stage, world, gathered, x, packed, norms, y1, y2, y3, out, stats, counts, local, workspace,
+                                                static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API int fiery_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t* desc, int32_t stage, int32_t world, const double* gathered,
+                                                   const float* grad_out, const float* x, const float* y1, const float* y2, const float* y3,
+                                                   const float* stats, const void* packed, const float* const* norms, float* grad_x,
+                                                   float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
+                                                   double* local, void* workspace, void* stream) {
+    const int rc = check_bottleneck_stage(desc, stage, world, gathered);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_out && x && y1 && y2 && y3 && stats && packed && norms && grad_norms && workspace, "bottleneck: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_out) && aligned16(x) && aligned16(y1) && aligned16(y2) && aligned16(y3) && aligned16(packed) &&
+                      aligned16(workspace) && (!grad_x || aligned16(grad_x)),
+                  "bottleneck: pointers must be 16-byte aligned");
+    if (stage < 3) FIERY_REQUIRE(local, "bottleneck: NULL local");
+    if (stage < 3) FIERY_REQUIRE(aligned8(local), "bottleneck: local must be 8-byte aligned");
+    return launch_bottleneck_sync_backward_stage(desc, stage, world, gathered, grad_out, x, y1, y2, y3, stats, packed, norms, grad_x,
+                                                 grad_w_down, grad_w_conv, grad_w_up, grad_norms, local, workspace,
+                                                 static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -304,8 +304,8 @@ def use_tensor_core_bottlenecks(model):
     unchanged) and runs it as ``torch.ops.fiery_b200.bottleneck``: each inner BatchNorm2d and ReLU is applied as the next convolution
     reads its input, forward and backward.  Works before or after ``use_tensor_core_future_prediction``.  Returns the model; a second
     call does nothing, a model without future prediction is returned untouched, and Bottlenecks the kernels do not cover (a skip
-    projection, another kernel size, dropout > 0, a norm other than BatchNorm2d -- a SyncBatchNorm stays torch's --, more than 128
-    channels) are left alone with one warning."""
+    projection, another kernel size, dropout > 0, a norm other than BatchNorm2d -- a SyncBatchNorm stays torch's here;
+    ``use_tensor_core_sync_bottlenecks`` swaps those --, more than 128 channels) are left alone with one warning."""
     from .bottleneck import TensorCoreBottleneck, module_reason
 
     def slots(res_blocks):
@@ -314,6 +314,36 @@ def use_tensor_core_bottlenecks(model):
                 yield stack, name, block, f"res_blocks[{i}][{name}]"
     return _swap(model, slots, TensorCoreBottleneck, module_reason, TensorCoreBottleneck.from_module,
                  "fiery_b200: Bottleneck(s) not covered by the tensor-core kernels, left as is: ", root=_res_blocks)
+
+
+def use_tensor_core_sync_bottlenecks(model):
+    """For every block in ``model.future_prediction.res_blocks`` of a ``Fiery`` instance (a reference ``Bottleneck`` or a
+    ``TensorCoreBottleneck``) with a norm of type exactly ``nn.SyncBatchNorm``: when the kernels cover it with its three norms of that
+    type, replace the three by ``fiery_b200.batch_norm.FusedSyncBatchNorm`` (same Parameters, buffers and ``process_group``;
+    ``state_dict`` keys unchanged) and the block by a ``fiery_b200.bottleneck.TensorCoreBottleneck`` holding the same ``layers``.  In
+    training over a group the block then runs ``SyncBottleneck``: the Bottleneck chain on the kernels with each norm's statistics
+    gathered over the group, one gather per norm each way, as torch's converted modules.  Call it after
+    ``SyncBatchNorm.convert_sync_batchnorm``; it works in any order with ``use_fused_sync_batch_norm``,
+    ``use_tensor_core_future_prediction`` and ``use_tensor_core_bottlenecks``.  Returns the model; a second call does nothing, a model
+    without future prediction is returned untouched, blocks without a SyncBatchNorm are left as they are, and converted blocks the
+    kernels do not cover (a skip projection, dropout > 0, another kernel size, a mix of norm kinds) are left alone with one warning."""
+    from .batch_norm import FusedSyncBatchNorm
+    from .bottleneck import TensorCoreBottleneck, module_reason
+
+    def slots(res_blocks):
+        for i, (_, stack) in enumerate(res_blocks._modules.items()):
+            for name, block in stack._modules.items():
+                layers = getattr(block, "layers", None)
+                norms = [m for m in layers.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)] if layers is not None else []
+                if any(type(m) is torch.nn.SyncBatchNorm for m in norms):
+                    yield stack, name, block, f"res_blocks[{i}][{name}]"
+
+    def make(block):
+        for abn in (block.layers.abn_down_project, block.layers.abn, block.layers.abn_up_project):
+            abn[0] = FusedSyncBatchNorm(abn[0])
+        return block if isinstance(block, TensorCoreBottleneck) else TensorCoreBottleneck(block)
+    return _swap(model, slots, (), lambda block: module_reason(block, kinds=(torch.nn.SyncBatchNorm,)), make,
+                 "fiery_b200: converted Bottleneck(s) not covered by the tensor-core kernels, left as is: ", root=_res_blocks)
 
 
 def uninstall():

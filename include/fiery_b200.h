@@ -704,6 +704,46 @@ FIERY_API int fiery_bottleneck_backward(const fiery_bottleneck_desc_t* desc, con
                                         float* grad_x, float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
                                         void* workspace, void* stream);
 
+/*
+ * The Bottleneck in training with each norm's batch statistics over a group of `world` ranks (its three norms SyncBatchNorms), split
+ * at the norms: the caller gathers every rank's (channels, 3) fp64 triplets `local` into `gathered` (world, channels, 3), rank r at
+ * [r], between two stages, as for fiery_batch_norm_local_stats / _forward_gathered and _local_grad_sums / _backward_gathered.
+ *   forward, stages 0 .. 3 in order:
+ *     0: y1 = W_down x;                                                          local = this rank's (n, mean, M2) of y1 (M channels)
+ *     1: bn1's gathered finalize (mean1, var1 into stats, counts[0] = the group's n); y2 = conv3x3(relu(bn1(y1)));  local of y2 (M)
+ *     2: bn2's gathered finalize (mean2, var2, counts[1]); y3 = W_up relu(bn2(y2));                                local of y3 (C)
+ *     3: bn3's gathered finalize (mean3, var3, counts[2]); out = relu(bn3(y3)) + x.
+ *   backward, stages 0 .. s, s the deepest stage a gradient asked for needs:
+ *     0: local = this rank's (n, S1, S2) of bn3's backward on (y3, grad_out); its own grad_norms[4], [5]
+ *     1: dy3 = bn3's backward from the gathered sums; grad_w_up; da2 = W_up^T dy3; local of bn2's backward on (y2, da2), grad_norms[2], [3]
+ *     2: dy2 = bn2's backward from the gathered sums; grad_w_conv; da1 = the 3x3 input gradient; local of bn1's, grad_norms[0], [1]
+ *     3: dy1 = bn1's backward from the gathered sums; grad_w_down; grad_x = W_down^T dy1 + grad_out.
+ *   s is 3 when grad_x or grad_w_down is asked for, else 2 for grad_w_conv or bn1's weight or bias, else 1 for grad_w_up or bn2's, else
+ *   0: it depends on which gradients are asked for only, so every rank runs as many gathers (s; 3 in the forward).  A NULL gradient
+ *   launches nothing for it, as in fiery_bottleneck_backward, and a stage past s launches nothing it does not need.
+ * Each stage's computation is fiery_bottleneck_forward's / _backward's with the group's statistics and sums, and the gathered finalize
+ * merges the ranks in ascending rank order (fiery_batch_norm_*_gathered), so every rank gets bit-identical statistics and counts.  The
+ * norms' weight and bias gradients are each rank's own (the local sums, as torch's SyncBatchNorm).  With world 1 every output,
+ * statistic and gradient is bit for bit fiery_bottleneck_forward's / _backward's: a group of one merges exactly as the single-rank
+ * finalize does, and the backward's prologue coefficients come from the saved mean and var through the same eval finalize.
+ * Arguments are fiery_bottleneck_forward's / _backward's, the same in every stage of a sequence; the forward's stages share one
+ * fiery_bottleneck_forward_workspace_bytes workspace and the backward's one fiery_bottleneck_backward_workspace_bytes workspace, kept
+ * from stage 0 to the last stage (the backward's intermediate gradients live there).  counts: 3 fp64, each norm's group n (the running
+ * variance's unbiased factor).  Limits as fiery_bottleneck_*, and: training 1; 0 <= stage <= 3; world >= 1 and gathered non-NULL in
+ * stages 1..3; local non-NULL in stages 0..2, counts in forward stages 1..3; gathered, local, counts 8-byte aligned.  A rank with no
+ * maps is the caller's to handle (the fiery_batch_norm_* group entries take n = 0).  Summation orders: fiery_bottleneck_*'s and
+ * fiery_batch_norm_*_gathered's.
+ */
+FIERY_API int fiery_bottleneck_sync_forward_stage(const fiery_bottleneck_desc_t* desc, int32_t stage, int32_t world, const double* gathered,
+                                                  const float* x, const void* packed, const float* const* norms, float* y1, float* y2,
+                                                  float* y3, float* out, float* stats, double* counts, double* local, void* workspace,
+                                                  void* stream);
+FIERY_API int fiery_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t* desc, int32_t stage, int32_t world, const double* gathered,
+                                                   const float* grad_out, const float* x, const float* y1, const float* y2, const float* y3,
+                                                   const float* stats, const void* packed, const float* const* norms, float* grad_x,
+                                                   float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
+                                                   double* local, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,6 +20,10 @@ Cases, per rank, training mode, fp32, forward + backward:
               swapped by use_fused_sync_batch_norm
   future   -- the 3-GRU FuturePrediction at baseline.yml (b 3, 4 steps of 200 x 200): the reference GRUs with converted norms, against
               use_fused_sync_batch_norm + use_tensor_core_future_prediction (the Bottlenecks' norms stay torch's SyncBatchNorm in both)
+  bottleneck -- one Bottleneck at baseline.yml (12 maps = b 3 x 4 steps, 64 channels, 200 x 200): the reference block with converted
+              norms, against use_tensor_core_sync_bottlenecks (TensorCoreBottleneck over FusedSyncBatchNorm norms)
+  future+bottlenecks -- the future case with use_tensor_core_sync_bottlenecks added to ours: the whole FuturePrediction on the kernels
+The first two cases are kept as they were, so their numbers stay comparable across versions.
 """
 from __future__ import annotations
 
@@ -39,6 +43,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from fiery_b200 import batch_norm as BN  # noqa: E402
+from fiery_b200 import bottleneck as BK  # noqa: E402
 from fiery_b200 import future_prediction as FP  # noqa: E402
 from fiery_b200 import install  # noqa: E402
 from fiery_b200.temporal import temporal_model_forward  # noqa: E402
@@ -75,6 +80,7 @@ def _force_sync():
         return (norm.process_group or dist.group.WORLD) if batch_stats and norm.training else None
     BN.sync_group = group_of
     FP.sync_group = group_of
+    BK.sync_group = group_of
 
     def torch_synced(self, x):                  # nn.SyncBatchNorm.forward with need_sync forced
         self._check_input_dim(x)
@@ -134,16 +140,35 @@ def _future_cases(dev):
     b, T, X, Y = FUTURE
     torch.manual_seed(7)
     ref = nn.SyncBatchNorm.convert_sync_batchnorm(FO.FuturePrediction(HIDDEN, LATENT)).to(dev).train()
-    holder = nn.Module()
-    holder.future_prediction = copy.deepcopy(ref)
-    install.use_fused_sync_batch_norm(holder)
-    install.use_tensor_core_future_prediction(holder)
-    ours = holder.future_prediction
     x = torch.randn(b, 1, LATENT, 1, 1, device=dev, requires_grad=True)
     h0 = torch.randn(b, HIDDEN, X, Y, device=dev, requires_grad=True)
-    leaves = [x, h0] + list(ref.parameters()) + list(ours.parameters())
     xin = lambda: x.expand(b, T, LATENT, X, Y)                       # noqa: E731
-    yield "future", _step(lambda: ref(xin(), h0), leaves), _step(lambda: ours(xin(), h0), leaves)
+    for name, bottlenecks in (("future", False), ("future+bottlenecks", True)):
+        holder = nn.Module()
+        holder.future_prediction = copy.deepcopy(ref)
+        install.use_fused_sync_batch_norm(holder)
+        install.use_tensor_core_future_prediction(holder)
+        if bottlenecks:
+            install.use_tensor_core_sync_bottlenecks(holder)
+        ours = holder.future_prediction
+        leaves = [x, h0] + list(ref.parameters()) + list(ours.parameters())
+        yield name, _step(lambda: ref(xin(), h0), leaves), _step(lambda: ours(xin(), h0), leaves)
+
+
+def _bottleneck_cases(dev):
+    b, T, X, Y = FUTURE
+    torch.manual_seed(7)
+    ref = nn.SyncBatchNorm.convert_sync_batchnorm(FO.Bottleneck(HIDDEN)).to(dev).train()
+    holder = nn.Module()
+    holder.future_prediction = nn.Module()
+    holder.future_prediction.res_blocks = nn.ModuleList([nn.Sequential(copy.deepcopy(ref))])
+    install.use_tensor_core_sync_bottlenecks(holder)
+    ours = holder.future_prediction.res_blocks[0][0]
+    if not isinstance(ours, BK.TensorCoreBottleneck):
+        raise SystemExit("the Bottleneck was not swapped")
+    x = torch.randn(b * T, HIDDEN, X, Y, device=dev, requires_grad=True)
+    leaves = [x] + list(ref.parameters()) + list(ours.parameters())
+    yield "bottleneck", _step(lambda: ref(x), leaves), _step(lambda: ours(x), leaves)
 
 
 def main():
@@ -161,7 +186,7 @@ def main():
         if world == 1:
             _force_sync()
         rows = []
-        for cases in (_temporal_cases, _future_cases):
+        for cases in (_temporal_cases, _future_cases, _bottleneck_cases):
             for name, ref, ours in cases(dev):
                 t_ref, t_ours = _time(ref, a.steps), _time(ours, a.steps)
                 row = dict(rank=rank, world=world, case=name, pass_="fwd+bwd", precision="fp32", torch_sync_ms=round(t_ref, 3),
