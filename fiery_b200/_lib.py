@@ -102,6 +102,13 @@ class BottleneckDesc(ctypes.Structure):
                 ("eps", c_double)]
 
 
+class OutputHeadDesc(ctypes.Structure):
+    """Mirror of ``fiery_output_head_desc_t``."""
+
+    _fields_ = [("maps", c_int32), ("grid_x", c_int32), ("grid_y", c_int32), ("channels", c_int32), ("n_out", c_int32),
+                ("training", c_int32), ("eps", c_double)]
+
+
 # name -> (restype, argtypes); every symbol include/fiery_b200.h declares
 SIGNATURES = {
     "fiery_abi_version": (c_int32, []),
@@ -196,6 +203,12 @@ SIGNATURES = {
                                             + [c_void_p] * 9),
     "fiery_bottleneck_sync_backward_stage": (c_int32, [POINTER(BottleneckDesc), c_int32, c_int32] + [c_void_p] * 8 + [POINTER(c_void_p)]
                                              + [c_void_p] * 4 + [POINTER(c_void_p)] + [c_void_p] * 3),
+    "fiery_output_head_packed_bytes": (c_size_t, [POINTER(OutputHeadDesc)]),
+    "fiery_output_head_pack_weights": (c_int32, [POINTER(OutputHeadDesc)] + [c_void_p] * 3),
+    "fiery_output_head_forward_workspace_bytes": (c_size_t, [POINTER(OutputHeadDesc)]),
+    "fiery_output_head_forward": (c_int32, [POINTER(OutputHeadDesc)] + [c_void_p] * 11),
+    "fiery_output_head_backward_workspace_bytes": (c_size_t, [POINTER(OutputHeadDesc)]),
+    "fiery_output_head_backward": (c_int32, [POINTER(OutputHeadDesc)] + [c_void_p] * 14),
     "fiery_warp_theta": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "fiery_warp_features_forward": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_int64, c_int32, c_void_p]),
@@ -284,7 +297,7 @@ def warn_once(key, msg: str, stacklevel: int = 2) -> None:
 # load.  One training step of a model with every layer swapped uses one pack per DepthLayer operand dtype, two for FirstConv (the
 # transposed one for the input gradient), four per TemporalBlock (its entry, two causal convolutions and its aggregation) and one per
 # Bottleneck3D: 19 for the four temporal blocks of a 5-frame receptive field, and one per SpatialGRU and Bottleneck: 12 for a swapped
-# FuturePrediction.  The bound leaves room for in-between layers (up to four per block there) without a step ever evicting a pack it
+# FuturePrediction, and one per output head: 4 for a swapped Decoder.  The bound leaves room for in-between layers (up to four per block there) without a step ever evicting a pack it
 # uses again.
 _PACK_CACHE_SIZE = 48
 _pack_cache: "collections.OrderedDict[tuple, tuple]" = collections.OrderedDict()

@@ -18,7 +18,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libfiery_b200.so")
 STAMP_PATH = os.path.join(PKG_DIR, "csrc", ".build_stamp")
-SOURCES = ["c_api.cu", "lift_plan.cu", "lift_fwd.cu", "lift_fwd_cols.cu", "lift_det.cu", "lift_bwd.cu", "bev_conv.cu", "bev_conv_bwd.cu", "depth_layer.cu", "voxels_summing.cu", "warp.cu", "temporal_entry.cu", "causal_conv.cu", "spatial_sums.cu", "batch_norm.cu", "spatial_gru.cu", "bottleneck.cu"]
+SOURCES = ["c_api.cu", "lift_plan.cu", "lift_fwd.cu", "lift_fwd_cols.cu", "lift_det.cu", "lift_bwd.cu", "bev_conv.cu", "bev_conv_bwd.cu", "depth_layer.cu", "voxels_summing.cu", "warp.cu", "temporal_entry.cu", "causal_conv.cu", "spatial_sums.cu", "batch_norm.cu", "spatial_gru.cu", "bottleneck.cu", "output_head.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math=false",

@@ -538,6 +538,187 @@ int launch_gru_blend_backward(const fiery_batch_norm_desc_t* d, const float* x, 
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
+// The decoder's output heads' backward (output_head.cu): out = W1 relu(bn(y)) + b1 on y (maps, C, 1, X, Y) contiguous, with n <= 8
+// outputs.  The 1x1's input gradient da[c, p] = sum_{j < n} W1[j, c] g[j, p] (fp32, fmaf in ascending j) is never stored: both passes below recompute it from the piece's n rows of g, which every channel's pieces read again
+// (from L2: g is n / C of y's size).  Over the pieces above:
+//   sums pass:  bn_grad_sums_kernel<RELU = true>'s (S1, S2) on (y, da), bit for bit; and each piece's 1x1 weight-gradient partials
+//               sum g[j, p] a[c, p] (a = relu(fmaf(scale, y, shift))) and, in channel 0's pieces, its bias-gradient partials
+//               sum g[j, p], each summed in the pieces' order (thread chunks ascending, a chunk as (p0 + p1) + (p2 + p3), the block sum);
+//   finalize:   bn_finalize_backward_kernel; dW1 and db1 the fp64 sums of their partials in ascending (map, piece) order;
+//   apply pass: bn_grad_apply_kernel<RELU = true, TRAINING>'s dx on (y, da), bit for bit.
+// g is (maps, n, X*Y) contiguous; W1[j][c] is at w1[j * ld + c].
+// ------------------------------------------------------------------------------------------------------------------------------
+struct HeadGrad {
+    const float* g;
+    const float* w1;
+    int n, ld;
+};
+
+// the piece's chunk q of da (g read at gp, the piece's first pixel in row 0 of its map's g)
+__device__ __forceinline__ float4 head_da(const HeadGrad& h, const float* gp, long long pixels, int c, int q, int n_px, bool vec) {
+    float4 da = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = 0; j < h.n; ++j) {
+        const float w = __ldg(h.w1 + static_cast<long long>(j) * h.ld + c);
+        const float4 gj = load_chunk4(gp + j * pixels, q, n_px, vec);
+        da = make_float4(fmaf(w, gj.x, da.x), fmaf(w, gj.y, da.y), fmaf(w, gj.z, da.z), fmaf(w, gj.w, da.w));
+    }
+    return da;
+}
+
+__device__ __forceinline__ float4 head_relu(float4 v, float scale, float shift) {
+    const BnCoef k{scale, shift, 0.f, 0.f, 0.f};
+    return make_float4(bn_relu_apply(k, v.x), bn_relu_apply(k, v.y), bn_relu_apply(k, v.z), bn_relu_apply(k, v.w));
+}
+
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) head_grad_sums_kernel(const BnShape s, const float* __restrict__ y, const HeadGrad h,
+                                                                    const float* __restrict__ w, const float* __restrict__ bias,
+                                                                    const float* __restrict__ mean, const float* __restrict__ var,
+                                                                    double eps, float2* __restrict__ part, float* __restrict__ wpart,
+                                                                    float* __restrict__ bpart) {
+    __shared__ float sh[BN_THREADS / 32];
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const GruPieceAt at = gru_piece_at(s, g);
+        const float* xp = y + p.x_off;
+        const float* gp = h.g + at.b * h.n * s.pixels + at.pix;
+        const bool vx = aligned16_ptr(xp), vg = aligned16_ptr(gp);
+        const float mu = mean[p.c];
+        float scale, shift;
+        bn_scale_shift(w, bias, mu, var[p.c], eps, p.c, scale, shift);
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            v[u] = q < n_chunks ? load_chunk4(xp, q, p.n, vx) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        // the 1x1's partials, row j at a time: sum g a over the piece, and (channel 0) sum g
+        const bool w_part = wpart != nullptr, b_part = bpart != nullptr && p.c == 0;
+        for (int j = 0; j < h.n && (w_part || b_part); ++j) {
+            float sw = 0.f, sb = 0.f;
+#pragma unroll
+            for (int u = 0; u < BN_CHUNKS; ++u) {
+                const int q = threadIdx.x + u * BN_THREADS;
+                if (q >= n_chunks) continue;
+                const float4 gj = load_chunk4(gp + static_cast<long long>(j) * s.pixels, q, p.n, vg);
+                const float4 a = head_relu(v[u], scale, shift);
+                sw += bn_chunk_sum(make_float4(gj.x * a.x, gj.y * a.y, gj.z * a.z, gj.w * a.w));
+                sb += bn_chunk_sum(gj);
+            }
+            if (w_part) {
+                sw = bn_block_sum(sw, sh);
+                if (threadIdx.x == 0) wpart[p.part * h.n + j] = sw;
+            }
+            if (b_part) {
+                sb = bn_block_sum(sb, sh);
+                if (threadIdx.x == 0) bpart[p.part * h.n + j] = sb;
+            }
+        }
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            const float4 d = q < n_chunks ? head_da(h, gp, s.pixels, p.c, q, p.n, vg) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4 gm = make_float4(bn_masked<true>(d.x, v[u].x, scale, shift), bn_masked<true>(d.y, v[u].y, scale, shift),
+                                          bn_masked<true>(d.z, v[u].z, scale, shift), bn_masked<true>(d.w, v[u].w, scale, shift));
+            s1 += bn_chunk_sum(gm);
+            s2 += bn_chunk_sum(make_float4(gm.x * (v[u].x - mu), gm.y * (v[u].y - mu), gm.z * (v[u].z - mu), gm.w * (v[u].w - mu)));
+        }
+        s1 = bn_block_sum(s1, sh);
+        s2 = bn_block_sum(s2, sh);
+        if (threadIdx.x == 0) part[p.part] = make_float2(s1, s2);
+    }
+}
+
+// One thread per output: i < n * C -> grad_w[i] (j = i / C, c = i % C) from channel c's pieces; else grad_b[i - n * C] from channel 0's
+__global__ void head_wgrad_finalize_kernel(const BnShape s, int n, const float* __restrict__ wpart, const float* __restrict__ bpart,
+                                           float* __restrict__ grad_w, float* __restrict__ grad_b) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int nw = n * s.channels;
+    if (i >= nw + n || (i < nw && !grad_w) || (i >= nw && !grad_b)) return;
+    const int j = i < nw ? i / s.channels : i - nw, c = i < nw ? i % s.channels : 0;
+    const float* pp = (i < nw ? wpart : bpart) + c * s.per_channel * n + j;
+    double acc = 0.0;
+    for (long long k = 0; k < s.per_channel; ++k) acc += static_cast<double>(pp[k * n]);
+    if (i < nw) grad_w[i] = static_cast<float>(acc);
+    else grad_b[j] = static_cast<float>(acc);
+}
+
+template <bool TRAINING>
+__global__ void __launch_bounds__(BN_THREADS, BN_MIN_CTAS) head_grad_apply_kernel(const BnShape s, const float* __restrict__ y, const HeadGrad h,
+                                                                     const BnCoef* __restrict__ coef, float* __restrict__ dx) {
+    for (long long g = blockIdx.x; g < s.pieces; g += gridDim.x) {
+        const BnPiece p = bn_piece(s, g);
+        const GruPieceAt at = gru_piece_at(s, g);
+        const float* xp = y + p.x_off;
+        const float* gp = h.g + at.b * h.n * s.pixels + at.pix;
+        float* op = dx + p.out_off;
+        const bool vx = aligned16_ptr(xp), vg = aligned16_ptr(gp), vo = aligned16_ptr(op);
+        const BnCoef k = coef[p.c];
+        const int n_chunks = (p.n + 3) / 4;
+        float4 v[BN_CHUNKS];
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q < n_chunks) v[u] = load_chunk4(xp, q, p.n, vx);
+        }
+#pragma unroll
+        for (int u = 0; u < BN_CHUNKS; ++u) {
+            const int q = threadIdx.x + u * BN_THREADS;
+            if (q >= n_chunks) continue;
+            const float4 d = head_da(h, gp, s.pixels, p.c, q, p.n, vg);
+            const float xs[4] = {v[u].x, v[u].y, v[u].z, v[u].w}, ds[4] = {d.x, d.y, d.z, d.w};
+            float o[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float gm = bn_masked<true>(ds[e], xs[e], k.scale, k.shift);
+                o[e] = TRAINING ? fmaf(k.scale, gm, fmaf(k.k1, xs[e] - k.mean, k.k0)) : k.scale * gm;
+            }
+            store_chunk4(op, q, p.n, vo, make_float4(o[0], o[1], o[2], o[3]));
+        }
+    }
+}
+
+// the backward's workspace: batch_norm_workspace_bytes(d) (coefficients, then the (S1, S2) partials), then n weight-gradient partials
+// per piece, then n bias-gradient partials per piece of channel 0
+struct HeadWork { BnCoef* coef; float2* part; float* wpart; float* bpart; };
+static size_t head_wpart_bytes(const BnShape& s, int n) { return (static_cast<size_t>(s.pieces) * n * sizeof(float) + 255) / 256 * 256; }
+
+size_t output_head_backward_workspace_bytes(const fiery_batch_norm_desc_t* d, int n) {
+    const BnShape s = bn_shape(d);
+    return (batch_norm_workspace_bytes(d) + 255) / 256 * 256 + head_wpart_bytes(s, n) + static_cast<size_t>(s.per_channel) * n * sizeof(float);
+}
+
+static HeadWork head_work(const fiery_batch_norm_desc_t* d, const BnShape& s, int n, void* workspace) {
+    const BnWork b = bn_work(d, workspace);
+    char* wp = static_cast<char*>(workspace) + (batch_norm_workspace_bytes(d) + 255) / 256 * 256;
+    return {b.coef, b.part, reinterpret_cast<float*>(wp), reinterpret_cast<float*>(wp + head_wpart_bytes(s, n))};
+}
+
+// d: the head's norm over y (relu 1); grad_y, grad_bn_w / grad_bn_b, grad_w (n, C) and grad_b (n) may each be NULL
+int launch_output_head_backward(const fiery_batch_norm_desc_t* d, const float* y, const float* g, const float* w1, int ld, int n,
+                                const float* w, const float* bias, const float* mean, const float* var, float* grad_y, float* grad_bn_w,
+                                float* grad_bn_b, float* grad_w, float* grad_b, void* workspace, cudaStream_t stream) {
+    const BnShape s = bn_shape(d);
+    const HeadWork k = head_work(d, s, n, workspace);
+    const HeadGrad h{g, w1, n, ld};
+    // the sums are needed for the norm's and the 1x1's weight and bias gradients, and for grad_y in training
+    const bool reduce = grad_bn_w || grad_bn_b || grad_w || grad_b || (grad_y && d->training);
+    if (reduce)
+        head_grad_sums_kernel<<<bn_grid(s), BN_THREADS, 0, stream>>>(s, y, h, w, bias, mean, var, d->eps, k.part, grad_w ? k.wpart : nullptr,
+                                                                     grad_b ? k.bpart : nullptr);
+    if (grad_y || grad_bn_w || grad_bn_b)
+        bn_finalize_backward_kernel<<<(d->channels + 127) / 128, 128, 0, stream>>>(s, k.part, reduce, w, bias, mean, var, d->training,
+                                                                                   d->eps, grad_bn_w, grad_bn_b, k.coef);
+    if (grad_w || grad_b)
+        head_wgrad_finalize_kernel<<<(n * (d->channels + 1) + 127) / 128, 128, 0, stream>>>(s, n, k.wpart, k.bpart, grad_w, grad_b);
+    if (grad_y && d->training) head_grad_apply_kernel<true><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, y, h, k.coef, grad_y);
+    else if (grad_y) head_grad_apply_kernel<false><<<bn_grid(s), BN_THREADS, 0, stream>>>(s, y, h, k.coef, grad_y);
+    FIERY_CUDA_CHECK(cudaGetLastError());
+    return FIERY_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
 // Statistics over several ranks (fiery_batch_norm_*_gathered, fiery_spatial_gru_*_step_*).  Each rank reduces its own pieces as
 // above into one fp64 triplet per channel -- (n, mean, M2) forward, (n, S1, S2) backward -- the caller gathers the ranks' triplets
 // into (world, channels, 3), and the gathered finalize merges them in ascending rank order with the same formulas, starting from

@@ -196,6 +196,16 @@ int launch_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t* d, int 
                                           const float* stats, const void* packed, const float* const* norms, float* grad_x,
                                           float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms, double* local,
                                           void* workspace, cudaStream_t stream);
+size_t output_head_packed_bytes(const fiery_output_head_desc_t* d);
+int launch_output_head_pack(const fiery_output_head_desc_t* d, const float* w, void* packed, cudaStream_t stream);
+size_t output_head_forward_workspace_bytes(const fiery_output_head_desc_t* d);
+int launch_output_head_forward(const fiery_output_head_desc_t* d, const float* y, const void* packed, const float* bn_w, const float* bn_b,
+                               const float* running_mean, const float* running_var, float* out, float* mean, float* var, void* workspace,
+                               cudaStream_t stream);
+size_t output_head_backward_workspace_bytes(const fiery_output_head_desc_t* d);
+int launch_output_head_backward(const fiery_output_head_desc_t* d, const float* grad_out, const float* y, const float* mean, const float* var,
+                                const float* w1, const float* bn_w, const float* bn_b, float* grad_y, float* grad_bn_w, float* grad_bn_b,
+                                float* grad_w, float* grad_b, void* workspace, cudaStream_t stream);
 int launch_causal_conv_forward(const fiery_causal_conv3d_desc_t* d, const float* x, const float* packed, float* y, cudaStream_t stream);
 int launch_causal_conv_dgrad(const fiery_causal_conv3d_desc_t* d, const float* gy, const float* packed, float* gx, cudaStream_t stream);
 size_t causal_conv_wgrad_workspace_bytes(const fiery_causal_conv3d_desc_t* d);
@@ -1151,6 +1161,72 @@ FIERY_API int fiery_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t
     return launch_bottleneck_sync_backward_stage(desc, stage, world, gathered, grad_out, x, y1, y2, y3, stats, packed, norms, grad_x,
                                                  grad_w_down, grad_w_conv, grad_w_up, grad_norms, local, workspace,
                                                  static_cast<cudaStream_t>(stream));
+}
+
+// The output head's limits, one place for every entry point.  The messages name the field.
+static int check_output_head_desc(const fiery_output_head_desc_t* d) {
+    FIERY_REQUIRE(d, "output head: NULL desc");
+    FIERY_REQUIRE(d->maps >= 1, "output head: maps = %d must be >= 1", d->maps);
+    FIERY_REQUIRE(d->channels >= 1 && d->channels <= 128, "output head: channels = %d must be in 1..128", d->channels);
+    FIERY_REQUIRE(d->n_out >= 1 && d->n_out <= 8, "output head: n_out = %d must be in 1..8", d->n_out);
+    FIERY_REQUIRE(d->grid_x >= 1, "output head: grid_x = %d must be >= 1", d->grid_x);
+    FIERY_REQUIRE(d->grid_y >= 1, "output head: grid_y = %d must be >= 1", d->grid_y);
+    const long long P = static_cast<long long>(d->grid_x) * d->grid_y;
+    FIERY_REQUIRE(P < (1ll << 31), "output head: grid_x * grid_y = %lld pixels must be < 2^31", P);
+    FIERY_REQUIRE(P % 4 == 0, "output head: grid_x * grid_y = %lld pixels must be a multiple of 4 (16-byte TMA plane pitch)", P);
+    FIERY_REQUIRE(d->training == 0 || d->training == 1, "output head: training = %d must be 0 or 1", d->training);
+    FIERY_REQUIRE(d->eps >= 0.0, "output head: eps = %g must be >= 0", d->eps);
+    FIERY_REQUIRE(!d->training || d->maps * P >= 2, "output head: maps * grid_x * grid_y = %lld values per channel must be >= 2 in training",
+                  d->maps * P);
+    return FIERY_OK;
+}
+
+FIERY_API size_t fiery_output_head_packed_bytes(const fiery_output_head_desc_t* desc) {
+    if (check_output_head_desc(desc) != FIERY_OK) return 0;
+    return output_head_packed_bytes(desc);
+}
+
+FIERY_API int fiery_output_head_pack_weights(const fiery_output_head_desc_t* desc, const float* w, void* packed, void* stream) {
+    const int rc = check_output_head_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(w && packed, "output head: NULL weight pointer");
+    FIERY_REQUIRE(aligned16(packed), "output head: packed weights must be 16-byte aligned");
+    return launch_output_head_pack(desc, w, packed, static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_output_head_forward_workspace_bytes(const fiery_output_head_desc_t* desc) {
+    if (check_output_head_desc(desc) != FIERY_OK) return 0;
+    return output_head_forward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_output_head_forward(const fiery_output_head_desc_t* desc, const float* y, const void* packed, const float* bn_weight,
+                                        const float* bn_bias, const float* running_mean, const float* running_var, float* out, float* mean,
+                                        float* var, void* workspace, void* stream) {
+    const int rc = check_output_head_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(y && packed && out && mean && var && workspace, "output head: NULL pointer");
+    FIERY_REQUIRE(desc->training || (running_mean && running_var), "output head: eval mode needs running_mean and running_var");
+    FIERY_REQUIRE(aligned16(y) && aligned16(packed) && aligned16(out) && aligned16(workspace), "output head: pointers must be 16-byte aligned");
+    return launch_output_head_forward(desc, y, packed, bn_weight, bn_bias, running_mean, running_var, out, mean, var, workspace,
+                                      static_cast<cudaStream_t>(stream));
+}
+
+FIERY_API size_t fiery_output_head_backward_workspace_bytes(const fiery_output_head_desc_t* desc) {
+    if (check_output_head_desc(desc) != FIERY_OK) return 0;
+    return output_head_backward_workspace_bytes(desc);
+}
+
+FIERY_API int fiery_output_head_backward(const fiery_output_head_desc_t* desc, const float* grad_out, const float* y, const float* mean,
+                                         const float* var, const float* w1, const float* bn_weight, const float* bn_bias, float* grad_y,
+                                         float* grad_bn_weight, float* grad_bn_bias, float* grad_w, float* grad_b, void* workspace,
+                                         void* stream) {
+    const int rc = check_output_head_desc(desc);
+    if (rc != FIERY_OK) return rc;
+    FIERY_REQUIRE(grad_out && y && mean && var && w1 && workspace, "output head: NULL pointer");
+    FIERY_REQUIRE(aligned16(grad_out) && aligned16(y) && aligned16(workspace) && (!grad_y || aligned16(grad_y)),
+                  "output head: pointers must be 16-byte aligned");
+    return launch_output_head_backward(desc, grad_out, y, mean, var, w1, bn_weight, bn_bias, grad_y, grad_bn_weight, grad_bn_bias,
+                                       grad_w, grad_b, workspace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

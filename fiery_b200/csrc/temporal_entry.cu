@@ -355,6 +355,16 @@ bottleneck_entry_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShap
     te_fwd_body<NCH, true>(maps, s, nullptr, nullptr, out, stages, tiles_per_frame, n_tiles, coef, s_coef);
 }
 
+// The decoder's output heads' 1x1 (output_head.cu): the Bottleneck's BN + ReLU prologue, and the head's bias folded in as the one
+// extra channel (E = 1) whose value `ones[f]` is 1 in every map f, so the epilogue adds fmaf(b1[o], 1, 0) = b1[o] exactly.  N <= 8.
+__global__ void __launch_bounds__(TE_FWD_THREADS, 1)
+output_head_fwd_kernel(const __grid_constant__ TeFwdMaps maps, const TeShape s, const float* __restrict__ ones,
+                       const float* __restrict__ w_extra, const TeOut out, int stages, int tiles_per_frame, int n_tiles,
+                       const BnCoef* __restrict__ coef) {
+    __shared__ BnCoef s_coef[128];
+    te_fwd_body<1, true>(maps, s, ones, w_extra, out, stages, tiles_per_frame, n_tiles, coef, s_coef);
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------
 // input gradient
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -666,7 +676,8 @@ static int te_stages(int fixed_bytes, int stage_bytes) {
 
 constexpr int TE_COEF_BYTES = 128 * sizeof(BnCoef);  // the BN instantiations' static shared memory
 
-// coef: nullptr (the entry's forward) or the Bottleneck's BN + ReLU prologue coefficients (K entries)
+// coef: nullptr (the entry's forward) or the Bottleneck's BN + ReLU prologue coefficients (K entries); coef with extra: the output
+// head's forward (extra the ones that carry the bias)
 static int te_launch_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* extra, const float* packed,
                              float* const* out, const BnCoef* coef, cudaStream_t stream) {
     const TeShape s = te_shape(d);
@@ -686,6 +697,14 @@ static int te_launch_forward(const fiery_temporal_entry_desc_t* d, const float* 
     unsigned grid = 0;
     if ((rc = persistent_grid(n_tiles, &grid)) != FIERY_OK) return rc;
     const float* we = packed + p.f_floats + p.t_floats;
+    if (coef && extra) {
+        FIERY_REQUIRE(s.E == 1 && p.nch == 1 && s.Kpad <= 128, "output head: one extra channel, n <= 8 outputs and C <= 128");
+        if ((rc = set_dynamic_smem(output_head_fwd_kernel, smem)) != FIERY_OK) return rc;
+        output_head_fwd_kernel<<<grid, TE_FWD_THREADS, smem, stream>>>(maps, s, extra, we, o, stages, tiles_per_frame,
+                                                                       static_cast<int>(n_tiles), coef);
+        FIERY_CUDA_CHECK(cudaGetLastError());
+        return FIERY_OK;
+    }
     if (coef) {
         FIERY_REQUIRE(s.E == 0 && s.Kpad <= 128, "bottleneck: the up projection takes no extra channels and K <= 128");
         switch (p.nch) {
@@ -725,6 +744,12 @@ int launch_temporal_entry_forward(const fiery_temporal_entry_desc_t* d, const fl
 int launch_bottleneck_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* packed, const BnCoef* coef, float* out,
                                     cudaStream_t stream) {
     return te_launch_forward(d, x, nullptr, packed, &out, coef, stream);
+}
+
+// ones: batch * frames floats of value 1, the extra channel that carries the bias
+int launch_output_head_entry_forward(const fiery_temporal_entry_desc_t* d, const float* x, const float* ones, const float* packed,
+                                     const BnCoef* coef, float* out, cudaStream_t stream) {
+    return te_launch_forward(d, x, ones, packed, &out, coef, stream);
 }
 
 // bias: nullptr (the entry's input gradient) or (batch * frames, K) fp32 added to every pixel of its frame's row k (the temporal

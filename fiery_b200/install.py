@@ -346,6 +346,32 @@ def use_tensor_core_sync_bottlenecks(model):
                  "fiery_b200: converted Bottleneck(s) not covered by the tensor-core kernels, left as is: ", root=_res_blocks)
 
 
+def _decoder(model):
+    return getattr(model, "decoder", None)
+
+
+_OUTPUT_HEADS = ("segmentation_head", "instance_offset_head", "instance_center_head", "instance_future_head")
+
+
+def use_tensor_core_output_heads(model):
+    """Replace each covered output head of ``model.decoder`` (fiery/models/decoder.py:24-50: ``segmentation_head``,
+    ``instance_offset_head``, ``instance_center_head`` and, when the model predicts future flow, ``instance_future_head``) of a ``Fiery``
+    instance by ``fiery_b200.decoder.FusedOutputHead``, which adopts the head's children (``state_dict`` keys unchanged) and runs its
+    BatchNorm2d, ReLU and 1x1 convolution as ``torch.ops.fiery_b200.output_head``, forward and backward; the 3x3 convolution stays
+    cuDNN's.  Returns the model; a second call does nothing, a model without a decoder is returned untouched, and heads the kernels do
+    not cover (a norm other than BatchNorm2d -- a SyncBatchNorm stays torch's --, more than 128 channels or 8 outputs, another
+    structure) are left alone with one warning."""
+    from .decoder import FusedOutputHead, module_reason
+
+    def slots(decoder):
+        for name in _OUTPUT_HEADS:
+            head = getattr(decoder, name, None)
+            if head is not None:
+                yield decoder, name, head, name
+    return _swap(model, slots, FusedOutputHead, module_reason, FusedOutputHead.from_module,
+                 "fiery_b200: output head(s) not covered by the kernels, left as is: ", root=_decoder)
+
+
 def uninstall():
     if not _saved:
         return

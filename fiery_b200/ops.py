@@ -550,4 +550,73 @@ bottleneck.register_autograd(_bottleneck_backward, setup_context=_bottleneck_set
 torch.library.register_autocast("fiery_b200::bottleneck", "cuda", torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# The decoder's output heads after their 3x3 convolution (fiery/models/decoder.py:24-50): ``output_head`` / ``output_head_backward``
+# (fiery_b200/decoder.py; csrc/output_head.cu).  The statistics outputs are not differentiable and the operator updates no running
+# buffer (FusedOutputHead does, from them).  Autocast: fp32, like the other operators; a 16-bit y is widened once by the autocast cast
+# and the gradients come back in the inputs' dtypes.
+# ------------------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op("fiery_b200::output_head", mutates_args=(), device_types="cuda")
+def output_head(y: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, bn_weight: Optional[torch.Tensor], bn_bias: Optional[torch.Tensor],
+                running_mean: Optional[torch.Tensor], running_var: Optional[torch.Tensor], training: bool,
+                eps: float) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """y (N, C, H, W) -> (out, mean, var): out the contiguous (N, n, H, W) fp32 ``conv2d(relu(batch_norm(y)), w1, b1)`` with w1 (n, C,
+    1, 1) and b1 (n,); mean and the biased var the (C,) fp32 statistics used (the batch's when ``training``, else copies of
+    ``running_mean`` / ``running_var``).  relu(batch_norm(y)) is never stored.  Bit-reproducible."""
+    from .decoder import forward
+    return forward(y, w1, b1, bn_weight, bn_bias, running_mean, running_var, training, eps)
+
+
+@output_head.register_fake
+def _(y, w1, b1, bn_weight, bn_bias, running_mean, running_var, training, eps):
+    n, c, h, w = y.shape
+    return (y.new_empty((n, w1.shape[0], h, w), dtype=torch.float32), y.new_empty((c,), dtype=torch.float32),
+            y.new_empty((c,), dtype=torch.float32))
+
+
+@torch.library.custom_op("fiery_b200::output_head_backward", mutates_args=(), device_types="cuda")
+def output_head_backward(grad_out: torch.Tensor, y: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, w1: torch.Tensor,
+                         b1: torch.Tensor, bn_weight: Optional[torch.Tensor], bn_bias: Optional[torch.Tensor], training: bool, eps: float,
+                         need: List[bool]) -> List[torch.Tensor]:
+    """[grad_y, grad_bn_weight, grad_bn_bias, grad_w1, grad_b1] of ``output_head``, each in its input's shape and dtype; ``need`` (5
+    flags in that order) says which are computed, the others come back empty.  Needs only y and the forward's (mean, var)."""
+    from .decoder import backward
+    g = backward(grad_out, y, mean, var, w1, b1, bn_weight, bn_bias, training, eps, need)
+    likes = [y, bn_weight, bn_bias, w1, b1]
+    return [_cast_back(gi, like if like is not None else y) for gi, like in zip(g, likes)]
+
+
+@output_head_backward.register_fake
+def _(grad_out, y, mean, var, w1, b1, bn_weight, bn_bias, training, eps, need):
+    likes = [y, bn_weight, bn_bias, w1, b1]
+    return [like.new_empty(like.shape) if nd and like is not None else y.new_empty((0,)) for like, nd in zip(likes, need)]
+
+
+def _output_head_setup_context(ctx, inputs, output):
+    y, w1, b1, bn_w, bn_b, _rm, _rv, training, eps = inputs
+    _out, mean, var = output
+    ctx.mark_non_differentiable(mean, var)
+    ctx.args = (training, eps)
+    ctx.save_for_backward(y, mean, var, w1, b1, bn_w, bn_b)
+
+
+_OUTPUT_HEAD_GRAD_SLOTS = (0, 3, 4, 1, 2)          # the inputs output_head_backward's gradients belong to
+
+
+def _output_head_backward(ctx, grad_out, _gm, _gv):
+    y, mean, var, w1, b1, bn_w, bn_b = ctx.saved_tensors
+    need = [bool(ctx.needs_input_grad[i]) for i in _OUTPUT_HEAD_GRAD_SLOTS]
+    grads = [None] * 9
+    if not any(need) or grad_out is None:
+        return tuple(grads)
+    g = torch.ops.fiery_b200.output_head_backward(grad_out, y, mean, var, w1, b1, bn_w, bn_b, *ctx.args, need)
+    for slot, gi, nd in zip(_OUTPUT_HEAD_GRAD_SLOTS, g, need):
+        grads[slot] = gi if nd else None
+    return tuple(grads)
+
+
+output_head.register_autograd(_output_head_backward, setup_context=_output_head_setup_context)
+torch.library.register_autocast("fiery_b200::output_head", "cuda", torch.float32)
+
+
 from . import bev_conv, causal_conv  # noqa: E402,F401  (they register first_conv and causal_conv3d through _register_conv)

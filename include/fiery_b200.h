@@ -744,6 +744,58 @@ FIERY_API int fiery_bottleneck_sync_backward_stage(const fiery_bottleneck_desc_t
                                                    float* grad_w_down, float* grad_w_conv, float* grad_w_up, float* const* grad_norms,
                                                    double* local, void* workspace, void* stream);
 
+/*
+ * One of the decoder's output heads after its 3x3 convolution (fiery/models/decoder.py:24-50: BatchNorm2d(C), ReLU, Conv2d(C, n, 1)
+ * with a bias) on `maps` independent (X, Y) maps y with C channels:
+ *   a   = relu(bn(y)) = max(fmaf(scale, y, shift), 0)       bn as fiery_batch_norm_forward's (relu 1): training this call's batch
+ *                                                           statistics, eval the running ones
+ *   out[m, j, p] = sum_c W1[j, c] a[m, c, p] + b1[j]
+ * a is never stored: each value is computed as the 1x1 reads it, exactly the fp32 value fiery_batch_norm_forward (relu 1) would write,
+ * and the tensor core truncates it to TF32; W1 is rounded to TF32 (nearest) when packed, the products accumulate in fp32, and b1 is
+ * added once, exactly, to the accumulator (it enters as the extra channel of a fiery_temporal_entry_forward with value 1).  So out is
+ * fiery_temporal_entry_forward's (batch = maps, frames = 1, E = 1, extra = 1) on fiery_batch_norm_forward's output of y, bit for bit.
+ *
+ * The backward, from g = grad_out: da[m, c, p] = sum_{j < n} W1[j, c] g[m, j, p] with the fp32 W1 (w1), fmaf in ascending j, in fp32; then grad_y, grad_bn_weight, grad_bn_bias are bit for bit fiery_batch_norm_backward's (relu 1) on (y, da), with
+ * scale and shift recomputed from the saved mean and var by the same fp64 formula; grad_w[j, c] = sum_{m, p} g[m, j, p] a[m, c, p] and
+ * grad_b[j] = sum_{m, p} g[m, j, p], a in fp32.  da is never stored: both backward passes recompute it from g.  The backward computes
+ * what is asked for: grad_y, grad_bn_weight, grad_bn_bias, grad_w and grad_b may each be NULL; the pass over y that sums runs only for
+ * a gradient that needs a sum (all but grad_y in eval), the pass that writes grad_y only for grad_y.
+ *
+ * y, grad_y: (maps, C, X, Y) fp32, contiguous; out, grad_out: (maps, n, X, Y) fp32, contiguous.  w: (n, C + 1) fp32, W1 with b1 as its
+ * last column (the pack's input); w1: (n, C) fp32, W1 alone (the backward's); grad_w (n, C), grad_b (n).  bn_weight / bn_bias may be NULL (1 / 0); running_mean / running_var are read in eval only.
+ * mean, var: (C,) fp32, written by the forward (the biased variance; copies of the running statistics in eval) and read by the
+ * backward.  Workspaces: the *_workspace_bytes, 16-byte aligned, contents irrelevant (0 bytes for a rejected descriptor).
+ * Limits (FIERY_E_INVALID, the message names the field): 1 <= channels <= 128 (the entry's K); 1 <= n_out <= 8; maps >= 1;
+ * grid_x, grid_y >= 1 with X*Y % 4 == 0 (16-byte TMA pixel-plane pitch) and X*Y < 2^31; training 0 or 1; eps >= 0; in training
+ * maps * X * Y >= 2; y, out, packed, grad_out, grad_y, workspace 16-byte aligned.
+ *
+ * Summation orders (no atomics, no host synchronisation; bit-reproducible and graph-capturable): the statistics and the norm's
+ * gradients as fiery_batch_norm_*; grad_w and grad_b over the same 4096-pixel pieces of each (m, c) plane -- a piece's partial summed
+ * as fiery_batch_norm_backward sums S1 (grad_b from channel 0's pieces) -- and the partials added in ascending (m, piece) order in
+ * fp64, rounded once.  Kernels: csrc/output_head.cu on csrc/temporal_entry.cu and csrc/batch_norm.cu.
+ */
+typedef struct {
+    int32_t maps;                 /* N: independent maps (batch * frames) */
+    int32_t grid_x;
+    int32_t grid_y;
+    int32_t channels;             /* C */
+    int32_t n_out;                /* n: the 1x1's outputs */
+    int32_t training;             /* 1: batch statistics; 0: running statistics */
+    double eps;
+} fiery_output_head_desc_t;
+
+FIERY_API size_t fiery_output_head_packed_bytes(const fiery_output_head_desc_t* desc);
+FIERY_API int fiery_output_head_pack_weights(const fiery_output_head_desc_t* desc, const float* w, void* packed, void* stream);
+FIERY_API size_t fiery_output_head_forward_workspace_bytes(const fiery_output_head_desc_t* desc);
+FIERY_API int fiery_output_head_forward(const fiery_output_head_desc_t* desc, const float* y, const void* packed, const float* bn_weight,
+                                        const float* bn_bias, const float* running_mean, const float* running_var, float* out, float* mean,
+                                        float* var, void* workspace, void* stream);
+FIERY_API size_t fiery_output_head_backward_workspace_bytes(const fiery_output_head_desc_t* desc);
+FIERY_API int fiery_output_head_backward(const fiery_output_head_desc_t* desc, const float* grad_out, const float* y, const float* mean,
+                                         const float* var, const float* w1, const float* bn_weight, const float* bn_bias, float* grad_y,
+                                         float* grad_bn_weight, float* grad_bn_bias, float* grad_w, float* grad_b, void* workspace,
+                                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif
