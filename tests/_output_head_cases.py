@@ -38,6 +38,90 @@ def _p(t):
     return t.data_ptr() if t is not None else 0
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# the envelope: a shape table, and a host model of the forward's launch (csrc/temporal_entry.cu's te_stages, csrc/common.cuh's
+# persistent_grid) that shows which tile, ring and piece cases the table reaches on a device of a given SM count
+# ------------------------------------------------------------------------------------------------------------------------------
+# (maps, C, n, X, Y): every channel count on both sides of each K padding class edge (Kpad = 32 / 64 / 96 / 128 for C = 1..32 /
+# 33..64 / 65..96 / 97..128) and C = 2 (C = 2 mod 4, so the planes are 8-byte aligned only); every n from 1 to 8 in at least two Kpad
+# classes; X * Y at every class of the 128-pixel tile's last-tile split between the two consumer warpgroups (P % 128 = 4, 60: warpgroup
+# 1 idle; 64: warpgroup 1 at n_valid 0; 68, 124: warpgroup 1 partial; 0: both full) and at the norm's 4096-pixel piece edges (4092,
+# 4096, 4100, 8188); the minimum count of 1 map of 4 pixels; and 7 maps of 19 full tiles (133 tiles: not a multiple of the grid on
+# 114 or 132 SMs).
+SHAPES = [
+    (1, 1, 1, 1, 4),
+    (3, 2, 2, 4, 33),
+    (2, 8, 3, 6, 10),
+    (3, 31, 4, 8, 8),
+    (2, 32, 5, 4, 17),
+    (2, 33, 6, 4, 31),
+    (3, 63, 7, 4, 32),
+    (2, 64, 8, 4, 47),
+    (2, 65, 1, 8, 24),
+    (3, 96, 2, 14, 14),
+    (2, 97, 3, 12, 21),
+    (2, 127, 4, 16, 16),
+    (2, 128, 5, 62, 66),
+    (2, 2, 6, 64, 64),
+    (2, 96, 7, 41, 100),
+    (1, 127, 8, 89, 92),
+    (7, 17, 2, 38, 64),
+]
+# (maps, C, n, X, Y, training): every shape in both modes
+ENVELOPE = [s + (t,) for s in SHAPES for t in (True, False)]
+# the shipped heads: 15 and 18 maps (3 and 6 frames of 5 / 3 samples) of the decoder's 64 x 200 x 200 output, segmentation (2) and
+# center (1): 313 tiles per map, the last with 64 pixels (warpgroup 1 at n_valid 0 in every map)
+SHIPPED = [(m, 64, n, 200, 200, True) for m in (15, 18) for n in (1, 2)]
+
+SMEM_MAX, SMEM_SLACK = 232448, 1024 + 256            # csrc/temporal_entry.cu: TE_SMEM_MAX, TE_SMEM_SLACK
+STG_BYTES, ROW_TABLE_BYTES = 2 * 32 * 66 * 4, 2 * 256 * (8 + 4)
+COEF_BYTES = 128 * 5 * 4                             # 128 BnCoef of 5 floats
+TILE_PX, PIECE_PX = 128, 4096
+KPADS = (32, 64, 96, 128)
+
+
+def kpad(c: int) -> int:
+    return -(-c // 32) * 32
+
+
+def ring_depth(c: int) -> int:
+    """te_stages for output_head_fwd_kernel: the forward weights (one 64-row block of Kpad columns), two staging tiles, the row tables
+    and the coefficients fixed; 128 pixels x Kpad channels per stage; at most 4"""
+    k = kpad(c)
+    fixed = 64 * k * 4 + STG_BYTES + ROW_TABLE_BYTES + COEF_BYTES
+    return min((SMEM_MAX - SMEM_SLACK - fixed) // (4 * k * TILE_PX), 4)
+
+
+def persistent_grid(n_tiles: int, sms: int) -> int:
+    waves = -(-n_tiles // sms)
+    return -(-n_tiles // waves)
+
+
+def reach(case, sms: int) -> dict:
+    """what one ENVELOPE case exercises on a device of ``sms`` SMs"""
+    maps, c, n, h, w, training = case
+    p = h * w
+    tiles = maps * -(-p // TILE_PX)
+    grid = persistent_grid(tiles, sms)
+    depth = ring_depth(c)
+    return {"kpad": kpad(c), "n": n, "depth": depth, "tiles": tiles, "grid": grid, "tail": p % TILE_PX,
+            "wg1_valid": (p - 1) % TILE_PX + 1 - 64,      # warpgroup 1's n_valid on each map's last tile
+            "min_per_cta": tiles // grid, "uneven": tiles % grid != 0,
+            "ring_wrap": tiles // grid >= 2 * depth + 1,  # every CTA uses each ring stage at least twice, so every phase flips
+            "frame_change": grid < tiles and -(-p // TILE_PX) < tiles, "piece_edge": p in (PIECE_PX - 4, PIECE_PX, PIECE_PX + 4, 2 * PIECE_PX - 4),
+            "min_count": training and maps * p == 4}
+
+
+def wrap_case(kp: int, sms: int):
+    """a training case at K padding kp whose tile count makes every CTA of a ``sms``-SM device wrap its ring twice: C = kp - 2, maps
+    of 100 x 130 pixels (102 tiles, the last with 72 pixels), as few maps as that takes"""
+    c, n = kp - 2, {32: 8, 64: 3, 96: 5, 128: 2}[kp]
+    maps = 1
+    while not reach((maps, c, n, 100, 130, True), sms)["ring_wrap"]:
+        maps += 1
+    return (maps, c, n, 100, 130, True)
+
+
 def fused_forward(y, w1, b1, norm, training, eps=1e-5):
     """The C ABI forward into NaN-filled memory between sentinels: ([out, mean, var], buffers)."""
     maps, c, h, w = y.shape
@@ -79,7 +163,16 @@ DEFECTS = {
     "batch_stats_in_eval": "the batch statistics used in eval",
     "unbiased_var": "the unbiased variance used to normalize",
     "da_wrong_operand": "da summed over the forward's output instead of grad_out",
+    "b1_tf32": "b1 rounded to TF32 like W1",
+    "da_packed_w1": "da formed with the packed (TF32-rounded) W1 instead of the fp32 one",
+    "dw1_rz_a": "dW1 formed from the truncated a the tensor core reads",
+    "a_rna": "a rounded to nearest instead of truncated",
+    "eps_outside_sqrt": "eps added outside the square root: weight / (sqrt(var) + eps)",
+    "db1_all_channels": "db1 summed over every channel's pieces instead of channel 0's",
 }
+# the defects that change the forward (the others change only the adjoint); and the module-level one (``running_update``)
+FORWARD_DEFECTS = ("w1_transposed", "unbiased_var", "batch_stats_in_eval", "b1_tf32", "a_rna", "eps_outside_sqrt")
+MODULE_DEFECTS = {"running_var_biased": "the running variance moved toward the biased batch variance"}
 
 
 def _w1(w1, dt, rounding, defect=None):
@@ -108,7 +201,13 @@ def forward(y, w1, b1, norm, training, eps, rounding=True, kernel=None, defect=N
     val, bnd = {"mean": mean, "var": var}, {"mean": em, "var": ev}
     if kernel is not None:
         mean, var = kernel[0].to(dt), kernel[1].to(dt)
-    if rounding:
+    if rounding and defect == "eps_outside_sqrt":
+        w64 = wt.double() if wt is not None else torch.ones_like(mean.double())
+        s = (w64 / (torch.sqrt(var.double()) + eps)).float().double()
+        sh_u = sh_c = ((bs.double() if bs is not None else 0.0) - mean.double() * s).float().double()
+        pre = fmaf(_ch(s), y, _ch(sh_c)).to(dt)
+        a, a_u = _relu(pre), _relu(pre)
+    elif rounding:
         s, sh_u, sh_c = _coef(wt, bs, mean, var, eps, y.device)
         pre = fmaf(_ch(s), y, _ch(sh_c)).to(dt)
         a, a_u = _relu(pre), _relu(fmaf(_ch(s), y, _ch(sh_u))).to(dt)
@@ -119,8 +218,11 @@ def forward(y, w1, b1, norm, training, eps, rounding=True, kernel=None, defect=N
         a = a_u = _relu(pre)
     W = _w1(w1, dt, rounding, defect)
     Z = gc.tf32_rz if rounding else (lambda t: t)
+    if rounding and defect == "a_rna":
+        Z = gc.tf32_rna
     az = Z(a)
-    out = _mm(W.view(*W.shape, 1, 1), az) + _ch(b1.to(dt))
+    bb = gc.tf32_rna(b1.to(dt)) if defect == "b1_tf32" else b1.to(dt)
+    out = _mm(W.view(*W.shape, 1, 1), az) + _ch(bb)
     c = y.shape[1]
     bnd["out"] = (c + 3) * SUM * (_mm(W.abs().view(*W.shape, 1, 1), az.abs()) + _ch(b1.to(dt).abs())) + \
         _mm(W.abs().view(*W.shape, 1, 1), (Z(a_u) - az).abs())
@@ -129,41 +231,84 @@ def forward(y, w1, b1, norm, training, eps, rounding=True, kernel=None, defect=N
     return {"value": val, "bound": bnd, "used": used, "rounding": rounding}
 
 
-def adjoint(fw, w1, b1, norm, g, training, eps, defect=None):
-    """The adjoint of ``forward`` (as it used the run's statistics, when given) in g's dtype: da = W1^T g (fp32 W1), the norm's backward on
-    (y, da) with the ReLU mask of the forward's fmaf, dW1 = g a^T, db1 = sum g; each with its absolute-value twin.  Returns (grads,
-    bounds) keyed as GRAD_KEYS."""
+def _masked_da(fw, w1, g, eps, defect=None):
+    """(gm, its twin, xhat, scale) in g's dtype: da = W1^T g (fp32 W1) through the forward's ReLU mask, and the normalized y"""
     dt = g.dtype
     u = fw["used"]
-    y, a, pre, s, mean, var = (u[k] for k in ("y", "a", "pre", "s", "mean", "var"))
-    maps, c, h, w = y.shape
-    n = g.shape[1]
-    W = _w1(w1, dt, False, defect).view(n, c, 1, 1)
+    y, pre, s, mean, var = (u[k] for k in ("y", "pre", "s", "mean", "var"))
+    n, c = g.shape[1], y.shape[1]
+    W = _w1(w1, dt, defect == "da_packed_w1", defect).view(n, c, 1, 1)
     src = fw["value"]["out"] if defect == "da_wrong_operand" else g
     da, mda = _mm(W.transpose(0, 1), src), _mm(W.abs().transpose(0, 1), src.abs())
     keep = (pre < 0) if defect == "mask_side" else ((pre > 0) | torch.isnan(pre))
     gm, mg = torch.where(keep, da, torch.zeros_like(da)), torch.where(keep, mda, torch.zeros_like(mda))
     inv = _ch(1.0 / torch.sqrt(var.to(dt) + eps))
-    xhat = (y - _ch(mean.to(dt))) * inv
-    sc = _ch(s.to(dt))
-    if training:
-        dy = sc * (gm - gm.mean((0, 2, 3), keepdim=True) - xhat * (gm * xhat).mean((0, 2, 3), keepdim=True))
-        mdy = sc.abs() * (mg + mg.mean((0, 2, 3), keepdim=True) + xhat.abs() * (mg * xhat.abs()).mean((0, 2, 3), keepdim=True))
-    else:
-        dy, mdy = sc * gm, sc.abs() * mg
-    grads = {"gy": dy, "gbw": (gm * xhat).sum((0, 2, 3)), "gbb": gm.sum((0, 2, 3)), "gW": _mm_w(a, g).view(n, c),
-             "gb": torch.zeros(n, dtype=dt, device=g.device) if defect == "bias_grad_dropped" else g.sum((0, 2, 3))}
-    twins = {"gy": mdy, "gbw": (mg * xhat.abs()).sum((0, 2, 3)), "gbb": mg.sum((0, 2, 3)), "gW": _mm_w(a.abs(), g.abs()).view(n, c),
-             "gb": g.abs().sum((0, 2, 3))}
+    return gm, mg, (y - _ch(mean.to(dt))) * inv, _ch(s.to(dt))
+
+
+def _gammas(n, maps, h, w):
+    """gamma along each gradient's longest path: the norm's backward, the pieces' sums and their fp64 sum, da's fmaf chain"""
     bnb = (BN_SUM + 8) * SUM + ELEM                                  # the norm's backward
     pieces = (maps * (-(-(h * w) // 4096)) + BN_SUM + 8) * SUM       # a piece sum, then the pieces' fp64 sum
     gda = (n + 1) * SUM                                              # da's fmaf chain
-    gam = {"gy": gda + bnb, "gbw": gda + pieces + ELEM, "gbb": gda + pieces, "gW": pieces + ELEM, "gb": pieces}
+    return {"gy": gda + bnb, "gbw": gda + pieces + ELEM, "gbb": gda + pieces, "gW": pieces + ELEM, "gb": pieces}
+
+
+def adjoint(fw, w1, b1, norm, g, training, eps, defect=None, totals=None, maps_total=None):
+    """The adjoint of ``forward`` (as it used the run's statistics, when given) in g's dtype: da = W1^T g (fp32 W1), the norm's backward on
+    (y, da) with the ReLU mask of the forward's fmaf, dW1 = g a^T, db1 = sum g; each with its absolute-value twin.  totals (optional):
+    ``batch_totals`` of the whole batch when fw and g are a slice of it, whose per-channel sums the training dy then uses; maps_total: the
+    whole batch's maps, for the reduction depths.  Returns (grads, bounds) keyed as GRAD_KEYS."""
+    dt = g.dtype
+    a = fw["used"]["a"]
+    maps, c, h, w = a.shape
+    n = g.shape[1]
+    gm, mg, xhat, sc = _masked_da(fw, w1, g, eps, defect)
+    if totals is None:
+        cnt = maps * h * w
+        t = {"s1": gm.sum((0, 2, 3)), "s2": (gm * xhat).sum((0, 2, 3)), "t1": mg.sum((0, 2, 3)), "t2": (mg * xhat.abs()).sum((0, 2, 3))}
+    else:
+        cnt, t = totals["count"], totals
+    mean_of = lambda k: _ch(t[k]) / cnt                              # noqa: E731
+    if training:
+        dy = sc * (gm - mean_of("s1") - xhat * mean_of("s2"))
+        mdy = sc.abs() * (mg + mean_of("t1") + xhat.abs() * mean_of("t2"))
+    else:
+        dy, mdy = sc * gm, sc.abs() * mg
+    aw = gc.tf32_rz(a) if defect == "dw1_rz_a" else a
+    gb = g.sum((0, 2, 3))
+    grads = {"gy": dy, "gbw": (gm * xhat).sum((0, 2, 3)), "gbb": gm.sum((0, 2, 3)), "gW": _mm_w(aw, g).view(n, c),
+             "gb": torch.zeros(n, dtype=dt, device=g.device) if defect == "bias_grad_dropped" else
+             gb * c if defect == "db1_all_channels" else gb}
+    twins = {"gy": mdy, "gbw": (mg * xhat.abs()).sum((0, 2, 3)), "gbb": mg.sum((0, 2, 3)), "gW": _mm_w(a.abs(), g.abs()).view(n, c),
+             "gb": g.abs().sum((0, 2, 3))}
+    gam = _gammas(n, maps_total or maps, h, w)
     for k, p in (("gbw", norm[0]), ("gbb", norm[1])):
         if p is None:
             grads[k] = twins[k] = None
     bounds = {k: (gam[k] * twins[k] if twins[k] is not None else None) for k in grads}
     return grads, bounds
+
+
+def batch_totals(y, g, w1, b1, norm, mean, var, training, eps, chunk=1):
+    """The whole batch's adjoint sums formed ``chunk`` maps at a time in fp64 (for a batch too large to restate at once): the per-channel
+    sums of the masked da and da x^ with their twins ({"count", "s1", "s2", "t1", "t2"}, for ``adjoint``'s totals), and the parameter
+    gradients dgamma, dbeta, dW1, db1 with their bounds (the sums of the per-map adjoints)"""
+    maps, c, h, w = y.shape
+    nd = [t.double() if t is not None else None for t in norm]
+    t = {"count": maps * h * w}
+    grads, bounds = {}, {}
+    for j in range(0, maps, chunk):
+        fw = forward(y[j:j + chunk].double(), w1, b1, nd, training, eps, True, (mean.double(), var.double()))
+        gm, mg, xhat, _ = _masked_da(fw, w1, g[j:j + chunk].double(), eps)
+        part = {"s1": gm.sum((0, 2, 3)), "s2": (gm * xhat).sum((0, 2, 3)), "t1": mg.sum((0, 2, 3)), "t2": (mg * xhat.abs()).sum((0, 2, 3))}
+        gj, bj = adjoint(fw, w1, b1, nd, g[j:j + chunk].double(), False, eps, maps_total=maps)    # the sums need no batch terms
+        for k, v in part.items():
+            t[k] = t.get(k, 0) + v
+        for k in ("gbw", "gbb", "gW", "gb"):
+            if gj[k] is not None:
+                grads[k], bounds[k] = grads.get(k, 0) + gj[k], bounds.get(k, 0) + bj[k]
+    return t, grads, bounds
 
 
 def stage_ratios(run, y, w1, b1, norm, training, eps, dtype=torch.float64):
@@ -182,3 +327,18 @@ def grad_ratios(fw, grads, w1, b1, norm, g, training, eps, dtype=torch.float64):
     want, bound = adjoint(fw, w1, b1, nd, g.to(dtype), training, eps)
     return {k: gc.excess(got.reshape(want[k].shape), want[k], bound[k]) for k, got in zip(GRAD_KEYS, grads)
             if got is not None and want[k] is not None}
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the module's running statistics
+# ------------------------------------------------------------------------------------------------------------------------------
+def running_update(rm, rv, mean, var, count, momentum, tracked, defect=None):
+    """torch's BatchNorm update of (running_mean, running_var) from a batch's mean and biased var over ``count`` values per channel:
+    factor = momentum (1 / num_batches_tracked after the increment when None), the variance moved toward the unbiased
+    count / (count - 1) var.  defect "running_var_biased": toward the biased one.  In fp64, with a bound for fp32 bookkeeping."""
+    f = 1.0 / tracked if momentum is None else momentum
+    rm, rv, mean, var = (t.double() for t in (rm, rv, mean, var))
+    v = var if defect == "running_var_biased" else var * (count / (count - 1))
+    want_m, want_v = rm * (1 - f) + mean * f, rv * (1 - f) + v * f
+    bound = lambda a, b, r: 8 * SUM * ((1 - f) * a.abs() + f * b.abs() + r.abs())        # noqa: E731
+    return (want_m, bound(rm, mean, want_m)), (want_v, bound(rv, v, want_v))

@@ -61,16 +61,91 @@ def test_bounds_hold_for_fp32_in_another_order(training):
     assert all(same and v <= 1.0 for v, same in r.values()), r
 
 
+# (training, eps) per defect where it is not (True, 1e-5): the batch statistics in eval need eval; with y's variance near 1/4 the two
+# placements of eps agree to first order in eps, so that defect is shown in eval (running var near 1.1) at eps 1e-3
+DEFECT_MODE = {"batch_stats_in_eval": (False, 1e-5), "eps_outside_sqrt": (False, 1e-3)}
+
+
 @pytest.mark.parametrize("defect", sorted(oc.DEFECTS))
 def test_planted_defects_caught(defect):
-    training = defect != "batch_stats_in_eval"
+    training, eps = DEFECT_MODE.get(defect, (True, 1e-5))
     y, w1, b1, norm, g = _case(training, seed=3)
     nd = [t.double() for t in norm]
-    clean = oc.forward(y.double(), w1, b1, nd, training, 1e-5)
-    bad = oc.forward(y.double(), w1, b1, nd, training, 1e-5, defect=defect)
+    clean = oc.forward(y.double(), w1, b1, nd, training, eps)
+    bad = oc.forward(y.double(), w1, b1, nd, training, eps, defect=defect)
     ratios = [gc.excess(bad["value"][k], clean["value"][k], clean["bound"][k])[0] for k in ("out", "mean", "var")]
-    want, bound = oc.adjoint(clean, w1, b1, nd, g.double(), training, 1e-5)
-    got, _ = oc.adjoint(bad if defect in ("w1_transposed", "unbiased_var", "batch_stats_in_eval") else clean, w1, b1, nd, g.double(),
-                        training, 1e-5, defect=defect)
+    want, bound = oc.adjoint(clean, w1, b1, nd, g.double(), training, eps)
+    got, _ = oc.adjoint(bad if defect in oc.FORWARD_DEFECTS else clean, w1, b1, nd, g.double(), training, eps, defect=defect)
     ratios += [gc.excess(got[k], want[k], bound[k])[0] for k in oc.GRAD_KEYS]
     assert max(ratios) > 10, (defect, ratios)
+
+
+@pytest.mark.parametrize("momentum", [0.1, None], ids=["momentum", "cumulative"])
+@pytest.mark.parametrize("defect", [None] + sorted(oc.MODULE_DEFECTS))
+def test_running_update_is_torchs(defect, momentum):
+    # the module tests hold the running statistics to running_update: it is torch's own update of nn.BatchNorm2d within its bound, and
+    # the biased-variance defect lands far outside it
+    c, count = 6, 2 * 5 * 6
+    bn = torch.nn.BatchNorm2d(c, momentum=momentum).double()
+    x = torch.randn(2, c, 5, 6, generator=torch.Generator().manual_seed(4), dtype=torch.float64) * 0.7 + 0.2
+    with torch.no_grad():
+        bn.running_mean.uniform_(-0.5, 0.5), bn.running_var.uniform_(0.5, 1.5)
+        bn.num_batches_tracked.fill_(2)
+    rm, rv = bn.running_mean.clone(), bn.running_var.clone()
+    bn.train()(x)
+    (wm, bm), (wv, bv) = oc.running_update(rm, rv, x.mean((0, 2, 3)), x.var((0, 2, 3), unbiased=False), count, momentum,
+                                            int(bn.num_batches_tracked), defect)
+    rm_ratio, _ = gc.excess(bn.running_mean, wm, bm)
+    rv_ratio, _ = gc.excess(bn.running_var, wv, bv)
+    if defect is None:
+        assert rm_ratio <= 1.0 and rv_ratio <= 1.0, (rm_ratio, rv_ratio)
+    else:
+        assert rv_ratio > 10, rv_ratio
+
+
+def test_batch_totals_give_the_whole_batch_adjoint():
+    # the chunked adjoint of a batch too large to restate at once: its parameter gradients and the training dy of any one map from the
+    # whole batch's totals are the whole-batch adjoint's
+    training, eps = True, 1e-5
+    y, w1, b1, norm, g = _case(training, seed=5)
+    nd = [t.double() for t in norm]
+    fw = oc.forward(y.double(), w1, b1, nd, training, eps)
+    mean, var = fw["value"]["mean"].float(), fw["value"]["var"].float()
+    fw = oc.forward(y.double(), w1, b1, nd, training, eps, True, (mean.double(), var.double()))
+    want, bound = oc.adjoint(fw, w1, b1, nd, g.double(), training, eps)
+    totals, grads, bounds = oc.batch_totals(y, g, w1, b1, norm, mean, var, training, eps, chunk=1)
+    close = lambda a, b: torch.testing.assert_close(a, b, rtol=1e-12, atol=1e-14)       # noqa: E731
+    for k in ("gbw", "gbb", "gW", "gb"):
+        close(grads[k], want[k])
+        close(bounds[k], bound[k])
+    for j in range(y.shape[0]):
+        fj = oc.forward(y[j:j + 1].double(), w1, b1, nd, training, eps, True, (mean.double(), var.double()))
+        gj, bj = oc.adjoint(fj, w1, b1, nd, g[j:j + 1].double(), training, eps, totals=totals, maps_total=y.shape[0])
+        close(gj["gy"], want["gy"][j:j + 1])
+        close(bj["gy"], bound["gy"][j:j + 1])
+
+
+@pytest.mark.parametrize("sms", [132, 114])
+def test_envelope_reaches_every_launch_case(sms):
+    # the host model of the forward's launch: the table reaches every K padding class with its ring depth, every n in two classes, each
+    # last-tile split, each piece edge, the minimum count and a tile count off the grid; the wrap cases make every CTA use each ring
+    # stage at least twice and change maps between its tiles, at every K padding class
+    assert {k: oc.ring_depth(k) for k in oc.KPADS} == {32: 4, 64: 4, 96: 3, 128: 2}
+    rs = [oc.reach(case, sms) for case in oc.ENVELOPE]
+    assert {c for _, c, *_ in oc.ENVELOPE} >= {1, 2, 8, 31, 32, 33, 63, 64, 65, 96, 97, 127, 128}
+    for n in range(1, 9):
+        assert len({r["kpad"] for r in rs if r["n"] == n}) >= 2, n
+    assert {r["tail"] for r in rs} >= {4, 60, 64, 68, 124, 0}
+    assert {r["wg1_valid"] for r in rs if r["wg1_valid"] <= 0} >= {-60, -4, 0} and any(0 < r["wg1_valid"] < 64 for r in rs)
+    assert {h * w for _, _, _, h, w, _ in oc.ENVELOPE} >= {4092, 4096, 4100, 8188}
+    assert any(r["min_count"] for r in rs)
+    assert any(r["uneven"] and r["min_per_cta"] < 2 for r in rs)
+    assert {t for *_, t in oc.ENVELOPE} == {True, False} and len(oc.ENVELOPE) == 2 * len(oc.SHAPES)
+    for kp in oc.KPADS:
+        case = oc.wrap_case(kp, sms)
+        r = oc.reach(case, sms)
+        assert r["kpad"] == kp and r["ring_wrap"] and r["frame_change"] and r["wg1_valid"] > 0, (kp, r)
+        assert not oc.reach((case[0] - 1,) + case[1:], sms)["ring_wrap"]
+    for case in oc.SHIPPED:
+        r = oc.reach(case, sms)
+        assert r["wg1_valid"] == 0 and r["tiles"] == case[0] * 313 and r["ring_wrap"]
